@@ -90,6 +90,10 @@ SYMBOLS = [
     ("cos_net_last_kernel_ms", _f, [_vp]),
     ("cos_net_launch_count", _i64, [_vp]),
     ("cos_net_fill", _i, [_vp, _i, _i, _u64, _u64, _f]),
+    ("cos_lrn_forward", _i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp]),
+    ("cos_lrn_backward", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp]),
+    ("cos_bias_relu_maxpool_forward", _i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    ("cos_bias_relu_maxpool_backward", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     ("cos_adapter_create", _vp, [_i, _i]),
     ("cos_adapter_destroy", None, [_vp]),
     ("cos_adapter_address", _cp, [_vp]),

@@ -6,11 +6,13 @@
 // "data is NULL", C++ exceptions -> error string instead of a Java exception).
 #include <string.h>
 
+#include <cmath>
 #include <exception>
 #include <string>
 #include <vector>
 
 #include "../../include/caffedistri_b200.h"
+#include "caffe_layers.hpp"
 #include "caffe_net.hpp"
 #include "caffe_proto_io.hpp"
 #include "hdf5_io.hpp"
@@ -355,6 +357,78 @@ int cos_net_fill(cos_net* net, int solver_index, int which, uint64_t seed, uint6
     if (!r->fill(which, seed, stream, amp, &err)) return fail(err);
     return 1;
   })
+}
+
+// ------------------------------------------------------ producer layers
+
+namespace {
+bool bad_nchw(int num, int channels, int height, int width) {
+  return num < 0 || channels < 0 || height < 1 || width < 1;
+}
+int launched(cudaError_t e, const char* what) {
+  if (e == cudaSuccess) return 1;
+  return fail(std::string(what) + ": " + cudaGetErrorString(e) + " (this library has no CPU path)");
+}
+const char* lrn_args(const void* a, const void* b, const void* c, int num, int channels, int height, int width,
+                     int local_size, float beta, float k) {
+  if (!a || !b || !c) return "NULL tensor";
+  if (bad_nchw(num, channels, height, width)) return "bad shape";
+  if (local_size < 1 || local_size % 2 == 0) return "LRN only supports odd values for local_size";
+  if (local_size > cosb::kLrnMaxLocalSize) return "LRN local_size > 15 is not supported";
+  if (!(k > 0.f) || !std::isfinite(beta)) return "LRN needs k > 0 and a finite beta";
+  return nullptr;
+}
+const char* pool_args(const void* a, const void* b, const void* c, int num, int channels, int height, int width,
+                      int kernel, int stride, int pooled_height, int pooled_width) {
+  if (!a || !b || !c) return "NULL tensor";
+  if (bad_nchw(num, channels, height, width)) return "bad shape";
+  if (kernel < 1 || kernel > 15 || stride < 1) return "pooling needs 1 <= kernel <= 15 and stride >= 1";
+  if (cosb::pooled_size(height, kernel, stride) != pooled_height ||
+      cosb::pooled_size(width, kernel, stride) != pooled_width)
+    return "pooled size does not match ceil-mode pooling of the input";
+  return nullptr;
+}
+}  // namespace
+
+int cos_lrn_forward(const float* x, float* y, int num, int channels, int height, int width, int local_size,
+                    float alpha, float beta, float k, void* cuda_stream) {
+  if (const char* e = lrn_args(x, y, y, num, channels, height, width, local_size, beta, k)) return fail(e);
+  return launched(cosb::lrn_forward(x, y, num, channels, height, width, local_size, alpha, beta, k,
+                                    static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_lrn_forward");
+}
+
+int cos_lrn_backward(const float* x, const float* dy, float* dx, int num, int channels, int height, int width,
+                     int local_size, float alpha, float beta, float k, void* cuda_stream) {
+  if (const char* e = lrn_args(x, dy, dx, num, channels, height, width, local_size, beta, k)) return fail(e);
+  return launched(cosb::lrn_backward(x, dy, dx, num, channels, height, width, local_size, alpha, beta, k,
+                                     static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_lrn_backward");
+}
+
+int cos_bias_relu_maxpool_forward(const float* x, const float* bias, float* y, uint8_t* index, int num, int channels,
+                                  int height, int width, int kernel, int stride, int pooled_height, int pooled_width,
+                                  void* cuda_stream) {
+  if (const char* e = pool_args(x, bias, y, num, channels, height, width, kernel, stride, pooled_height, pooled_width))
+    return fail(e);
+  if (!index) return fail("NULL tensor");
+  return launched(cosb::bias_relu_maxpool_forward(x, bias, y, index, num, channels, height, width, kernel, stride,
+                                                  pooled_height, pooled_width,
+                                                  static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_bias_relu_maxpool_forward");
+}
+
+int cos_bias_relu_maxpool_backward(const float* dy, const uint8_t* index, float* dx, float* bias_partials,
+                                   float* dbias, int num, int channels, int height, int width, int kernel, int stride,
+                                   int pooled_height, int pooled_width, void* cuda_stream) {
+  if (const char* e =
+          pool_args(dy, index, dx, num, channels, height, width, kernel, stride, pooled_height, pooled_width))
+    return fail(e);
+  if (!bias_partials || !dbias) return fail("NULL tensor");
+  return launched(cosb::bias_relu_maxpool_backward(dy, index, dx, bias_partials, dbias, num, channels, height, width,
+                                                   kernel, stride, pooled_height, pooled_width,
+                                                   static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_bias_relu_maxpool_backward");
 }
 
 // ------------------------------------------------------------- adapter API

@@ -171,18 +171,42 @@ def write_prototxts(name, directory):
     return solver_file
 
 
+def _relu_maxpool_after(layers, i):
+    """The MAX pool tuple when layers[i+1:i+3] is relu + MAX pool in either order, else None."""
+    nxt = layers[i + 1:i + 3]
+    kinds = sorted(L[0] for L in nxt)
+    if kinds != ["pool", "relu"]:
+        return None
+    pool = next(L for L in nxt if L[0] == "pool")
+    return pool if pool[2] == "MAX" else None
+
+
 def torch_module(name):
-    """PyTorch gradient producer with parameters in learnable_params() order."""
+    """PyTorch gradient producer with parameters in learnable_params() order.  LRN layers and every conv followed
+    by ReLU + MAX pool (either order) run on the library's native kernels (layers.py); the rest is PyTorch."""
     import torch.nn as nn
+    from .layers import LRN, ConvReluMaxPool
     net = NETS[name]
     c, h, w = net["input"]
-    mods, flat = [], None
-    for L in net["layers"]:
+    layers = net["layers"]
+    mods, flat, skip = [], None, 0
+    for i, L in enumerate(layers):
+        if skip:
+            skip -= 1
+            continue
         kind = L[0]
         if kind == "conv":
             _, _, cout, k, s, p, g, _, _ = L
-            mods.append(nn.Conv2d(c, cout, k, stride=s, padding=p, groups=g))
+            conv = nn.Conv2d(c, cout, k, stride=s, padding=p, groups=g)
             h, w, c = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1, cout
+            pool = _relu_maxpool_after(layers, i)
+            if pool is None:
+                mods.append(conv)
+            else:
+                _, _, _, pk, ps = pool
+                mods.append(ConvReluMaxPool(conv, pk, ps))
+                h, w = _pool_out(h, pk, ps), _pool_out(w, pk, ps)
+                skip = 2
         elif kind == "pool":
             _, _, mode, k, s = L
             mods.append((nn.MaxPool2d if mode == "MAX" else nn.AvgPool2d)(k, s, ceil_mode=True))
@@ -196,7 +220,7 @@ def torch_module(name):
         elif kind == "relu":
             mods.append(nn.ReLU(inplace=True))
         elif kind == "lrn":
-            mods.append(nn.LocalResponseNorm(L[2], alpha=L[3], beta=L[4], k=1.0))
+            mods.append(LRN(L[2], alpha=L[3], beta=L[4], k=1.0))
         elif kind == "drop":
             mods.append(nn.Dropout(L[2]))
     return nn.Sequential(*mods)

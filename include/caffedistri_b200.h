@@ -247,6 +247,35 @@ COS_API int64_t cos_net_launch_count(cos_net* net);
  * 4P-byte tensors.  Asynchronous on the net's stream; 1/0. */
 COS_API int cos_net_fill(cos_net* net, int solver_index, int which, uint64_t seed, uint64_t stream, float amp);
 
+/* ------------ native layers for the gradient producer (DESIGN.md section 10) ------ */
+/* Memory-bound layers of CaffeNet / CIFAR-10-quick as single passes.  Every tensor is a
+ * contiguous NCHW fp32 DEVICE buffer of the given sizes.  The calls only enqueue kernels on
+ * `cuda_stream` (NULL = the legacy default stream): they never allocate, synchronise or query
+ * the device, so they may be captured into a CUDA graph.  1 = launched; 0 = bad arguments or a
+ * failed launch (no GPU: there is no CPU path), with the reason in cos_last_error(). */
+
+/* Cross-channel LRN (Caffe's ACROSS_CHANNELS, zero padding at the channel ends), local_size
+ * odd and <= 15:  s_c = k + alpha/local_size * sum_{|c'-c| <= local_size/2} x_c'^2,
+ * y_c = x_c * s_c^-beta.  The backward recomputes s from x (nothing else is stored). */
+COS_API int cos_lrn_forward(const float* x, float* y, int num, int channels, int height, int width, int local_size,
+                            float alpha, float beta, float k, void* cuda_stream);
+COS_API int cos_lrn_backward(const float* x, const float* dy, float* dx, int num, int channels, int height, int width,
+                             int local_size, float alpha, float beta, float k, void* cuda_stream);
+
+/* conv bias + ReLU + MAX pooling (ceil mode, pad 0; either order of ReLU and pooling gives the same
+ * result).  x is the conv output WITHOUT bias, bias has `channels` elements, y and index are
+ * num x channels x pooled_height x pooled_width with pooled_* the ceil-mode sizes (checked).
+ * index holds the position of the window's first maximum of x + bias (0 .. kernel^2-1), or 255
+ * when that maximum is <= 0 (no gradient flows).  kernel <= 15. */
+COS_API int cos_bias_relu_maxpool_forward(const float* x, const float* bias, float* y, uint8_t* index, int num,
+                                          int channels, int height, int width, int kernel, int stride,
+                                          int pooled_height, int pooled_width, void* cuda_stream);
+/* dx (num x channels x height x width, written densely) and dbias (channels, overwritten) from dy and
+ * the forward's index.  bias_partials is num * channels floats of scratch.  Deterministic. */
+COS_API int cos_bias_relu_maxpool_backward(const float* dy, const uint8_t* index, float* dx, float* bias_partials,
+                                           float* dbias, int num, int channels, int height, int width, int kernel,
+                                           int stride, int pooled_height, int pooled_width, void* cuda_stream);
+
 /* --------------------- transport object (reference: util/socket.hpp) ------ */
 /* PeerAdapter = SocketAdapter + SocketChannel of the reference
  * (socket.hpp:22-89): a listener thread on a per-process endpoint whose
