@@ -9,6 +9,11 @@
 //    maximum is <= 0).  The backward gathers dy per conv-output element in PyTorch's max_pool_backward_nchw
 //    order, so dx is bit-identical to threshold_backward(max_pool2d_backward(...)), and reduces the bias
 //    gradient with per-plane partials and a fixed-order second pass (no float atomics: deterministic).
+//
+// Every kernel is a template on the activation storage type T (x, y, dy, dx): fp32, or bf16 for the mixed-precision
+// producer.  Arithmetic is fp32 for both, in the same expressions, so a bf16 kernel's output is the fp32 kernel's
+// output on the upcast inputs rounded once to bf16 (round to nearest even).  The bias, its gradient and the
+// gradient's partials are fp32 for both.
 #include <math.h>
 
 #include "caffe_layers.hpp"
@@ -27,13 +32,22 @@ struct FastDiv {
   __device__ __forceinline__ unsigned div(unsigned n) const { return (__umulhi(n, m) + n) >> s; }
 };
 
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <typename T>
+__device__ __forceinline__ T from_f32(float v);
+template <>
+__device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <>
+__device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
 constexpr int kLrnChunk = 16;   // channels per thread; the halo costs 2*HALF (fwd) / 4*HALF (bwd) extra loads
 constexpr int kLrnBlock = 128;
 
 // blockIdx.x = pixel_block * nchunks + chunk: the chunks of one pixel range run side by side, so the halo
 // loads of neighbouring chunks hit L2.
-template <int HALF>
-__global__ void __launch_bounds__(kLrnBlock) lrn_forward_kernel(const float* __restrict__ x, float* __restrict__ y,
+template <typename T, int HALF>
+__global__ void __launch_bounds__(kLrnBlock) lrn_forward_kernel(const T* __restrict__ x, T* __restrict__ y,
                                                                 int C, FastDiv fd_hw, unsigned npix, int nchunks,
                                                                 float alpha_over_n, float beta, float k) {
   const int chunk = blockIdx.x % nchunks;
@@ -46,7 +60,7 @@ __global__ void __launch_bounds__(kLrnBlock) lrn_forward_kernel(const float* __r
 #pragma unroll
   for (int i = 0; i < kLrnChunk + 2 * HALF; ++i) {
     const int c = c0 - HALF + i;
-    xv[i] = (c >= 0 && c < C) ? x[base + (size_t)c * HW] : 0.f;
+    xv[i] = (c >= 0 && c < C) ? to_f32(x[base + (size_t)c * HW]) : 0.f;
   }
 #pragma unroll
   for (int t = 0; t < kLrnChunk; ++t) {
@@ -56,15 +70,15 @@ __global__ void __launch_bounds__(kLrnBlock) lrn_forward_kernel(const float* __r
 #pragma unroll
       for (int j = 0; j <= 2 * HALF; ++j) ss += xv[t + j] * xv[t + j];
       const float s = k + alpha_over_n * ss;
-      y[base + (size_t)c * HW] = xv[t + HALF] * powf(s, -beta);
+      y[base + (size_t)c * HW] = from_f32<T>(xv[t + HALF] * powf(s, -beta));
     }
   }
 }
 
 // dx_c = dy_c s_c^-beta - (2 alpha beta / n) x_c sum_{c' in window(c)} r_c',  r_c' = dy_c' x_c' s_c'^(-beta-1)
-template <int HALF>
-__global__ void __launch_bounds__(kLrnBlock) lrn_backward_kernel(const float* __restrict__ x,
-                                                                 const float* __restrict__ dy, float* __restrict__ dx,
+template <typename T, int HALF>
+__global__ void __launch_bounds__(kLrnBlock) lrn_backward_kernel(const T* __restrict__ x,
+                                                                 const T* __restrict__ dy, T* __restrict__ dx,
                                                                  int C, FastDiv fd_hw, unsigned npix, int nchunks,
                                                                  float alpha_over_n, float beta, float k, float coef) {
   const int chunk = blockIdx.x % nchunks;
@@ -79,12 +93,12 @@ __global__ void __launch_bounds__(kLrnBlock) lrn_backward_kernel(const float* __
 #pragma unroll
   for (int i = 0; i < NR + 2 * HALF; ++i) {
     const int c = c0 - 2 * HALF + i;
-    xv[i] = (c >= 0 && c < C) ? x[base + (size_t)c * HW] : 0.f;
+    xv[i] = (c >= 0 && c < C) ? to_f32(x[base + (size_t)c * HW]) : 0.f;
   }
 #pragma unroll
   for (int i = 0; i < NR; ++i) {
     const int c = c0 - HALF + i;
-    dv[i] = (c >= 0 && c < C) ? dy[base + (size_t)c * HW] : 0.f;
+    dv[i] = (c >= 0 && c < C) ? to_f32(dy[base + (size_t)c * HW]) : 0.f;
   }
   float r[NR], sb[NR];  // sb = s^-beta
 #pragma unroll
@@ -104,7 +118,7 @@ __global__ void __launch_bounds__(kLrnBlock) lrn_backward_kernel(const float* __
       float acc = 0.f;
 #pragma unroll
       for (int j = 0; j <= 2 * HALF; ++j) acc += r[t + j];
-      dx[base + (size_t)c * HW] = dv[t + HALF] * sb[t + HALF] - coef * xv[t + 2 * HALF] * acc;
+      dx[base + (size_t)c * HW] = from_f32<T>(dv[t + HALF] * sb[t + HALF] - coef * xv[t + 2 * HALF] * acc);
     }
   }
 }
@@ -138,9 +152,10 @@ struct LrnGrid {
 
 template <int HALF>
 struct LrnFwd {
-  static cudaError_t run(const float* x, float* y, int C, const LrnGrid& g, float aon, float beta, float k,
+  template <typename T>
+  static cudaError_t run(const T* x, T* y, int C, const LrnGrid& g, float aon, float beta, float k,
                          cudaStream_t st) {
-    lrn_forward_kernel<HALF><<<(unsigned)g.blocks, kLrnBlock, 0, st>>>(x, y, C, g.fd_hw, (unsigned)g.npix,
+    lrn_forward_kernel<T, HALF><<<(unsigned)g.blocks, kLrnBlock, 0, st>>>(x, y, C, g.fd_hw, (unsigned)g.npix,
                                                                         g.nchunks, aon, beta, k);
     return cudaGetLastError();
   }
@@ -148,9 +163,10 @@ struct LrnFwd {
 
 template <int HALF>
 struct LrnBwd {
-  static cudaError_t run(const float* x, const float* dy, float* dx, int C, const LrnGrid& g, float aon, float beta,
+  template <typename T>
+  static cudaError_t run(const T* x, const T* dy, T* dx, int C, const LrnGrid& g, float aon, float beta,
                          float k, float coef, cudaStream_t st) {
-    lrn_backward_kernel<HALF><<<(unsigned)g.blocks, kLrnBlock, 0, st>>>(x, dy, dx, C, g.fd_hw, (unsigned)g.npix,
+    lrn_backward_kernel<T, HALF><<<(unsigned)g.blocks, kLrnBlock, 0, st>>>(x, dy, dx, C, g.fd_hw, (unsigned)g.npix,
                                                                          g.nchunks, aon, beta, k, coef);
     return cudaGetLastError();
   }
@@ -159,9 +175,9 @@ struct LrnBwd {
 // ---------------------------------------------------------------- bias + ReLU + MAX pool
 
 // KERNEL/STRIDE > 0: compile-time pooling geometry (CaffeNet and CIFAR-10-quick: 3/2); 0: the runtime values
-template <int KERNEL, int STRIDE>
-__global__ void pool_forward_kernel(const float* __restrict__ x, const float* __restrict__ bias,
-                                    float* __restrict__ y, uint8_t* __restrict__ index, unsigned total, FastDiv fd_pp,
+template <typename T, int KERNEL, int STRIDE>
+__global__ void pool_forward_kernel(const T* __restrict__ x, const float* __restrict__ bias,
+                                    T* __restrict__ y, uint8_t* __restrict__ index, unsigned total, FastDiv fd_pp,
                                     FastDiv fd_pw, FastDiv fd_c, int H, int W, int kernel_rt, int stride_rt) {
   const int kernel = KERNEL ? KERNEL : kernel_rt, stride = STRIDE ? STRIDE : stride_rt;
   const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -171,7 +187,7 @@ __global__ void pool_forward_kernel(const float* __restrict__ x, const float* __
   const int ph = (int)fd_pw.div(e);
   const int pw = (int)(e - ph * fd_pw.d);
   const float b = bias[plane - fd_c.div(plane) * fd_c.d];
-  const float* xp = x + (size_t)plane * H * W;
+  const T* xp = x + (size_t)plane * H * W;
   const int hs = ph * stride, ws = pw * stride;
   float vmax = -INFINITY;
   int pos = 0;
@@ -181,7 +197,7 @@ __global__ void pool_forward_kernel(const float* __restrict__ x, const float* __
 #pragma unroll
     for (int dw = 0; dw < (KERNEL ? KERNEL : 15); ++dw) {
       if (dw >= kernel || ws + dw >= W) break;
-      const float v = xp[(hs + dh) * W + ws + dw] + b;
+      const float v = to_f32(xp[(hs + dh) * W + ws + dw]) + b;
       if (v > vmax || isnan(v)) {  // first maximum wins; NaN propagates (max_pool_forward_nchw)
         vmax = v;
         pos = dh * kernel + dw;
@@ -189,23 +205,23 @@ __global__ void pool_forward_kernel(const float* __restrict__ x, const float* __
     }
   }
   const bool pass = vmax > 0.f || isnan(vmax);
-  y[i] = pass ? vmax : 0.f;
+  y[i] = from_f32<T>(pass ? vmax : 0.f);
   index[i] = pass ? (uint8_t)pos : kPoolNoGrad;
 }
 
 // One block per (n, c) plane: dx of every conv-output element is the sum, over ph then pw, of the dy of the
 // windows whose stored position is this element; the plane's sum of dx (= its share of dbias) is reduced in a
 // fixed order into partials[plane].
-template <int KERNEL, int STRIDE>
-__global__ void pool_backward_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ index,
-                                     float* __restrict__ dx, float* __restrict__ partials, FastDiv fd_w, int H,
+template <typename T, int KERNEL, int STRIDE>
+__global__ void pool_backward_kernel(const T* __restrict__ dy, const uint8_t* __restrict__ index,
+                                     T* __restrict__ dx, float* __restrict__ partials, FastDiv fd_w, int H,
                                      int kernel_rt, int stride_rt, int PH, int PW) {
   const int kernel = KERNEL ? KERNEL : kernel_rt, stride = STRIDE ? STRIDE : stride_rt;
   const int W = (int)fd_w.d;
   const long long plane = blockIdx.x;
-  const float* dyp = dy + (size_t)plane * PH * PW;
+  const T* dyp = dy + (size_t)plane * PH * PW;
   const uint8_t* ip = index + (size_t)plane * PH * PW;
-  float* dxp = dx + (size_t)plane * H * W;
+  T* dxp = dx + (size_t)plane * H * W;
   float part = 0.f;
   for (int e = threadIdx.x; e < H * W; e += blockDim.x) {
     const int h = (int)fd_w.div(e), w = e - h * W;
@@ -225,7 +241,7 @@ __global__ void pool_backward_kernel(const float* __restrict__ dy, const uint8_t
           const bool ok = phs + a < phe && pws + b < pwe;
           const int o = ok ? (phs + a) * PW + pws + b : 0;
           id[a][b] = ok ? ip[o] : kPoolNoGrad;
-          v[a][b] = ok ? dyp[o] : 0.f;
+          v[a][b] = ok ? to_f32(dyp[o]) : 0.f;
         }
       }
 #pragma unroll
@@ -237,12 +253,12 @@ __global__ void pool_backward_kernel(const float* __restrict__ dy, const uint8_t
     } else {
       for (int ph = phs; ph < phe; ++ph) {
         for (int pw = pws; pw < pwe; ++pw) {
-          if (ip[ph * PW + pw] == (h - ph * stride) * kernel + (w - pw * stride)) g += dyp[ph * PW + pw];
+          if (ip[ph * PW + pw] == (h - ph * stride) * kernel + (w - pw * stride)) g += to_f32(dyp[ph * PW + pw]);
         }
       }
     }
-    dxp[e] = g;
-    part += g;
+    dxp[e] = from_f32<T>(g);
+    part += g;  // the unrounded g: dbias does not depend on the storage type
   }
   __shared__ float warp_sums[32];
 #pragma unroll
@@ -265,23 +281,89 @@ __global__ void bias_grad_kernel(const float* __restrict__ partials, float* __re
   dbias[c] = s;
 }
 
-}  // namespace
-
-cudaError_t lrn_forward(const float* x, float* y, int num, int channels, int height, int width, int local_size,
-                        float alpha, float beta, float k, cudaStream_t stream) {
+template <typename T>
+cudaError_t lrn_forward_t(const T* x, T* y, int num, int channels, int height, int width, int local_size, float alpha,
+                          float beta, float k, cudaStream_t stream) {
   const LrnGrid g(num, channels, height * width);
   if (g.blocks == 0) return cudaSuccess;
   if (!g.fits()) return cudaErrorInvalidValue;
   return lrn_dispatch<LrnFwd>(local_size / 2, x, y, channels, g, alpha / local_size, beta, k, stream);
 }
 
-cudaError_t lrn_backward(const float* x, const float* dy, float* dx, int num, int channels, int height, int width,
-                         int local_size, float alpha, float beta, float k, cudaStream_t stream) {
+template <typename T>
+cudaError_t lrn_backward_t(const T* x, const T* dy, T* dx, int num, int channels, int height, int width,
+                           int local_size, float alpha, float beta, float k, cudaStream_t stream) {
   const LrnGrid g(num, channels, height * width);
   if (g.blocks == 0) return cudaSuccess;
   if (!g.fits()) return cudaErrorInvalidValue;
   return lrn_dispatch<LrnBwd>(local_size / 2, x, dy, dx, channels, g, alpha / local_size, beta, k,
                               2.f * alpha * beta / local_size, stream);
+}
+
+template <typename T>
+cudaError_t pool_forward_t(const T* x, const float* bias, T* y, uint8_t* index, int num, int channels, int height,
+                           int width, int kernel, int stride, int pooled_h, int pooled_w, cudaStream_t stream) {
+  const long long total = (long long)num * channels * pooled_h * pooled_w;
+  if (total == 0) return cudaSuccess;
+  if (total >= (1ll << 31) || (long long)height * width >= (1ll << 31)) return cudaErrorInvalidValue;
+  const int block = 256;
+  const unsigned grid = (unsigned)((total + block - 1) / block);
+  const FastDiv fpp(pooled_h * pooled_w), fpw(pooled_w), fc(channels);
+  if (kernel == 3 && stride == 2)
+    pool_forward_kernel<T, 3, 2><<<grid, block, 0, stream>>>(x, bias, y, index, (unsigned)total, fpp, fpw, fc,
+                                                             height, width, kernel, stride);
+  else
+    pool_forward_kernel<T, 0, 0><<<grid, block, 0, stream>>>(x, bias, y, index, (unsigned)total, fpp, fpw, fc,
+                                                             height, width, kernel, stride);
+  return cudaGetLastError();
+}
+
+template <typename T>
+cudaError_t pool_backward_t(const T* dy, const uint8_t* index, T* dx, float* dbias_partials, float* dbias, int num,
+                            int channels, int height, int width, int kernel, int stride, int pooled_h, int pooled_w,
+                            cudaStream_t stream) {
+  const long long planes = (long long)num * channels;
+  if (channels == 0) return cudaSuccess;
+  if (planes > 0) {
+    if (planes >= (1ll << 31) || (long long)height * width >= (1ll << 31)) return cudaErrorInvalidValue;
+    // the block size depends on the shape only, so the partials' summation order is fixed
+    const int hw = height * width;
+    const int block = hw >= 256 ? 256 : ((hw + 31) / 32) * 32;
+    const FastDiv fw(width);
+    if (kernel == 3 && stride == 2)
+      pool_backward_kernel<T, 3, 2><<<(unsigned)planes, block, 0, stream>>>(dy, index, dx, dbias_partials, fw,
+                                                                            height, kernel, stride, pooled_h,
+                                                                            pooled_w);
+    else
+      pool_backward_kernel<T, 0, 0><<<(unsigned)planes, block, 0, stream>>>(dy, index, dx, dbias_partials, fw,
+                                                                            height, kernel, stride, pooled_h,
+                                                                            pooled_w);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  bias_grad_kernel<<<(channels + 127) / 128, 128, 0, stream>>>(dbias_partials, dbias, num, channels);
+  return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t lrn_forward(const float* x, float* y, int num, int channels, int height, int width, int local_size,
+                        float alpha, float beta, float k, cudaStream_t stream) {
+  return lrn_forward_t(x, y, num, channels, height, width, local_size, alpha, beta, k, stream);
+}
+cudaError_t lrn_forward(const __nv_bfloat16* x, __nv_bfloat16* y, int num, int channels, int height, int width,
+                        int local_size, float alpha, float beta, float k, cudaStream_t stream) {
+  return lrn_forward_t(x, y, num, channels, height, width, local_size, alpha, beta, k, stream);
+}
+
+cudaError_t lrn_backward(const float* x, const float* dy, float* dx, int num, int channels, int height, int width,
+                         int local_size, float alpha, float beta, float k, cudaStream_t stream) {
+  return lrn_backward_t(x, dy, dx, num, channels, height, width, local_size, alpha, beta, k, stream);
+}
+cudaError_t lrn_backward(const __nv_bfloat16* x, const __nv_bfloat16* dy, __nv_bfloat16* dx, int num, int channels,
+                         int height, int width, int local_size, float alpha, float beta, float k,
+                         cudaStream_t stream) {
+  return lrn_backward_t(x, dy, dx, num, channels, height, width, local_size, alpha, beta, k, stream);
 }
 
 int pooled_size(int in, int kernel, int stride) {
@@ -295,43 +377,26 @@ int pooled_size(int in, int kernel, int stride) {
 cudaError_t bias_relu_maxpool_forward(const float* x, const float* bias, float* y, uint8_t* index, int num,
                                       int channels, int height, int width, int kernel, int stride, int pooled_h,
                                       int pooled_w, cudaStream_t stream) {
-  const long long total = (long long)num * channels * pooled_h * pooled_w;
-  if (total == 0) return cudaSuccess;
-  if (total >= (1ll << 31) || (long long)height * width >= (1ll << 31)) return cudaErrorInvalidValue;
-  const int block = 256;
-  const unsigned grid = (unsigned)((total + block - 1) / block);
-  const FastDiv fpp(pooled_h * pooled_w), fpw(pooled_w), fc(channels);
-  if (kernel == 3 && stride == 2)
-    pool_forward_kernel<3, 2><<<grid, block, 0, stream>>>(x, bias, y, index, (unsigned)total, fpp, fpw, fc, height,
-                                                          width, kernel, stride);
-  else
-    pool_forward_kernel<0, 0><<<grid, block, 0, stream>>>(x, bias, y, index, (unsigned)total, fpp, fpw, fc, height,
-                                                          width, kernel, stride);
-  return cudaGetLastError();
+  return pool_forward_t(x, bias, y, index, num, channels, height, width, kernel, stride, pooled_h, pooled_w, stream);
+}
+cudaError_t bias_relu_maxpool_forward(const __nv_bfloat16* x, const float* bias, __nv_bfloat16* y, uint8_t* index,
+                                      int num, int channels, int height, int width, int kernel, int stride,
+                                      int pooled_h, int pooled_w, cudaStream_t stream) {
+  return pool_forward_t(x, bias, y, index, num, channels, height, width, kernel, stride, pooled_h, pooled_w, stream);
 }
 
 cudaError_t bias_relu_maxpool_backward(const float* dy, const uint8_t* index, float* dx, float* dbias_partials,
                                        float* dbias, int num, int channels, int height, int width, int kernel,
                                        int stride, int pooled_h, int pooled_w, cudaStream_t stream) {
-  const long long planes = (long long)num * channels;
-  if (channels == 0) return cudaSuccess;
-  if (planes > 0) {
-    if (planes >= (1ll << 31) || (long long)height * width >= (1ll << 31)) return cudaErrorInvalidValue;
-    // the block size depends on the shape only, so the partials' summation order is fixed
-    const int hw = height * width;
-    const int block = hw >= 256 ? 256 : ((hw + 31) / 32) * 32;
-    const FastDiv fw(width);
-    if (kernel == 3 && stride == 2)
-      pool_backward_kernel<3, 2><<<(unsigned)planes, block, 0, stream>>>(dy, index, dx, dbias_partials, fw, height,
-                                                                         kernel, stride, pooled_h, pooled_w);
-    else
-      pool_backward_kernel<0, 0><<<(unsigned)planes, block, 0, stream>>>(dy, index, dx, dbias_partials, fw, height,
-                                                                         kernel, stride, pooled_h, pooled_w);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-  }
-  bias_grad_kernel<<<(channels + 127) / 128, 128, 0, stream>>>(dbias_partials, dbias, num, channels);
-  return cudaGetLastError();
+  return pool_backward_t(dy, index, dx, dbias_partials, dbias, num, channels, height, width, kernel, stride, pooled_h,
+                         pooled_w, stream);
+}
+cudaError_t bias_relu_maxpool_backward(const __nv_bfloat16* dy, const uint8_t* index, __nv_bfloat16* dx,
+                                       float* dbias_partials, float* dbias, int num, int channels, int height,
+                                       int width, int kernel, int stride, int pooled_h, int pooled_w,
+                                       cudaStream_t stream) {
+  return pool_backward_t(dy, index, dx, dbias_partials, dbias, num, channels, height, width, kernel, stride, pooled_h,
+                         pooled_w, stream);
 }
 
 }  // namespace cosb

@@ -431,6 +431,53 @@ int cos_bias_relu_maxpool_backward(const float* dy, const uint8_t* index, float*
                   "cos_bias_relu_maxpool_backward");
 }
 
+namespace {
+// extern "C" linkage rules out overloading: one name per constness
+const __nv_bfloat16* bf16_in(const uint16_t* p) { return reinterpret_cast<const __nv_bfloat16*>(p); }
+__nv_bfloat16* bf16_out(uint16_t* p) { return reinterpret_cast<__nv_bfloat16*>(p); }
+}  // namespace
+
+int cos_lrn_forward_bf16(const uint16_t* x, uint16_t* y, int num, int channels, int height, int width,
+                         int local_size, float alpha, float beta, float k, void* cuda_stream) {
+  if (const char* e = lrn_args(x, y, y, num, channels, height, width, local_size, beta, k)) return fail(e);
+  return launched(cosb::lrn_forward(bf16_in(x), bf16_out(y), num, channels, height, width, local_size, alpha, beta, k,
+                                    static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_lrn_forward_bf16");
+}
+
+int cos_lrn_backward_bf16(const uint16_t* x, const uint16_t* dy, uint16_t* dx, int num, int channels, int height,
+                          int width, int local_size, float alpha, float beta, float k, void* cuda_stream) {
+  if (const char* e = lrn_args(x, dy, dx, num, channels, height, width, local_size, beta, k)) return fail(e);
+  return launched(cosb::lrn_backward(bf16_in(x), bf16_in(dy), bf16_out(dx), num, channels, height, width, local_size, alpha,
+                                     beta, k, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_lrn_backward_bf16");
+}
+
+int cos_bias_relu_maxpool_forward_bf16(const uint16_t* x, const float* bias, uint16_t* y, uint8_t* index, int num,
+                                       int channels, int height, int width, int kernel, int stride,
+                                       int pooled_height, int pooled_width, void* cuda_stream) {
+  if (const char* e = pool_args(x, bias, y, num, channels, height, width, kernel, stride, pooled_height, pooled_width))
+    return fail(e);
+  if (!index) return fail("NULL tensor");
+  return launched(cosb::bias_relu_maxpool_forward(bf16_in(x), bias, bf16_out(y), index, num, channels, height, width, kernel,
+                                                  stride, pooled_height, pooled_width,
+                                                  static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_bias_relu_maxpool_forward_bf16");
+}
+
+int cos_bias_relu_maxpool_backward_bf16(const uint16_t* dy, const uint8_t* index, uint16_t* dx, float* bias_partials,
+                                        float* dbias, int num, int channels, int height, int width, int kernel,
+                                        int stride, int pooled_height, int pooled_width, void* cuda_stream) {
+  if (const char* e =
+          pool_args(dy, index, dx, num, channels, height, width, kernel, stride, pooled_height, pooled_width))
+    return fail(e);
+  if (!bias_partials || !dbias) return fail("NULL tensor");
+  return launched(cosb::bias_relu_maxpool_backward(bf16_in(dy), index, bf16_out(dx), bias_partials, dbias, num, channels,
+                                                   height, width, kernel, stride, pooled_height, pooled_width,
+                                                   static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_bias_relu_maxpool_backward_bf16");
+}
+
 // ------------------------------------------------------------- adapter API
 
 cos_adapter* cos_adapter_create(int cluster_size, int rank) {

@@ -21,8 +21,18 @@ from .caffenet import CaffeNet, CosError, _DevArray
 from . import nets
 
 
+PRECISIONS = ("fp32", "bf16")
+
+
 class TorchProducer:
-    def __init__(self, net: CaffeNet, module: torch.nn.Module, seed=1234, use_graph=True):
+    """precision="bf16" runs forward/backward under torch.autocast(bfloat16): convolutions, FC layers and the
+    native layers take bf16 activations, while parameters, their gradients (diff_) and the solver state stay
+    fp32.  An opt-in trade of bitwise parity for speed; "fp32" (the default) is the full-precision producer."""
+
+    def __init__(self, net: CaffeNet, module: torch.nn.Module, seed=1234, use_graph=True, precision="fp32"):
+        if precision not in PRECISIONS:
+            raise CosError(f"unknown producer precision {precision!r} (expected one of {', '.join(PRECISIONS)})")
+        self.precision = precision
         self.net = net
         self.device = torch.device(f"cuda:{net.deviceID(0)}")
         self.module = module.to(self.device)
@@ -51,8 +61,14 @@ class TorchProducer:
 
     def forward_backward(self, x, label):
         """Accumulates d(loss)/d(w) into diff_ (the kernel zeroes it after use)."""
-        logits = self.module(x)
-        loss = self.loss_fn(logits, label)
+        if self.precision == "bf16":
+            # cache_enabled=False: autocast's weight-cast cache must not outlive a CUDA-graph capture; the casts
+            # are recomputed every call, so a replay always reads the current fp32 weights
+            with torch.autocast("cuda", dtype=torch.bfloat16, cache_enabled=False):
+                loss = self.loss_fn(self.module(x), label)
+        else:
+            logits = self.module(x)
+            loss = self.loss_fn(logits, label)
         loss.backward()
         return loss.detach()
 
@@ -128,5 +144,5 @@ class Cluster:
         return net
 
 
-def make_producer(name, net, seed=1234, use_graph=True):
-    return TorchProducer(net, nets.torch_module(name), seed=seed, use_graph=use_graph)
+def make_producer(name, net, seed=1234, use_graph=True, precision="fp32"):
+    return TorchProducer(net, nets.torch_module(name), seed=seed, use_graph=use_graph, precision=precision)

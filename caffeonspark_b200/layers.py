@@ -1,6 +1,10 @@
 """Native producer layers: autograd Functions and modules over the library's LRN and fused
 conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10).
 
+Activations may be fp32 or bf16 (the mixed-precision producer runs these layers under
+torch.autocast, where the convolutions hand them bf16).  bf16 tensors take the bf16 entry points,
+which compute in fp32 and round each output once; the conv bias and its gradient stay fp32.
+
 Every call enqueues on torch.cuda.current_stream() and takes its buffers from torch.empty, so
 forward/backward can be captured with torch.cuda.graph.  CUDA tensors always take the native
 kernels: a missing library or a failed launch raises.  The modules evaluate CPU tensors with the
@@ -20,11 +24,24 @@ def _call(fn, *args):
         raise CosError(_lib.lib().cos_last_error().decode())
 
 
+_ENTRY = {torch.float32: "", torch.bfloat16: "_bf16"}  # activation dtype -> suffix of the C entry point
+
+
 def _check(t):
-    if not t.is_cuda or t.dtype != torch.float32 or t.dim() != 4:
-        raise CosError(f"native producer layers take 4-d fp32 CUDA tensors (no CPU path), got {t.dtype} "
+    if not t.is_cuda or t.dtype not in _ENTRY or t.dim() != 4:
+        raise CosError(f"native producer layers take 4-d fp32 or bf16 CUDA tensors (no CPU path), got {t.dtype} "
                        f"{tuple(t.shape)} on {t.device}")
     return t.contiguous()
+
+
+def _entry(name, dtype):
+    return getattr(_lib.lib(), name + _ENTRY[dtype])
+
+
+def _grad(dy, dtype):
+    if dy.dtype != dtype:
+        raise CosError(f"gradient dtype {dy.dtype} does not match the activation dtype {dtype}")
+    return dy.contiguous()
 
 
 def _stream():
@@ -42,7 +59,8 @@ class LRNFunction(torch.autograd.Function):
     def forward(ctx, x, size, alpha, beta, k):
         x = _check(x)
         y = torch.empty_like(x)
-        _call(_lib.lib().cos_lrn_forward, x.data_ptr(), y.data_ptr(), *x.shape, size, alpha, beta, k, _stream())
+        _call(_entry("cos_lrn_forward", x.dtype), x.data_ptr(), y.data_ptr(), *x.shape, size, alpha, beta, k,
+              _stream())
         ctx.save_for_backward(x)
         ctx.hyper = (size, alpha, beta, k)
         return y
@@ -50,26 +68,31 @@ class LRNFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         (x,) = ctx.saved_tensors
-        dy = dy.contiguous()
+        dy = _grad(dy, x.dtype)
         dx = torch.empty_like(x)
-        _call(_lib.lib().cos_lrn_backward, x.data_ptr(), dy.data_ptr(), dx.data_ptr(), *x.shape, *ctx.hyper,
+        _call(_entry("cos_lrn_backward", x.dtype), x.data_ptr(), dy.data_ptr(), dx.data_ptr(), *x.shape, *ctx.hyper,
               _stream())
         return dx, None, None, None, None
 
 
 class BiasReluMaxPoolFunction(torch.autograd.Function):
-    """y = max_pool2d(relu(x + bias), kernel, stride, ceil_mode=True) for a bias-free conv output x."""
+    """y = max_pool2d(relu(x + bias), kernel, stride, ceil_mode=True) for a bias-free conv output x (fp32 or bf16)
+    and an fp32 bias; y and dx have x's dtype, the bias gradient is fp32."""
 
     @staticmethod
     def forward(ctx, x, bias, kernel, stride):
         x = _check(x)
+        if not bias.is_cuda or bias.dtype != torch.float32 or bias.shape != (x.shape[1],):
+            raise CosError(f"the pool block's bias must be an fp32 CUDA tensor of {x.shape[1]} elements, got "
+                           f"{bias.dtype} {tuple(bias.shape)} on {bias.device}")
         n, c, h, w = x.shape
         ph, pw = pooled_size(h, kernel, stride), pooled_size(w, kernel, stride)
         y = torch.empty((n, c, ph, pw), dtype=x.dtype, device=x.device)
         index = torch.empty((n, c, ph, pw), dtype=torch.uint8, device=x.device)
-        _call(_lib.lib().cos_bias_relu_maxpool_forward, x.data_ptr(), bias.contiguous().data_ptr(), y.data_ptr(),
-              index.data_ptr(), n, c, h, w, kernel, stride, ph, pw, _stream())
+        _call(_entry("cos_bias_relu_maxpool_forward", x.dtype), x.data_ptr(), bias.contiguous().data_ptr(),
+              y.data_ptr(), index.data_ptr(), n, c, h, w, kernel, stride, ph, pw, _stream())
         ctx.save_for_backward(index)
+        ctx.dtype = x.dtype
         ctx.geom = (n, c, h, w, kernel, stride, ph, pw)
         ctx.mark_non_differentiable(index)
         return y
@@ -78,11 +101,11 @@ class BiasReluMaxPoolFunction(torch.autograd.Function):
     def backward(ctx, dy):
         (index,) = ctx.saved_tensors
         n, c, h, w, kernel, stride, ph, pw = ctx.geom
-        dy = dy.contiguous()
+        dy = _grad(dy, ctx.dtype)
         dx = torch.empty((n, c, h, w), dtype=dy.dtype, device=dy.device)
-        partials = torch.empty((n, c), dtype=dy.dtype, device=dy.device)
-        db = torch.empty((c,), dtype=dy.dtype, device=dy.device)
-        _call(_lib.lib().cos_bias_relu_maxpool_backward, dy.data_ptr(), index.data_ptr(), dx.data_ptr(),
+        partials = torch.empty((n, c), dtype=torch.float32, device=dy.device)
+        db = torch.empty((c,), dtype=torch.float32, device=dy.device)
+        _call(_entry("cos_bias_relu_maxpool_backward", ctx.dtype), dy.data_ptr(), index.data_ptr(), dx.data_ptr(),
               partials.data_ptr(), db.data_ptr(), *ctx.geom, _stream())
         return dx, db, None, None
 

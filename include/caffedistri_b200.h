@@ -276,6 +276,24 @@ COS_API int cos_bias_relu_maxpool_backward(const float* dy, const uint8_t* index
                                            float* dbias, int num, int channels, int height, int width, int kernel,
                                            int stride, int pooled_height, int pooled_width, void* cuda_stream);
 
+/* The same four layers with bf16 activations (x, y, dy, dx: uint16_t bit patterns of bfloat16, for the
+ * mixed-precision producer).  Arguments, checks and launch rules are those of the fp32 calls above; bias,
+ * bias_partials and dbias stay fp32.  Arithmetic is fp32 as in the fp32 calls: every y and dx element is the
+ * fp32 call's result on the upcast inputs rounded once to bf16 (round to nearest even), index is the fp32 call's
+ * index, and dbias equals the fp32 call's dbias on the upcast dy bit for bit. */
+COS_API int cos_lrn_forward_bf16(const uint16_t* x, uint16_t* y, int num, int channels, int height, int width,
+                                 int local_size, float alpha, float beta, float k, void* cuda_stream);
+COS_API int cos_lrn_backward_bf16(const uint16_t* x, const uint16_t* dy, uint16_t* dx, int num, int channels,
+                                  int height, int width, int local_size, float alpha, float beta, float k,
+                                  void* cuda_stream);
+COS_API int cos_bias_relu_maxpool_forward_bf16(const uint16_t* x, const float* bias, uint16_t* y, uint8_t* index,
+                                               int num, int channels, int height, int width, int kernel, int stride,
+                                               int pooled_height, int pooled_width, void* cuda_stream);
+COS_API int cos_bias_relu_maxpool_backward_bf16(const uint16_t* dy, const uint8_t* index, uint16_t* dx,
+                                                float* bias_partials, float* dbias, int num, int channels, int height,
+                                                int width, int kernel, int stride, int pooled_height,
+                                                int pooled_width, void* cuda_stream);
+
 /* --------------------- transport object (reference: util/socket.hpp) ------ */
 /* PeerAdapter = SocketAdapter + SocketChannel of the reference
  * (socket.hpp:22-89): a listener thread on a per-process endpoint whose
