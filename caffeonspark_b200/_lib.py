@@ -33,7 +33,8 @@ class cos_solver_desc(ctypes.Structure):
                 ("nstepvalues", ctypes.c_int), ("max_iter", ctypes.c_int), ("momentum", ctypes.c_float),
                 ("weight_decay", ctypes.c_float), ("test_iter", ctypes.c_int), ("test_interval", ctypes.c_int),
                 ("snapshot_prefix", ctypes.c_char_p), ("grad_dtype", ctypes.c_int), ("init_iter", ctypes.c_int),
-                ("regularization_l1", ctypes.c_int)]
+                ("regularization_l1", ctypes.c_int), ("solver_type", ctypes.c_int), ("momentum2", ctypes.c_float),
+                ("delta", ctypes.c_float)]
 
 
 FORWARD_BACKWARD_FN = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(cos_blob),

@@ -39,13 +39,16 @@ def learning_rate(lr_policy, base_lr, gamma=0.0, power=0.0, stepsize=1, stepvalu
     return r, step.value
 
 
+SOLVER_TYPES = {"SGD": 0, "Adam": 1}  # COS_SOLVER_SGD / COS_SOLVER_ADAM
+
+
 class SolverDesc:
     """Solver hyper-parameters + learnable blob layout (cos_solver_desc)."""
 
     def __init__(self, counts, lr_mult=None, decay_mult=None, lr_policy="fixed", base_lr=0.01, gamma=0.0, power=0.0,
                  stepsize=1, stepvalues=(), max_iter=0, momentum=0.0, weight_decay=0.0, test_iter=0,
                  test_interval=0, snapshot_prefix="", grad_dtype="fp32", init_iter=0, batch_size=0,
-                 regularization_type="L2"):
+                 regularization_type="L2", type="SGD", momentum2=0.999, delta=1e-8):
         self.counts = [int(c) for c in counts]
         self.lr_mult = [float(x) for x in (lr_mult if lr_mult is not None else [1.0] * len(self.counts))]
         self.decay_mult = [float(x) for x in (decay_mult if decay_mult is not None else [1.0] * len(self.counts))]
@@ -55,6 +58,14 @@ class SolverDesc:
         self.test_iter, self.test_interval, self.snapshot_prefix = test_iter, test_interval, snapshot_prefix
         self.grad_dtype, self.init_iter, self.batch_size = grad_dtype, init_iter, batch_size
         self.regularization_type = regularization_type
+        if type not in SOLVER_TYPES:
+            raise ValueError(f"solver type must be one of {sorted(SOLVER_TYPES)}, not {type!r}")
+        self.type, self.momentum2, self.delta = type, momentum2, delta  # Adam: momentum is beta1
+
+    @property
+    def history_count(self):
+        """Floats in the solver's history: P for SGD, 2P (m then v) for Adam."""
+        return self.param_count * (2 if self.type == "Adam" else 1)
 
     @property
     def param_count(self):
@@ -62,10 +73,13 @@ class SolverDesc:
 
     def hyper(self):
         """Keyword arguments understood by oracle.Simulation / run_ref_*."""
-        return dict(lr_policy=self.lr_policy, base_lr=self.base_lr, gamma=self.gamma, power=self.power,
+        h = dict(lr_policy=self.lr_policy, base_lr=self.base_lr, gamma=self.gamma, power=self.power,
                     stepsize=self.stepsize, stepvalues=self.stepvalues, max_iter=self.max_iter,
                     momentum=self.momentum, weight_decay=self.weight_decay,
                     regularization_type=self.regularization_type)
+        if self.type == "Adam":
+            h.update(solver_type="Adam", momentum2=self.momentum2, delta=self.delta)
+        return h
 
     def to_c(self):
         n = len(self.counts)
@@ -83,6 +97,8 @@ class SolverDesc:
         d.grad_dtype = 1 if self.grad_dtype == "bf16" else 0
         d.init_iter = int(self.init_iter)
         d.regularization_l1 = 1 if self.regularization_type == "L1" else 0
+        d.solver_type = SOLVER_TYPES[self.type]
+        d.momentum2, d.delta = self.momentum2, self.delta
         return d, keep
 
 
@@ -102,7 +118,9 @@ def parse_solver(solver_conf_file):
                       gamma=d.gamma, power=d.power, stepsize=d.stepsize, stepvalues=list(sv[:d.nstepvalues]),
                       max_iter=d.max_iter, momentum=d.momentum, weight_decay=d.weight_decay, test_iter=d.test_iter,
                       test_interval=d.test_interval, snapshot_prefix=pre.value.decode(), batch_size=bs.value,
-                      regularization_type="L1" if d.regularization_l1 else "L2")
+                      regularization_type="L1" if d.regularization_l1 else "L2",
+                      type="Adam" if d.solver_type == SOLVER_TYPES["Adam"] else "SGD", momentum2=d.momentum2,
+                      delta=d.delta)
 
 
 def read_caffemodel_blob(path, layer_name, blob_index=0):
@@ -307,7 +325,10 @@ class CaffeNet:
         return self._torch_view(self.diff_ptr(solver_index), solver_index)
 
     def history(self, solver_index=0):
-        return self._torch_view(self.history_ptr(solver_index), solver_index)
+        """Solver::history_ flat: P floats for SGD, 2P for Adam (m of every blob, then v of every blob)."""
+        import torch
+        return torch.as_tensor(_DevArray(self.history_ptr(solver_index), self.desc.history_count),
+                               device=f"cuda:{self.deviceID(solver_index)}")
 
     def global_rank(self, solver_index=0):
         """Rank of local solver `solver_index` in the collective of cluster_size x num_local_devices ranks."""

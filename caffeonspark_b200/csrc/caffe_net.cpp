@@ -159,7 +159,7 @@ bool CaffeNet::allocate_device(int start_device_id, bool peer_mappable, std::str
   off_diff_ = off;
   off = align_up(off + fbytes, 4096);
   off_hist_ = off;
-  off = align_up(off + fbytes, 4096);
+  off = align_up(off + fbytes * spec_.history_sets(), 4096);  // Adam: m then v
   off_wire_ = off;
   if (spec_.grad_dtype == COS_GRAD_BF16) off = align_up(off + static_cast<size_t>(count_) * 2, 4096);
   off_recv_ = off;
@@ -272,7 +272,8 @@ int CaffeNet::resolved_kernel() const {
   const int algo = resolved_algo();
   const bool fp32 = spec_.grad_dtype == COS_GRAD_FP32;
   const int64_t bytes = static_cast<int64_t>(count_ * sizeof(float));
-  const bool nvls_ok = nvls_active_ && fp32 && algo == kModeTwoShot;
+  const bool sgd = spec_.solver_type == COS_SOLVER_SGD;  // the TMA and NVLS kernels implement SGD only
+  const bool nvls_ok = sgd && nvls_active_ && fp32 && algo == kModeTwoShot;
   const bool push_ok = world_ > 1 && algo == kModeTwoShot && recv_stride_ > 0;
   const bool ll_ok = world_ > 1 && algo == kModeTwoShot && ll_grad_stride_ > 0;
   if (opt_kernel_ == 0 || opt_kernel_ == 1) return opt_kernel_;
@@ -280,11 +281,11 @@ int CaffeNet::resolved_kernel() const {
   if (opt_kernel_ == 3 && nvls_ok) return 3;
   if (opt_kernel_ == 4 && ll_ok) return 4;
   if (world_ == 1) return 0;
-  if (algo != kModeTwoShot) return bytes >= (2 << 20) ? 1 : 0;
+  if (algo != kModeTwoShot) return sgd && bytes >= (2 << 20) ? 1 : 0;
   if (nvls_ok && (opt_nvls_ == 1 || (world_ >= kNvlsAutoMinWorld && bytes >= opt_nvls_min_bytes_))) return 3;
   if (ll_ok && bytes < opt_ll_max_bytes_) return 4;
-  if (push_ok && (!fp32 || bytes < opt_push_max_bytes_)) return 2;
-  return bytes >= (2 << 20) ? 1 : 0;
+  if (push_ok && (!fp32 || !sgd || bytes < opt_push_max_bytes_)) return 2;
+  return sgd && bytes >= (2 << 20) ? 1 : 0;
 }
 
 float CaffeNet::current_rate() {
@@ -334,6 +335,13 @@ bool CaffeNet::launch(int mode, cudaStream_t stream, std::string* err) {
   p.timeout_ns = static_cast<unsigned long long>(opt_timeout_ms_) * 1000000ull;
   p.status = status_;
   p.trace = opt_trace_ ? reinterpret_cast<unsigned long long*>(status_) + 2 : nullptr;
+  p.solver = spec_.solver_type == COS_SOLVER_ADAM ? kSolverAdam : kSolverSgd;
+  if (p.solver == kSolverAdam) {
+    p.hist2 = hist_ + count_;
+    p.beta2 = spec_.momentum2;
+    p.delta = spec_.delta;
+    p.correction = adam_correction(spec_.momentum, spec_.momentum2, iter_);
+  }
   if (mode != kModeAllGather) {
     if (!learning_rate(spec_.lr_policy, spec_.base_lr, spec_.gamma, spec_.power, spec_.stepsize,
                        spec_.stepvalues.empty() ? nullptr : spec_.stepvalues.data(),
@@ -347,6 +355,11 @@ bool CaffeNet::launch(int mode, cudaStream_t stream, std::string* err) {
   if (opt_timing_) COS_RT(cudaEventRecord(ev_start_, stream));
   const int grid = opt_grid_;
   const int kern = (mode == kModeAllGather) ? 0 : resolved_kernel();
+  if (p.solver != kSolverSgd && (kern == 1 || kern == 3 || opt_kernel_ == 1 || opt_kernel_ == 3)) {
+    *err = "kernel " + std::to_string(opt_kernel_) + " (" + (opt_kernel_ == 1 ? "TMA" : "NVLS") +
+           ") implements SGD only; an Adam net runs on kernel -1 (auto), 0, 2 or 4";
+    return false;
+  }
   cudaError_t e;
   switch (kern) {
     case 1: e = launch_fused_sync_sgd_tma(p, grid, stream); break;
@@ -444,7 +457,8 @@ bool CaffeNet::fill(int which, uint64_t seed, uint64_t stream_id, float amp, std
     return false;
   }
   COS_RT(cudaSetDevice(device_));
-  COS_RT(launch_fill(dst, count_, seed, stream_id, amp, stream_));
+  const uint64_t n = which == 2 ? count_ * spec_.history_sets() : count_;
+  COS_RT(launch_fill(dst, n, seed, stream_id, amp, stream_));
   COS_RT(cudaStreamSynchronize(stream_));
   return true;
 }
@@ -657,7 +671,8 @@ int CaffeNet::snapshot(std::string* err) {
     return -1;
   }
   if (!check_status(err)) return -1;
-  std::vector<float> w(count_), h(count_);
+  const int sets = spec_.history_sets();  // Adam: every owner's shard of m and of v
+  std::vector<float> w(count_), h(count_ * sets);
   cudaError_t e = cudaMemcpy(w.data(), data_, count_ * sizeof(float), cudaMemcpyDeviceToHost);
   const bool sharded_hist = world_ > 1 && resolved_algo() == kModeTwoShot;
   for (int r = 0; r < world_ && e == cudaSuccess; ++r) {
@@ -669,7 +684,16 @@ int CaffeNet::snapshot(std::string* err) {
       *err = "snapshot: history of rank " + std::to_string(r) + " is not mapped (connect() first)";
       return -1;
     }
-    if (size) e = cudaMemcpy(h.data() + offs, src + offs, size * sizeof(float), cudaMemcpyDeviceToHost);
+    for (int q = 0; q < sets && e == cudaSuccess; ++q) {
+      const uint64_t o = static_cast<uint64_t>(q) * count_ + offs;
+      if (size) e = cudaMemcpy(h.data() + o, src + o, size * sizeof(float), cudaMemcpyDeviceToHost);
+    }
+  }
+  // SolverState.history = history_: nblobs blobs for SGD; for Adam the m blobs, then the v blobs
+  std::vector<BlobView> hv = blob_views(h.data());
+  if (sets == 2) {
+    std::vector<BlobView> v2 = blob_views(h.data() + count_);
+    hv.insert(hv.end(), v2.begin(), v2.end());
   }
   if (e != cudaSuccess) {
     *err = rt_err("snapshot: copy to host", e);
@@ -678,11 +702,11 @@ int CaffeNet::snapshot(std::string* err) {
   const std::string model = snapshot_filename(iter_, false), state = snapshot_filename(iter_, true);
   if (spec_.snapshot_hdf5) {  // solver.cpp:417-418 SnapshotToHDF5 + sgd_solver.cpp:251-252 (csrc/hdf5_io.cpp)
     if (!write_caffemodel_h5(model, blob_views(w.data()), err)) return -1;
-    if (!write_solverstate_h5(state, iter_, current_step_, model, blob_views(h.data()), err)) return -1;
+    if (!write_solverstate_h5(state, iter_, current_step_, model, hv, err)) return -1;
     return iter_;
   }
   if (!write_caffemodel(model, spec_.net_name, blob_views(w.data()), err)) return -1;
-  if (!write_solverstate(state, iter_, current_step_, model, blob_views(h.data()), err)) return -1;
+  if (!write_solverstate(state, iter_, current_step_, model, hv, err)) return -1;
   return iter_;
 }
 
@@ -696,24 +720,27 @@ bool CaffeNet::restore(const std::string& model_file, const std::string& state_f
     std::string learned;
     std::vector<ParsedBlob> hist;
     if (!read_solverstate(state_file, &it, &step, &learned, &hist, err)) return false;
-    if (hist.size() != spec_.counts.size()) {
+    const size_t nb = spec_.counts.size(), sets = static_cast<size_t>(spec_.history_sets());
+    if (hist.size() != nb * sets) {
       *err = "'" + state_file + "' is not a matching snapshot of this net: " + std::to_string(hist.size()) +
-             " history blobs, the net has " + std::to_string(spec_.counts.size()) + " learnable blobs";
+             " history blobs, the net has " + std::to_string(nb) + " learnable blobs" +
+             (sets == 2 ? " and an Adam solver, which keeps " + std::to_string(nb * sets) : std::string());
       return false;
     }
-    std::vector<float> flat(count_, 0.f);
+    std::vector<float> flat(count_ * sets, 0.f);
     uint64_t off = 0;
     for (size_t k = 0; k < hist.size(); ++k) {
-      if (hist[k].data.size() != static_cast<size_t>(spec_.counts[k])) {
+      if (k == nb) off = count_;  // Adam: the v blobs start the second half
+      if (hist[k].data.size() != static_cast<size_t>(spec_.counts[k % nb])) {
         *err = "'" + state_file + "' is not a matching snapshot of this net: history blob " + std::to_string(k) +
                " has " + std::to_string(hist[k].data.size()) + " elements, expected " +
-               std::to_string(spec_.counts[k]);
+               std::to_string(spec_.counts[k % nb]);
         return false;
       }
       memcpy(flat.data() + off, hist[k].data.data(), hist[k].data.size() * sizeof(float));
       off += hist[k].data.size();
     }
-    COS_RT(cudaMemcpy(hist_, flat.data(), count_ * sizeof(float), cudaMemcpyHostToDevice));
+    COS_RT(cudaMemcpy(hist_, flat.data(), flat.size() * sizeof(float), cudaMemcpyHostToDevice));
     iter_ = it;
     current_step_ = step;
     spec_.init_iter = it;

@@ -81,6 +81,15 @@ bool spec_from_desc(const cos_solver_desc* d, SolverSpec* s, std::string* err) {
   s->grad_dtype = d->grad_dtype;
   s->init_iter = d->init_iter;
   s->regularization_type = d->regularization_l1 ? "L1" : "L2";
+  if (d->solver_type != COS_SOLVER_SGD && d->solver_type != COS_SOLVER_ADAM) {
+    *err = "solver_type must be COS_SOLVER_SGD (0) or COS_SOLVER_ADAM (1)";
+    return false;
+  }
+  s->solver_type = d->solver_type;
+  s->type = d->solver_type == COS_SOLVER_ADAM ? "Adam" : "SGD";
+  s->momentum2 = d->momentum2;
+  s->delta = d->delta;
+  if (!cosb::check_solver_layout(*s, err)) return false;
   float r;
   int step = 0;
   if (!cosb::learning_rate(s->lr_policy, s->base_lr, s->gamma, s->power, s->stepsize,
@@ -741,6 +750,9 @@ int cos_parse_solver(const char* solver_conf_file, cos_solver_desc* desc, int64_
     desc->momentum = s.momentum;
     desc->weight_decay = s.weight_decay;
     desc->regularization_l1 = s.regularization_type == "L1" ? 1 : 0;
+    desc->solver_type = s.solver_type;
+    desc->momentum2 = s.momentum2;
+    desc->delta = s.delta;
     desc->test_iter = s.test_iter;
     desc->test_interval = s.test_interval;
     if (batch_size) *batch_size = s.batch_size;

@@ -97,7 +97,8 @@ __device__ __forceinline__ float4 reduce_vec_any(const SyncParams& p, int s, uin
 
 // N = compile-time world size (0 = runtime world, any size up to kMaxRanks).
 // (The in-switch NVLS variant lives in fused_sync_sgd_nvls.cu.)
-template <int N, bool BF16>
+// ADAM: Adam update with the second history half (sync_device.cuh), false = SGD.
+template <int N, bool BF16, bool ADAM = false>
 __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(const SyncParams p) {
   extern __shared__ unsigned char smem_raw[];
   __shared__ int s_abort;
@@ -207,6 +208,8 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
         const uint64_t i = (r.vec_lo + j) << 2;
         float4 w = *reinterpret_cast<const float4*>(wl + i);
         float4 h = *reinterpret_cast<const float4*>(hl + i);
+        float4 v;
+        load_v<ADAM>(p, i, v);
         float4 g;
         if (p.mode == kModeLocal) {
           g = ld_stream(p.diff[rank] + i);  // no scale at N == 1 (CaffeNet.cpp:206-216: no sync object)
@@ -219,8 +222,9 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
         } else {
           g = reduce_vec_any<N, BF16>(p, s, i);
         }
-        sgd_vec(p, cur, i, g, w, h);
+        update_vec<ADAM>(p, cur, i, g, w, h, v);
         *reinterpret_cast<float4*>(hl + i) = h;
+        store_v<ADAM>(p, i, v);
         *reinterpret_cast<float4*>(wl + i) = w;
         if (push) {
 #pragma unroll
@@ -249,8 +253,7 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
           float g = (p.mode == kModeLocal) ? p.diff[rank][i] : reduce_scalar<BF16>(p, s, i);
           if (BF16 && p.mode == kModeLocal) g = bf16_bits_to_float(float_to_bf16_bits(g));
           float w = wl[i], h = hl[i];
-          sgd_element(g, w, h, __fmul_rn(p.rate, c2.lr_mult[c2.k]), __fmul_rn(p.weight_decay, c2.decay_mult[c2.k]),
-                      p.momentum, p.l1);
+          update_element<ADAM>(p, c2, i, g, w, h);
           hl[i] = h;
           wl[i] = w;
           if (push) {
@@ -318,8 +321,14 @@ uint64_t host_mix64(uint64_t z) {
 
 template <int N>
 cudaError_t launch_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (p.grad_bf16) fused_sync_sgd_kernel<N, true><<<grid, block, smem, stream>>>(p);
-  else fused_sync_sgd_kernel<N, false><<<grid, block, smem, stream>>>(p);
+  if (p.solver == kSolverAdam) {
+    if (p.grad_bf16) fused_sync_sgd_kernel<N, true, true><<<grid, block, smem, stream>>>(p);
+    else fused_sync_sgd_kernel<N, false, true><<<grid, block, smem, stream>>>(p);
+  } else if (p.grad_bf16) {
+    fused_sync_sgd_kernel<N, true><<<grid, block, smem, stream>>>(p);
+  } else {
+    fused_sync_sgd_kernel<N, false><<<grid, block, smem, stream>>>(p);
+  }
   return cudaGetLastError();
 }
 

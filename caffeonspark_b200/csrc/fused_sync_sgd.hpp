@@ -66,7 +66,16 @@ struct SyncParams {
   int* status;                      // local device word: 0 ok, else error code
   unsigned long long* trace;        // optional: 13 x %globaltimer of CTA 0: [0..4] phase boundaries, [5..8] / [9..12]
                                     // inside barrier A / B (entered, release fence done, flag arrived, acquire done)
+  // Appended so that the fields above keep their offsets.  Adam (solver == kSolverAdam): hist holds m, hist2 = hist
+  // + count holds v, momentum is beta1, and correction = sqrt(1 - beta2^t) / (1 - beta1^t) of this iteration.
+  int solver;
+  float* hist2;
+  float beta2;
+  float delta;
+  float correction;
 };
+
+enum SolverKind : int { kSolverSgd = 0, kSolverAdam = 1 };
 
 // Launches the vector (LDG/STG) kernel.  grid/block 0 = defaults.
 cudaError_t launch_fused_sync_sgd(const SyncParams& p, int grid, int block, cudaStream_t stream);

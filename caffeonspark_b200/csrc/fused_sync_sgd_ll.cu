@@ -131,7 +131,8 @@ __device__ __forceinline__ uint64_t edge_of_thread(const ShardRange& r, unsigned
 }
 
 // N = compile-time world size, 2..8 (the N-1 polled slots live in registers)
-template <int N, bool BF16>
+// ADAM: Adam update with the second history half (sync_device.cuh), false = SGD.
+template <int N, bool BF16, bool ADAM = false>
 __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const SyncParams p) {
   extern __shared__ unsigned char smem_raw[];
   __shared__ int s_abort;
@@ -249,6 +250,8 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
       float4 x = ld_stream(g + i);
       float4 w = *reinterpret_cast<const float4*>(wl + i);
       float4 h = *reinterpret_cast<const float4*>(hl + i);
+      float4 v;
+      load_v<ADAM>(p, i, v);
       if (BF16) {
         x.x = bf16_bits_to_float(float_to_bf16_bits(x.x)); x.y = bf16_bits_to_float(float_to_bf16_bits(x.y));
         x.z = bf16_bits_to_float(float_to_bf16_bits(x.z)); x.w = bf16_bits_to_float(float_to_bf16_bits(x.w));
@@ -285,8 +288,9 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
         acc.w = __fadd_rn(__fmul_rn(inv, y.w), acc.w);
       }
       if (!alive) break;
-      sgd_vec(p, cur, i, acc, w, h);
+      update_vec<ADAM>(p, cur, i, acc, w, h, v);
       *reinterpret_cast<float4*>(hl + i) = h;
+      store_v<ADAM>(p, i, v);
       *reinterpret_cast<float4*>(wl + i) = w;
       const uint64_t wa = ll_word(__float_as_uint(w.x), flag), wb = ll_word(__float_as_uint(w.y), flag);
       const uint64_t wc = ll_word(__float_as_uint(w.z), flag), wd = ll_word(__float_as_uint(w.w), flag);
@@ -315,8 +319,7 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
         }
         if (alive) {
           float w = wl[e], h = hl[e];
-          sgd_element(acc, w, h, __fmul_rn(p.rate, c2.lr_mult[c2.k]), __fmul_rn(p.weight_decay, c2.decay_mult[c2.k]),
-                      p.momentum, p.l1);
+          update_element<ADAM>(p, c2, e, acc, w, h);
           hl[e] = h;
           wl[e] = w;
           for (int k = 1; k < world; ++k) {
@@ -387,8 +390,14 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
 
 template <int N>
 cudaError_t launch_ll_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (p.grad_bf16) fused_sync_sgd_ll_kernel<N, true><<<grid, block, smem, stream>>>(p);
-  else fused_sync_sgd_ll_kernel<N, false><<<grid, block, smem, stream>>>(p);
+  if (p.solver == kSolverAdam) {
+    if (p.grad_bf16) fused_sync_sgd_ll_kernel<N, true, true><<<grid, block, smem, stream>>>(p);
+    else fused_sync_sgd_ll_kernel<N, false, true><<<grid, block, smem, stream>>>(p);
+  } else if (p.grad_bf16) {
+    fused_sync_sgd_ll_kernel<N, true><<<grid, block, smem, stream>>>(p);
+  } else {
+    fused_sync_sgd_ll_kernel<N, false><<<grid, block, smem, stream>>>(p);
+  }
   return cudaGetLastError();
 }
 

@@ -283,6 +283,7 @@ cudaError_t launch_share(const SyncParams& p, int grid, size_t smem, cudaStream_
 cudaError_t launch_fused_sync_sgd_nvls(const SyncParams& p, int grid, cudaStream_t stream) {
   if (p.world < 2 || p.world > kMaxRanks || p.rank < 0 || p.rank >= p.world) return cudaErrorInvalidValue;
   if (p.mode != kModeTwoShot || p.grad_bf16 || !p.mc_data || !p.mc_diff) return cudaErrorInvalidValue;
+  if (p.solver != kSolverSgd) return cudaErrorInvalidValue;  // SGD only
   int dev = 0, sms = kTargetSms;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);

@@ -65,7 +65,8 @@ __device__ __forceinline__ uint64_t edge_element(const ShardRange& r, unsigned t
 }
 
 // N = compile-time world size (2..8), 0 = run-time world (<= kMaxRanks)
-template <int N, bool BF16>
+// ADAM: Adam update with the second history half (sync_device.cuh), false = SGD.
+template <int N, bool BF16, bool ADAM = false>
 __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(const SyncParams p) {
   extern __shared__ unsigned char smem_raw[];
   __shared__ int s_abort;
@@ -229,6 +230,8 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
       }
       float4 w = *reinterpret_cast<const float4*>(wl + i);
       float4 h = *reinterpret_cast<const float4*>(hl + i);
+      float4 v;
+      load_v<ADAM>(p, i, v);
       if (BF16) {
         x[0].x = round_bf16(x[0].x); x[0].y = round_bf16(x[0].y);
         x[0].z = round_bf16(x[0].z); x[0].w = round_bf16(x[0].w);
@@ -258,8 +261,9 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
           acc.w = __fadd_rn(__fmul_rn(inv, y.w), acc.w);
         }
       }
-      sgd_vec(p, cur, i, acc, w, h);
+      update_vec<ADAM>(p, cur, i, acc, w, h, v);
       *reinterpret_cast<float4*>(hl + i) = h;
+      store_v<ADAM>(p, i, v);
       *reinterpret_cast<float4*>(wl + i) = w;
       if (N > 0) {
 #pragma unroll
@@ -292,8 +296,7 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
           acc = __fadd_rn(__fmul_rn(inv, y), acc);
         }
         float w = wl[i], h = hl[i];
-        sgd_element(acc, w, h, __fmul_rn(p.rate, c2.lr_mult[c2.k]), __fmul_rn(p.weight_decay, c2.decay_mult[c2.k]),
-                    p.momentum, p.l1);
+        update_element<ADAM>(p, c2, i, acc, w, h);
         hl[i] = h;
         wl[i] = w;
         for (int k = 1; k < world; ++k) {
@@ -325,8 +328,14 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
 
 template <int N>
 cudaError_t launch_push_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (p.grad_bf16) fused_sync_sgd_push_kernel<N, true><<<grid, block, smem, stream>>>(p);
-  else fused_sync_sgd_push_kernel<N, false><<<grid, block, smem, stream>>>(p);
+  if (p.solver == kSolverAdam) {
+    if (p.grad_bf16) fused_sync_sgd_push_kernel<N, true, true><<<grid, block, smem, stream>>>(p);
+    else fused_sync_sgd_push_kernel<N, false, true><<<grid, block, smem, stream>>>(p);
+  } else if (p.grad_bf16) {
+    fused_sync_sgd_push_kernel<N, true><<<grid, block, smem, stream>>>(p);
+  } else {
+    fused_sync_sgd_push_kernel<N, false><<<grid, block, smem, stream>>>(p);
+  }
   return cudaGetLastError();
 }
 

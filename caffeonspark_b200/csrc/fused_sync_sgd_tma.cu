@@ -438,7 +438,7 @@ fused_sync_sgd_tma_kernel(const SyncParams p, const int tile_elems) {
 
 cudaError_t launch_fused_sync_sgd_tma(const SyncParams& p, int grid, cudaStream_t stream) {
   if (p.world < 1 || p.world > kMaxRanks || p.rank < 0 || p.rank >= p.world) return cudaErrorInvalidValue;
-  if (p.mode == kModeAllGather) return cudaErrorInvalidValue;
+  if (p.mode == kModeAllGather || p.solver != kSolverSgd) return cudaErrorInvalidValue;  // SGD only
   int dev = 0;
   cudaGetDevice(&dev);
   int sms = kTargetSms;

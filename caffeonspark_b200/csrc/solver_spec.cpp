@@ -29,6 +29,12 @@ void chunk(uint64_t param_count, int cluster_size, int peer, uint64_t* offs, uin
 // sgd_solver.cpp:27-63 with Dtype = float.  The reference's unqualified
 // pow()/exp() take float sub-expressions, evaluate in double and the product
 // with base_lr is rounded to float when assigned to `Dtype rate`.
+float adam_correction(float beta1, float beta2, int iter) {
+  const int t = iter + 1;
+  return static_cast<float>(sqrt(1.0 - pow(static_cast<double>(beta2), t)) /
+                            (1.0 - pow(static_cast<double>(beta1), t)));
+}
+
 bool learning_rate(const std::string& policy, float base_lr, float gamma, float power, int stepsize,
                    const int* stepvalues, int nstepvalues, int max_iter, int iter, int* current_step,
                    float* rate) {
@@ -467,6 +473,17 @@ bool parse_net_prototxt_text(const std::string& text, SolverSpec* spec, std::str
   return net_layout(net, spec, err);
 }
 
+bool check_solver_layout(const SolverSpec& spec, std::string* err) {
+  uint64_t n = 0;
+  for (int64_t c : spec.counts) n += static_cast<uint64_t>(c);
+  if (spec.solver_type == 1 && n == 0) {
+    *err = "solver type 'Adam' needs learnable parameters; for a net without any, only SGD is on the accelerated "
+           "path (with no history blobs, its Adam and SGD solver states could not be told apart)";
+    return false;
+  }
+  return true;
+}
+
 bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std::string* err) {
   std::string text;
   if (!read_file(solver_path, &text)) {
@@ -501,10 +518,14 @@ bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std
     type = st;
   }
   spec->type = type;
-  if (spec->type != "SGD") {
+  if (spec->type != "SGD" && spec->type != "Adam" && spec->type != "ADAM") {
     *err = "solver type '" + spec->type + "' is not on the accelerated path (only SGD with momentum is)";
     return false;
   }
+  if (spec->type == "ADAM") spec->type = "Adam";  // deprecated enum spelling (caffe.proto SolverType)
+  spec->solver_type = spec->type == "Adam" ? 1 : 0;
+  spec->momentum2 = static_cast<float>(s.num("momentum2", 0.999));
+  spec->delta = static_cast<float>(s.num("delta", 1e-8));
   if (spec->regularization_type != "L2" && spec->regularization_type != "L1") {
     *err = "Unknown regularization type: " + spec->regularization_type;  // sgd_solver.cpp:169-171
     return false;
@@ -519,7 +540,7 @@ bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std
   }
   // locate the net definition
   if (const Node* inl = s.first("net_param") ? s.first("net_param") : s.first("train_net_param")) {
-    return net_layout(*inl, spec, err);
+    return net_layout(*inl, spec, err) && check_solver_layout(*spec, err);
   }
   std::string net_path = s.str("net", "");
   if (net_path.empty()) net_path = s.str("train_net", "");
@@ -542,7 +563,7 @@ bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std
     *err = "cannot read net file '" + net_path + "' named by '" + solver_path + "'";
     return false;
   }
-  return parse_net_prototxt_text(net_text, spec, err);
+  return parse_net_prototxt_text(net_text, spec, err) && check_solver_layout(*spec, err);
 }
 
 }  // namespace cosb

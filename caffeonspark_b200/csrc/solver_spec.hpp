@@ -37,6 +37,8 @@ struct SolverSpec {
   std::string snapshot_prefix;
   std::string regularization_type = "L2";
   std::string type = "SGD";
+  int solver_type = 0;                   // COS_SOLVER_SGD / COS_SOLVER_ADAM (from type)
+  float momentum2 = 0.999f, delta = 1e-8f;  // Adam's beta2 and epsilon (caffe.proto:213-218); momentum is beta1
   int iter_size = 1;
   float clip_gradients = -1.f;
   bool solver_mode_gpu = true;
@@ -48,10 +50,16 @@ struct SolverSpec {
   int init_iter = 0;
 
   uint64_t param_count() const;  // max(1, sum counts): parallel.cpp:60-68
+  // history blobs per learnable blob: 1 for SGD, 2 for Adam (AdamPreSolve appends v, adam_solver.cpp:8-17)
+  int history_sets() const { return solver_type == 1 ? 2 : 1; }
 };
 
 // SocketSync::chunk (socket_sync_cpu.cpp:46-54).
 void chunk(uint64_t param_count, int cluster_size, int peer, uint64_t* offs, uint64_t* size);
+
+// Adam's bias correction sqrt(1 - beta2^t) / (1 - beta1^t) for t = iter + 1 (adam_solver.cpp:39-41): pow with a
+// float base and an int exponent is the double pow, so the whole expression is double, rounded once to float.
+float adam_correction(float beta1, float beta2, int iter);
 
 // SGDSolver::GetLearningRate (sgd_solver.cpp:27-63), Dtype = float.
 // Returns false for an unknown policy.
@@ -62,6 +70,9 @@ bool learning_rate(const std::string& policy, float base_lr, float gamma, float 
 // Parses a solver prototxt and the net it references (net:, train_net: or
 // inline net_param/train_net_param) and fills `spec`.
 bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std::string* err);
+// Checks that apply once the layout is known: an Adam solver needs at least one learnable element (a snapshot of a
+// net without any holds no history blobs, so restore could not refuse a state of the other solver kind).
+bool check_solver_layout(const SolverSpec& spec, std::string* err);
 // Parses only a net prototxt text (TRAIN phase) into the layout part of spec.
 bool parse_net_prototxt_text(const std::string& text, SolverSpec* spec, std::string* err);
 

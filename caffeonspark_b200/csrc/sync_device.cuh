@@ -10,6 +10,7 @@
 #include <stdint.h>
 
 #include "fused_sync_sgd.hpp"
+#include "powf_half.h"
 
 namespace cosb {
 namespace {
@@ -258,6 +259,126 @@ __device__ __forceinline__ void sgd_vec(const SyncParams& p, SegCursor& c, uint6
     }
     w = make_float4(ww[0], ww[1], ww[2], ww[3]);
     h = make_float4(hh[0], hh[1], hh[2], hh[3]);
+  }
+}
+
+// ---------------------------------------------------------- Adam element
+
+// The same Regularize, then AdamSolver::ComputeUpdateValue's CPU branch (adam_solver.cpp:46-73; caffe_cpu_axpby =
+// scal then axpy, mkl_alternate.hpp) and Blob::Update, one rounding per operation (m = h, v = second history half):
+//   m = b1*m ; m = (1-b1)*g + m
+//   t = g*g ; v = b2*v ; v = (1-b2)*t + v
+//   t = powf(v, 0.5) ; t = t + delta ; t = m / t        (powf as glibc rounds it, powf_half.h)
+//   g = lrc*t ; w = (-1*g) + w                           lrc = (rate*lr_mult)*correction
+template <bool L1>
+__device__ __forceinline__ void adam_element_t(float g, float& w, float& m, float& v, float lrc, float ld,
+                                               const SyncParams& p) {
+  if (ld != 0.f) {
+    const float x = L1 ? static_cast<float>((0.f < w) - (w < 0.f)) : w;
+    g = __fadd_rn(__fmul_rn(ld, x), g);
+  }
+  const float b1 = p.momentum, b2 = p.beta2;
+  m = __fmul_rn(b1, m);
+  m = __fadd_rn(__fmul_rn(__fsub_rn(1.f, b1), g), m);
+  float t = __fmul_rn(g, g);
+  v = __fmul_rn(b2, v);
+  v = __fadd_rn(__fmul_rn(__fsub_rn(1.f, b2), t), v);
+  t = cos_powf_half(v);
+  t = __fadd_rn(t, p.delta);
+  t = __fdiv_rn(m, t);
+  g = __fmul_rn(lrc, t);
+  w = __fadd_rn(__fmul_rn(-1.0f, g), w);
+}
+
+// one element of blob k
+__device__ __forceinline__ void adam_element(const SyncParams& p, float g, float& w, float& m, float& v, float lr_mult,
+                                             float decay_mult) {
+  const float lrc = __fmul_rn(__fmul_rn(p.rate, lr_mult), p.correction);
+  const float ld = __fmul_rn(p.weight_decay, decay_mult);
+  if (p.l1) adam_element_t<true>(g, w, m, v, lrc, ld, p);
+  else adam_element_t<false>(g, w, m, v, lrc, ld, p);
+}
+
+__device__ __forceinline__ void adam_vec(const SyncParams& p, SegCursor& c, uint64_t i, const float4& g, float4& w,
+                                         float4& m, float4& v) {
+  c.advance(i);
+  int k = c.k;
+  // One element per trip, picked and written back with selects: the four double-precision powf evaluations are
+  // not interleaved, which keeps the update inside the kernels' register budget (no spills at N = 8).
+#pragma unroll 1
+  for (int e = 0; e < 4; ++e) {  // the vector may straddle blob boundaries
+    while (k < c.nseg - 1 && i + e >= c.end[k]) ++k;
+    float ge = e == 0 ? g.x : e == 1 ? g.y : e == 2 ? g.z : g.w;
+    float we = e == 0 ? w.x : e == 1 ? w.y : e == 2 ? w.z : w.w;
+    float me = e == 0 ? m.x : e == 1 ? m.y : e == 2 ? m.z : m.w;
+    float ve = e == 0 ? v.x : e == 1 ? v.y : e == 2 ? v.z : v.w;
+    adam_element(p, ge, we, me, ve, c.lr_mult[k], c.decay_mult[k]);
+    if (e == 0) { w.x = we; m.x = me; v.x = ve; }
+    else if (e == 1) { w.y = we; m.y = me; v.y = ve; }
+    else if (e == 2) { w.z = we; m.z = me; v.z = ve; }
+    else { w.w = we; m.w = me; v.w = ve; }
+  }
+}
+
+// ---------------------------------------------- solver as a kernel parameter
+// The kernels are templates on ADAM (false = SGD, the default).  The SGD instantiations only ever see sgd_vec /
+// sgd_element; Adam loads and stores v at h's index in hist2.  hist2 = hist + P is 16-byte aligned only when P is a
+// multiple of 4 (the history is Caffe's history_ laid out flat, m then v); i is, so the access width follows from
+// the alignment of hist2, the same for the whole launch.
+
+template <bool ADAM>
+__device__ __forceinline__ void load_v(const SyncParams& p, uint64_t i, float4& v) {
+  if (ADAM) {
+    const float* q = p.hist2 + i;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p.hist2);
+    if ((a & 15) == 0) {
+      v = *reinterpret_cast<const float4*>(q);
+    } else if ((a & 7) == 0) {
+      const float2 lo = *reinterpret_cast<const float2*>(q), hi = *reinterpret_cast<const float2*>(q + 2);
+      v = make_float4(lo.x, lo.y, hi.x, hi.y);
+    } else {
+      v = make_float4(q[0], q[1], q[2], q[3]);
+    }
+  }
+}
+
+template <bool ADAM>
+__device__ __forceinline__ void store_v(const SyncParams& p, uint64_t i, const float4& v) {
+  if (ADAM) {
+    float* q = p.hist2 + i;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p.hist2);
+    if ((a & 15) == 0) {
+      *reinterpret_cast<float4*>(q) = v;
+    } else if ((a & 7) == 0) {
+      *reinterpret_cast<float2*>(q) = make_float2(v.x, v.y);
+      *reinterpret_cast<float2*>(q + 2) = make_float2(v.z, v.w);
+    } else {
+      q[0] = v.x;
+      q[1] = v.y;
+      q[2] = v.z;
+      q[3] = v.w;
+    }
+  }
+}
+
+template <bool ADAM>
+__device__ __forceinline__ void update_vec(const SyncParams& p, SegCursor& c, uint64_t i, const float4& g, float4& w,
+                                           float4& h, float4& v) {
+  if (ADAM) adam_vec(p, c, i, g, w, h, v);
+  else sgd_vec(p, c, i, g, w, h);
+}
+
+// scalar head / tail element i of blob c.k
+template <bool ADAM>
+__device__ __forceinline__ void update_element(const SyncParams& p, const SegCursor& c, uint64_t i, float g, float& w,
+                                               float& h) {
+  if (ADAM) {
+    float v = p.hist2[i];
+    adam_element(p, g, w, h, v, c.lr_mult[c.k], c.decay_mult[c.k]);
+    p.hist2[i] = v;
+  } else {
+    sgd_element(g, w, h, __fmul_rn(p.rate, c.lr_mult[c.k]), __fmul_rn(p.weight_decay, c.decay_mult[c.k]),
+                p.momentum, p.l1);
   }
 }
 

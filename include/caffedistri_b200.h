@@ -43,6 +43,10 @@ extern "C" {
 #define COS_GRAD_FP32 0
 #define COS_GRAD_BF16 1
 
+/* solver type (SolverParameter.type); history layout per type, see cos_net_history */
+#define COS_SOLVER_SGD 0  /* "SGD": momentum SGD, history = P floats */
+#define COS_SOLVER_ADAM 1 /* "Adam": history = 2P floats, m of every blob then v of every blob */
+
 /* all-reduce algorithm selection (cos_net_set_option "algo") */
 #define COS_ALGO_AUTO 0
 #define COS_ALGO_TWO_SHOT 1 /* reduce-scatter -> fused SGD -> weight push (sharded PS, reference structure) */
@@ -78,6 +82,9 @@ typedef struct cos_solver_desc {
   int grad_dtype;              /* COS_GRAD_FP32 | COS_GRAD_BF16 */
   int init_iter;               /* iteration to resume from (0) */
   int regularization_l1;       /* SolverParameter.regularization_type: 0 = "L2" (default), 1 = "L1" */
+  int solver_type;             /* COS_SOLVER_SGD (0, default) | COS_SOLVER_ADAM; momentum is Adam's beta1 */
+  float momentum2;             /* Adam's beta2 (SolverParameter.momentum2, 0.999 in a prototxt) */
+  float delta;                 /* Adam's epsilon (SolverParameter.delta, 1e-8 in a prototxt) */
 } cos_solver_desc;
 
 /* Gradient producer = Net::ForwardBackward of the reference (solver.cpp:221-223),
@@ -177,9 +184,11 @@ COS_API int cos_net_get_validation_output_blobs(cos_net* net, int length, cos_bl
 /* Register Net::ForwardBackward (see cos_forward_backward_fn). */
 COS_API int cos_net_set_forward_backward(cos_net* net, cos_forward_backward_fn fn, void* user);
 
-/* Flat device buffers of Params<Dtype> (parallel.hpp:22-45): data_, diff_ and
- * the SGD history, each cos_net_param_count() fp32 elements, blobs laid out
- * back to back in learnable_params() order. */
+/* Flat device buffers of Params<Dtype> (parallel.hpp:22-45): data_ and diff_,
+ * each cos_net_param_count() = P fp32 elements, blobs laid out back to back in
+ * learnable_params() order, and the start of the solver's history_: P floats for
+ * SGD; 2P for Adam, the m of every blob followed by the v of every blob
+ * (AdamPreSolve order, adam_solver.cpp:8-17). */
 COS_API float* cos_net_data(cos_net* net, int solver_index);
 COS_API float* cos_net_diff(cos_net* net, int solver_index);
 COS_API float* cos_net_history(cos_net* net, int solver_index);
@@ -218,7 +227,7 @@ COS_API int cos_net_synchronize(cos_net* net);
  * (flag-in-data words, no barrier / fence; small nets, cluster_size <= 8)),
  * "barrier_timeout_ms", "one_shot_max_bytes", "ll_max_bytes" / "push_max_bytes" /
  * "nvls_min_bytes" (AUTO thresholds on the message size 4P), "push_vecs" (push / LL
- * kernel grid sizing),
+ * kernel grid sizing; an Adam net refuses 1 and 3: cos_net_sync_step then returns 0 without launching),
  * "timing" (CUDA events around each launch, default 0), "initial_gather" (0 =
  * connect() skips the first on_start(); the caller then runs
  * cos_net_all_gather_weights itself), "nvls" (-1 = auto: join an NVSwitch
@@ -241,7 +250,7 @@ COS_API float cos_net_last_kernel_ms(cos_net* net);
 /* Kernels launched by this net so far (bench.py gpu_launches). */
 COS_API int64_t cos_net_launch_count(cos_net* net);
 /* Seeded synthetic fill of one flat buffer ON THE DEVICE (which: 0 = data_, 1 = diff_,
- * 2 = history): out[i] = amp * u_i, u_i uniform in [-1, 1) from a counter-based
+ * 2 = the whole history, 2P floats for Adam): out[i] = amp * u_i, u_i uniform in [-1, 1) from a counter-based
  * generator keyed by (seed, stream) -- the generator the oracle's driver uses
  * (oracle/ref_driver.cpp), so benchmarks and parity runs need no host copy of the
  * 4P-byte tensors.  Asynchronous on the net's stream; 1/0. */
