@@ -34,7 +34,7 @@ class cos_solver_desc(ctypes.Structure):
                 ("weight_decay", ctypes.c_float), ("test_iter", ctypes.c_int), ("test_interval", ctypes.c_int),
                 ("snapshot_prefix", ctypes.c_char_p), ("grad_dtype", ctypes.c_int), ("init_iter", ctypes.c_int),
                 ("regularization_l1", ctypes.c_int), ("solver_type", ctypes.c_int), ("momentum2", ctypes.c_float),
-                ("delta", ctypes.c_float)]
+                ("delta", ctypes.c_float), ("iter_size", ctypes.c_int)]
 
 
 FORWARD_BACKWARD_FN = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(cos_blob),
@@ -55,6 +55,7 @@ SYMBOLS = [
     ("cos_net_sync", _i, [_vp]),
     ("cos_net_init", _i, [_vp, _i, _i]),
     ("cos_net_train", _i, [_vp, _i, _c.POINTER(cos_blob), _i]),
+    ("cos_net_train_accumulate", _i, [_vp, _i, _c.POINTER(cos_blob), _i, _i]),
     ("cos_net_predict", _i, [_vp, _i, _c.POINTER(cos_blob), _i, _pcp, _i, _c.POINTER(cos_blob)]),
     ("cos_net_validation", _i, [_vp, _c.POINTER(cos_blob), _i]),
     ("cos_net_aggregate_validation_outputs", _i, [_vp]),

@@ -48,7 +48,7 @@ class SolverDesc:
     def __init__(self, counts, lr_mult=None, decay_mult=None, lr_policy="fixed", base_lr=0.01, gamma=0.0, power=0.0,
                  stepsize=1, stepvalues=(), max_iter=0, momentum=0.0, weight_decay=0.0, test_iter=0,
                  test_interval=0, snapshot_prefix="", grad_dtype="fp32", init_iter=0, batch_size=0,
-                 regularization_type="L2", type="SGD", momentum2=0.999, delta=1e-8):
+                 regularization_type="L2", type="SGD", momentum2=0.999, delta=1e-8, iter_size=1):
         self.counts = [int(c) for c in counts]
         self.lr_mult = [float(x) for x in (lr_mult if lr_mult is not None else [1.0] * len(self.counts))]
         self.decay_mult = [float(x) for x in (decay_mult if decay_mult is not None else [1.0] * len(self.counts))]
@@ -61,6 +61,9 @@ class SolverDesc:
         if type not in SOLVER_TYPES:
             raise ValueError(f"solver type must be one of {sorted(SOLVER_TYPES)}, not {type!r}")
         self.type, self.momentum2, self.delta = type, momentum2, delta  # Adam: momentum is beta1
+        if int(iter_size) != iter_size or iter_size < 1:
+            raise ValueError(f"iter_size must be an integer >= 1, not {iter_size!r}")
+        self.iter_size = int(iter_size)  # forward/backward passes per step; the step scales diff_ by 1/iter_size
 
     @property
     def history_count(self):
@@ -79,6 +82,8 @@ class SolverDesc:
                     regularization_type=self.regularization_type)
         if self.type == "Adam":
             h.update(solver_type="Adam", momentum2=self.momentum2, delta=self.delta)
+        if self.iter_size != 1:
+            h.update(iter_size=self.iter_size)
         return h
 
     def to_c(self):
@@ -99,6 +104,7 @@ class SolverDesc:
         d.regularization_l1 = 1 if self.regularization_type == "L1" else 0
         d.solver_type = SOLVER_TYPES[self.type]
         d.momentum2, d.delta = self.momentum2, self.delta
+        d.iter_size = self.iter_size
         return d, keep
 
 
@@ -120,7 +126,7 @@ def parse_solver(solver_conf_file):
                       test_interval=d.test_interval, snapshot_prefix=pre.value.decode(), batch_size=bs.value,
                       regularization_type="L1" if d.regularization_l1 else "L2",
                       type="Adam" if d.solver_type == SOLVER_TYPES["Adam"] else "SGD", momentum2=d.momentum2,
-                      delta=d.delta)
+                      delta=d.delta, iter_size=d.iter_size)
 
 
 def read_caffemodel_blob(path, layer_name, blob_index=0):
@@ -249,6 +255,21 @@ class CaffeNet:
             raise CosError(_err())
         blobs, keep = _blob_array(data)
         ok = bool(self._L.cos_net_train(self._h, solver_index, blobs, len(data)))
+        del keep
+        return ok
+
+    def train_accumulate(self, solver_index, micro_batches):
+        """One Solver::Step over iter_size distinct micro-batches (gradient accumulation): `micro_batches` is a
+        list of iter_size lists of host blobs, pass i runs the producer on micro_batches[i].  Raises CosError on a
+        bad argument (a wrong number of micro-batches, blobs of unequal count); returns False when the step fails."""
+        if micro_batches is None:
+            self._L.cos_net_train_accumulate(self._h, solver_index, None, 0, 0)
+            raise CosError(_err())
+        groups = [list(g) for g in micro_batches]
+        if not groups or any(len(g) != len(groups[0]) for g in groups):
+            raise CosError("train_accumulate(): every micro-batch must have the same number of blobs")
+        blobs, keep = _blob_array([b for g in groups for b in g])
+        ok = bool(self._L.cos_net_train_accumulate(self._h, solver_index, blobs, len(groups[0]), len(groups)))
         del keep
         return ok
 

@@ -103,6 +103,7 @@ CaffeNet::~CaffeNet() {
     if (seg_lr_) cudaFree(seg_lr_);
     if (seg_dm_) cudaFree(seg_dm_);
     if (loss_dev_) cudaFree(loss_dev_);
+    if (loss_slots_) cudaFree(loss_slots_);
     if (loss_host_) cudaFreeHost(loss_host_);
     if (status_) cudaFreeHost(status_);
     if (ev_start_) cudaEventDestroy(ev_start_);
@@ -224,6 +225,10 @@ bool CaffeNet::allocate_device(int start_device_id, bool peer_mappable, std::str
   memset(status_, 0, 16 * sizeof(unsigned long long));
   COS_RT(cudaMalloc(reinterpret_cast<void**>(&loss_dev_), sizeof(float)));
   COS_RT(cudaMemset(loss_dev_, 0, sizeof(float)));
+  if (spec_.iter_size > 1) {
+    COS_RT(cudaMalloc(reinterpret_cast<void**>(&loss_slots_), spec_.iter_size * sizeof(float)));
+    COS_RT(cudaMemset(loss_slots_, 0, spec_.iter_size * sizeof(float)));
+  }
   COS_RT(cudaHostAlloc(reinterpret_cast<void**>(&loss_host_), 2 * sizeof(float), cudaHostAllocDefault));
   loss_host_[0] = loss_host_[1] = 0.f;
   COS_RT(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
@@ -342,6 +347,9 @@ bool CaffeNet::launch(int mode, cudaStream_t stream, std::string* err) {
     p.delta = spec_.delta;
     p.correction = adam_correction(spec_.momentum, spec_.momentum2, iter_);
   }
+  // sgd_solver.cpp:118-142 Normalize: Dtype(1.) / param_.iter_size(); iter_size 1 returns early (accum_norm 1 =
+  // the launchers' instantiations without Normalize)
+  p.accum_norm = spec_.iter_size > 1 ? 1.0f / static_cast<float>(spec_.iter_size) : 1.0f;
   if (mode != kModeAllGather) {
     if (!learning_rate(spec_.lr_policy, spec_.base_lr, spec_.gamma, spec_.power, spec_.stepsize,
                        spec_.stepvalues.empty() ? nullptr : spec_.stepvalues.data(),
@@ -478,7 +486,8 @@ float CaffeNet::last_kernel_ms() {
   return ms;
 }
 
-// CaffeNet.cpp:707-729 train(): feed the batch, Solver::Step(1).
+// CaffeNet.cpp:707-729 train(): feed the batch, Solver::Step(1).  MemoryInputAdapter::feed only Resets the data
+// layer to this batch, so with iter_size k every one of the step's k passes reads it (solver.cpp:221-223).
 bool CaffeNet::train(int solver_index, const cos_blob* data, int ndata, std::string* err) {
   if (solver_index != 0) {
     *err = "solver_index must be 0";
@@ -488,6 +497,32 @@ bool CaffeNet::train(int solver_index, const cos_blob* data, int ndata, std::str
     *err = "data is NULL";  // JniCaffeNet.cpp:391-395
     return false;
   }
+  return run_step(solver_index, data, ndata, 1, err);
+}
+
+// Gradient accumulation over distinct micro-batches: pass i of the step reads data[i*ndata .. (i+1)*ndata).
+bool CaffeNet::train_accumulate(int solver_index, const cos_blob* data, int ndata, int passes, std::string* err) {
+  if (solver_index != 0) {
+    *err = "solver_index must be 0";
+    return false;
+  }
+  if (!data) {
+    *err = "data is NULL";
+    return false;
+  }
+  if (ndata < 1) {
+    *err = "train_accumulate: ndata must be >= 1 (blobs per pass), got " + std::to_string(ndata);
+    return false;
+  }
+  if (passes != spec_.iter_size) {
+    *err = "train_accumulate: passes (" + std::to_string(passes) + ") must equal the solver's iter_size (" +
+           std::to_string(spec_.iter_size) + ")";
+    return false;
+  }
+  return run_step(solver_index, data, ndata, passes, err);
+}
+
+bool CaffeNet::run_step(int solver_index, const cos_blob* data, int ndata, int groups, std::string* err) {
   if (!fb_fn_) {
     *err = "train: no gradient producer registered (cos_net_set_forward_backward); Net::ForwardBackward is "
            "outside this library";
@@ -498,13 +533,14 @@ bool CaffeNet::train(int solver_index, const cos_blob* data, int ndata, std::str
   // MemoryInputAdapter::feed (MemoryInputAdapter.cpp:24-32) equivalent: stage the host blobs on the device.
   // Stage k was last read by step t-2: its H2D may only start once that step is done (device-side wait).
   InputStage& st = stage_[stage_idx_];
-  if (static_cast<int>(st.dev.size()) < ndata) {
-    st.dev.resize(ndata, nullptr);
-    st.bytes.resize(ndata, 0);
+  const int nblobs = ndata * groups;
+  if (static_cast<int>(st.dev.size()) < nblobs) {
+    st.dev.resize(nblobs, nullptr);
+    st.bytes.resize(nblobs, 0);
   }
   if (st.consumed_valid) COS_RT(cudaStreamWaitEvent(copy_stream_, st.consumed, 0));
-  std::vector<cos_blob> dev_blobs(ndata);
-  for (int i = 0; i < ndata; ++i) {
+  std::vector<cos_blob> dev_blobs(nblobs);
+  for (int i = 0; i < nblobs; ++i) {
     if (!data[i].data) {
       *err = "data[" + std::to_string(i) + "] is NULL";
       return false;
@@ -525,11 +561,19 @@ bool CaffeNet::train(int solver_index, const cos_blob* data, int ndata, std::str
   }
   COS_RT(cudaEventRecord(st.copied, copy_stream_));
   COS_RT(cudaStreamWaitEvent(stream_, st.copied, 0));
-  int rc = fb_fn_(fb_user_, solver_index_, dev_blobs.data(), ndata, loss_dev_, stream_);
-  if (rc != 0) {
-    *err = "gradient producer failed with code " + std::to_string(rc);
-    return false;
+  // solver.cpp:219-224: for i < iter_size: loss += ForwardBackward(); the producers accumulate into diff_
+  const int passes = spec_.iter_size;
+  for (int i = 0; i < passes; ++i) {
+    const cos_blob* in = dev_blobs.data() + static_cast<size_t>(groups == 1 ? 0 : i) * ndata;
+    float* loss = passes > 1 ? loss_slots_ + i : loss_dev_;
+    int rc = fb_fn_(fb_user_, solver_index_, in, ndata, loss, stream_);
+    if (rc != 0) {
+      *err = "gradient producer failed with code " + std::to_string(rc) +
+             (passes > 1 ? " in pass " + std::to_string(i) + " of " + std::to_string(passes) : std::string());
+      return false;
+    }
   }
+  if (passes > 1) COS_RT(launch_loss_mean(loss_slots_, passes, loss_dev_, stream_));  // loss /= iter_size
   if (!sync_step(solver_index, stream_, true, err)) return false;
   COS_RT(cudaEventRecord(st.consumed, stream_));
   st.consumed_valid = true;

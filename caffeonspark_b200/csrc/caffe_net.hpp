@@ -53,6 +53,8 @@ class CaffeNet {
   int deviceID(int solver_index) const;
   bool init(int solver_index, bool enable_nn, std::string* err);
   bool train(int solver_index, const cos_blob* data, int ndata, std::string* err);
+  // one step over `passes` (== iter_size) groups of ndata blobs, one distinct micro-batch per pass
+  bool train_accumulate(int solver_index, const cos_blob* data, int ndata, int passes, std::string* err);
   virtual int snapshot(std::string* err);
   std::string snapshot_filename(int iter, bool is_state) const;  // Solver::SnapshotFilename
   std::vector<BlobView> blob_views(const float* flat) const;
@@ -95,6 +97,9 @@ class CaffeNet {
   bool allocate_device(int start_device_id, bool peer_mappable, std::string* err);
   bool launch(int mode, cudaStream_t stream, std::string* err);
   bool check_status(std::string* err);
+  // Solver::Step: stage `groups` x ndata host blobs, run the producer iter_size times (pass i reads group i, or
+  // group 0 when groups == 1), the loss mean, then sync_step
+  bool run_step(int solver_index, const cos_blob* data, int ndata, int groups, std::string* err);
   int resolved_algo() const;
   int resolved_kernel() const;
 
@@ -123,6 +128,7 @@ class CaffeNet {
   int nseg_ = 0;
   int* status_ = nullptr;          // pinned + mapped: device-side error word
   float* loss_dev_ = nullptr;
+  float* loss_slots_ = nullptr;    // iter_size > 1: one device loss per forward/backward pass
   float* loss_host_ = nullptr;     // pinned
 
   // pointer tables for the kernel ([rank_] = local)

@@ -89,6 +89,11 @@ bool spec_from_desc(const cos_solver_desc* d, SolverSpec* s, std::string* err) {
   s->type = d->solver_type == COS_SOLVER_ADAM ? "Adam" : "SGD";
   s->momentum2 = d->momentum2;
   s->delta = d->delta;
+  if (d->iter_size < 0) {
+    *err = "iter_size must be >= 1 (0 reads as 1), got " + std::to_string(d->iter_size);
+    return false;
+  }
+  s->iter_size = d->iter_size == 0 ? 1 : d->iter_size;
   if (!cosb::check_solver_layout(*s, err)) return false;
   float r;
   int step = 0;
@@ -214,6 +219,19 @@ int cos_net_train(cos_net* net, int solver_index, const cos_blob* data, int ndat
     CaffeNet* r = R(net, solver_index);
     if (!r) return fail("invalid solver_index");
     if (!r->train(0, data, ndata, &err)) return fail(err);
+    return 1;
+  })
+}
+
+int cos_net_train_accumulate(cos_net* net, int solver_index, const cos_blob* data, int ndata, int passes) {
+  COS_GUARD(0, {
+    if (!net) return fail("net is NULL");
+    if (solver_index < 0) return fail("invalid solver_index");
+    if (!data) return fail("data is NULL");
+    std::string err;
+    CaffeNet* r = R(net, solver_index);
+    if (!r) return fail("invalid solver_index");
+    if (!r->train_accumulate(0, data, ndata, passes, &err)) return fail(err);
     return 1;
   })
 }
@@ -753,6 +771,7 @@ int cos_parse_solver(const char* solver_conf_file, cos_solver_desc* desc, int64_
     desc->solver_type = s.solver_type;
     desc->momentum2 = s.momentum2;
     desc->delta = s.delta;
+    desc->iter_size = s.iter_size;
     desc->test_iter = s.test_iter;
     desc->test_interval = s.test_interval;
     if (batch_size) *batch_size = s.batch_size;

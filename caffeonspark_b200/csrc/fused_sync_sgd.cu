@@ -98,7 +98,8 @@ __device__ __forceinline__ float4 reduce_vec_any(const SyncParams& p, int s, uin
 // N = compile-time world size (0 = runtime world, any size up to kMaxRanks).
 // (The in-switch NVLS variant lives in fused_sync_sgd_nvls.cu.)
 // ADAM: Adam update with the second history half (sync_device.cuh), false = SGD.
-template <int N, bool BF16, bool ADAM = false>
+// NORM: Normalize (iter_size > 1) before the update (sync_device.cuh), false = none.
+template <int N, bool BF16, bool ADAM = false, bool NORM = false>
 __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(const SyncParams p) {
   extern __shared__ unsigned char smem_raw[];
   __shared__ int s_abort;
@@ -222,7 +223,7 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
         } else {
           g = reduce_vec_any<N, BF16>(p, s, i);
         }
-        update_vec<ADAM>(p, cur, i, g, w, h, v);
+        update_vec<ADAM, NORM>(p, cur, i, g, w, h, v);
         *reinterpret_cast<float4*>(hl + i) = h;
         store_v<ADAM>(p, i, v);
         *reinterpret_cast<float4*>(wl + i) = w;
@@ -253,7 +254,7 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
           float g = (p.mode == kModeLocal) ? p.diff[rank][i] : reduce_scalar<BF16>(p, s, i);
           if (BF16 && p.mode == kModeLocal) g = bf16_bits_to_float(float_to_bf16_bits(g));
           float w = wl[i], h = hl[i];
-          update_element<ADAM>(p, c2, i, g, w, h);
+          update_element<ADAM, NORM>(p, c2, i, g, w, h);
           hl[i] = h;
           wl[i] = w;
           if (push) {
@@ -313,22 +314,36 @@ __global__ void fill_kernel(float* out, uint64_t n, uint64_t key, float amp) {
   }
 }
 
+// Solver::Step's loss over iter_size passes (solver.cpp:221-224): loss = 0; loss += ForwardBackward() per pass, in
+// pass order; loss /= iter_size -- float arithmetic, one rounding per operation.
+__global__ void loss_mean_kernel(const float* slots, int passes, float* out) {
+  float s = 0.f;
+  for (int i = 0; i < passes; ++i) s = __fadd_rn(s, slots[i]);
+  *out = __fdiv_rn(s, static_cast<float>(passes));
+}
+
 uint64_t host_mix64(uint64_t z) {
   z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ULL;
   z = (z ^ (z >> 27)) * 0x94d049bb133111ebULL;
   return z ^ (z >> 31);
 }
 
+template <int N, bool NORM>
+void launch_solver(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
+  if (p.solver == kSolverAdam) {
+    if (p.grad_bf16) fused_sync_sgd_kernel<N, true, true, NORM><<<grid, block, smem, stream>>>(p);
+    else fused_sync_sgd_kernel<N, false, true, NORM><<<grid, block, smem, stream>>>(p);
+  } else if (p.grad_bf16) {
+    fused_sync_sgd_kernel<N, true, false, NORM><<<grid, block, smem, stream>>>(p);
+  } else {
+    fused_sync_sgd_kernel<N, false, false, NORM><<<grid, block, smem, stream>>>(p);
+  }
+}
+
 template <int N>
 cudaError_t launch_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (p.solver == kSolverAdam) {
-    if (p.grad_bf16) fused_sync_sgd_kernel<N, true, true><<<grid, block, smem, stream>>>(p);
-    else fused_sync_sgd_kernel<N, false, true><<<grid, block, smem, stream>>>(p);
-  } else if (p.grad_bf16) {
-    fused_sync_sgd_kernel<N, true><<<grid, block, smem, stream>>>(p);
-  } else {
-    fused_sync_sgd_kernel<N, false><<<grid, block, smem, stream>>>(p);
-  }
+  if (sync_normalizes(p)) launch_solver<N, true>(p, grid, block, smem, stream);
+  else launch_solver<N, false>(p, grid, block, smem, stream);
   return cudaGetLastError();
 }
 
@@ -375,6 +390,12 @@ cudaError_t launch_fused_sync_sgd(const SyncParams& p, int grid, int block, cuda
 }
 
 // TMA (cp.async.bulk) pipelined variant: see fused_sync_sgd_tma.cu.
+
+cudaError_t launch_loss_mean(const float* slots, int passes, float* out, cudaStream_t stream) {
+  if (passes < 1) return cudaErrorInvalidValue;
+  loss_mean_kernel<<<1, 1, 0, stream>>>(slots, passes, out);
+  return cudaGetLastError();
+}
 
 cudaError_t launch_fill(float* out, uint64_t n, uint64_t seed, uint64_t stream_id, float amp, cudaStream_t stream) {
   const uint64_t key = host_mix64(seed * 0x9e3779b97f4a7c15ULL + stream_id);

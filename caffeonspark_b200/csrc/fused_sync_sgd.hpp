@@ -73,7 +73,14 @@ struct SyncParams {
   float beta2;
   float delta;
   float correction;
+  // Appended likewise.  iter_size > 1: SGDSolver::Normalize (sgd_solver.cpp:118-142) scales the reduced gradient by
+  // accum_norm = 1.0f / iter_size before Regularize.  0 or 1: no Normalize (the launchers pick the instantiations
+  // without it, so an iter_size 1 net runs exactly the kernels it ran before).
+  float accum_norm;
 };
+
+// true when the launch must apply Normalize (iter_size > 1)
+inline bool sync_normalizes(const SyncParams& p) { return p.accum_norm != 0.f && p.accum_norm != 1.f; }
 
 enum SolverKind : int { kSolverSgd = 0, kSolverAdam = 1 };
 
@@ -99,6 +106,8 @@ constexpr uint64_t kLLRegionMaxBytes = 8ull << 20;
 uint64_t push_recv_stride(uint64_t count, int world);
 // Occupancy-derived default grid (co-resident CTAs) for the vector kernel.
 int default_sync_grid(int device);
+// *out = (0 + slots[0] + ... + slots[passes-1]) / passes in float, in that order, on one device thread.
+cudaError_t launch_loss_mean(const float* slots, int passes, float* out, cudaStream_t stream);
 // Device-side synthetic fill, identical to cos_oracle_fill (tests/bench).
 cudaError_t launch_fill(float* out, uint64_t n, uint64_t seed, uint64_t stream_id, float amp,
                         cudaStream_t stream);

@@ -132,7 +132,8 @@ __device__ __forceinline__ uint64_t edge_of_thread(const ShardRange& r, unsigned
 
 // N = compile-time world size, 2..8 (the N-1 polled slots live in registers)
 // ADAM: Adam update with the second history half (sync_device.cuh), false = SGD.
-template <int N, bool BF16, bool ADAM = false>
+// NORM: Normalize (iter_size > 1) before the update (sync_device.cuh), false = none.
+template <int N, bool BF16, bool ADAM = false, bool NORM = false>
 __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const SyncParams p) {
   extern __shared__ unsigned char smem_raw[];
   __shared__ int s_abort;
@@ -288,7 +289,7 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
         acc.w = __fadd_rn(__fmul_rn(inv, y.w), acc.w);
       }
       if (!alive) break;
-      update_vec<ADAM>(p, cur, i, acc, w, h, v);
+      update_vec<ADAM, NORM>(p, cur, i, acc, w, h, v);
       *reinterpret_cast<float4*>(hl + i) = h;
       store_v<ADAM>(p, i, v);
       *reinterpret_cast<float4*>(wl + i) = w;
@@ -319,7 +320,7 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
         }
         if (alive) {
           float w = wl[e], h = hl[e];
-          update_element<ADAM>(p, c2, e, acc, w, h);
+          update_element<ADAM, NORM>(p, c2, e, acc, w, h);
           hl[e] = h;
           wl[e] = w;
           for (int k = 1; k < world; ++k) {
@@ -388,16 +389,22 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
   if (tracer) p.trace[4] = globaltimer_ns();
 }
 
+template <int N, bool NORM>
+void launch_ll_solver(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
+  if (p.solver == kSolverAdam) {
+    if (p.grad_bf16) fused_sync_sgd_ll_kernel<N, true, true, NORM><<<grid, block, smem, stream>>>(p);
+    else fused_sync_sgd_ll_kernel<N, false, true, NORM><<<grid, block, smem, stream>>>(p);
+  } else if (p.grad_bf16) {
+    fused_sync_sgd_ll_kernel<N, true, false, NORM><<<grid, block, smem, stream>>>(p);
+  } else {
+    fused_sync_sgd_ll_kernel<N, false, false, NORM><<<grid, block, smem, stream>>>(p);
+  }
+}
+
 template <int N>
 cudaError_t launch_ll_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (p.solver == kSolverAdam) {
-    if (p.grad_bf16) fused_sync_sgd_ll_kernel<N, true, true><<<grid, block, smem, stream>>>(p);
-    else fused_sync_sgd_ll_kernel<N, false, true><<<grid, block, smem, stream>>>(p);
-  } else if (p.grad_bf16) {
-    fused_sync_sgd_ll_kernel<N, true><<<grid, block, smem, stream>>>(p);
-  } else {
-    fused_sync_sgd_ll_kernel<N, false><<<grid, block, smem, stream>>>(p);
-  }
+  if (sync_normalizes(p)) launch_ll_solver<N, true>(p, grid, block, smem, stream);
+  else launch_ll_solver<N, false>(p, grid, block, smem, stream);
   return cudaGetLastError();
 }
 

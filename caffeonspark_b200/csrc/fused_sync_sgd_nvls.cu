@@ -47,7 +47,8 @@ constexpr uint32_t kIterBits = 16;               // progress word = (epoch << 16
 
 __device__ __forceinline__ void work_bar() { asm volatile("bar.sync 1, %0;" ::"n"(kWorkThreads) : "memory"); }
 
-template <int UN, int UP, int N>
+// NORM: Normalize (iter_size > 1) before the update (sync_device.cuh), false = none.
+template <int UN, int UP, int N, bool NORM = false>
 __global__ void __launch_bounds__(kNvlsThreads, 1) fused_sync_sgd_nvls_kernel(const SyncParams p) {
   extern __shared__ unsigned char smem_raw[];
   __shared__ int s_abort;
@@ -145,6 +146,7 @@ __global__ void __launch_bounds__(kNvlsThreads, 1) fused_sync_sgd_nvls_kernel(co
             }
           }
           cur.seek(i);
+          if (NORM) g = normalize_vec(p, g);
           sgd_vec(p, cur, i, g, w[u], h[u]);
           st_vec(hl + i, h[u]);
           if (u < UN) {
@@ -183,6 +185,7 @@ __global__ void __launch_bounds__(kNvlsThreads, 1) fused_sync_sgd_nvls_kernel(co
           const float y = __fmul_rn(inv, p.diff[src][i]);
           acc = (k == 0) ? y : __fadd_rn(y, acc);
         }
+        if (NORM) acc = __fmul_rn(p.accum_norm, acc);
         float w = wl[i], h = hl[i];
         sgd_element(acc, w, h, __fmul_rn(p.rate, cur.lr_mult[cur.k]), __fmul_rn(p.weight_decay, cur.decay_mult[cur.k]),
                     p.momentum, p.l1);
@@ -264,7 +267,8 @@ __global__ void __launch_bounds__(kNvlsThreads, 1) fused_sync_sgd_nvls_kernel(co
 
 template <int UN, int UP, int N>
 cudaError_t launch_cfg(const SyncParams& p, int grid, size_t smem, cudaStream_t stream) {
-  fused_sync_sgd_nvls_kernel<UN, UP, N><<<grid, kNvlsThreads, smem, stream>>>(p);
+  if (sync_normalizes(p)) fused_sync_sgd_nvls_kernel<UN, UP, N, true><<<grid, kNvlsThreads, smem, stream>>>(p);
+  else fused_sync_sgd_nvls_kernel<UN, UP, N><<<grid, kNvlsThreads, smem, stream>>>(p);
   return cudaGetLastError();
 }
 

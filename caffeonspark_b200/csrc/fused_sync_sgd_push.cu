@@ -66,7 +66,8 @@ __device__ __forceinline__ uint64_t edge_element(const ShardRange& r, unsigned t
 
 // N = compile-time world size (2..8), 0 = run-time world (<= kMaxRanks)
 // ADAM: Adam update with the second history half (sync_device.cuh), false = SGD.
-template <int N, bool BF16, bool ADAM = false>
+// NORM: Normalize (iter_size > 1) before the update (sync_device.cuh), false = none.
+template <int N, bool BF16, bool ADAM = false, bool NORM = false>
 __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(const SyncParams p) {
   extern __shared__ unsigned char smem_raw[];
   __shared__ int s_abort;
@@ -261,7 +262,7 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
           acc.w = __fadd_rn(__fmul_rn(inv, y.w), acc.w);
         }
       }
-      update_vec<ADAM>(p, cur, i, acc, w, h, v);
+      update_vec<ADAM, NORM>(p, cur, i, acc, w, h, v);
       *reinterpret_cast<float4*>(hl + i) = h;
       store_v<ADAM>(p, i, v);
       *reinterpret_cast<float4*>(wl + i) = w;
@@ -296,7 +297,7 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
           acc = __fadd_rn(__fmul_rn(inv, y), acc);
         }
         float w = wl[i], h = hl[i];
-        update_element<ADAM>(p, c2, i, acc, w, h);
+        update_element<ADAM, NORM>(p, c2, i, acc, w, h);
         hl[i] = h;
         wl[i] = w;
         for (int k = 1; k < world; ++k) {
@@ -326,16 +327,22 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
   if (tracer) p.trace[4] = globaltimer_ns();
 }
 
+template <int N, bool NORM>
+void launch_push_solver(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
+  if (p.solver == kSolverAdam) {
+    if (p.grad_bf16) fused_sync_sgd_push_kernel<N, true, true, NORM><<<grid, block, smem, stream>>>(p);
+    else fused_sync_sgd_push_kernel<N, false, true, NORM><<<grid, block, smem, stream>>>(p);
+  } else if (p.grad_bf16) {
+    fused_sync_sgd_push_kernel<N, true, false, NORM><<<grid, block, smem, stream>>>(p);
+  } else {
+    fused_sync_sgd_push_kernel<N, false, false, NORM><<<grid, block, smem, stream>>>(p);
+  }
+}
+
 template <int N>
 cudaError_t launch_push_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (p.solver == kSolverAdam) {
-    if (p.grad_bf16) fused_sync_sgd_push_kernel<N, true, true><<<grid, block, smem, stream>>>(p);
-    else fused_sync_sgd_push_kernel<N, false, true><<<grid, block, smem, stream>>>(p);
-  } else if (p.grad_bf16) {
-    fused_sync_sgd_push_kernel<N, true><<<grid, block, smem, stream>>>(p);
-  } else {
-    fused_sync_sgd_push_kernel<N, false><<<grid, block, smem, stream>>>(p);
-  }
+  if (sync_normalizes(p)) launch_push_solver<N, true>(p, grid, block, smem, stream);
+  else launch_push_solver<N, false>(p, grid, block, smem, stream);
   return cudaGetLastError();
 }
 

@@ -161,7 +161,8 @@ struct StageView {
   float* h;             // history tile
 };
 
-template <bool BF16>
+// NORM: Normalize (iter_size > 1) before the update (sync_device.cuh), false = none.
+template <bool BF16, bool NORM = false>
 __global__ void __launch_bounds__(kTmaThreads, 1)
 fused_sync_sgd_tma_kernel(const SyncParams p, const int tile_elems) {
   extern __shared__ __align__(128) unsigned char smem[];
@@ -332,6 +333,7 @@ fused_sync_sgd_tma_kernel(const SyncParams p, const int tile_elems) {
         cur.seek(i0 + e);
         cur_seeked = true;
       }
+      if (NORM) acc = normalize_vec(p, acc);
       sgd_vec(p, cur, i0 + e, acc, w, h);
       *reinterpret_cast<float4*>(v.w + e) = w;
       *reinterpret_cast<float4*>(v.h + e) = h;
@@ -391,6 +393,7 @@ fused_sync_sgd_tma_kernel(const SyncParams p, const int tile_elems) {
             g = (q == 0) ? x : __fadd_rn(x, g);
           }
         }
+        if (NORM) g = __fmul_rn(p.accum_norm, g);
         float w = wl[i], h = hl[i];
         sgd_element(g, w, h, __fmul_rn(p.rate, c2.lr_mult[c2.k]), __fmul_rn(p.weight_decay, c2.decay_mult[c2.k]),
                     p.momentum, p.l1);
@@ -434,6 +437,15 @@ fused_sync_sgd_tma_kernel(const SyncParams p, const int tile_elems) {
   }
 }
 
+template <bool BF16, bool NORM>
+cudaError_t launch_tma(const SyncParams& p, int grid, int tile, size_t smem, cudaStream_t stream) {
+  const cudaError_t e = cudaFuncSetAttribute(fused_sync_sgd_tma_kernel<BF16, NORM>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (e != cudaSuccess) return e;
+  fused_sync_sgd_tma_kernel<BF16, NORM><<<grid, kTmaThreads, smem, stream>>>(p, tile);
+  return cudaGetLastError();
+}
+
 }  // namespace
 
 cudaError_t launch_fused_sync_sgd_tma(const SyncParams& p, int grid, cudaStream_t stream) {
@@ -464,19 +476,11 @@ cudaError_t launch_fused_sync_sgd_tma(const SyncParams& p, int grid, cudaStream_
   smem = (smem + 127) & ~static_cast<size_t>(127);
   smem += static_cast<size_t>(kStages) * (per_elem * tile);
   smem += 128;
-  cudaError_t e;
+  const bool norm = sync_normalizes(p);
   if (p.grad_bf16) {
-    e = cudaFuncSetAttribute(fused_sync_sgd_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-    fused_sync_sgd_tma_kernel<true><<<grid, kTmaThreads, smem, stream>>>(p, tile);
-  } else {
-    e = cudaFuncSetAttribute(fused_sync_sgd_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-    fused_sync_sgd_tma_kernel<false><<<grid, kTmaThreads, smem, stream>>>(p, tile);
+    return norm ? launch_tma<true, true>(p, grid, tile, smem, stream) : launch_tma<true, false>(p, grid, tile, smem, stream);
   }
-  return cudaGetLastError();
+  return norm ? launch_tma<false, true>(p, grid, tile, smem, stream) : launch_tma<false, false>(p, grid, tile, smem, stream);
 }
 
 }  // namespace cosb

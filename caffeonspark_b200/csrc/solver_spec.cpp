@@ -530,8 +530,8 @@ bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std
     *err = "Unknown regularization type: " + spec->regularization_type;  // sgd_solver.cpp:169-171
     return false;
   }
-  if (spec->iter_size != 1) {
-    *err = "iter_size != 1 is not supported";
+  if (spec->iter_size < 1) {  // solver.cpp:37-38 CHECK_GE(iter_size, 1) (caffe.proto: iter_size default 1)
+    *err = "iter_size must be >= 1 (got " + std::to_string(spec->iter_size) + ")";
     return false;
   }
   if (spec->clip_gradients >= 0.f) {

@@ -361,17 +361,29 @@ __device__ __forceinline__ void store_v(const SyncParams& p, uint64_t i, const f
   }
 }
 
-template <bool ADAM>
+// ------------------------------------------- Normalize as a kernel parameter
+// iter_size > 1 (SGDSolver::Normalize, sgd_solver.cpp:118-142): caffe_scal(count, Dtype(1.)/iter_size, diff) on the
+// reduced gradient, before Regularize, for SGD and Adam alike.  One rounding: g = accum_norm * g.  The kernels are
+// templates on NORM (false = no Normalize, the default); NORM is applied to the reduced gradient right before the
+// element update, so it only adds one FMUL per element.
+__device__ __forceinline__ float4 normalize_vec(const SyncParams& p, const float4& g) {
+  const float a = p.accum_norm;
+  return make_float4(__fmul_rn(a, g.x), __fmul_rn(a, g.y), __fmul_rn(a, g.z), __fmul_rn(a, g.w));
+}
+
+template <bool ADAM, bool NORM = false>
 __device__ __forceinline__ void update_vec(const SyncParams& p, SegCursor& c, uint64_t i, const float4& g, float4& w,
                                            float4& h, float4& v) {
-  if (ADAM) adam_vec(p, c, i, g, w, h, v);
-  else sgd_vec(p, c, i, g, w, h);
+  const float4 gn = NORM ? normalize_vec(p, g) : g;
+  if (ADAM) adam_vec(p, c, i, gn, w, h, v);
+  else sgd_vec(p, c, i, gn, w, h);
 }
 
 // scalar head / tail element i of blob c.k
-template <bool ADAM>
+template <bool ADAM, bool NORM = false>
 __device__ __forceinline__ void update_element(const SyncParams& p, const SegCursor& c, uint64_t i, float g, float& w,
                                                float& h) {
+  if (NORM) g = __fmul_rn(p.accum_norm, g);
   if (ADAM) {
     float v = p.hist2[i];
     adam_element(p, g, w, h, v, c.lr_mult[c.k], c.decay_mult[c.k]);

@@ -85,6 +85,8 @@ typedef struct cos_solver_desc {
   int solver_type;             /* COS_SOLVER_SGD (0, default) | COS_SOLVER_ADAM; momentum is Adam's beta1 */
   float momentum2;             /* Adam's beta2 (SolverParameter.momentum2, 0.999 in a prototxt) */
   float delta;                 /* Adam's epsilon (SolverParameter.delta, 1e-8 in a prototxt) */
+  int iter_size;               /* SolverParameter.iter_size: forward/backward passes per step (0 is read as 1);
+                                  the step scales the accumulated gradient by 1/iter_size (SGDSolver::Normalize) */
 } cos_solver_desc;
 
 /* Gradient producer = Net::ForwardBackward of the reference (solver.cpp:221-223),
@@ -93,7 +95,9 @@ typedef struct cos_solver_desc {
  * to the device: `inputs[i]` are DEVICE pointers (same shapes as the host
  * blobs), it must enqueue on `cuda_stream` work that ACCUMULATES the local
  * gradient into cos_net_diff() using the weights in cos_net_data(), and write
- * the scalar loss to the DEVICE float `loss_dev`.  Return 0 on success. */
+ * the scalar loss to the DEVICE float `loss_dev`.  Return 0 on success.
+ * With iter_size k > 1 it is called k times per step, each time with its own
+ * `loss_dev`; cos_net_last_loss() then reports the float mean of the k losses. */
 typedef int (*cos_forward_backward_fn)(void* user, int solver_index, const cos_blob* inputs, int ninputs,
                                        float* loss_dev, void* cuda_stream);
 
@@ -139,10 +143,19 @@ COS_API int cos_net_sync(cos_net* net);
 COS_API int cos_net_init(cos_net* net, int solver_index, int enable_nn);
 
 /* J:120 train / JN:383-413, CN:707-729: ONE Solver::Step (solver.cpp:194-273):
- * stage the input blobs host->device, run the gradient producer, then the
- * fused scale + reduce-scatter + SGD/momentum update + weight all-gather
- * kernel, ++iter.  data==NULL -> 0 with error "data is NULL" (JN:391-395). */
+ * stage the input blobs host->device, run the gradient producer iter_size
+ * times on that one batch (the reference's data layer is Reset to the fed
+ * batch, so every pass of a Step reads it), then the fused scale +
+ * reduce-scatter + Normalize + SGD/momentum update + weight all-gather kernel,
+ * ++iter.  data==NULL -> 0 with error "data is NULL" (JN:391-395). */
 COS_API int cos_net_train(cos_net* net, int solver_index, const cos_blob* data, int ndata);
+
+/* One Solver::Step over `passes` distinct micro-batches: `data` holds passes
+ * groups of ndata blobs, group i is what pass i's producer call sees.  passes
+ * must equal the solver's iter_size; the effective batch is passes x the
+ * micro-batch.  Same staging, pipelining, loss and sync as cos_net_train.
+ * 1/0 with the reason in cos_last_error(). */
+COS_API int cos_net_train_accumulate(cos_net* net, int solver_index, const cos_blob* data, int ndata, int passes);
 
 /* J:110 predict / JN:277-376: forward-only; not on the sync path -> always
  * fails with "predict: not supported" (returns -1).  Kept for symbol parity. */
