@@ -100,6 +100,10 @@ SYMBOLS = [
     ("cos_lrn_backward_bf16", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp]),
     ("cos_bias_relu_maxpool_forward_bf16", _i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     ("cos_bias_relu_maxpool_backward_bf16", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    ("cos_batch_norm_forward", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    ("cos_batch_norm_backward", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
+    ("cos_batch_norm_forward_bf16", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    ("cos_batch_norm_backward_bf16", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
     ("cos_adapter_create", _vp, [_i, _i]),
     ("cos_adapter_destroy", None, [_vp]),
     ("cos_adapter_address", _cp, [_vp]),

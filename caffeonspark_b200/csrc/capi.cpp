@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/caffedistri_b200.h"
+#include "batch_norm.hpp"
 #include "caffe_layers.hpp"
 #include "caffe_net.hpp"
 #include "caffe_proto_io.hpp"
@@ -503,6 +504,77 @@ int cos_bias_relu_maxpool_backward_bf16(const uint16_t* dy, const uint8_t* index
                                                    height, width, kernel, stride, pooled_height, pooled_width,
                                                    static_cast<cudaStream_t>(cuda_stream)),
                   "cos_bias_relu_maxpool_backward_bf16");
+}
+
+namespace {
+const char* bn_args(const void* a, const void* b, const void* c, const void* save, const void* workspace, int num,
+                    int channels, int height, int width, float eps) {
+  if (!a || !b || !c || !save || !workspace) return "NULL tensor";
+  if (num < 1 || channels < 1 || height < 1 || width < 1 || (long long)height * width >= (1ll << 31))
+    return "bad shape";
+  if (!(eps >= 0.f) || !std::isfinite(eps)) return "BatchNorm needs a finite eps >= 0";
+  return nullptr;
+}
+const char* bn_forward_args(const void* x, const void* y, const float* mean_blob, const float* var_blob,
+                            const float* scale_blob, const float* save, const float* workspace, int num, int channels,
+                            int height, int width, float fraction, float eps) {
+  if (const char* e = bn_args(x, y, mean_blob, save, workspace, num, channels, height, width, eps)) return e;
+  if (!var_blob || !scale_blob) return "NULL tensor";
+  if (!std::isfinite(fraction)) return "BatchNorm needs a finite moving_average_fraction";
+  if (x == y) return "BatchNorm cannot run in place: y must not alias x";
+  return nullptr;
+}
+// the backward reads x and dy for the channel sums and again for dx
+const char* bn_backward_args(const void* x, const void* dy, const void* dx, const float* save,
+                             const float* workspace, int num, int channels, int height, int width, float eps) {
+  if (const char* e = bn_args(x, dy, dx, save, workspace, num, channels, height, width, eps)) return e;
+  if (dx == x || dx == dy) return "BatchNorm cannot run in place: dx must not alias x or dy";
+  return nullptr;
+}
+}  // namespace
+
+int cos_batch_norm_forward(const float* x, float* y, float* mean_blob, float* var_blob, float* scale_blob, float* save,
+                           float* workspace, int num, int channels, int height, int width, int use_global_stats,
+                           float moving_average_fraction, float eps, void* cuda_stream) {
+  if (const char* e = bn_forward_args(x, y, mean_blob, var_blob, scale_blob, save, workspace, num, channels, height,
+                                      width, moving_average_fraction, eps))
+    return fail(e);
+  return launched(cosb::batch_norm_forward(x, y, mean_blob, var_blob, scale_blob, save, workspace, num, channels,
+                                           height, width, use_global_stats != 0, moving_average_fraction, eps,
+                                           static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_batch_norm_forward");
+}
+
+int cos_batch_norm_backward(const float* x, const float* dy, float* dx, const float* save, float* workspace, int num,
+                            int channels, int height, int width, int use_global_stats, float eps, void* cuda_stream) {
+  if (const char* e = bn_backward_args(x, dy, dx, save, workspace, num, channels, height, width, eps))
+    return fail(e);
+  return launched(cosb::batch_norm_backward(x, dy, dx, save, workspace, num, channels, height, width,
+                                            use_global_stats != 0, eps, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_batch_norm_backward");
+}
+
+int cos_batch_norm_forward_bf16(const uint16_t* x, uint16_t* y, float* mean_blob, float* var_blob, float* scale_blob,
+                                float* save, float* workspace, int num, int channels, int height, int width,
+                                int use_global_stats, float moving_average_fraction, float eps, void* cuda_stream) {
+  if (const char* e = bn_forward_args(x, y, mean_blob, var_blob, scale_blob, save, workspace, num, channels, height,
+                                      width, moving_average_fraction, eps))
+    return fail(e);
+  return launched(cosb::batch_norm_forward(bf16_in(x), bf16_out(y), mean_blob, var_blob, scale_blob, save, workspace,
+                                           num, channels, height, width, use_global_stats != 0,
+                                           moving_average_fraction, eps, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_batch_norm_forward_bf16");
+}
+
+int cos_batch_norm_backward_bf16(const uint16_t* x, const uint16_t* dy, uint16_t* dx, const float* save,
+                                 float* workspace, int num, int channels, int height, int width, int use_global_stats,
+                                 float eps, void* cuda_stream) {
+  if (const char* e = bn_backward_args(x, dy, dx, save, workspace, num, channels, height, width, eps))
+    return fail(e);
+  return launched(cosb::batch_norm_backward(bf16_in(x), bf16_in(dy), bf16_out(dx), save, workspace, num, channels,
+                                            height, width, use_global_stats != 0, eps,
+                                            static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_batch_norm_backward_bf16");
 }
 
 // ------------------------------------------------------------- adapter API

@@ -443,6 +443,16 @@ bool net_layout(const Node& net, SolverSpec* spec, std::string* err) {
     } else if (type == "SoftmaxWithLoss" || type == "Accuracy" || type == "EuclideanLoss" ||
                type == "SigmoidCrossEntropyLoss" || type == "HingeLoss" || type == "MultinomialLogisticLoss") {
       for (const std::string& t : tops) blobs[t] = Shape{};
+    } else if (type == "BatchNorm") {
+      // batch_norm_layer.cpp:17-36: mean [C], variance [C], moving-average scale factor [1]; C = shape(1), or 1
+      // for a 1-axis bottom.  The forward pass rewrites them; their lr_mult is whatever the prototxt says.
+      Shape in;
+      if (!bottom_shape(0, &in)) return false;
+      if (in.empty()) { *err = "layer '" + name + "': bad BatchNorm bottom"; return false; }
+      const long C = in.size() == 1 ? 1 : in[1];
+      param_counts = {C, C, 1};
+      param_shapes = {{C}, {C}, {1}};
+      for (const std::string& t : tops) blobs[t] = in;
     } else if (type == "Silence") {
     } else {
       *err = "layer '" + name + "' of type '" + type +

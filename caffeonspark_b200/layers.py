@@ -1,5 +1,6 @@
 """Native producer layers: autograd Functions and modules over the library's LRN and fused
-conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10).
+conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10) and its
+BatchNorm entry points (csrc/batch_norm.cu, DESIGN.md section 13).
 
 Activations may be fp32 or bf16 (the mixed-precision producer runs these layers under
 torch.autocast, where the convolutions hand them bf16).  bf16 tensors take the bf16 entry points,
@@ -110,6 +111,82 @@ class BiasReluMaxPoolFunction(torch.autograd.Function):
         return dx, db, None, None
 
 
+def _bn_geometry(x):
+    """(num, channels, height, width) of Caffe's BatchNorm view of x: channels = shape(1) (1 for a 1-axis bottom),
+    the remaining axes flattened into height."""
+    n = x.shape[0]
+    c = x.shape[1] if x.dim() > 1 else 1
+    return n, c, x[0].numel() // c if n else 0, 1
+
+
+def _bn_blob(t, c):
+    if not t.is_cuda or t.dtype != torch.float32 or t.numel() != c or not t.is_contiguous():
+        raise CosError(f"BatchNorm statistics must be contiguous fp32 CUDA tensors of {c} elements, got {t.dtype} "
+                       f"{tuple(t.shape)} on {t.device}")
+    return t
+
+
+class BatchNormFunction(torch.autograd.Function):
+    """Caffe's BatchNorm on fp32 or bf16 activations.  The forward updates mean/variance/scale (fp32, usually
+    views of data_) in place unless use_global_stats; the backward returns dx only."""
+
+    @staticmethod
+    def forward(ctx, x, mean, variance, scale, use_global_stats, moving_average_fraction, eps):
+        if not x.is_cuda or x.dtype not in _ENTRY or x.dim() < 1 or x.numel() == 0:
+            raise CosError(f"BatchNorm takes non-empty fp32 or bf16 CUDA tensors (no CPU path), got {x.dtype} "
+                           f"{tuple(x.shape)} on {x.device}")
+        x = x.contiguous()
+        geom = _bn_geometry(x)
+        n, c = geom[0], geom[1]
+        for t, k in ((mean, c), (variance, c), (scale, 1)):
+            _bn_blob(t, k)
+        y = torch.empty_like(x)
+        save = torch.empty(2 * c, dtype=torch.float32, device=x.device)
+        work = torch.empty(2 * (n + 1) * c, dtype=torch.float32, device=x.device)
+        _call(_entry("cos_batch_norm_forward", x.dtype), x.data_ptr(), y.data_ptr(), mean.data_ptr(),
+              variance.data_ptr(), scale.data_ptr(), save.data_ptr(), work.data_ptr(), *geom, int(use_global_stats),
+              moving_average_fraction, eps, _stream())
+        ctx.save_for_backward(x, save)
+        ctx.hyper = (geom, int(use_global_stats), eps)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, save = ctx.saved_tensors
+        geom, use_global_stats, eps = ctx.hyper
+        dy = _grad(dy, x.dtype)
+        dx = torch.empty_like(x)
+        work = torch.empty(2 * (geom[0] + 1) * geom[1], dtype=torch.float32, device=x.device)
+        _call(_entry("cos_batch_norm_backward", x.dtype), x.data_ptr(), dy.data_ptr(), dx.data_ptr(), save.data_ptr(),
+              work.data_ptr(), *geom, use_global_stats, eps, _stream())
+        return dx, None, None, None, None, None, None
+
+
+def batch_norm_composite(x, mean, variance, scale, use_global_stats=False, moving_average_fraction=0.999, eps=1e-5):
+    """Caffe's BatchNorm as a PyTorch composition of the same formulas (any device, autograd through x).  Updates
+    the three statistics tensors in place unless use_global_stats, as the native forward does."""
+    n, c = x.shape[0], (x.shape[1] if x.dim() > 1 else 1)
+    xf = x.float().reshape(n, c, -1)
+    if use_global_stats:
+        s = scale.detach()[0]
+        sf = torch.where(s == 0, torch.zeros_like(s), 1 / s)
+        mu, var = sf * mean.detach(), sf * variance.detach()
+    else:
+        # batch statistics as functions of x: autograd then gives Caffe's (dy - mean(dy) - x^ mean(dy x^)) / std
+        m = xf.shape[0] * xf.shape[2]
+        mu = xf.mean((0, 2))
+        var = ((xf - mu.view(1, c, 1)) ** 2).mean((0, 2))
+        f = moving_average_fraction
+        corr = float(torch.tensor(m, dtype=torch.float32) / torch.tensor(m - 1, dtype=torch.float32)) if m > 1 else 1.0
+        with torch.no_grad():
+            scale.mul_(f).add_(1)
+            mean.copy_(mu + f * mean)
+            variance.copy_(corr * var + f * variance)
+    sd = torch.pow(var + eps, 0.5)
+    y = (xf - mu.view(1, c, 1)) / sd.view(1, c, 1)
+    return y.reshape(x.shape).to(x.dtype)
+
+
 class LRN(nn.Module):
     """Caffe's cross-channel LRN (nn.LocalResponseNorm's function) on the native kernels."""
 
@@ -123,6 +200,31 @@ class LRN(nn.Module):
         if not x.is_cuda:
             return F.local_response_norm(x, self.size, self.alpha, self.beta, self.k)
         return LRNFunction.apply(x, self.size, self.alpha, self.beta, self.k)
+
+
+class BatchNorm(nn.Module):
+    """Caffe's BatchNorm layer.  Its three blobs (mean sum, variance sum, scale factor) are parameters, in that
+    order, so a producer aliases them into data_ like any weight; the forward pass writes them (training mode) and
+    they never receive a gradient.  CUDA tensors take the native kernels; CPU tensors batch_norm_composite."""
+
+    def __init__(self, channels, use_global_stats=False, moving_average_fraction=0.999, eps=1e-5):
+        super().__init__()
+        self.mean = nn.Parameter(torch.zeros(channels), requires_grad=False)
+        self.variance = nn.Parameter(torch.zeros(channels), requires_grad=False)
+        self.scale_factor = nn.Parameter(torch.zeros(1), requires_grad=False)
+        self.use_global_stats = use_global_stats
+        self.moving_average_fraction, self.eps = moving_average_fraction, eps
+
+    def reset_parameters(self):
+        with torch.no_grad():  # batch_norm_layer.cpp LayerSetUp: caffe_set(0)
+            for p in (self.mean, self.variance, self.scale_factor):
+                p.zero_()
+
+    def forward(self, x):
+        hyper = (self.use_global_stats, self.moving_average_fraction, self.eps)
+        if not x.is_cuda:
+            return batch_norm_composite(x, self.mean, self.variance, self.scale_factor, *hyper)
+        return BatchNormFunction.apply(x, self.mean, self.variance, self.scale_factor, *hyper)
 
 
 class ConvReluMaxPool(nn.Module):

@@ -1,4 +1,4 @@
-"""The three BASELINE nets as layer lists -> (a) Caffe prototxt text for the C
+"""The three BASELINE nets and the reference's BatchNorm example as layer lists -> (a) Caffe prototxt text for the C
 library's layout parser, (b) the learnable-blob layout, (c) a PyTorch module
 used ONLY as the gradient producer (Net::ForwardBackward is out of scope of
 the sync library; SURVEY.md section 8 row f1).
@@ -7,18 +7,21 @@ Architectures follow the reference's configuration files
   data/lenet_memory_train_test.prototxt, data/lenet_memory_solver.prototxt
   data/cifar10_quick_train_test.prototxt, data/cifar10_quick_solver.prototxt
   data/bvlc_reference_net.prototxt, data/bvlc_reference_solver.prototxt
+  caffe-public/examples/cifar10/cifar10_full_sigmoid_train_test_bn.prototxt (+ _solver_bn)
 (batch 256/device for CaffeNet per
  caffe-public/models/bvlc_reference_caffenet/train_val.prototxt:25).
 """
 from .caffenet import SolverDesc
 
 # layer tuples:
-#   ("conv", name, cout, k, stride, pad, group, (lr_w, dm_w), (lr_b, dm_b))
+#   ("conv", name, cout, k, stride, pad, group, (lr_w, dm_w), (lr_b, dm_b) or None for bias_term: false)
 #   ("ip",   name, nout, (lr_w, dm_w), (lr_b, dm_b))
 #   ("pool", name, "MAX"|"AVE", k, stride)   ("relu", name)  ("lrn", name, size, alpha, beta)
-#   ("drop", name, ratio)
+#   ("drop", name, ratio)   ("sigmoid", name)
+#   ("bn",   name): Caffe BatchNorm, blobs mean [C], variance [C], scale factor [1], each lr_mult 0 decay_mult 1
 _W, _B = (1.0, 1.0), (2.0, 1.0)
 _B0 = (2.0, 0.0)  # CaffeNet biases: lr_mult 2, decay_mult 0
+_BN = (0.0, 1.0)  # BatchNorm statistics: written by the forward pass, never by the solver
 
 NETS = {
     "lenet": dict(
@@ -50,10 +53,25 @@ NETS = {
                 ("ip", "fc8", 1000, _W, _B0)],
         solver=dict(lr_policy="step", base_lr=0.01, gamma=0.1, stepsize=100000, momentum=0.9, weight_decay=0.0005,
                     max_iter=450000, test_iter=0, test_interval=0, snapshot_prefix="bvlc_reference_caffenet")),
+    # caffe-public/examples/cifar10/cifar10_full_sigmoid_{train_test,solver}_bn.prototxt
+    "cifar10_full_bn": dict(
+        input=(3, 32, 32), batch=100, classes=10,
+        layers=[("conv", "conv1", 32, 5, 1, 2, 1, _W, None), ("pool", "pool1", "MAX", 3, 2), ("bn", "bn1"),
+                ("sigmoid", "Sigmoid1"),
+                ("conv", "conv2", 32, 5, 1, 2, 1, _W, None), ("bn", "bn2"), ("sigmoid", "Sigmoid2"),
+                ("pool", "pool2", "AVE", 3, 2),
+                ("conv", "conv3", 64, 5, 1, 2, 1, _W, None), ("bn", "bn3"), ("sigmoid", "Sigmoid3"),
+                ("pool", "pool3", "AVE", 3, 2),
+                ("ip", "ip1", 10, _W, (1.0, 0.0))],
+        solver=dict(lr_policy="step", base_lr=0.001, gamma=1, stepsize=5000, momentum=0.9, max_iter=60000,
+                    test_iter=10, test_interval=1000, snapshot_prefix="cifar10_full_sigmoid_bn")),
 }
 
 # SURVEY.md App. D: expected flat sizes (checked by tests)
 EXPECTED_PARAM_COUNT = {"lenet": 431080, "cifar10_quick": 145578, "caffenet": 60965224}
+# Nets with BatchNorm statistics among their learnable blobs: the forward pass writes those, and no backward
+# gives them a gradient.  3x32x32 -> conv1 2400, bn1 65, conv2 25600, bn2 65, conv3 51200, bn3 129, ip1 10240 + 10
+STATS_NET_PARAM_COUNT = {"cifar10_full_bn": 89709}
 
 
 def _pool_out(h, k, s):
@@ -71,10 +89,15 @@ def layout(name):
         kind = L[0]
         if kind == "conv":
             _, nm, cout, k, s, p, g, pw, pb = L
-            counts += [cout * (c // g) * k * k, cout]
-            lr += [pw[0], pb[0]]
-            dm += [pw[1], pb[1]]
-            names += [nm + ".w", nm + ".b"]
+            counts.append(cout * (c // g) * k * k)
+            lr.append(pw[0])
+            dm.append(pw[1])
+            names.append(nm + ".w")
+            if pb is not None:
+                counts.append(cout)
+                lr.append(pb[0])
+                dm.append(pb[1])
+                names.append(nm + ".b")
             h, w, c = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1, cout
         elif kind == "pool":
             _, nm, _mode, k, s = L
@@ -87,6 +110,12 @@ def layout(name):
             dm += [pw[1], pb[1]]
             names += [nm + ".w", nm + ".b"]
             flat = nout
+        elif kind == "bn":
+            nm = L[1]
+            counts += [c, c, 1]
+            lr += [_BN[0]] * 3
+            dm += [_BN[1]] * 3
+            names += [nm + ".mean", nm + ".variance", nm + ".scale"]
     return counts, lr, dm, names
 
 
@@ -113,10 +142,11 @@ def net_prototxt(name):
             _, _, cout, k, s, p, g, pw, pb = L
             grp = f" group: {g}" if g != 1 else ""
             pad = f" pad: {p}" if p else ""
+            bias = (f' param {{ lr_mult: {pb[0]:g} decay_mult: {pb[1]:g} }}' if pb is not None else "")
             out.append(f'layer {{ name: "{nm}" type: "Convolution" bottom: "{bottom}" top: "{nm}"\n'
-                       f'  param {{ lr_mult: {pw[0]:g} decay_mult: {pw[1]:g} }} param {{ lr_mult: {pb[0]:g} '
-                       f'decay_mult: {pb[1]:g} }}\n'
-                       f'  convolution_param {{ num_output: {cout} kernel_size: {k} stride: {s}{pad}{grp} }} }}')
+                       f'  param {{ lr_mult: {pw[0]:g} decay_mult: {pw[1]:g} }}{bias}\n'
+                       f'  convolution_param {{ num_output: {cout} kernel_size: {k} stride: {s}{pad}{grp}'
+                       f'{"" if pb is not None else " bias_term: false"} }} }}')
             bottom = nm
         elif kind == "pool":
             _, _, mode, k, s = L
@@ -140,6 +170,14 @@ def net_prototxt(name):
         elif kind == "drop":
             out.append(f'layer {{ name: "{nm}" type: "Dropout" bottom: "{bottom}" top: "{bottom}" '
                        f'dropout_param {{ dropout_ratio: {L[2]:g} }} }}')
+        elif kind == "bn":
+            out.append(f'layer {{ name: "{nm}" type: "BatchNorm" bottom: "{bottom}" top: "{nm}"\n'
+                       + "".join(f'  param {{ lr_mult: {_BN[0]:g} decay_mult: {_BN[1]:g} }}' for _ in range(3))
+                       + ' }')
+            bottom = nm
+        elif kind == "sigmoid":
+            out.append(f'layer {{ name: "{nm}" type: "Sigmoid" bottom: "{bottom}" top: "{nm}" }}')
+            bottom = nm
     out.append(f'layer {{ name: "accuracy" type: "Accuracy" bottom: "{bottom}" bottom: "label" top: "accuracy" '
                f'include {{ phase: TEST }} }}')
     out.append(f'layer {{ name: "loss" type: "SoftmaxWithLoss" bottom: "{bottom}" bottom: "label" top: "loss" }}')
@@ -182,10 +220,11 @@ def _relu_maxpool_after(layers, i):
 
 
 def torch_module(name):
-    """PyTorch gradient producer with parameters in learnable_params() order.  LRN layers and every conv followed
-    by ReLU + MAX pool (either order) run on the library's native kernels (layers.py); the rest is PyTorch."""
+    """PyTorch gradient producer with parameters in learnable_params() order.  LRN and BatchNorm layers and every
+    conv with a bias followed by ReLU + MAX pool (either order) run on the library's native kernels (layers.py); the
+    rest is PyTorch."""
     import torch.nn as nn
-    from .layers import LRN, ConvReluMaxPool
+    from .layers import LRN, BatchNorm, ConvReluMaxPool
     net = NETS[name]
     c, h, w = net["input"]
     layers = net["layers"]
@@ -196,10 +235,10 @@ def torch_module(name):
             continue
         kind = L[0]
         if kind == "conv":
-            _, _, cout, k, s, p, g, _, _ = L
-            conv = nn.Conv2d(c, cout, k, stride=s, padding=p, groups=g)
+            _, _, cout, k, s, p, g, _, pb = L
+            conv = nn.Conv2d(c, cout, k, stride=s, padding=p, groups=g, bias=pb is not None)
             h, w, c = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1, cout
-            pool = _relu_maxpool_after(layers, i)
+            pool = _relu_maxpool_after(layers, i) if pb is not None else None
             if pool is None:
                 mods.append(conv)
             else:
@@ -223,4 +262,8 @@ def torch_module(name):
             mods.append(LRN(L[2], alpha=L[3], beta=L[4], k=1.0))
         elif kind == "drop":
             mods.append(nn.Dropout(L[2]))
+        elif kind == "bn":
+            mods.append(BatchNorm(c))
+        elif kind == "sigmoid":
+            mods.append(nn.Sigmoid())
     return nn.Sequential(*mods)

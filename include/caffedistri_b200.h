@@ -316,6 +316,36 @@ COS_API int cos_bias_relu_maxpool_backward_bf16(const uint16_t* dy, const uint8_
                                                 int width, int kernel, int stride, int pooled_height,
                                                 int pooled_width, void* cuda_stream);
 
+/* Caffe's BatchNorm layer (batch_norm_layer.cpp; DESIGN.md section 13), x contiguous NCHW (a 2-axis
+ * num x channels bottom passes height = width = 1).  mean_blob and var_blob have `channels` floats and
+ * scale_blob one: the layer's three learnable blobs, usually pointers into data_.  save holds 2 * channels
+ * floats: the mean, then the variance, the forward normalised with (the backward reads them).  workspace is
+ * 2 * (num + 1) * channels floats of scratch.  Same launch rules as the calls above; deterministic.
+ * Not in place: y must not alias x, and dx must not alias x or dy (the backward reads both twice); such
+ * calls are rejected.  A Caffe net with top == bottom passes a separate output buffer.
+ * use_global_stats 0: y = (x - mean) / powf(var + eps, 0.5) with the biased batch variance E((x - mean)^2),
+ *   and the blobs are updated in place: s = s * f + 1, mean_blob = mean + f * mean_blob,
+ *   var_blob = M / (M - 1) * var + f * var_blob (M = num * height * width, factor 1 when M <= 1),
+ *   f = moving_average_fraction, one fp32 rounding per operation.
+ * use_global_stats 1: mean = mean_blob / s and var = var_blob / s (0 when s == 0); the blobs are only read.
+ * The backward writes dx only: (dy - sum(dy) / M - x^ * sum(dy * x^) / M) / std in training mode and dy / std
+ * with global statistics; the blobs get no gradient. */
+COS_API int cos_batch_norm_forward(const float* x, float* y, float* mean_blob, float* var_blob, float* scale_blob,
+                                   float* save, float* workspace, int num, int channels, int height, int width,
+                                   int use_global_stats, float moving_average_fraction, float eps, void* cuda_stream);
+COS_API int cos_batch_norm_backward(const float* x, const float* dy, float* dx, const float* save, float* workspace,
+                                    int num, int channels, int height, int width, int use_global_stats, float eps,
+                                    void* cuda_stream);
+/* bf16 activations (x, y, dy, dx); statistics, save and workspace stay fp32.  Every y and dx element is the fp32
+ * call's result on the upcast inputs rounded once to bf16, and save and the blobs equal the fp32 call's bit for bit. */
+COS_API int cos_batch_norm_forward_bf16(const uint16_t* x, uint16_t* y, float* mean_blob, float* var_blob,
+                                        float* scale_blob, float* save, float* workspace, int num, int channels,
+                                        int height, int width, int use_global_stats, float moving_average_fraction,
+                                        float eps, void* cuda_stream);
+COS_API int cos_batch_norm_backward_bf16(const uint16_t* x, const uint16_t* dy, uint16_t* dx, const float* save,
+                                         float* workspace, int num, int channels, int height, int width,
+                                         int use_global_stats, float eps, void* cuda_stream);
+
 /* --------------------- transport object (reference: util/socket.hpp) ------ */
 /* PeerAdapter = SocketAdapter + SocketChannel of the reference
  * (socket.hpp:22-89): a listener thread on a per-process endpoint whose
