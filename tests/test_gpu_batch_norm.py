@@ -16,9 +16,13 @@ from test_hdf5_io import MiniH5
 pytestmark = pytest.mark.gpu
 
 EPS, FRAC = 1e-5, 0.999
-# the example net's three BN inputs at batch 100, then ragged ones
+# the example net's three BN inputs at batch 100, then ragged ones, then one per thread group the kernels pick from
+# H*W (the smallest power of two >= H*W up to a warp, the whole block above 1024), on the 32/33 and 1024/1025 edges:
+# H*W 2 -> 2 threads, 3 and 4 -> 4, 5 and 8 -> 8, 32 and 33 -> 32, 1024 -> 32, 1025 -> 256
 SHAPES = [(100, 32, 16, 16), (100, 32, 16, 16), (100, 64, 8, 8), (1, 5, 3, 3), (7, 1, 9, 11), (3, 6, 1, 1),
-          (5, 3, 7, 7), (2, 3, 37, 41), (1, 1, 1, 1)]
+          (5, 3, 7, 7), (2, 3, 37, 41), (1, 1, 1, 1),
+          (4, 3, 1, 2), (3, 4, 3, 1), (3, 5, 2, 2), (2, 3, 1, 5), (2, 3, 1, 7), (2, 3, 2, 4), (2, 3, 4, 8),
+          (2, 3, 3, 11), (2, 2, 32, 32), (2, 2, 1, 1025)]
 SHAPES = list(dict.fromkeys(SHAPES))
 
 _libm = ctypes.CDLL(ctypes.util.find_library("m"))

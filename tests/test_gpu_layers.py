@@ -26,16 +26,41 @@ POOL_CASES = {
     "cifar10_quick_conv1": ((100, 32, 32, 32), 3, 2),  # 32 -> 16: the last window is clipped
     "ragged": ((3, 3, 17, 23), 3, 2),
     "ragged_k2": ((2, 3, 9, 7), 2, 2),
+    # the runtime-geometry kernels: overlapping windows (kernel > stride), stride > kernel, kernel 1, kernel 15
+    "k1s1": ((2, 3, 5, 6), 1, 1),
+    "k1s2": ((2, 3, 7, 6), 1, 2),
+    "k2s1": ((2, 3, 9, 7), 2, 1),
+    "k3s1": ((2, 3, 9, 10), 3, 1),
+    "k4s3": ((2, 3, 10, 11), 4, 3),
+    "k5s3_clipped": ((2, 3, 13, 12), 5, 3),
+    "k7s2": ((2, 3, 15, 16), 7, 2),
+    "k2s3_gaps": ((2, 3, 9, 8), 2, 3),
+    "k15s1": ((1, 2, 17, 16), 15, 1),
+    "k15s17": ((1, 2, 33, 40), 15, 17),
+    # H*W = 33 and 257 (the backward's block sizes 64 and 256 with two strided passes), N*C > 65535, C > 128
+    "hw33": ((2, 3, 3, 11), 3, 2),
+    "hw257": ((2, 3, 257, 1), 1, 1),
+    "planes65792": ((257, 256, 3, 3), 3, 2),
+    "c257_k2s1": ((2, 257, 5, 5), 2, 1),
 }
-# (N, C, H, W), local_size, alpha, beta
+# (N, C, H, W), local_size, alpha, beta, k: every window half-width 0..7 has its own kernel instantiation
 LRN_CASES = {
-    "caffenet_norm1_b256": ((256, 96, 27, 27), 5, 1e-4, 0.75),
-    "caffenet_norm2_b256": ((256, 256, 13, 13), 5, 1e-4, 0.75),
-    "caffenet_norm1_b4": ((4, 96, 27, 27), 5, 1e-4, 0.75),
-    "caffenet_norm2_b4": ((4, 256, 13, 13), 5, 1e-4, 0.75),
-    "ragged": ((3, 3, 7, 9), 5, 1e-4, 0.75),
-    "ragged_size3_strong": ((2, 37, 5, 11), 3, 5e-2, 0.75),
-    "size7": ((2, 40, 6, 6), 7, 1e-3, 0.5),
+    "caffenet_norm1_b256": ((256, 96, 27, 27), 5, 1e-4, 0.75, 1.0),
+    "caffenet_norm2_b256": ((256, 256, 13, 13), 5, 1e-4, 0.75, 1.0),
+    "caffenet_norm1_b4": ((4, 96, 27, 27), 5, 1e-4, 0.75, 1.0),
+    "caffenet_norm2_b4": ((4, 256, 13, 13), 5, 1e-4, 0.75, 1.0),
+    "ragged": ((3, 3, 7, 9), 5, 1e-4, 0.75, 1.0),
+    "ragged_size3_strong": ((2, 37, 5, 11), 3, 5e-2, 0.75, 1.0),
+    "size7": ((2, 40, 6, 6), 7, 1e-3, 0.5, 1.0),
+    "size1": ((2, 20, 3, 7), 1, 1e-2, 0.75, 1.0),
+    "size9": ((2, 40, 6, 6), 9, 1e-3, 0.75, 1.0),
+    "size11": ((3, 35, 5, 7), 11, 1e-3, 0.75, 1.0),
+    "size13": ((2, 40, 4, 9), 13, 1e-3, 0.6, 1.0),
+    "size15": ((2, 33, 4, 5), 15, 1e-3, 0.75, 1.0),
+    "k2": ((2, 33, 5, 7), 5, 1e-4, 0.75, 2.0),
+    "k1e-3_size3": ((2, 17, 3, 43), 3, 1e-4, 0.75, 1e-3),
+    "size15_k2": ((1, 16, 8, 16), 15, 1e-3, 0.5, 2.0),
+    "size7_k1e-3": ((3, 31, 1, 43), 7, 1e-3, 1.0, 1e-3),
 }
 
 
@@ -94,13 +119,13 @@ def _rel(a, ref):
 
 @pytest.mark.parametrize("case", list(LRN_CASES))
 def test_lrn_matches_pytorch(case):
-    shape, size, alpha, beta = LRN_CASES[case]
+    shape, size, alpha, beta, k = LRN_CASES[case]
     x, dy = _lrn_inputs(shape, 21)
     xr = x.clone().requires_grad_()
-    yr = nn.LocalResponseNorm(size, alpha=alpha, beta=beta, k=1.0)(xr)
+    yr = nn.LocalResponseNorm(size, alpha=alpha, beta=beta, k=k)(xr)
     yr.backward(dy)
     xn = x.clone().requires_grad_()
-    y = layers.LRN(size, alpha=alpha, beta=beta, k=1.0)(xn)
+    y = layers.LRN(size, alpha=alpha, beta=beta, k=k)(xn)
     y.backward(dy)
     assert _rel(y, yr.detach()) <= 1e-6, case
     assert _rel(xn.grad, xr.grad) <= 1e-5, case
