@@ -1,0 +1,192 @@
+"""Forward/backward time of the built-in producer against the PyTorch fp32 producer (DESIGN.md section 14).
+
+Workloads: the three nets the engine runs, at their reference batch sizes (LeNet b64, CIFAR-10-quick b100,
+cifar10_full_bn b100).  For each, one process times the native engine, the PyTorch module with TF32 off and with
+TF32 on (cuDNN's default, here applied to matmuls too), alternating the three in every round; each sample is CUDA events around `--iters`
+back-to-back forward/backward calls on one stream after `--warmup` untimed ones.  Prints one JSON line per
+workload with median / min / max ms per call and images/s, and the card's name and power limit.
+
+--profile adds a torch.profiler run of the native engine: per-kernel device time per call, and the achieved FLOP/s of
+each net's largest GEMM (2*M*N*K from the plan's shapes over that launch's kernel time) against the H100 SXM data
+sheet's 67 TFLOP/s FP32.
+"""
+import argparse
+import json
+import os
+import re
+import statistics
+import subprocess
+import sys
+import tempfile
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, ROOT)
+
+WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn")
+FP32_PEAK = 67e12  # H100 SXM data sheet, dense FP32, at up to 700 W
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        return out[0] if out else "unknown"
+    except Exception:
+        return "unknown"
+
+
+def plan_gemms(text):
+    """(label, flops) of every GEMM one forward/backward launches, in launch order (native_producer.cu)."""
+    fwd, bwd = [], []
+    for line in text.splitlines():
+        if not line.startswith("op "):
+            continue
+        f = line.split()
+        kind, name = f[2], f[3]
+        ins = [int(v) for v in f[4].split("x")]
+        w = int(re.search(r" w=\d+:(\d+)", line).group(1)) if " w=" in line else 0
+        need_dx = " staged-bottom" not in line  # the plan's rule: no data gradient into a staged input
+        if kind in ("Convolution", "ConvBiasReLUMaxPool"):
+            kh, kw = (int(v) for v in re.search(r" k(\d+)x(\d+)", line).groups())
+            sh, sw = (int(v) for v in re.search(r" s(\d+)x(\d+)", line).groups())
+            ph, pw = (int(v) for v in re.search(r" p(\d+)x(\d+)", line).groups())
+            n, cin, h, wd = ins
+            cout = w // (cin * kh * kw)
+            oh, ow = (h + 2 * ph - kh) // sh + 1, (wd + 2 * pw - kw) // sw + 1
+            k, cols = cin * kh * kw, n * oh * ow
+            fwd.append((f"{name} forward", 2 * cout * cols * k))
+            back = [(f"{name} weight gradient", 2 * cout * k * cols)]
+            if need_dx:
+                back.append((f"{name} data gradient", 2 * cin * n * h * wd * cout * kh * kw))
+            bwd.append(back)
+        elif kind == "InnerProduct":
+            b = ins[0]
+            k = 1
+            for d in ins[1:]:
+                k *= d
+            nout = w // k
+            fwd.append((f"{name} forward", 2 * b * nout * k))
+            back = [(f"{name} weight gradient", 2 * nout * k * b)]
+            if need_dx:
+                back.append((f"{name} data gradient", 2 * b * k * nout))
+            bwd.append(back)
+    return fwd + [g for back in reversed(bwd) for g in back]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=7)
+    ap.add_argument("--iters", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--workloads", default=",".join(WORKLOADS))
+    args = ap.parse_args()
+
+    import numpy as np
+    import torch
+    import torch.nn.functional as F
+    import caffeonspark_b200 as C
+    from caffeonspark_b200 import nets
+
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_native_producer.py needs a CUDA device (there is no CPU path)")
+    gpu = card()
+    tmp = tempfile.mkdtemp(prefix="bench_native_producer_")
+    for name in args.workloads.split(","):
+        solver = nets.write_prototxts(name, tmp)
+        net = C.CaffeNet(solver, "", "", 1, 1, 0, True, C.CaffeNet.NONE, -1, 0)
+        net.use_native_producer(fill_weights=False)
+        net.fill("data", 1, 0, 0.05)
+        torch.cuda.synchronize()
+        batch = nets.NETS[name]["batch"]
+        rng = np.random.RandomState(0)
+        x = torch.from_numpy(rng.rand(batch, *nets.NETS[name]["input"]).astype(np.float32)).cuda()
+        y = torch.from_numpy(rng.randint(0, 10, batch).astype(np.float32)).cuda()
+        loss = torch.zeros(1, device="cuda")
+        # a stream of its own: the legacy default stream's handle is 0, which would send the engine to the net's
+        # stream, outside the events
+        stream = torch.cuda.Stream()
+        torch.cuda.synchronize()
+        torch.cuda.set_stream(stream)
+
+        def native():
+            assert net.forward_backward([x, y], loss.data_ptr(), stream=stream.cuda_stream), net.last_error()
+
+        module = nets.torch_module(name).cuda()
+        with torch.no_grad():
+            w, off = net.data().clone(), 0
+            for p in module.parameters():
+                p.copy_(w[off:off + p.numel()].view(p.shape))
+                off += p.numel()
+        ylong = y.long()
+
+        def torch_fb():
+            out = module(x)
+            F.cross_entropy(out, ylong).backward()
+
+        default_tf32 = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
+
+        def with_tf32(on, fn):
+            def run():
+                torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = on
+                fn()
+            return run
+
+        impls = {"native": native, "torch_fp32": with_tf32(False, torch_fb),
+                 "torch_tf32": with_tf32(True, torch_fb)}
+        samples = {k: [] for k in impls}
+        for fn in impls.values():  # every shape warmed before the first timed round
+            for _ in range(args.warmup):
+                fn()
+        for _ in range(args.rounds):
+            for k, fn in impls.items():
+                for _ in range(args.warmup):
+                    fn()
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                for _ in range(args.iters):
+                    fn()
+                b.record()
+                b.synchronize()
+                samples[k].append(a.elapsed_time(b) / args.iters)
+        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = default_tf32
+        res = {"workload": name, "batch": batch, "gpu": gpu, "rounds": args.rounds, "iters": args.iters}
+        for k, v in samples.items():
+            med = statistics.median(v)
+            res[k] = {"ms_median": round(med, 4), "ms_min": round(min(v), 4), "ms_max": round(max(v), 4),
+                      "images_per_s": round(batch / med * 1e3, 1)}
+        if args.profile:
+            from torch.profiler import ProfilerActivity, profile
+            calls = 10
+            native()
+            torch.cuda.synchronize()
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(calls):
+                    native()
+                torch.cuda.synchronize()
+            kernels = [e for e in prof.events() if e.device_type.name == "CUDA" and "Memcpy" not in e.name
+                       and "Memset" not in e.name]
+            res["profile_kernel_ms_per_call_total"] = round(sum(e.device_time for e in kernels) / 1e3 / calls, 4)
+            per = {}
+            for e in kernels:
+                short = re.sub(r"\(anonymous namespace\)::|cosb::", "", e.name)[:90]
+                per[short] = per.get(short, 0.0) + e.device_time / 1e3 / calls
+            res["profile_ms_per_call"] = {k: round(v, 4) for k, v in sorted(per.items(), key=lambda t: -t[1])}
+            gemms = plan_gemms(C.native_producer_plan(solver))
+            times = [e.device_time / 1e3 for e in kernels if "gemm_kernel" in e.name]
+            if len(times) == len(gemms) * calls:
+                big = max(range(len(gemms)), key=lambda i: gemms[i][1])
+                t = statistics.median(times[big::len(gemms)])
+                res["largest_gemm"] = {"gemm": gemms[big][0], "gflop": round(gemms[big][1] / 1e9, 3),
+                                       "ms": round(t, 4), "tflops": round(gemms[big][1] / t / 1e9, 2),
+                                       "share_of_67_tflops": round(gemms[big][1] / t / 1e-3 / FP32_PEAK, 3)}
+            else:
+                res["largest_gemm"] = f"not measured ({len(times)} GEMM launches, expected {len(gemms) * calls})"
+        print(json.dumps(res), flush=True)
+        torch.cuda.synchronize()
+        torch.cuda.set_stream(torch.cuda.default_stream())
+        net.deallocate()
+
+
+if __name__ == "__main__":
+    main()

@@ -76,6 +76,9 @@ SYMBOLS = [
     ("cos_net_get_validation_output_blob_names", _i, [_vp, _c.POINTER(_pcp)]),
     ("cos_net_get_validation_output_blobs", _i, [_vp, _i, _c.POINTER(cos_blob)]),
     ("cos_net_set_forward_backward", _i, [_vp, FORWARD_BACKWARD_FN, _vp]),
+    ("cos_net_use_native_producer", _i, [_vp, _cp, _i]),
+    ("cos_net_forward_backward", _i, [_vp, _i, _c.POINTER(cos_blob), _i, _vp, _vp]),
+    ("cos_native_producer_plan", _i, [_cp, _cp, _i]),
     ("cos_net_data", _vp, [_vp, _i]),
     ("cos_net_diff", _vp, [_vp, _i]),
     ("cos_net_history", _vp, [_vp, _i]),

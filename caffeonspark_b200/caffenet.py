@@ -129,6 +129,18 @@ def parse_solver(solver_conf_file):
                       delta=d.delta, iter_size=d.iter_size)
 
 
+def native_producer_plan(prototxt):
+    """The built-in producer's plan for a solver or net prototxt, one op per line (host only).  Raises CosError
+    naming the first layer the engine cannot run."""
+    L = _lib.lib()
+    n = L.cos_native_producer_plan(str(prototxt).encode(), None, 0)
+    if n < 0:
+        raise CosError(_err())
+    buf = ctypes.create_string_buffer(n + 1)
+    L.cos_native_producer_plan(str(prototxt).encode(), buf, n + 1)
+    return buf.value.decode()
+
+
 def read_caffemodel_blob(path, layer_name, blob_index=0):
     """One blob of a Caffe .caffemodel (ours or stock Caffe's) as a flat float32 numpy array."""
     import numpy as np
@@ -321,6 +333,28 @@ class CaffeNet:
                 return 1
         self._fb_keep = FORWARD_BACKWARD_FN(tramp)
         return bool(self._L.cos_net_set_forward_backward(self._h, self._fb_keep, None))
+
+    def use_native_producer(self, net_prototxt=None, fill_weights=True):
+        """Attach the built-in sm_90a producer to every local solver and register it (replacing any other).
+        net_prototxt None = the net the solver file named; fill_weights = initialise data_ from the prototxt fillers
+        unless a model file was restored.  Raises CosError when the engine refuses the net."""
+        path = None if net_prototxt is None else str(net_prototxt).encode()
+        if not self._L.cos_net_use_native_producer(self._h, path, int(bool(fill_weights))):
+            raise CosError(_err())
+        self._fb_keep = None
+
+    def forward_backward(self, inputs, loss_dev, solver_index=0, stream=None):
+        """One call of the registered producer without a sync: inputs are [(device_ptr, (n, c, h, w))] or CUDA
+        tensors, loss_dev a device float pointer; the gradient is added into diff_.  Returns True/False."""
+        blobs = (cos_blob * max(1, len(inputs)))()
+        for i, a in enumerate(inputs):
+            if hasattr(a, "data_ptr"):
+                ptr, shape = a.data_ptr(), tuple(a.shape)
+            else:
+                ptr, shape = a
+            shape = tuple(int(d) for d in shape) + (1,) * (4 - len(shape))
+            blobs[i].data, blobs[i].num, blobs[i].channels, blobs[i].height, blobs[i].width = ptr, *shape
+        return bool(self._L.cos_net_forward_backward(self._h, solver_index, blobs, len(inputs), loss_dev, stream))
 
     def param_count(self):
         return self._L.cos_net_param_count(self._h)

@@ -2,6 +2,7 @@
 #include "caffe_net.hpp"
 
 #include "caffe_proto_io.hpp"
+#include "native_producer.hpp"
 
 #include <stdio.h>
 #include <stdlib.h>
@@ -90,6 +91,7 @@ CaffeNet::~CaffeNet() {
     cudaSetDevice(device_);
     if (stream_) cudaStreamSynchronize(stream_);
     cudaDeviceSynchronize();
+    native_.reset();
     for (InputStage& st : stage_) {
       for (void* p : st.dev)
         if (p) cudaFree(p);
@@ -431,6 +433,11 @@ bool CaffeNet::check_status(std::string* err) {
   if (s == 400) {  // fused_sync_sgd_nvls.cu: the zeroing warp never saw an owner finish its reduce phase
     os << "device-side NVLS reduce phase of a peer did not finish within " << opt_timeout_ms_ << " ms (status 400)";
     *err = os.str();
+    return false;
+  }
+  if (s == kStatusBadLabel) {  // native_producer.cu softmax_loss_kernel
+    *err = "SoftmaxWithLoss: a label outside [0, number of classes) reached the native producer; its row added no "
+           "loss and no gradient (status 500)";
     return false;
   }
   if (s == 300) {  // fused_sync_sgd_tma.cu: an mbarrier never completed (a bulk copy was lost or a peer died mid-tile)
@@ -820,6 +827,44 @@ bool CaffeNet::restore(const std::string& model_file, const std::string& state_f
       return false;
     }
     COS_RT(cudaMemcpy(data_, flat.data(), count_ * sizeof(float), cudaMemcpyHostToDevice));
+    restored_model_ = true;
+  }
+  return true;
+}
+
+std::unique_ptr<NativeProducer> CaffeNet::build_native(const Plan& plan, bool fill, uint64_t seed, std::string* err) {
+  if (cudaSetDevice(device_) != cudaSuccess) {
+    *err = rt_err("cudaSetDevice", cudaGetLastError());
+    return nullptr;
+  }
+  std::unique_ptr<NativeProducer> p(NativeProducer::create(plan, device_, data_, diff_, status_, err));
+  if (p && fill && !restored_model_ && !p->fill(seed, stream_, err)) p.reset();
+  return p;
+}
+
+void CaffeNet::install_native(std::unique_ptr<NativeProducer> engine) {
+  native_ = std::move(engine);  // the replaced engine's destructor waits for its last call
+  fb_fn_ = &NativeProducer::callback;
+  fb_user_ = native_.get();
+}
+
+void CaffeNet::set_forward_backward(cos_forward_backward_fn fn, void* user) {
+  fb_fn_ = fn;
+  fb_user_ = user;
+  native_.reset();  // another producer replaces the built-in one: free its activations and workspace
+}
+
+bool CaffeNet::forward_backward(const cos_blob* inputs, int ninputs, float* loss_dev, cudaStream_t stream,
+                                std::string* err) {
+  if (!fb_fn_) {
+    *err = "forward_backward: no gradient producer registered";
+    return false;
+  }
+  COS_RT(cudaSetDevice(device_));
+  const int rc = fb_fn_(fb_user_, solver_index_, inputs, ninputs, loss_dev, stream ? stream : stream_);
+  if (rc != 0) {
+    *err = "gradient producer failed with code " + std::to_string(rc);
+    return false;
   }
   return true;
 }

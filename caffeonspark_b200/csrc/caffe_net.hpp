@@ -28,6 +28,9 @@
 
 namespace cosb {
 
+class NativeProducer;
+struct Plan;
+
 // AUTO uses the NVLS kernel from this world size on.  NVLink bytes per direction: NVLS 4P(1+1/N), P2P 8P(N-1)/N, but
 // multimem traffic carries more protocol overhead than plain stores, so the byte saving has to be large before NVLS
 // pays off.  Multi-GPU crossovers have not been measured on H100; this and the other AUTO thresholds below are
@@ -72,7 +75,15 @@ class CaffeNet {
   // seeded device-side fill of data_ (0) / diff_ (1) / history (2), see cos_net_fill
   bool fill(int which, uint64_t seed, uint64_t stream_id, float amp, std::string* err);
 
-  virtual void set_forward_backward(cos_forward_backward_fn fn, void* user) { fb_fn_ = fn; fb_user_ = user; }
+  // Registers a producer; a built-in one that was attached is released.
+  virtual void set_forward_backward(cos_forward_backward_fn fn, void* user);
+  // Builds the built-in producer of `plan` on this net's device and fills data_ from its fillers when `fill` and no
+  // model file was restored; nullptr + err on failure.  Not registered yet: see install_native.
+  std::unique_ptr<NativeProducer> build_native(const Plan& plan, bool fill, uint64_t seed, std::string* err);
+  // Registers a built engine as the producer, replacing (and releasing) any earlier one.  Cannot fail.
+  void install_native(std::unique_ptr<NativeProducer> engine);
+  // One call of the registered producer on device inputs (stream NULL = the net's stream); only enqueues.
+  bool forward_backward(const cos_blob* inputs, int ninputs, float* loss_dev, cudaStream_t stream, std::string* err);
   void set_solver_index(int i) { solver_index_ = i; }
   float* data() const { return data_; }
   float* diff() const { return diff_; }
@@ -176,6 +187,8 @@ class CaffeNet {
 
   cos_forward_backward_fn fb_fn_ = nullptr;
   void* fb_user_ = nullptr;
+  std::unique_ptr<NativeProducer> native_;  // the built-in producer, when attached
+  bool restored_model_ = false;             // restore() loaded weights from a model file
   int solver_index_ = 0;  // index the gradient producer sees (local device number inside the executor)
   // Input path (row f3): the reference keeps a 2-deep Free/Full queue of host blobs between the transformer
   // threads and the solver thread (CaffeProcessor.scala:32-35,442-452) and MemoryInputAdapter::feed points the

@@ -17,6 +17,7 @@
 #include "caffe_net.hpp"
 #include "caffe_proto_io.hpp"
 #include "hdf5_io.hpp"
+#include "native_producer.hpp"
 #include "peer_adapter.hpp"
 #include "solver_spec.hpp"
 
@@ -300,6 +301,64 @@ int cos_net_set_forward_backward(cos_net* net, cos_forward_backward_fn fn, void*
   if (!net) return fail("net is NULL");
   N(net)->set_forward_backward(fn, user);
   return 1;
+}
+
+int cos_net_use_native_producer(cos_net* net, const char* net_prototxt, int fill_weights) {
+  COS_GUARD(0, {
+    if (!net) return fail("net is NULL");
+    CaffeNet* r0 = R(net, 0);
+    const std::string path = net_prototxt ? net_prototxt : r0->spec().solver_file;
+    if (path.empty())
+      return fail("use_native_producer: this net was allocated from a layout descriptor, not a prototxt; pass the net "
+                  "prototxt");
+    SolverSpec s;
+    cosb::Plan plan;
+    std::string err;
+    if (!cosb::plan_from_prototxt(path, &s, &plan, &err)) return fail(err);
+    if (s.counts != r0->spec().counts)
+      return fail("use_native_producer: '" + path + "' has " + std::to_string(s.counts.size()) + " learnable blobs of " +
+                  std::to_string(plan.param_count) + " floats, which is not the layout of this net (" +
+                  std::to_string(r0->spec().counts.size()) + " blobs of " + std::to_string(r0->param_count()) + ")");
+    // the solver's random_seed (caffe.proto default -1: absent or negative fills with seed 0)
+    const int64_t seed = s.random_seed >= 0 ? s.random_seed : r0->spec().random_seed;
+    // every local solver's engine is built (and filled) before any is registered: a failure on one device leaves
+    // every solver with the producer it had
+    std::vector<std::unique_ptr<cosb::NativeProducer>> engines;
+    for (int i = 0; i < N(net)->num_local_devices(); ++i) {
+      engines.push_back(
+          R(net, i)->build_native(plan, fill_weights != 0, seed >= 0 ? static_cast<uint64_t>(seed) : 0, &err));
+      if (!engines.back()) return fail("local device " + std::to_string(i) + ": " + err);
+    }
+    for (int i = 0; i < N(net)->num_local_devices(); ++i) R(net, i)->install_native(std::move(engines[i]));
+    return 1;
+  })
+}
+
+int cos_net_forward_backward(cos_net* net, int solver_index, const cos_blob* inputs, int ninputs, float* loss_dev,
+                             void* cuda_stream) {
+  COS_GUARD(0, {
+    if (!net) return fail("net is NULL");
+    CaffeNet* r = R(net, solver_index);
+    if (!r) return fail("invalid solver_index");
+    if (!inputs || ninputs < 1) return fail("inputs is NULL");
+    if (!loss_dev) return fail("loss_dev is NULL");
+    std::string err;
+    if (!r->forward_backward(inputs, ninputs, loss_dev, static_cast<cudaStream_t>(cuda_stream), &err)) return fail(err);
+    return 1;
+  })
+}
+
+int cos_native_producer_plan(const char* prototxt, char* buf, int cap) {
+  COS_GUARD(-1, {
+    if (!prototxt) return fail("prototxt is NULL", -1);
+    SolverSpec s;
+    cosb::Plan plan;
+    std::string err;
+    if (!cosb::plan_from_prototxt(prototxt, &s, &plan, &err)) return fail(err, -1);
+    const std::string t = plan.text();
+    if (buf && cap > static_cast<int>(t.size())) memcpy(buf, t.c_str(), t.size() + 1);
+    return static_cast<int>(t.size());
+  })
 }
 
 float* cos_net_data(cos_net* net, int solver_index) {

@@ -107,6 +107,10 @@ JNIEXPORT jboolean JNICALL Java_com_yahoo_ml_jcaffe_CaffeNet_allocate(
     throw_java(env, cos_last_error());
     return JNI_FALSE;
   }
+  // train() needs a gradient producer: attach the built-in one when it can run this net (DESIGN.md section 14),
+  // filling the weights from the prototxt unless a model file was restored.  A net it refuses behaves as before:
+  // train() then fails until a producer is registered.
+  if (is_training) cos_net_use_native_producer(net, nullptr, (m.c && *m.c) ? 0 : 1);
   return set_native(env, self, net) ? JNI_TRUE : JNI_FALSE;
 }
 

@@ -1,0 +1,288 @@
+// native_producer.cpp -- the built-in producer's net plan (host only); see native_producer.hpp.
+#include "native_producer.hpp"
+
+#include <map>
+#include <sstream>
+
+namespace cosb {
+namespace {
+
+bool is_data_layer(const std::string& t) { return t == "MemoryData" || t == "CoSData" || t == "Input"; }
+
+std::string why(const NetLayer& L, const std::string& reason) {
+  return "layer '" + L.name + "' (" + L.type + "): " + reason + " (native producer)";
+}
+
+int64_t count_of(const std::vector<int64_t>& s) {
+  int64_t n = 1;
+  for (int64_t d : s) n *= d;
+  return n;
+}
+
+std::string shape_str(const std::vector<int64_t>& s) {
+  std::ostringstream os;
+  for (size_t i = 0; i < s.size(); ++i) os << (i ? "x" : "") << s[i];
+  return s.empty() ? "scalar" : os.str();
+}
+
+bool filler_ok(const FillerSpec& f, std::string* reason) {
+  static const char* types[] = {"constant", "uniform", "gaussian", "xavier", "msra"};
+  bool known = false;
+  for (const char* t : types) known = known || f.type == t;
+  if (!known) {
+    *reason = "filler type '" + f.type + "' is not supported (constant, uniform, gaussian, xavier, msra are)";
+    return false;
+  }
+  if (f.variance_norm != "FAN_IN" && f.variance_norm != "FAN_OUT" && f.variance_norm != "AVERAGE") {
+    *reason = "filler variance_norm '" + f.variance_norm + "' is not FAN_IN, FAN_OUT or AVERAGE";
+    return false;
+  }
+  return true;
+}
+
+// Caffe's ReLU and MAX pool as the existing fused block accepts them: slope 0; square window, pad 0, kernel <= 15.
+bool fusable_relu(const NetLayer& L) {
+  return L.type == "ReLU" && L.negative_slope == 0.f && L.bottoms.size() == 1 && L.tops.size() == 1;
+}
+bool fusable_pool(const NetLayer& L) {
+  return L.type == "Pooling" && L.pool == "MAX" && !L.global_pooling && L.pad_h == 0 && L.pad_w == 0 &&
+         L.kernel_h == L.kernel_w && L.stride_h == L.stride_w && L.kernel_h <= 15 && L.bottoms.size() == 1 &&
+         L.tops.size() == 1 && L.bottom_shapes[0].size() == 4;
+}
+
+}  // namespace
+
+bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Plan* plan, std::string* err) {
+  Plan P;
+  int64_t off = 0;
+  for (size_t k = 0; k < spec.counts.size(); ++k) {
+    P.blob_off.push_back(off);
+    P.blob_count.push_back(spec.counts[k]);
+    P.blob_shape.push_back(k < spec.shapes.size() ? spec.shapes[k] : std::vector<int64_t>{spec.counts[k]});
+    P.blob_filler.push_back(FillerSpec());
+    off += spec.counts[k];
+  }
+  P.param_count = off;
+  std::map<std::string, int> cur;  // blob name -> tensor id it currently names
+  std::vector<std::string> consumer;  // per tensor: the layer that reads it ("" = none yet)
+  auto new_tensor = [&](int64_t n, int storage) {
+    P.tensor_count.push_back(n);
+    P.storage.push_back(storage < 0 ? static_cast<int>(P.tensor_count.size()) - 1 : storage);
+    consumer.emplace_back();
+    return static_cast<int>(P.tensor_count.size()) - 1;
+  };
+  for (const NetLayer& L : layers) {  // staged inputs first: tensors 0 .. ninputs-1
+    if (!is_data_layer(L.type)) continue;
+    for (size_t t = 0; t < L.tops.size(); ++t) {
+      cur[L.tops[t]] = new_tensor(count_of(L.top_shapes[t]), -1);
+      P.input_names.push_back(L.tops[t]);
+    }
+  }
+  P.ninputs = static_cast<int>(P.tensor_count.size());
+  int losses = 0;
+  for (size_t i = 0; i < layers.size(); ++i) {
+    const NetLayer& L = layers[i];
+    if (is_data_layer(L.type) || L.type == "Accuracy" || L.type == "Silence") continue;  // no TRAIN work
+    if (L.has_loss_param) {
+      *err = why(L, "loss_param is not supported (only the default VALID normalisation without ignore_label is)");
+      return false;
+    }
+    const bool known = L.type == "Convolution" || L.type == "Pooling" || L.type == "InnerProduct" || L.type == "ReLU" ||
+                       L.type == "Sigmoid" || L.type == "BatchNorm" || L.type == "SoftmaxWithLoss";
+    if (!known) {
+      *err = why(L, "layer type not supported");
+      return false;
+    }
+    const size_t want_bottoms = L.type == "SoftmaxWithLoss" ? 2 : 1;
+    if (L.bottoms.size() != want_bottoms || L.tops.size() != 1) {
+      *err = why(L, "needs " + std::to_string(want_bottoms) + " bottom(s) and one top");
+      return false;
+    }
+    Op op;
+    op.name = L.name;
+    auto take = [&](const std::string& name, int* id) {
+      auto it = cur.find(name);
+      if (it == cur.end()) {
+        *err = why(L, "bottom '" + name + "' is not produced by an earlier TRAIN layer");
+        return false;
+      }
+      if (!consumer[it->second].empty()) {
+        *err = why(L, "bottom '" + name + "' already feeds layer '" + consumer[it->second] +
+                          "'; a blob read by two layers needs a Split");
+        return false;
+      }
+      consumer[it->second] = L.name;
+      *id = it->second;
+      return true;
+    };
+    if (!take(L.bottoms[0], &op.in)) return false;
+    op.in_shape = L.bottom_shapes[0];
+    op.out_shape = L.top_shapes[0];
+    op.need_dx = op.in >= P.ninputs;
+    int storage = -1;
+    std::string reason;
+    if (L.type == "Convolution") {
+      if (L.group != 1) {
+        *err = why(L, "group " + std::to_string(L.group) + " > 1 is not supported");
+        return false;
+      }
+      if (L.dilation_h != 1 || L.dilation_w != 1) {
+        *err = why(L, "dilation other than 1 is not supported");
+        return false;
+      }
+      if (!filler_ok(L.weight_filler, &reason) || (L.bias_term && !filler_ok(L.bias_filler, &reason))) {
+        *err = why(L, reason);
+        return false;
+      }
+      op.kind = OpKind::kConv;
+      op.kh = static_cast<int>(L.kernel_h), op.kw = static_cast<int>(L.kernel_w);
+      op.sh = static_cast<int>(L.stride_h), op.sw = static_cast<int>(L.stride_w);
+      op.ph = static_cast<int>(L.pad_h), op.pw = static_cast<int>(L.pad_w);
+      op.w_off = P.blob_off[L.first_blob], op.w_count = P.blob_count[L.first_blob];
+      P.blob_filler[L.first_blob] = L.weight_filler;
+      if (L.bias_term) {
+        op.b_off = P.blob_off[L.first_blob + 1], op.b_count = P.blob_count[L.first_blob + 1];
+        P.blob_filler[L.first_blob + 1] = L.bias_filler;
+      }
+      // conv + bias followed by ReLU and MAX pool in either order: the existing fused block (caffe_layers.cu)
+      if (L.bias_term && i + 2 < layers.size()) {
+        const NetLayer& a = layers[i + 1];
+        const NetLayer& b = layers[i + 2];
+        const bool order = (fusable_relu(a) && fusable_pool(b)) || (fusable_pool(a) && fusable_relu(b));
+        if (order && a.bottoms[0] == L.tops[0] && b.bottoms[0] == a.tops[0]) {
+          bool private_mid = true;  // the intermediates must not be read by any later layer
+          for (size_t j = i + 3; j < layers.size(); ++j)
+            for (const std::string& bn : layers[j].bottoms)
+              if ((bn == L.tops[0] || bn == a.tops[0]) && bn != b.tops[0]) private_mid = false;
+          if (private_mid) {
+            const NetLayer& pool = a.type == "Pooling" ? a : b;
+            op.kind = OpKind::kConvBiasReluMaxPool;
+            op.name = L.name + "+" + a.name + "+" + b.name;
+            op.pool_kernel = static_cast<int>(pool.kernel_h);
+            op.pool_stride = static_cast<int>(pool.stride_h);
+            op.out_shape = b.top_shapes[0];
+            const int out = new_tensor(count_of(op.out_shape), -1);
+            cur[b.tops[0]] = out;
+            op.out = out;
+            P.ops.push_back(op);
+            i += 2;
+            continue;
+          }
+        }
+      }
+    } else if (L.type == "Pooling") {
+      if (L.pool != "MAX" && L.pool != "AVE") {
+        *err = why(L, "pool method " + L.pool + " is not supported (MAX and AVE are)");
+        return false;
+      }
+      op.kind = OpKind::kPool;
+      op.max_pool = L.pool == "MAX";
+      op.kh = static_cast<int>(L.kernel_h), op.kw = static_cast<int>(L.kernel_w);
+      op.sh = static_cast<int>(L.stride_h), op.sw = static_cast<int>(L.stride_w);
+      op.ph = static_cast<int>(L.pad_h), op.pw = static_cast<int>(L.pad_w);
+    } else if (L.type == "InnerProduct") {
+      if (L.transpose) {
+        *err = why(L, "transpose: true is not supported");
+        return false;
+      }
+      if (L.axis != 1) {
+        *err = why(L, "axis other than 1 is not supported");
+        return false;
+      }
+      if (!filler_ok(L.weight_filler, &reason) || (L.bias_term && !filler_ok(L.bias_filler, &reason))) {
+        *err = why(L, reason);
+        return false;
+      }
+      op.kind = OpKind::kInnerProduct;
+      op.w_off = P.blob_off[L.first_blob], op.w_count = P.blob_count[L.first_blob];
+      P.blob_filler[L.first_blob] = L.weight_filler;
+      if (L.bias_term) {
+        op.b_off = P.blob_off[L.first_blob + 1], op.b_count = P.blob_count[L.first_blob + 1];
+        P.blob_filler[L.first_blob + 1] = L.bias_filler;
+      }
+    } else if (L.type == "ReLU" || L.type == "Sigmoid") {
+      op.kind = L.type == "ReLU" ? OpKind::kReLU : OpKind::kSigmoid;
+      op.slope = L.negative_slope;
+      // top == bottom shares the bottom's memory, except on a staged input: that is never written (every pass of an
+      // iter_size step reads it again), so the top gets storage of its own
+      op.in_place = L.tops[0] == L.bottoms[0] && op.in >= P.ninputs;
+      if (op.in_place) storage = P.storage[op.in];
+    } else if (L.type == "BatchNorm") {
+      op.kind = OpKind::kBatchNorm;  // separate top storage even when top == bottom: the kernels are not in place
+      op.w_off = P.blob_off[L.first_blob];
+      op.global_stats = L.use_global_stats;
+      op.fraction = L.moving_average_fraction;
+      op.eps = L.eps;
+    } else {  // SoftmaxWithLoss
+      if (++losses > 1) {
+        *err = why(L, "a second loss layer is not supported");
+        return false;
+      }
+      op.kind = OpKind::kSoftmaxLoss;
+      op.loss_weight = L.loss_weight;
+      auto it = cur.find(L.bottoms[1]);
+      if (it == cur.end()) {
+        *err = why(L, "label bottom '" + L.bottoms[1] + "' is not produced by an earlier TRAIN layer");
+        return false;
+      }
+      op.label = it->second;
+      const int64_t rows = op.in_shape.empty() ? 0 : count_of(op.in_shape) / (op.in_shape.size() > 1 ? op.in_shape[1] : 1);
+      if (op.in_shape.size() < 2 || P.tensor_count[op.label] != rows) {
+        *err = why(L, "label count " + std::to_string(P.tensor_count[op.label]) + " does not match the " +
+                          std::to_string(rows) + " rows of the scores");
+        return false;
+      }
+    }
+    op.out = new_tensor(count_of(op.out_shape), storage);
+    cur[L.tops[0]] = op.out;
+    P.ops.push_back(op);
+  }
+  if (losses == 0) {
+    *err = "the net has no SoftmaxWithLoss layer in its TRAIN phase (native producer)";
+    return false;
+  }
+  for (size_t t = 0; t < P.tensor_count.size(); ++t) {
+    if (P.tensor_count[t] <= 0 || P.tensor_count[t] >= (int64_t(1) << 31)) {
+      *err = "a blob of " + std::to_string(P.tensor_count[t]) + " elements is outside the native producer's range";
+      return false;
+    }
+  }
+  *plan = std::move(P);
+  return true;
+}
+
+bool plan_from_prototxt(const std::string& path, SolverSpec* spec, Plan* plan, std::string* err) {
+  std::vector<NetLayer> layers;
+  return parse_train_net(path, spec, &layers, err) && build_plan(*spec, layers, plan, err);
+}
+
+std::string Plan::text() const {
+  static const char* kinds[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling", "InnerProduct",
+                                "ReLU",        "Sigmoid",             "BatchNorm", "SoftmaxWithLoss"};
+  std::ostringstream os;
+  for (int i = 0; i < ninputs; ++i) os << "input " << i << " " << input_names[i] << " " << tensor_count[i] << "\n";
+  for (size_t i = 0; i < ops.size(); ++i) {
+    const Op& op = ops[i];
+    os << "op " << i << " " << kinds[static_cast<int>(op.kind)];
+    if (op.kind == OpKind::kPool) os << "(" << (op.max_pool ? "MAX" : "AVE") << ")";
+    os << " " << op.name << " " << shape_str(op.in_shape) << " -> " << shape_str(op.out_shape);
+    if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kPool)
+      os << " k" << op.kh << "x" << op.kw << " s" << op.sh << "x" << op.sw << " p" << op.ph << "x" << op.pw;
+    if (op.kind == OpKind::kConvBiasReluMaxPool) os << " pool" << op.pool_kernel << "/" << op.pool_stride;
+    if (op.kind == OpKind::kReLU && op.slope != 0.f) os << " slope=" << op.slope;
+    if (op.w_off >= 0 && op.kind != OpKind::kBatchNorm) os << " w=" << op.w_off << ":" << op.w_count;
+    if (op.b_off >= 0) os << " b=" << op.b_off << ":" << op.b_count;
+    if (op.kind == OpKind::kBatchNorm) os << " stats=" << op.w_off;
+    if (op.kind == OpKind::kSoftmaxLoss) os << " label=" << op.label << " loss_weight=" << op.loss_weight;
+    if (op.in_place) os << " in-place";
+    if (!op.need_dx) os << " staged-bottom";  // no data gradient is propagated into a staged input
+    os << "\n";
+  }
+  os << "params " << param_count << " blobs " << blob_count.size() << "\n";
+  for (size_t k = 0; k < blob_off.size(); ++k)
+    os << "blob " << k << " " << blob_off[k] << ":" << blob_count[k] << " " << shape_str(blob_shape[k]) << " "
+       << blob_filler[k].type << "\n";
+  return os.str();
+}
+
+}  // namespace cosb

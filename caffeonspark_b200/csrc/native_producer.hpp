@@ -1,0 +1,100 @@
+// native_producer.hpp -- the built-in gradient producer (Net::ForwardBackward for the TRAIN phase of the LeNet,
+// CIFAR-10-quick and CIFAR-10-full-BN family of nets; DESIGN.md section 14).
+//
+// build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
+// with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
+// of every learnable blob, or refuses the net naming the first layer it cannot run.  NativeProducer holds the device
+// buffers of one plan on one device and enqueues forward + backward (native_producer.cu).
+#ifndef COS_NATIVE_PRODUCER_HPP_
+#define COS_NATIVE_PRODUCER_HPP_
+
+#include <cuda_runtime_api.h>
+#include <stdint.h>
+
+#include <string>
+#include <vector>
+
+#include "../../include/caffedistri_b200.h"
+#include "solver_spec.hpp"
+
+namespace cosb {
+
+enum class OpKind { kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss };
+
+struct Op {
+  OpKind kind;
+  std::string name;                    // layer name (the fused block: "conv1+relu1+pool1")
+  int in = -1, out = -1, label = -1;   // tensor ids (label: SoftmaxWithLoss only)
+  std::vector<int64_t> in_shape, out_shape;
+  bool need_dx = true;                 // false when the bottom is a staged input
+  bool in_place = false;               // ReLU / Sigmoid with top == bottom: out shares in's storage (never a staged
+                                       // input's: those are not written)
+  // Convolution, Pooling, the fused block's convolution
+  int kh = 0, kw = 0, sh = 1, sw = 1, ph = 0, pw = 0;
+  bool max_pool = true;
+  int pool_kernel = 0, pool_stride = 0;  // the fused block's MAX pool (square, pad 0)
+  int64_t w_off = -1, w_count = 0, b_off = -1, b_count = 0;  // flat offsets into data_ / diff_
+  float slope = 0.f;                   // ReLU negative_slope
+  float loss_weight = 1.f;             // SoftmaxWithLoss
+  bool global_stats = false;           // BatchNorm
+  float fraction = 0.999f, eps = 1e-5f;
+};
+
+struct Plan {
+  std::vector<Op> ops;
+  std::vector<int64_t> tensor_count;   // elements per tensor id
+  std::vector<int> storage;            // tensor id -> tensor id that owns its memory (itself unless in place)
+  int ninputs = 0;                     // tensors 0 .. ninputs-1 are the staged inputs, in data-layer top order
+  std::vector<std::string> input_names;
+  std::vector<int64_t> blob_off, blob_count;  // every learnable blob, learnable_params() order
+  std::vector<std::vector<int64_t>> blob_shape;
+  std::vector<FillerSpec> blob_filler;
+  int64_t param_count = 0;
+  std::string text() const;  // one op per line (cos_native_producer_plan)
+};
+
+// Builds the plan of a parsed TRAIN net; false with "layer '<name>' (<type>): <reason>" when it cannot be run.
+bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Plan* plan, std::string* err);
+// parse_train_net + build_plan.
+bool plan_from_prototxt(const std::string& path, SolverSpec* spec, Plan* plan, std::string* err);
+
+// Status word value of a label outside [0, classes) (CaffeNet::check_status turns it into an error).
+constexpr int kStatusBadLabel = 500;
+
+class NativeProducer {
+ public:
+  // Allocates every activation, gradient, index, BatchNorm save area and split-K workspace of `plan` on `device`.
+  static NativeProducer* create(const Plan& plan, int device, float* data, float* diff, int* status, std::string* err);
+  ~NativeProducer();
+  // Fills data_ from the prototxt fillers with the counter-based generator keyed by (seed, blob index).  Synchronous.
+  bool fill(uint64_t seed, cudaStream_t stream, std::string* err);
+  // One forward + backward on `stream`: accumulates every gradient into diff_ once and writes the loss.  Only enqueues
+  // (no allocation, synchronisation or device query).  0 on success, else a cudaError_t or -1 for bad inputs.
+  int forward_backward(const cos_blob* inputs, int ninputs, float* loss_dev, cudaStream_t stream);
+  // cos_forward_backward_fn trampoline; `user` is the NativeProducer
+  static int callback(void* user, int solver_index, const cos_blob* inputs, int ninputs, float* loss_dev,
+                      void* cuda_stream);
+
+ private:
+  NativeProducer(const Plan& plan, int device, float* data, float* diff, int* status)
+      : plan_(plan), device_(device), data_(data), diff_(diff), status_(status) {}
+  bool allocate(std::string* err);
+  cudaError_t run_op_forward(const Op& op, size_t i, cudaStream_t s);
+  cudaError_t run_op_backward(const Op& op, size_t i, cudaStream_t s);
+
+  Plan plan_;
+  int device_;
+  float* data_;
+  float* diff_;
+  int* status_;
+  std::vector<float*> act_, grad_;        // per tensor id (staged inputs: act_ is the caller's buffer, set per call)
+  std::vector<void*> op_aux_;             // per op: MAX pool argmax (int32), fused block index (uint8), BN save
+  std::vector<float*> op_z_, op_dz_;      // fused block: conv output without bias and its gradient
+  cudaEvent_t done_ = nullptr;            // recorded at the end of every call: the destructor waits for it
+  float* workspace_ = nullptr;            // split-K partials, bias partials, BatchNorm scratch (ops run in order)
+  size_t workspace_floats_ = 0;
+  std::vector<void*> allocations_;
+};
+
+}  // namespace cosb
+#endif

@@ -265,8 +265,25 @@ HW pair_field(const Node& p, const std::string& rep, const std::string& h, const
   return r;
 }
 
-bool net_layout(const Node& net, SolverSpec* spec, std::string* err) {
+FillerSpec filler(const Node* f) {
+  FillerSpec s;
+  if (!f || !f->is_msg) return s;
+  s.type = f->str("type", "constant");
+  s.value = static_cast<float>(f->num("value", 0.0));
+  s.min = static_cast<float>(f->num("min", 0.0));
+  s.max = static_cast<float>(f->num("max", 1.0));
+  s.mean = static_cast<float>(f->num("mean", 0.0));
+  s.std = static_cast<float>(f->num("std", 1.0));
+  s.variance_norm = f->str("variance_norm", "FAN_IN");
+  return s;
+}
+
+std::vector<int64_t> to64(const Shape& s) { return std::vector<int64_t>(s.begin(), s.end()); }
+
+// `out` (optional) receives every TRAIN-phase layer with its blob shapes and the parameters the native producer reads.
+bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, std::string* err) {
   std::map<std::string, Shape> blobs;
+  if (out) out->clear();
   spec->counts.clear();
   spec->lr_mult.clear();
   spec->decay_mult.clear();
@@ -285,6 +302,16 @@ bool net_layout(const Node& net, SolverSpec* spec, std::string* err) {
       if (i < shapes.size()) for (const Node* d : shapes[i]->all("dim")) s.push_back(atol(d->value.c_str()));
       else for (size_t k = 4 * i; k < 4 * i + 4 && k < dims.size(); ++k) s.push_back(atol(dims[k]->value.c_str()));
       blobs[inputs[i]->value] = s;
+    }
+    if (out && !inputs.empty()) {
+      NetLayer rec;
+      rec.name = "input";
+      rec.type = "Input";
+      for (const Node* in : inputs) {
+        rec.tops.push_back(in->value);
+        rec.top_shapes.push_back(to64(blobs[in->value]));
+      }
+      out->push_back(rec);
     }
   }
   auto layers = net.all("layer");
@@ -310,6 +337,15 @@ bool net_layout(const Node& net, SolverSpec* spec, std::string* err) {
     };
     std::vector<long> param_counts;  // learnable blobs this layer owns, in order
     std::vector<std::vector<int64_t>> param_shapes;
+    NetLayer rec;
+    rec.name = name;
+    rec.type = type;
+    rec.bottoms = bottoms;
+    rec.tops = tops;
+    for (const std::string& b : bottoms) rec.bottom_shapes.push_back(blobs.count(b) ? to64(blobs[b]) : std::vector<int64_t>());
+    rec.first_blob = static_cast<int>(spec->counts.size());
+    rec.has_loss_param = L->first("loss_param") != nullptr;
+    if (const Node* lw = L->first("loss_weight")) rec.loss_weight = static_cast<float>(atof(lw->value.c_str()));
     if (type == "MemoryData") {
       const Node* p = L->first("memory_data_param");
       if (!p) { *err = "MemoryData layer without memory_data_param"; return false; }
@@ -361,6 +397,13 @@ bool net_layout(const Node& net, SolverSpec* spec, std::string* err) {
         *err = "layer '" + name + "': bad convolution_param";
         return false;
       }
+      rec.num_output = nout;
+      rec.group = group;
+      rec.kernel_h = k.h, rec.kernel_w = k.w, rec.stride_h = st.h, rec.stride_w = st.w;
+      rec.pad_h = pad.h, rec.pad_w = pad.w, rec.dilation_h = dil.h, rec.dilation_w = dil.w;
+      rec.bias_term = bias;
+      rec.weight_filler = filler(p->first("weight_filler"));
+      rec.bias_filler = filler(p->first("bias_filler"));
       Shape out(4);
       out[0] = in[0];
       if (type == "Convolution") {
@@ -400,6 +443,10 @@ bool net_layout(const Node& net, SolverSpec* spec, std::string* err) {
         if ((oh - 1) * st.h >= in[2] + pad.h) --oh;
         if ((ow - 1) * st.w >= in[3] + pad.w) --ow;
       }
+      rec.kernel_h = k.h, rec.kernel_w = k.w, rec.stride_h = st.h, rec.stride_w = st.w;
+      rec.pad_h = pad.h, rec.pad_w = pad.w;
+      rec.pool = p->str("pool", "MAX");
+      rec.global_pooling = p->boolean("global_pooling", false);
       for (const std::string& t : tops) blobs[t] = Shape{in[0], in[1], oh, ow};
     } else if (type == "InnerProduct") {
       const Node* p = L->first("inner_product_param");
@@ -418,12 +465,19 @@ bool net_layout(const Node& net, SolverSpec* spec, std::string* err) {
       Shape out(in.begin(), in.begin() + axis);
       out.push_back(nout);
       if (!tops.empty()) blobs[tops[0]] = out;
+      rec.num_output = nout;
+      rec.axis = axis;
+      rec.bias_term = p->boolean("bias_term", true);
+      rec.transpose = p->boolean("transpose", false);
+      rec.weight_filler = filler(p->first("weight_filler"));
+      rec.bias_filler = filler(p->first("bias_filler"));
     } else if (type == "ReLU" || type == "LRN" || type == "Dropout" || type == "Sigmoid" || type == "TanH" ||
                type == "Softmax" || type == "Power" || type == "AbsVal" || type == "BNLL" || type == "ELU" ||
                type == "Exp" || type == "Log" || type == "Threshold" || type == "Split" || type == "Eltwise") {
       Shape in;
       if (!bottom_shape(0, &in)) return false;
       for (const std::string& t : tops) blobs[t] = in;
+      if (const Node* p = L->first("relu_param")) rec.negative_slope = static_cast<float>(p->num("negative_slope", 0.0));
     } else if (type == "Flatten") {
       Shape in;
       if (!bottom_shape(0, &in) || in.empty()) return false;
@@ -453,6 +507,11 @@ bool net_layout(const Node& net, SolverSpec* spec, std::string* err) {
       param_counts = {C, C, 1};
       param_shapes = {{C}, {C}, {1}};
       for (const std::string& t : tops) blobs[t] = in;
+      if (const Node* p = L->first("batch_norm_param")) {  // caffe.proto BatchNormParameter
+        rec.use_global_stats = p->boolean("use_global_stats", false);
+        rec.moving_average_fraction = static_cast<float>(p->num("moving_average_fraction", 0.999));
+        rec.eps = static_cast<float>(p->num("eps", 1e-5));
+      }
     } else if (type == "Silence") {
     } else {
       *err = "layer '" + name + "' of type '" + type +
@@ -470,9 +529,16 @@ bool net_layout(const Node& net, SolverSpec* spec, std::string* err) {
       spec->layer_types.push_back(type);
       spec->shapes.push_back(param_shapes[i]);
     }
+    if (out) {
+      rec.nblobs = static_cast<int>(param_counts.size());
+      for (const std::string& t : tops) rec.top_shapes.push_back(blobs.count(t) ? to64(blobs[t]) : std::vector<int64_t>());
+      out->push_back(rec);
+    }
   }
   return true;
 }
+
+bool parse_solver(const std::string& solver_path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err);
 
 }  // namespace
 
@@ -480,7 +546,25 @@ bool parse_net_prototxt_text(const std::string& text, SolverSpec* spec, std::str
   Node net;
   TextParser tp(text);
   if (!tp.parse(&net, err)) return false;
-  return net_layout(net, spec, err);
+  return net_layout(net, spec, nullptr, err);
+}
+
+bool parse_train_net(const std::string& path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err) {
+  std::string text;
+  if (!read_file(path, &text)) {
+    *err = "cannot read prototxt '" + path + "'";
+    return false;
+  }
+  Node top;
+  TextParser tp(text);
+  if (!tp.parse(&top, err)) return false;
+  if (!top.all("layer").empty() || !top.all("layers").empty() || !top.all("input").empty())
+    return net_layout(top, spec, layers, err);
+  return parse_solver(path, spec, layers, err);
+}
+
+bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std::string* err) {
+  return parse_solver(solver_path, spec, nullptr, err);
 }
 
 bool check_solver_layout(const SolverSpec& spec, std::string* err) {
@@ -494,7 +578,8 @@ bool check_solver_layout(const SolverSpec& spec, std::string* err) {
   return true;
 }
 
-bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std::string* err) {
+namespace {
+bool parse_solver(const std::string& solver_path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err) {
   std::string text;
   if (!read_file(solver_path, &text)) {
     *err = "cannot read solver file '" + solver_path + "'";
@@ -522,6 +607,8 @@ bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std
   spec->clip_gradients = static_cast<float>(s.num("clip_gradients", -1.0));
   spec->solver_mode_gpu = s.str("solver_mode", "GPU") != "CPU";
   spec->snapshot_hdf5 = s.str("snapshot_format", "BINARYPROTO") == "HDF5";
+  spec->random_seed = s.integer("random_seed", -1);
+  spec->solver_file = solver_path;
   std::string type = s.str("type", "");
   if (type.empty()) {
     std::string st = s.str("solver_type", "SGD");  // deprecated enum field
@@ -550,7 +637,7 @@ bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std
   }
   // locate the net definition
   if (const Node* inl = s.first("net_param") ? s.first("net_param") : s.first("train_net_param")) {
-    return net_layout(*inl, spec, err) && check_solver_layout(*spec, err);
+    return net_layout(*inl, spec, layers, err) && check_solver_layout(*spec, err);
   }
   std::string net_path = s.str("net", "");
   if (net_path.empty()) net_path = s.str("train_net", "");
@@ -573,7 +660,11 @@ bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std
     *err = "cannot read net file '" + net_path + "' named by '" + solver_path + "'";
     return false;
   }
-  return parse_net_prototxt_text(net_text, spec, err) && check_solver_layout(*spec, err);
+  Node net;
+  TextParser np(net_text);
+  if (!np.parse(&net, err)) return false;
+  return net_layout(net, spec, layers, err) && check_solver_layout(*spec, err);
 }
+}  // namespace
 
 }  // namespace cosb

@@ -16,6 +16,33 @@
 
 namespace cosb {
 
+// FillerParameter (caffe.proto:43-62): what a weight_filler / bias_filler block says.  Caffe's default is constant 0.
+struct FillerSpec {
+  std::string type = "constant";
+  float value = 0.f, min = 0.f, max = 1.f, mean = 0.f, std = 1.f;
+  std::string variance_norm = "FAN_IN";
+};
+
+// One TRAIN-phase layer as the layout parser saw it: its blobs' shapes (from the same shape inference that derives
+// the learnable layout) and the parameters a forward/backward engine needs.  Fields a layer type does not have keep
+// their defaults.
+struct NetLayer {
+  std::string name, type;
+  std::vector<std::string> bottoms, tops;
+  std::vector<std::vector<int64_t>> bottom_shapes, top_shapes;
+  int first_blob = 0, nblobs = 0;  // learnable blobs of this layer: SolverSpec index first_blob ..
+  int64_t num_output = 0, axis = 1, group = 1;
+  int64_t kernel_h = 0, kernel_w = 0, stride_h = 1, stride_w = 1, pad_h = 0, pad_w = 0, dilation_h = 1, dilation_w = 1;
+  bool bias_term = true, transpose = false, global_pooling = false;
+  std::string pool = "MAX";
+  float negative_slope = 0.f;
+  bool use_global_stats = false;  // BatchNorm in TRAIN: default false
+  float moving_average_fraction = 0.999f, eps = 1e-5f;
+  float loss_weight = 1.f;
+  bool has_loss_param = false;
+  FillerSpec weight_filler, bias_filler;
+};
+
 struct SolverSpec {
   // learnable blobs in learnable_params() order
   std::vector<int64_t> counts;
@@ -42,6 +69,8 @@ struct SolverSpec {
   int iter_size = 1;
   float clip_gradients = -1.f;
   bool solver_mode_gpu = true;
+  int64_t random_seed = -1;  // SolverParameter.random_seed (caffe.proto: default -1)
+  std::string solver_file;   // the solver prototxt this spec was parsed from ("" for a descriptor)
   // training input layer
   int batch_size = 0;
   std::vector<int> input_shape;  // N,C,H,W of the first top of the data layer
@@ -75,6 +104,9 @@ bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std
 bool check_solver_layout(const SolverSpec& spec, std::string* err);
 // Parses only a net prototxt text (TRAIN phase) into the layout part of spec.
 bool parse_net_prototxt_text(const std::string& text, SolverSpec* spec, std::string* err);
+// A solver prototxt (its net is read as parse_solver_prototxt reads it) or a net prototxt, told apart by whether the
+// file has top-level layers: fills spec (solver fields only for a solver file) and the TRAIN-phase layer list.
+bool parse_train_net(const std::string& path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err);
 
 }  // namespace cosb
 #endif

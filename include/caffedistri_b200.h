@@ -197,6 +197,26 @@ COS_API int cos_net_get_validation_output_blobs(cos_net* net, int length, cos_bl
 /* Register Net::ForwardBackward (see cos_forward_backward_fn). */
 COS_API int cos_net_set_forward_backward(cos_net* net, cos_forward_backward_fn fn, void* user);
 
+/* The built-in gradient producer (DESIGN.md section 14): a forward/backward engine built from the TRAIN phase of a
+ * Caffe net prototxt, on this library's own sm_90a kernels.  It runs MemoryData / CoSData / Input, Convolution (group
+ * 1, dilation 1), Pooling (MAX, AVE), InnerProduct (axis 1), ReLU, Sigmoid, BatchNorm and SoftmaxWithLoss (default
+ * normalisation); Accuracy and Silence are skipped.  Every other layer, and loss_param or an unknown filler type, is
+ * refused with an error naming the layer.  Gradients are added into diff_ once per call and are bitwise reproducible.
+ * A label outside [0, classes) sets the net's device status word: the next synchronising call fails with a message. */
+/* Attach the built-in engine to every local solver of `net` and register it as the producer.
+ * net_prototxt NULL = the net the solver file named at allocate; otherwise a solver or net prototxt whose layout must
+ * equal the net's.  fill_weights 1 = initialise data_ from the prototxt fillers (only when no model_file was
+ * restored), drawn from the cos_net_fill generator keyed by (the solver's random_seed, blob index); random_seed absent
+ * or negative = seed 0, so every rank fills identically.  1/0. */
+COS_API int cos_net_use_native_producer(cos_net* net, const char* net_prototxt, int fill_weights);
+/* One Net::ForwardBackward with the registered producer on DEVICE inputs, no sync: accumulates into diff_, writes the
+ * loss to the device float loss_dev.  cuda_stream NULL = the net's stream.  1/0. */
+COS_API int cos_net_forward_backward(cos_net* net, int solver_index, const cos_blob* inputs, int ninputs,
+                                     float* loss_dev, void* cuda_stream);
+/* Host only, no device: the engine's plan for a solver or net prototxt as text (one op per line).  Returns the text
+ * length and copies it with its NUL when cap exceeds it (buf may be NULL to ask for the length), or -1 + error. */
+COS_API int cos_native_producer_plan(const char* prototxt, char* buf, int cap);
+
 /* Flat device buffers of Params<Dtype> (parallel.hpp:22-45): data_ and diff_,
  * each cos_net_param_count() = P fp32 elements, blobs laid out back to back in
  * learnable_params() order, and the start of the solver's history_: P floats for
