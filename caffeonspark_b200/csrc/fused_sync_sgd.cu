@@ -37,7 +37,6 @@ namespace cosb {
 namespace {
 
 constexpr int kDefaultThreads = 512;
-constexpr int kMaxSegSmem = 1024;
 
 // --------------------------------------------------------- reduce (phase 1)
 
@@ -51,40 +50,16 @@ __device__ __forceinline__ float4 reduce_vec(const SyncParams& p, int s, uint64_
   for (int j = 0; j < N; ++j) {  // all loads first: N independent 128-bit requests in flight
     int src = s + j;
     if (src >= N) src -= N;
-    if (BF16) {
-      uint2 u = ld_stream_u2(p.wire[src] + i);
-      x[j] = make_float4(bf16_bits_to_float(u.x & 0xffffu), bf16_bits_to_float(u.x >> 16),
-                         bf16_bits_to_float(u.y & 0xffffu), bf16_bits_to_float(u.y >> 16));
-    } else {
-      x[j] = ld_stream(p.diff[src] + i);
-    }
+    x[j] = BF16 ? unpack_bf16x4(ld_stream_u2(p.wire[src] + i)) : ld_stream(p.diff[src] + i);
   }
   const float inv = p.inv_scale;
-  float4 acc = make_float4(__fmul_rn(inv, x[0].x), __fmul_rn(inv, x[0].y), __fmul_rn(inv, x[0].z),
-                           __fmul_rn(inv, x[0].w));
+  float4 acc = scale4(inv, x[0]);
 #pragma unroll
-  for (int j = 1; j < N; ++j) {
-    acc.x = __fadd_rn(__fmul_rn(inv, x[j].x), acc.x);
-    acc.y = __fadd_rn(__fmul_rn(inv, x[j].y), acc.y);
-    acc.z = __fadd_rn(__fmul_rn(inv, x[j].z), acc.z);
-    acc.w = __fadd_rn(__fmul_rn(inv, x[j].w), acc.w);
-  }
+  for (int j = 1; j < N; ++j) add_scaled(acc, inv, x[j]);
   return acc;
 }
 
-// runtime-world fallback (N not instantiated): sequential accumulate
-template <bool BF16>
-__device__ __forceinline__ float reduce_scalar(const SyncParams& p, int s, uint64_t i) {
-  float acc = 0.f;
-  for (int j = 0; j < p.world; ++j) {
-    int src = s + j;
-    if (src >= p.world) src -= p.world;
-    float x = BF16 ? bf16_bits_to_float(p.wire[src][i]) : p.diff[src][i];
-    x = __fmul_rn(p.inv_scale, x);
-    acc = (j == 0) ? x : __fadd_rn(x, acc);
-  }
-  return acc;
-}
+// runtime-world fallback (N not instantiated): sequential accumulate (reduce_scalar, sync_device.cuh)
 
 template <int N, bool BF16>
 __device__ __forceinline__ float4 reduce_vec_any(const SyncParams& p, int s, uint64_t i) {
@@ -140,18 +115,9 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
       const ShardRange r = shard_range(p.count, world, s);
       for (uint64_t j = tid; j < r.nvec; j += stride) {
         const uint64_t i = (r.vec_lo + j) << 2;
-        float4 v = ld_stream(g + i);
-        uint2 o;
-        o.x = static_cast<uint32_t>(float_to_bf16_bits(v.x)) | (static_cast<uint32_t>(float_to_bf16_bits(v.y)) << 16);
-        o.y = static_cast<uint32_t>(float_to_bf16_bits(v.z)) | (static_cast<uint32_t>(float_to_bf16_bits(v.w)) << 16);
-        *reinterpret_cast<uint2*>(wv + i) = o;
+        *reinterpret_cast<uint2*>(wv + i) = pack_bf16x4(ld_stream(g + i));
       }
-      if (blockIdx.x == 0) {
-        const uint64_t nhead = r.head_end - r.lo, ntail = r.hi - r.tail_begin;
-        if (threadIdx.x < nhead) wv[r.lo + threadIdx.x] = float_to_bf16_bits(g[r.lo + threadIdx.x]);
-        else if (threadIdx.x - nhead < ntail)
-          wv[r.tail_begin + (threadIdx.x - nhead)] = float_to_bf16_bits(g[r.tail_begin + (threadIdx.x - nhead)]);
-      }
+      if (blockIdx.x == 0) for_edge_element(r, threadIdx.x, [&](uint64_t i) { wv[i] = float_to_bf16_bits(g[i]); });
     }
   }
 
@@ -176,10 +142,7 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
       }
     }
     if (blockIdx.x == 0) {
-      const uint64_t nhead = r.head_end - r.lo, ntail = r.hi - r.tail_begin;
-      uint64_t i = ~0ull;
-      if (threadIdx.x < nhead) i = r.lo + threadIdx.x;
-      else if (threadIdx.x - nhead < ntail) i = r.tail_begin + (threadIdx.x - nhead);
+      const uint64_t i = edge_element(r, threadIdx.x);
       if (i != ~0ull) {
         const float v = w[i];
         for (int q = 1; q < world; ++q) {
@@ -214,12 +177,8 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
         float4 g;
         if (p.mode == kModeLocal) {
           g = ld_stream(p.diff[rank] + i);  // no scale at N == 1 (CaffeNet.cpp:206-216: no sync object)
-          if (BF16) {  // bf16 gradient inputs: same rounding the wire applies at N > 1
-            g.x = bf16_bits_to_float(float_to_bf16_bits(g.x));
-            g.y = bf16_bits_to_float(float_to_bf16_bits(g.y));
-            g.z = bf16_bits_to_float(float_to_bf16_bits(g.z));
-            g.w = bf16_bits_to_float(float_to_bf16_bits(g.w));
-          }
+          if (BF16)  // bf16 gradient inputs: same rounding the wire applies at N > 1
+            g = make_float4(round_bf16(g.x), round_bf16(g.y), round_bf16(g.z), round_bf16(g.w));
         } else {
           g = reduce_vec_any<N, BF16>(p, s, i);
         }
@@ -244,15 +203,12 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
         }
       }
       if (blockIdx.x == 0) {  // scalar head / tail of the range (<= 3 elements each)
-        const uint64_t nhead = r.head_end - r.lo, ntail = r.hi - r.tail_begin;
-        uint64_t i = ~0ull;
-        if (threadIdx.x < nhead) i = r.lo + threadIdx.x;
-        else if (threadIdx.x - nhead < ntail) i = r.tail_begin + (threadIdx.x - nhead);
+        const uint64_t i = edge_element(r, threadIdx.x);
         if (i != ~0ull) {
           SegCursor c2 = cur;
           c2.seek(i);
           float g = (p.mode == kModeLocal) ? p.diff[rank][i] : reduce_scalar<BF16>(p, s, i);
-          if (BF16 && p.mode == kModeLocal) g = bf16_bits_to_float(float_to_bf16_bits(g));
+          if (BF16 && p.mode == kModeLocal) g = round_bf16(g);
           float w = wl[i], h = hl[i];
           update_element<ADAM, NORM>(p, c2, i, g, w, h);
           hl[i] = h;
@@ -288,18 +244,14 @@ __global__ void __launch_bounds__(kDefaultThreads, 2) fused_sync_sgd_kernel(cons
       for (int s = 0; s < world; ++s) {
         const ShardRange r = shard_range(p.count, world, s);
         for (uint64_t j = tid; j < r.nvec; j += stride) *reinterpret_cast<float4*>(g + ((r.vec_lo + j) << 2)) = z;
-        if (blockIdx.x == 0) {
-          const uint64_t nhead = r.head_end - r.lo, ntail = r.hi - r.tail_begin;
-          if (threadIdx.x < nhead) g[r.lo + threadIdx.x] = 0.f;
-          else if (threadIdx.x - nhead < ntail) g[r.tail_begin + (threadIdx.x - nhead)] = 0.f;
-        }
+        if (blockIdx.x == 0) for_edge_element(r, threadIdx.x, [&](uint64_t i) { g[i] = 0.f; });
       }
     }
   }
   if (tracer) p.trace[4] = globaltimer_ns();
 }
 
-__device__ __forceinline__ uint64_t mix64(uint64_t z) {
+__host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {
   z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ULL;
   z = (z ^ (z >> 27)) * 0x94d049bb133111ebULL;
   return z ^ (z >> 31);
@@ -322,30 +274,10 @@ __global__ void loss_mean_kernel(const float* slots, int passes, float* out) {
   *out = __fdiv_rn(s, static_cast<float>(passes));
 }
 
-uint64_t host_mix64(uint64_t z) {
-  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ULL;
-  z = (z ^ (z >> 27)) * 0x94d049bb133111ebULL;
-  return z ^ (z >> 31);
-}
-
-template <int N, bool NORM>
-void launch_solver(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (p.solver == kSolverAdam) {
-    if (p.grad_bf16) fused_sync_sgd_kernel<N, true, true, NORM><<<grid, block, smem, stream>>>(p);
-    else fused_sync_sgd_kernel<N, false, true, NORM><<<grid, block, smem, stream>>>(p);
-  } else if (p.grad_bf16) {
-    fused_sync_sgd_kernel<N, true, false, NORM><<<grid, block, smem, stream>>>(p);
-  } else {
-    fused_sync_sgd_kernel<N, false, false, NORM><<<grid, block, smem, stream>>>(p);
-  }
-}
-
-template <int N>
-cudaError_t launch_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (sync_normalizes(p)) launch_solver<N, true>(p, grid, block, smem, stream);
-  else launch_solver<N, false>(p, grid, block, smem, stream);
-  return cudaGetLastError();
-}
+struct LdgKernel {
+  template <int N, bool BF16, bool ADAM, bool NORM>
+  static constexpr auto kernel = fused_sync_sgd_kernel<N, BF16, ADAM, NORM>;
+};
 
 }  // namespace
 
@@ -359,7 +291,7 @@ int default_sync_grid(int device) {
 }
 
 cudaError_t launch_fused_sync_sgd(const SyncParams& p, int grid, int block, cudaStream_t stream) {
-  if (p.world < 1 || p.world > kMaxRanks || p.rank < 0 || p.rank >= p.world) return cudaErrorInvalidValue;
+  if (!valid_world(p, 1)) return cudaErrorInvalidValue;
   if (block <= 0) block = kDefaultThreads;
   if (block > kDefaultThreads || block < kMaxRanks || (block & 31)) return cudaErrorInvalidValue;
   if (grid <= 0) {
@@ -375,18 +307,8 @@ cudaError_t launch_fused_sync_sgd(const SyncParams& p, int grid, int block, cuda
   uint64_t need = (work_vecs + block - 1) / block;
   if (need < 1) need = 1;
   if (static_cast<uint64_t>(grid) > need) grid = static_cast<int>(need);
-  size_t smem = p.nseg <= kMaxSegSmem ? static_cast<size_t>(p.nseg) * (sizeof(uint64_t) + 2 * sizeof(float)) : 0;
   const int n = (p.mode == kModeLocal || p.mode == kModeAllGather) ? 0 : p.world;
-  switch (n) {
-    case 2: return launch_n<2>(p, grid, block, smem, stream);
-    case 3: return launch_n<3>(p, grid, block, smem, stream);
-    case 4: return launch_n<4>(p, grid, block, smem, stream);
-    case 5: return launch_n<5>(p, grid, block, smem, stream);
-    case 6: return launch_n<6>(p, grid, block, smem, stream);
-    case 7: return launch_n<7>(p, grid, block, smem, stream);
-    case 8: return launch_n<8>(p, grid, block, smem, stream);
-    default: return launch_n<0>(p, grid, block, smem, stream);
-  }
+  return launch_sync<LdgKernel, true>(p, n, grid, block, seg_smem_bytes(p.nseg), stream);
 }
 
 // TMA (cp.async.bulk) pipelined variant: see fused_sync_sgd_tma.cu.
@@ -398,7 +320,7 @@ cudaError_t launch_loss_mean(const float* slots, int passes, float* out, cudaStr
 }
 
 cudaError_t launch_fill(float* out, uint64_t n, uint64_t seed, uint64_t stream_id, float amp, cudaStream_t stream) {
-  const uint64_t key = host_mix64(seed * 0x9e3779b97f4a7c15ULL + stream_id);
+  const uint64_t key = mix64(seed * 0x9e3779b97f4a7c15ULL + stream_id);
   int grid = static_cast<int>((n + 255) / 256);
   if (grid > kTargetSms * 16) grid = kTargetSms * 16;
   if (grid < 1) grid = 1;

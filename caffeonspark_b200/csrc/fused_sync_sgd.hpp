@@ -2,8 +2,9 @@
 //
 // One launch performs what the reference spreads over on_gradients_ready()
 // (parallel_cpu.cpp:120-122 scale, socket_sync_cpu.cpp:108-133 reduce-scatter),
-// SGDSolver::ApplyUpdate (sgd_solver.cpp:102-116) and the next Step's
-// on_start() (socket_sync_cpu.cpp:102-105 all-gather), see fused_sync_sgd.cu.
+// the solver's ApplyUpdate (SGD: sgd_solver.cpp:102-116, Adam: adam_solver.cpp,
+// with Normalize for iter_size > 1) and the next Step's on_start()
+// (socket_sync_cpu.cpp:102-105 all-gather), see fused_sync_sgd.cu.
 #ifndef COS_FUSED_SYNC_SGD_HPP_
 #define COS_FUSED_SYNC_SGD_HPP_
 

@@ -34,7 +34,6 @@ namespace cosb {
 namespace {
 
 constexpr int kLLThreads = 512;
-constexpr int kLLMaxSeg = 1024;
 constexpr int kEdgeWords = 8;  // scalar head/tail elements of a shard travel in 8 extra words behind the body
 
 __device__ __forceinline__ void st_ll2(uint64_t* p, uint64_t a, uint64_t b) {  // two atomic 8-byte words
@@ -123,12 +122,6 @@ __device__ __forceinline__ bool poll1(const uint64_t* w, uint32_t flag, Poll& po
 __device__ __forceinline__ uint64_t edge_index(const ShardRange& r, uint64_t e) {
   return e < r.head_end ? e - r.lo : 4 + (e - r.tail_begin);
 }
-__device__ __forceinline__ uint64_t edge_of_thread(const ShardRange& r, unsigned t) {
-  const uint64_t nhead = r.head_end - r.lo, ntail = r.hi - r.tail_begin;
-  if (t < nhead) return r.lo + t;
-  if (t - nhead < ntail) return r.tail_begin + (t - nhead);
-  return ~0ull;
-}
 
 // N = compile-time world size, 2..8 (the N-1 polled slots live in registers)
 // ADAM: Adam update with the second history half (sync_device.cuh), false = SGD.
@@ -140,7 +133,7 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
   uint64_t* s_end = reinterpret_cast<uint64_t*>(smem_raw);
   float* s_lr = reinterpret_cast<float*>(s_end + p.nseg);
   float* s_dm = s_lr + p.nseg;
-  const bool seg_in_smem = p.nseg <= kLLMaxSeg;
+  const bool seg_in_smem = p.nseg <= kMaxSegSmem;
   if (seg_in_smem) {
     for (int k = threadIdx.x; k < p.nseg; k += blockDim.x) {
       s_end[k] = p.seg_end[k];
@@ -206,10 +199,10 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
       int q = rank + d;
       if (q >= world) q -= world;
       const ShardRange r = shard_range(p.count, world, q);
-      const uint64_t e = edge_of_thread(r, threadIdx.x);
+      const uint64_t e = edge_element(r, threadIdx.x);
       if (e != ~0ull) {
         float x = g[e];
-        if (BF16) x = bf16_bits_to_float(float_to_bf16_bits(x));
+        if (BF16) x = round_bf16(x);
         st_ll1(p.ll_grad[q] + static_cast<uint64_t>(rank) * gslot + gedge + edge_index(r, e), ll_word(__float_as_uint(x), flag));
       }
     }
@@ -222,7 +215,7 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
       const ShardRange r = shard_range(p.count, world, q);
       for (uint64_t j = tid; j < r.nvec; j += stride) st_vec(g + ((r.vec_lo + j) << 2), z4);
       if (blockIdx.x == 0) {
-        const uint64_t e = edge_of_thread(r, threadIdx.x);
+        const uint64_t e = edge_element(r, threadIdx.x);
         if (e != ~0ull) g[e] = 0.f;
       }
     }
@@ -253,11 +246,8 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
       float4 h = *reinterpret_cast<const float4*>(hl + i);
       float4 v;
       load_v<ADAM>(p, i, v);
-      if (BF16) {
-        x.x = bf16_bits_to_float(float_to_bf16_bits(x.x)); x.y = bf16_bits_to_float(float_to_bf16_bits(x.y));
-        x.z = bf16_bits_to_float(float_to_bf16_bits(x.z)); x.w = bf16_bits_to_float(float_to_bf16_bits(x.w));
-      }
-      float4 acc = make_float4(__fmul_rn(inv, x.x), __fmul_rn(inv, x.y), __fmul_rn(inv, x.z), __fmul_rn(inv, x.w));
+      if (BF16) x = make_float4(round_bf16(x.x), round_bf16(x.y), round_bf16(x.z), round_bf16(x.w));
+      float4 acc = scale4(inv, x);
       constexpr int K = N - 1;  // the N-1 slots, polled together
       constexpr int W = BF16 ? 2 : 4;
       const uint64_t* ptr[K];
@@ -274,19 +264,14 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
       for (int k = 0; k < K; ++k) {  // reference order: rank+1, rank+2, ... (mod N)
         float4 y;
         if (BF16) {
-          const uint32_t u0 = static_cast<uint32_t>(words[k][0]), u1 = static_cast<uint32_t>(words[k][1]);
-          y = make_float4(bf16_bits_to_float(u0 & 0xffffu), bf16_bits_to_float(u0 >> 16),
-                          bf16_bits_to_float(u1 & 0xffffu), bf16_bits_to_float(u1 >> 16));
+          y = unpack_bf16x4(make_uint2(static_cast<uint32_t>(words[k][0]), static_cast<uint32_t>(words[k][1])));
         } else {
           y = make_float4(__uint_as_float(static_cast<uint32_t>(words[k][0])),
                           __uint_as_float(static_cast<uint32_t>(words[k][1])),
                           __uint_as_float(static_cast<uint32_t>(words[k][W - 2])),
                           __uint_as_float(static_cast<uint32_t>(words[k][W - 1])));
         }
-        acc.x = __fadd_rn(__fmul_rn(inv, y.x), acc.x);
-        acc.y = __fadd_rn(__fmul_rn(inv, y.y), acc.y);
-        acc.z = __fadd_rn(__fmul_rn(inv, y.z), acc.z);
-        acc.w = __fadd_rn(__fmul_rn(inv, y.w), acc.w);
+        add_scaled(acc, inv, y);
       }
       if (!alive) break;
       update_vec<ADAM, NORM>(p, cur, i, acc, w, h, v);
@@ -304,12 +289,12 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
       }
     }
     if (alive && blockIdx.x == 0) {  // scalar head / tail of my shard
-      const uint64_t e = edge_of_thread(r, threadIdx.x);
+      const uint64_t e = edge_element(r, threadIdx.x);
       if (e != ~0ull) {
         SegCursor c2 = cur;
         c2.seek(e);
         float x = g[e];
-        if (BF16) x = bf16_bits_to_float(float_to_bf16_bits(x));
+        if (BF16) x = round_bf16(x);
         float acc = __fmul_rn(inv, x);
         for (int k = 1; alive && k < world; ++k) {
           int src = rank + k;
@@ -335,7 +320,7 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
     if (zero) {  // my own shard of diff_ (read above by exactly these threads)
       for (uint64_t j = tid; j < r.nvec; j += stride) st_vec(g + ((r.vec_lo + j) << 2), z4);
       if (blockIdx.x == 0) {
-        const uint64_t e = edge_of_thread(r, threadIdx.x);
+        const uint64_t e = edge_element(r, threadIdx.x);
         if (e != ~0ull) g[e] = 0.f;
       }
     }
@@ -377,7 +362,7 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
         int q = rank + d;
         if (q >= world) q -= world;
         const ShardRange r = shard_range(p.count, world, q);
-        const uint64_t e = edge_of_thread(r, threadIdx.x);
+        const uint64_t e = edge_element(r, threadIdx.x);
         if (e != ~0ull) {
           uint32_t u;
           alive = poll1(p.ll_weight[rank] + static_cast<uint64_t>(q) * wslot + wedge + edge_index(r, e), flag, poll, q, u);
@@ -389,24 +374,10 @@ __global__ void __launch_bounds__(kLLThreads, 1) fused_sync_sgd_ll_kernel(const 
   if (tracer) p.trace[4] = globaltimer_ns();
 }
 
-template <int N, bool NORM>
-void launch_ll_solver(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (p.solver == kSolverAdam) {
-    if (p.grad_bf16) fused_sync_sgd_ll_kernel<N, true, true, NORM><<<grid, block, smem, stream>>>(p);
-    else fused_sync_sgd_ll_kernel<N, false, true, NORM><<<grid, block, smem, stream>>>(p);
-  } else if (p.grad_bf16) {
-    fused_sync_sgd_ll_kernel<N, true, false, NORM><<<grid, block, smem, stream>>>(p);
-  } else {
-    fused_sync_sgd_ll_kernel<N, false, false, NORM><<<grid, block, smem, stream>>>(p);
-  }
-}
-
-template <int N>
-cudaError_t launch_ll_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (sync_normalizes(p)) launch_ll_solver<N, true>(p, grid, block, smem, stream);
-  else launch_ll_solver<N, false>(p, grid, block, smem, stream);
-  return cudaGetLastError();
-}
+struct LLKernel {
+  template <int N, bool BF16, bool ADAM, bool NORM>
+  static constexpr auto kernel = fused_sync_sgd_ll_kernel<N, BF16, ADAM, NORM>;
+};
 
 }  // namespace
 
@@ -421,7 +392,7 @@ void ll_slot_words(uint64_t count, int world, bool bf16, uint64_t* grad_words, u
 
 cudaError_t launch_fused_sync_sgd_ll(const SyncParams& p, int grid, int block, int vecs_per_thread,
                                      cudaStream_t stream) {
-  if (p.world < 2 || p.world > kMaxRanks || p.rank < 0 || p.rank >= p.world) return cudaErrorInvalidValue;
+  if (!valid_world(p, 2)) return cudaErrorInvalidValue;
   if (p.mode != kModeTwoShot || p.ll_grad_stride == 0 || p.ll_weight_stride == 0) return cudaErrorInvalidValue;
   if (block <= 0) block = kLLThreads;
   if (block > kLLThreads || block < kMaxRanks || (block & 31)) return cudaErrorInvalidValue;
@@ -440,17 +411,8 @@ cudaError_t launch_fused_sync_sgd_ll(const SyncParams& p, int grid, int block, i
     grid = static_cast<int>(need > static_cast<uint64_t>(cap) ? cap : need);
   }
   if (grid > cap) grid = cap;
-  const size_t smem = p.nseg <= kLLMaxSeg ? static_cast<size_t>(p.nseg) * (sizeof(uint64_t) + 2 * sizeof(float)) : 0;
-  switch (p.world) {
-    case 2: return launch_ll_n<2>(p, grid, block, smem, stream);
-    case 3: return launch_ll_n<3>(p, grid, block, smem, stream);
-    case 4: return launch_ll_n<4>(p, grid, block, smem, stream);
-    case 5: return launch_ll_n<5>(p, grid, block, smem, stream);
-    case 6: return launch_ll_n<6>(p, grid, block, smem, stream);
-    case 7: return launch_ll_n<7>(p, grid, block, smem, stream);
-    case 8: return launch_ll_n<8>(p, grid, block, smem, stream);
-    default: return cudaErrorInvalidValue;  // world sizes 9..16 use the barrier-based kernels
-  }
+  // world sizes 9..16 use the barrier-based kernels
+  return launch_sync<LLKernel, false>(p, p.world, grid, block, seg_smem_bytes(p.nseg), stream);
 }
 
 }  // namespace cosb

@@ -40,7 +40,6 @@ namespace cosb {
 namespace {
 
 constexpr int kNvlsThreads = 512;
-constexpr int kNvlsMaxSeg = 1024;
 
 constexpr int kWorkThreads = kNvlsThreads - 32;  // warps 0..14 reduce, warp 15 zeroes diff_ behind them
 constexpr uint32_t kIterBits = 16;               // progress word = (epoch << 16) | iterations done (< 65536)
@@ -55,7 +54,7 @@ __global__ void __launch_bounds__(kNvlsThreads, 1) fused_sync_sgd_nvls_kernel(co
   uint64_t* s_end = reinterpret_cast<uint64_t*>(smem_raw);
   float* s_lr = reinterpret_cast<float*>(s_end + p.nseg);
   float* s_dm = s_lr + p.nseg;
-  const bool seg_in_smem = p.nseg <= kNvlsMaxSeg;
+  const bool seg_in_smem = p.nseg <= kMaxSegSmem;
   if (seg_in_smem) {
     for (int k = threadIdx.x; k < p.nseg; k += blockDim.x) {
       s_end[k] = p.seg_end[k];
@@ -285,7 +284,7 @@ cudaError_t launch_share(const SyncParams& p, int grid, size_t smem, cudaStream_
 }  // namespace
 
 cudaError_t launch_fused_sync_sgd_nvls(const SyncParams& p, int grid, cudaStream_t stream) {
-  if (p.world < 2 || p.world > kMaxRanks || p.rank < 0 || p.rank >= p.world) return cudaErrorInvalidValue;
+  if (!valid_world(p, 2)) return cudaErrorInvalidValue;
   if (p.mode != kModeTwoShot || p.grad_bf16 || !p.mc_data || !p.mc_diff) return cudaErrorInvalidValue;
   if (p.solver != kSolverSgd) return cudaErrorInvalidValue;  // SGD only
   int dev = 0, sms = kTargetSms;
@@ -296,7 +295,7 @@ cudaError_t launch_fused_sync_sgd_nvls(const SyncParams& p, int grid, cudaStream
   uint64_t need = (((p.count / p.world) >> 2) + kWorkThreads - 1) / kWorkThreads;  // one vector per work thread
   if (need < 1) need = 1;
   if (static_cast<uint64_t>(grid) > need) grid = static_cast<int>(need);
-  const size_t smem = p.nseg <= kNvlsMaxSeg ? static_cast<size_t>(p.nseg) * (sizeof(uint64_t) + 2 * sizeof(float)) : 0;
+  const size_t smem = seg_smem_bytes(p.nseg);
   {  // the per-CTA progress counter has kIterBits bits
     const uint64_t u = static_cast<uint64_t>((p.nvls_unroll > 0 ? p.nvls_unroll : 1) + (p.nvls_p2p > 0 ? 1 : 0));
     const uint64_t per_round = static_cast<uint64_t>(grid) * kWorkThreads * u;

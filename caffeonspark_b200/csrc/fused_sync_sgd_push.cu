@@ -40,29 +40,6 @@ namespace cosb {
 namespace {
 
 constexpr int kPushThreads = 512;
-constexpr int kPushMaxSeg = 1024;
-
-__device__ __forceinline__ float round_bf16(float x) { return bf16_bits_to_float(float_to_bf16_bits(x)); }
-
-__device__ __forceinline__ uint2 pack_bf16x4(const float4& v) {
-  uint2 o;
-  o.x = static_cast<uint32_t>(float_to_bf16_bits(v.x)) | (static_cast<uint32_t>(float_to_bf16_bits(v.y)) << 16);
-  o.y = static_cast<uint32_t>(float_to_bf16_bits(v.z)) | (static_cast<uint32_t>(float_to_bf16_bits(v.w)) << 16);
-  return o;
-}
-
-__device__ __forceinline__ float4 unpack_bf16x4(const uint2& u) {
-  return make_float4(bf16_bits_to_float(u.x & 0xffffu), bf16_bits_to_float(u.x >> 16),
-                     bf16_bits_to_float(u.y & 0xffffu), bf16_bits_to_float(u.y >> 16));
-}
-
-// scalar head / tail element of a shard range handled by thread t of CTA 0 (or ~0)
-__device__ __forceinline__ uint64_t edge_element(const ShardRange& r, unsigned t) {
-  const uint64_t nhead = r.head_end - r.lo, ntail = r.hi - r.tail_begin;
-  if (t < nhead) return r.lo + t;
-  if (t - nhead < ntail) return r.tail_begin + (t - nhead);
-  return ~0ull;
-}
 
 // N = compile-time world size (2..8), 0 = run-time world (<= kMaxRanks)
 // ADAM: Adam update with the second history half (sync_device.cuh), false = SGD.
@@ -74,7 +51,7 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
   uint64_t* s_end = reinterpret_cast<uint64_t*>(smem_raw);
   float* s_lr = reinterpret_cast<float*>(s_end + p.nseg);
   float* s_dm = s_lr + p.nseg;
-  const bool seg_in_smem = p.nseg <= kPushMaxSeg;
+  const bool seg_in_smem = p.nseg <= kMaxSegSmem;
   if (seg_in_smem) {
     for (int k = threadIdx.x; k < p.nseg; k += blockDim.x) {
       s_end[k] = p.seg_end[k];
@@ -237,16 +214,10 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
         x[0].x = round_bf16(x[0].x); x[0].y = round_bf16(x[0].y);
         x[0].z = round_bf16(x[0].z); x[0].w = round_bf16(x[0].w);
       }
-      float4 acc = make_float4(__fmul_rn(inv, x[0].x), __fmul_rn(inv, x[0].y), __fmul_rn(inv, x[0].z),
-                               __fmul_rn(inv, x[0].w));
+      float4 acc = scale4(inv, x[0]);
       if (N > 0) {
 #pragma unroll
-        for (int k = 1; k < M; ++k) {
-          acc.x = __fadd_rn(__fmul_rn(inv, x[k].x), acc.x);
-          acc.y = __fadd_rn(__fmul_rn(inv, x[k].y), acc.y);
-          acc.z = __fadd_rn(__fmul_rn(inv, x[k].z), acc.z);
-          acc.w = __fadd_rn(__fmul_rn(inv, x[k].w), acc.w);
-        }
+        for (int k = 1; k < M; ++k) add_scaled(acc, inv, x[k]);
       } else {
         for (int k = 1; k < world; ++k) {
           int src = rank + k;
@@ -256,10 +227,7 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
             y = unpack_bf16x4(ld_stream_u2(static_cast<const uint16_t*>(p.recv[rank]) + src * slot + (i - base)));
           else
             y = ld_stream(static_cast<const float*>(p.recv[rank]) + src * slot + (i - base));
-          acc.x = __fadd_rn(__fmul_rn(inv, y.x), acc.x);
-          acc.y = __fadd_rn(__fmul_rn(inv, y.y), acc.y);
-          acc.z = __fadd_rn(__fmul_rn(inv, y.z), acc.z);
-          acc.w = __fadd_rn(__fmul_rn(inv, y.w), acc.w);
+          add_scaled(acc, inv, y);
         }
       }
       update_vec<ADAM, NORM>(p, cur, i, acc, w, h, v);
@@ -327,24 +295,10 @@ __global__ void __launch_bounds__(kPushThreads, 2) fused_sync_sgd_push_kernel(co
   if (tracer) p.trace[4] = globaltimer_ns();
 }
 
-template <int N, bool NORM>
-void launch_push_solver(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (p.solver == kSolverAdam) {
-    if (p.grad_bf16) fused_sync_sgd_push_kernel<N, true, true, NORM><<<grid, block, smem, stream>>>(p);
-    else fused_sync_sgd_push_kernel<N, false, true, NORM><<<grid, block, smem, stream>>>(p);
-  } else if (p.grad_bf16) {
-    fused_sync_sgd_push_kernel<N, true, false, NORM><<<grid, block, smem, stream>>>(p);
-  } else {
-    fused_sync_sgd_push_kernel<N, false, false, NORM><<<grid, block, smem, stream>>>(p);
-  }
-}
-
-template <int N>
-cudaError_t launch_push_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
-  if (sync_normalizes(p)) launch_push_solver<N, true>(p, grid, block, smem, stream);
-  else launch_push_solver<N, false>(p, grid, block, smem, stream);
-  return cudaGetLastError();
-}
+struct PushKernel {
+  template <int N, bool BF16, bool ADAM, bool NORM>
+  static constexpr auto kernel = fused_sync_sgd_push_kernel<N, BF16, ADAM, NORM>;
+};
 
 }  // namespace
 
@@ -355,7 +309,7 @@ uint64_t push_recv_stride(uint64_t count, int world) {
 
 cudaError_t launch_fused_sync_sgd_push(const SyncParams& p, int grid, int block, int vecs_per_thread,
                                        cudaStream_t stream) {
-  if (p.world < 2 || p.world > kMaxRanks || p.rank < 0 || p.rank >= p.world) return cudaErrorInvalidValue;
+  if (!valid_world(p, 2)) return cudaErrorInvalidValue;
   if (p.mode != kModeTwoShot || p.recv_stride == 0) return cudaErrorInvalidValue;
   if (block <= 0) block = kPushThreads;
   if (block > kPushThreads || block < kMaxRanks || (block & 31)) return cudaErrorInvalidValue;
@@ -372,17 +326,7 @@ cudaError_t launch_fused_sync_sgd_push(const SyncParams& p, int grid, int block,
     grid = static_cast<int>(need > static_cast<uint64_t>(cap) ? cap : need);
   }
   if (grid > kMaxCtas) grid = kMaxCtas;
-  const size_t smem = p.nseg <= kPushMaxSeg ? static_cast<size_t>(p.nseg) * (sizeof(uint64_t) + 2 * sizeof(float)) : 0;
-  switch (p.world) {
-    case 2: return launch_push_n<2>(p, grid, block, smem, stream);
-    case 3: return launch_push_n<3>(p, grid, block, smem, stream);
-    case 4: return launch_push_n<4>(p, grid, block, smem, stream);
-    case 5: return launch_push_n<5>(p, grid, block, smem, stream);
-    case 6: return launch_push_n<6>(p, grid, block, smem, stream);
-    case 7: return launch_push_n<7>(p, grid, block, smem, stream);
-    case 8: return launch_push_n<8>(p, grid, block, smem, stream);
-    default: return launch_push_n<0>(p, grid, block, smem, stream);
-  }
+  return launch_sync<PushKernel, true>(p, p.world, grid, block, seg_smem_bytes(p.nseg), stream);
 }
 
 }  // namespace cosb

@@ -449,7 +449,7 @@ cudaError_t launch_tma(const SyncParams& p, int grid, int tile, size_t smem, cud
 }  // namespace
 
 cudaError_t launch_fused_sync_sgd_tma(const SyncParams& p, int grid, cudaStream_t stream) {
-  if (p.world < 1 || p.world > kMaxRanks || p.rank < 0 || p.rank >= p.world) return cudaErrorInvalidValue;
+  if (!valid_world(p, 1)) return cudaErrorInvalidValue;
   if (p.mode == kModeAllGather || p.solver != kSolverSgd) return cudaErrorInvalidValue;  // SGD only
   int dev = 0;
   cudaGetDevice(&dev);
@@ -471,8 +471,7 @@ cudaError_t launch_fused_sync_sgd_tma(const SyncParams& p, int grid, cudaStream_
   if (p.zero_diff || p.grad_bf16) tiles = (p.count / (p.mode == kModeLocal ? 1 : p.world) + tile - 1) / tile;
   if (tiles < 1) tiles = 1;
   if (static_cast<uint64_t>(grid) > tiles) grid = static_cast<int>(tiles);
-  const int nseg_s = p.nseg <= kMaxSegSmemTma ? p.nseg : 0;
-  size_t smem = 128 + static_cast<size_t>(nseg_s) * 16;
+  size_t smem = 128 + seg_smem_bytes(p.nseg, kMaxSegSmemTma);
   smem = (smem + 127) & ~static_cast<size_t>(127);
   smem += static_cast<size_t>(kStages) * (per_elem * tile);
   smem += 128;

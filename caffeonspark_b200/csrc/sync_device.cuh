@@ -1,8 +1,11 @@
-// sync_device.cuh -- device-side building blocks shared by the two variants of
-// the fused sync kernel (fused_sync_sgd.cu: vector LDG/STG path,
-// fused_sync_sgd_tma.cu: cp.async.bulk pipeline): PTX wrappers, the per-CTA
-// cross-GPU barrier, the shard/vector partition, the blob (segment) cursor and
-// the SGD element update in the reference's operation order.
+// sync_device.cuh -- building blocks shared by the five variants of the fused
+// sync kernel (fused_sync_sgd.cu: vector LDG/STG, _tma.cu: cp.async.bulk
+// pipeline, _push.cu: stores only, _ll.cu: flag-in-data, _nvls.cu: in-switch
+// reduction): PTX wrappers, bf16 packing, the per-CTA cross-GPU barrier, the
+// shard/vector partition and its scalar edges, the reduce in the reference's
+// order, the blob (segment) cursor, the SGD and Adam element updates in the
+// reference's operation order, and the host-side dispatch of a launch to its
+// <N, BF16, ADAM, NORM> instantiation.
 #ifndef COS_SYNC_DEVICE_CUH_
 #define COS_SYNC_DEVICE_CUH_
 
@@ -65,6 +68,21 @@ __device__ __forceinline__ float bf16_bits_to_float(uint32_t bits16) { return __
 
 __device__ __forceinline__ uint16_t float_to_bf16_bits(float f) {
   return __bfloat16_as_ushort(__float2bfloat16_rn(f));
+}
+
+// the rounding the bf16 wire applies to a gradient element
+__device__ __forceinline__ float round_bf16(float x) { return bf16_bits_to_float(float_to_bf16_bits(x)); }
+
+__device__ __forceinline__ uint2 pack_bf16x4(const float4& v) {
+  uint2 o;
+  o.x = static_cast<uint32_t>(float_to_bf16_bits(v.x)) | (static_cast<uint32_t>(float_to_bf16_bits(v.y)) << 16);
+  o.y = static_cast<uint32_t>(float_to_bf16_bits(v.z)) | (static_cast<uint32_t>(float_to_bf16_bits(v.w)) << 16);
+  return o;
+}
+
+__device__ __forceinline__ float4 unpack_bf16x4(const uint2& u) {
+  return make_float4(bf16_bits_to_float(u.x & 0xffffu), bf16_bits_to_float(u.x >> 16),
+                     bf16_bits_to_float(u.y & 0xffffu), bf16_bits_to_float(u.y >> 16));
 }
 
 // ------------------------------------------------------ cross-GPU barrier
@@ -184,6 +202,53 @@ __device__ __forceinline__ ShardRange shard_range(uint64_t count, int world, int
   return r;
 }
 
+// f(i) for the scalar head / tail element i of range r (ShardRange or the TMA kernel's BodyRange) that thread t of
+// CTA 0 handles, if there is one
+template <class Range, class F>
+__device__ __forceinline__ void for_edge_element(const Range& r, unsigned t, F f) {
+  const uint64_t nhead = r.head_end - r.lo, ntail = r.hi - r.tail_begin;
+  if (t < nhead) f(r.lo + t);
+  else if (t - nhead < ntail) f(r.tail_begin + (t - nhead));
+}
+
+// the same element as an index, ~0 when thread t has none
+template <class Range>
+__device__ __forceinline__ uint64_t edge_element(const Range& r, unsigned t) {
+  uint64_t i = ~0ull;
+  for_edge_element(r, t, [&](uint64_t e) { i = e; });
+  return i;
+}
+
+// ------------------------------------------------------------- reduce
+
+// One term of the reduce, with the 1/N scale applied BEFORE the sum (parallel_cpu.cpp:120-122 runs before
+// socket_sync_cpu.cpp:112-132): the first term is scale4(inv, x), each further one add_scaled(acc, inv, x).
+__device__ __forceinline__ float4 scale4(float inv, const float4& x) {
+  return make_float4(__fmul_rn(inv, x.x), __fmul_rn(inv, x.y), __fmul_rn(inv, x.z), __fmul_rn(inv, x.w));
+}
+
+__device__ __forceinline__ void add_scaled(float4& acc, float inv, const float4& x) {
+  acc.x = __fadd_rn(__fmul_rn(inv, x.x), acc.x);
+  acc.y = __fadd_rn(__fmul_rn(inv, x.y), acc.y);
+  acc.z = __fadd_rn(__fmul_rn(inv, x.z), acc.z);
+  acc.w = __fadd_rn(__fmul_rn(inv, x.w), acc.w);
+}
+
+// Element i of shard s summed over the world's diff_ (or bf16 wire buffers) in the reference's order s, s+1, ...
+// (mod N), each term scaled by 1/N first.
+template <bool BF16>
+__device__ __forceinline__ float reduce_scalar(const SyncParams& p, int s, uint64_t i) {
+  float acc = 0.f;
+  for (int j = 0; j < p.world; ++j) {
+    int src = s + j;
+    if (src >= p.world) src -= p.world;
+    float x = BF16 ? bf16_bits_to_float(p.wire[src][i]) : p.diff[src][i];
+    x = __fmul_rn(p.inv_scale, x);
+    acc = (j == 0) ? x : __fadd_rn(x, acc);
+  }
+  return acc;
+}
+
 // ----------------------------------------------------------- SGD element
 
 struct SegCursor {
@@ -204,6 +269,15 @@ struct SegCursor {
     while (k < nseg - 1 && i >= end[k]) ++k;
   }
 };
+
+// Segments a kernel copies into dynamic shared memory at most (ends, then lr_mult, then decay_mult); with more the
+// cursor reads the global table.  The TMA kernel has its own, smaller limit.
+constexpr int kMaxSegSmem = 1024;
+
+// dynamic shared memory the segment table takes when at most max_smem segments are copied
+inline size_t seg_smem_bytes(int nseg, int max_smem = kMaxSegSmem) {
+  return nseg <= max_smem ? static_cast<size_t>(nseg) * (sizeof(uint64_t) + 2 * sizeof(float)) : 0;
+}
 
 // Regularize + ComputeUpdateValue + Blob::Update for one element, in the
 // reference's operation order with one rounding per operation:
@@ -366,10 +440,7 @@ __device__ __forceinline__ void store_v(const SyncParams& p, uint64_t i, const f
 // reduced gradient, before Regularize, for SGD and Adam alike.  One rounding: g = accum_norm * g.  The kernels are
 // templates on NORM (false = no Normalize, the default); NORM is applied to the reduced gradient right before the
 // element update, so it only adds one FMUL per element.
-__device__ __forceinline__ float4 normalize_vec(const SyncParams& p, const float4& g) {
-  const float a = p.accum_norm;
-  return make_float4(__fmul_rn(a, g.x), __fmul_rn(a, g.y), __fmul_rn(a, g.z), __fmul_rn(a, g.w));
-}
+__device__ __forceinline__ float4 normalize_vec(const SyncParams& p, const float4& g) { return scale4(p.accum_norm, g); }
 
 template <bool ADAM, bool NORM = false>
 __device__ __forceinline__ void update_vec(const SyncParams& p, SegCursor& c, uint64_t i, const float4& g, float4& w,
@@ -394,6 +465,51 @@ __device__ __forceinline__ void update_element(const SyncParams& p, const SegCur
   }
 }
 
+// ------------------------------------------------------------ host: launch
+
+// world size and rank a launcher accepts (its kernel needs at least min_world ranks)
+inline bool valid_world(const SyncParams& p, int min_world) {
+  return p.world >= min_world && p.world <= kMaxRanks && p.rank >= 0 && p.rank < p.world;
+}
+
+// Launches the <N, BF16, ADAM, NORM> instantiation of a kernel family that SyncParams selects: BF16 = grad_bf16,
+// ADAM = (solver == kSolverAdam), NORM = sync_normalizes(p).  K::kernel<N, BF16, ADAM, NORM> names the family's
+// kernel.  N = n for n = 2..8; any other n launches the run-time-world instantiation N = 0 when GENERIC, else is
+// refused.
+template <class K, int N, bool NORM>
+void launch_solver(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
+  if (p.solver == kSolverAdam) {
+    if (p.grad_bf16) K::template kernel<N, true, true, NORM><<<grid, block, smem, stream>>>(p);
+    else K::template kernel<N, false, true, NORM><<<grid, block, smem, stream>>>(p);
+  } else if (p.grad_bf16) {
+    K::template kernel<N, true, false, NORM><<<grid, block, smem, stream>>>(p);
+  } else {
+    K::template kernel<N, false, false, NORM><<<grid, block, smem, stream>>>(p);
+  }
+}
+
+template <class K, int N>
+cudaError_t launch_n(const SyncParams& p, int grid, int block, size_t smem, cudaStream_t stream) {
+  if (sync_normalizes(p)) launch_solver<K, N, true>(p, grid, block, smem, stream);
+  else launch_solver<K, N, false>(p, grid, block, smem, stream);
+  return cudaGetLastError();
+}
+
+template <class K, bool GENERIC>
+cudaError_t launch_sync(const SyncParams& p, int n, int grid, int block, size_t smem, cudaStream_t stream) {
+  switch (n) {
+    case 2: return launch_n<K, 2>(p, grid, block, smem, stream);
+    case 3: return launch_n<K, 3>(p, grid, block, smem, stream);
+    case 4: return launch_n<K, 4>(p, grid, block, smem, stream);
+    case 5: return launch_n<K, 5>(p, grid, block, smem, stream);
+    case 6: return launch_n<K, 6>(p, grid, block, smem, stream);
+    case 7: return launch_n<K, 7>(p, grid, block, smem, stream);
+    case 8: return launch_n<K, 8>(p, grid, block, smem, stream);
+    default:
+      if constexpr (GENERIC) return launch_n<K, 0>(p, grid, block, smem, stream);
+      else return cudaErrorInvalidValue;
+  }
+}
 
 }  // namespace
 }  // namespace cosb
