@@ -1,7 +1,7 @@
 """Forward/backward time of the built-in producer against the PyTorch fp32 producer (DESIGN.md section 14).
 
-Workloads: the three nets the engine runs, at their reference batch sizes (LeNet b64, CIFAR-10-quick b100,
-cifar10_full_bn b100).  For each, one process times the native engine, the PyTorch module with TF32 off and with
+Workloads: the four nets the engine runs, at their reference batch sizes (LeNet b64, CIFAR-10-quick b100,
+cifar10_full_bn b100, cifar10_full b100).  For each, one process times the native engine, the PyTorch module with TF32 off and with
 TF32 on (cuDNN's default, here applied to matmuls too), alternating the three in every round; each sample is CUDA events around `--iters`
 back-to-back forward/backward calls on one stream after `--warmup` untimed ones.  Prints one JSON line per
 workload with median / min / max ms per call and images/s, and the card's name and power limit.
@@ -22,7 +22,7 @@ import tempfile
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn")
+WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full")
 FP32_PEAK = 67e12  # H100 SXM data sheet, dense FP32, at up to 700 W
 
 

@@ -101,6 +101,10 @@ SYMBOLS = [
     ("cos_bias_relu_maxpool_backward", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     ("cos_lrn_forward_bf16", _i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp]),
     ("cos_lrn_backward_bf16", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp]),
+    ("cos_lrn_within_forward", _i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    ("cos_lrn_within_backward", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    ("cos_lrn_within_forward_bf16", _i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    ("cos_lrn_within_backward_bf16", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
     ("cos_bias_relu_maxpool_forward_bf16", _i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     ("cos_bias_relu_maxpool_backward_bf16", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     ("cos_batch_norm_forward", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),

@@ -4,6 +4,8 @@
 //  * cross-channel LRN, forward and backward.  The scale s is never stored: the backward recomputes it from x.
 //    One thread walks CH consecutive channels of one pixel with the window (and the backward's second window)
 //    in registers; pixels are the fast thread index, so every load and store is coalesced along w.
+//  * within-channel LRN (cifar10_full), forward and backward: a 2-D stencil over each plane from a shared-memory
+//    tile with a halo; the backward recomputes s as well.
 //  * conv bias + ReLU + MAX pool, forward and backward.  The forward adds the bias to the bias-free conv
 //    output, takes the first maximum of each window and stores a 1-byte window position (kPoolNoGrad when the
 //    maximum is <= 0).  The backward gathers dy per conv-output element in PyTorch's max_pool_backward_nchw
@@ -172,6 +174,156 @@ struct LrnBwd {
   }
 };
 
+// ---------------------------------------------------------------- within-channel LRN
+//
+// One block per kLrwTileH x kLrwTileW tile of one (n, c) plane, one output per thread.  The block stages x over the
+// tile plus a halo (HALF = n/2 for the forward, 2*HALF for the backward: s is needed on the tile plus HALF) in shared
+// memory, zero outside the plane, so every global load is a row segment (coalesced along w) and the window sums are
+// separable: each window row's n terms are added from 0.f in increasing w, then the n row sums from 0.f in increasing
+// h.  A zero cell adds +0.f to a sum of squares, which leaves it unchanged, so this equals the clipped window's sum.
+constexpr int kLrwTileW = 32, kLrwTileH = 8, kLrwThreads = kLrwTileW * kLrwTileH;
+
+__device__ __forceinline__ float sq(float v) { return __fmul_rn(v, v); }  // never contracted into an FMA
+
+// s = 1 + alpha * S / n^2 (Caffe's AVE pool divisor counts the pad cells: always n^2 here)
+__device__ __forceinline__ float lrw_scale(float S, float nn, float alpha) { return fmaf(alpha, S / nn, 1.f); }
+
+template <typename T, int HALF>
+__global__ void __launch_bounds__(kLrwThreads) lrn_within_forward_kernel(const T* __restrict__ x, T* __restrict__ y,
+                                                                         int H, int W, int tiles_w, int tiles,
+                                                                         float nn, float alpha, float beta) {
+  constexpr int N = 2 * HALF + 1, RH = kLrwTileH + 2 * HALF, RW = kLrwTileW + 2 * HALF;
+  __shared__ float xs[RH][RW];        // x on the tile + HALF
+  __shared__ float hs[RH][kLrwTileW];  // window-row sums of x^2
+  const unsigned plane = blockIdx.x / tiles;
+  const int t = blockIdx.x - plane * tiles;
+  const int h0 = (t / tiles_w) * kLrwTileH, w0 = (t % tiles_w) * kLrwTileW;
+  const size_t base = (size_t)plane * H * W;
+  const int tid = threadIdx.y * kLrwTileW + threadIdx.x;
+  for (int i = tid; i < RH * RW; i += kLrwThreads) {
+    const int r = i / RW, c = i - r * RW, h = h0 - HALF + r, w = w0 - HALF + c;
+    xs[r][c] = (h >= 0 && h < H && w >= 0 && w < W) ? to_f32(x[base + (size_t)h * W + w]) : 0.f;
+  }
+  __syncthreads();
+  for (int i = tid; i < RH * kLrwTileW; i += kLrwThreads) {
+    const int r = i / kLrwTileW, c = i - r * kLrwTileW;
+    float a = 0.f;
+#pragma unroll
+    for (int b = 0; b < N; ++b) a += sq(xs[r][c + b]);
+    hs[r][c] = a;
+  }
+  __syncthreads();
+  const int ty = threadIdx.y, tx = threadIdx.x, h = h0 + ty, w = w0 + tx;
+  if (h >= H || w >= W) return;
+  float S = 0.f;
+#pragma unroll
+  for (int a = 0; a < N; ++a) S += hs[ty + a][tx];
+  y[base + (size_t)h * W + w] = from_f32<T>(xs[ty + HALF][tx + HALF] * powf(lrw_scale(S, nn, alpha), -beta));
+}
+
+// dx_i = dy_i s_i^-beta - (2 alpha beta / n^2) x_i sum_{j in window(i)} r_j,  r_j = dy_j x_j s_j^-beta / s_j
+template <typename T, int HALF>
+__global__ void __launch_bounds__(kLrwThreads) lrn_within_backward_kernel(const T* __restrict__ x,
+                                                                          const T* __restrict__ dy,
+                                                                          T* __restrict__ dx, int H, int W,
+                                                                          int tiles_w, int tiles, float nn,
+                                                                          float alpha, float beta, float coef) {
+  constexpr int N = 2 * HALF + 1;
+  constexpr int XH = kLrwTileH + 4 * HALF, XW = kLrwTileW + 4 * HALF;  // x: the tile + 2*HALF
+  constexpr int MH = kLrwTileH + 2 * HALF, MW = kLrwTileW + 2 * HALF;  // r: the tile + HALF
+  __shared__ float xs[XH][XW];
+  __shared__ float hs[XH][MW];  // window-row sums of x^2 over r's columns
+  __shared__ float rs[MH][MW];  // r, 0 outside the plane
+  __shared__ float hr[MH][kLrwTileW];  // window-row sums of r
+  __shared__ float dyc[kLrwTileH][kLrwTileW], sbc[kLrwTileH][kLrwTileW];  // dy and s^-beta on the tile
+  const unsigned plane = blockIdx.x / tiles;
+  const int t = blockIdx.x - plane * tiles;
+  const int h0 = (t / tiles_w) * kLrwTileH, w0 = (t % tiles_w) * kLrwTileW;
+  const size_t base = (size_t)plane * H * W;
+  const int tid = threadIdx.y * kLrwTileW + threadIdx.x;
+  for (int i = tid; i < XH * XW; i += kLrwThreads) {
+    const int r = i / XW, c = i - r * XW, h = h0 - 2 * HALF + r, w = w0 - 2 * HALF + c;
+    xs[r][c] = (h >= 0 && h < H && w >= 0 && w < W) ? to_f32(x[base + (size_t)h * W + w]) : 0.f;
+  }
+  __syncthreads();
+  for (int i = tid; i < XH * MW; i += kLrwThreads) {
+    const int r = i / MW, c = i - r * MW;
+    float a = 0.f;
+#pragma unroll
+    for (int b = 0; b < N; ++b) a += sq(xs[r][c + b]);
+    hs[r][c] = a;
+  }
+  __syncthreads();
+  for (int i = tid; i < MH * MW; i += kLrwThreads) {
+    const int r = i / MW, c = i - r * MW, h = h0 - HALF + r, w = w0 - HALF + c;
+    float rv = 0.f;
+    if (h >= 0 && h < H && w >= 0 && w < W) {
+      float S = 0.f;
+#pragma unroll
+      for (int a = 0; a < N; ++a) S += hs[r + a][c];
+      const float s = lrw_scale(S, nn, alpha), sb = powf(s, -beta);
+      const float d = to_f32(dy[base + (size_t)h * W + w]);
+      rv = d * xs[r + HALF][c + HALF] * sb / s;
+      const int cr = r - HALF, cc = c - HALF;
+      if (cr >= 0 && cr < kLrwTileH && cc >= 0 && cc < kLrwTileW) {
+        dyc[cr][cc] = d;
+        sbc[cr][cc] = sb;
+      }
+    }
+    rs[r][c] = rv;
+  }
+  __syncthreads();
+  for (int i = tid; i < MH * kLrwTileW; i += kLrwThreads) {
+    const int r = i / kLrwTileW, c = i - r * kLrwTileW;
+    float a = 0.f;
+#pragma unroll
+    for (int b = 0; b < N; ++b) a += rs[r][c + b];
+    hr[r][c] = a;
+  }
+  __syncthreads();
+  const int ty = threadIdx.y, tx = threadIdx.x, h = h0 + ty, w = w0 + tx;
+  if (h >= H || w >= W) return;
+  float acc = 0.f;
+#pragma unroll
+  for (int a = 0; a < N; ++a) acc += hr[ty + a][tx];
+  const float xv = xs[ty + 2 * HALF][tx + 2 * HALF];
+  dx[base + (size_t)h * W + w] = from_f32<T>(fmaf(-(coef * xv), acc, dyc[ty][tx] * sbc[ty][tx]));
+}
+
+struct LrwGrid {
+  int tiles_w, tiles;
+  long long blocks;
+  LrwGrid(int num, int channels, int height, int width)
+      : tiles_w((width + kLrwTileW - 1) / kLrwTileW), tiles(tiles_w * ((height + kLrwTileH - 1) / kLrwTileH)),
+        blocks((long long)num * channels * tiles) {}
+  // plane offsets are size_t; in-plane offsets and the block count must fit the kernels' 32-bit arithmetic
+  static bool fits(long long blocks, int height, int width) {
+    return blocks < (1ll << 31) && (long long)height * width < (1ll << 31);
+  }
+};
+
+template <int HALF>
+struct LrwFwd {
+  template <typename T>
+  static cudaError_t run(const T* x, T* y, int H, int W, const LrwGrid& g, float nn, float alpha, float beta,
+                         cudaStream_t st) {
+    lrn_within_forward_kernel<T, HALF><<<(unsigned)g.blocks, dim3(kLrwTileW, kLrwTileH), 0, st>>>(
+        x, y, H, W, g.tiles_w, g.tiles, nn, alpha, beta);
+    return cudaGetLastError();
+  }
+};
+
+template <int HALF>
+struct LrwBwd {
+  template <typename T>
+  static cudaError_t run(const T* x, const T* dy, T* dx, int H, int W, const LrwGrid& g, float nn, float alpha,
+                         float beta, float coef, cudaStream_t st) {
+    lrn_within_backward_kernel<T, HALF><<<(unsigned)g.blocks, dim3(kLrwTileW, kLrwTileH), 0, st>>>(
+        x, dy, dx, H, W, g.tiles_w, g.tiles, nn, alpha, beta, coef);
+    return cudaGetLastError();
+  }
+};
+
 // ---------------------------------------------------------------- bias + ReLU + MAX pool
 
 // KERNEL/STRIDE > 0: compile-time pooling geometry (CaffeNet and CIFAR-10-quick: 3/2); 0: the runtime values
@@ -301,6 +453,27 @@ cudaError_t lrn_backward_t(const T* x, const T* dy, T* dx, int num, int channels
 }
 
 template <typename T>
+cudaError_t lrn_within_forward_t(const T* x, T* y, int num, int channels, int height, int width, int local_size,
+                                 float alpha, float beta, cudaStream_t stream) {
+  const LrwGrid g(num, channels, height, width);
+  if (g.blocks == 0) return cudaSuccess;
+  if (!LrwGrid::fits(g.blocks, height, width)) return cudaErrorInvalidValue;
+  return lrn_dispatch<LrwFwd>(local_size / 2, x, y, height, width, g, (float)(local_size * local_size), alpha, beta,
+                              stream);
+}
+
+template <typename T>
+cudaError_t lrn_within_backward_t(const T* x, const T* dy, T* dx, int num, int channels, int height, int width,
+                                  int local_size, float alpha, float beta, cudaStream_t stream) {
+  const LrwGrid g(num, channels, height, width);
+  if (g.blocks == 0) return cudaSuccess;
+  if (!LrwGrid::fits(g.blocks, height, width)) return cudaErrorInvalidValue;
+  const float nn = (float)(local_size * local_size);
+  return lrn_dispatch<LrwBwd>(local_size / 2, x, dy, dx, height, width, g, nn, alpha, beta,
+                              2.f * alpha * beta / nn, stream);
+}
+
+template <typename T>
 cudaError_t pool_forward_t(const T* x, const float* bias, T* y, uint8_t* index, int num, int channels, int height,
                            int width, int kernel, int stride, int pooled_h, int pooled_w, cudaStream_t stream) {
   const long long total = (long long)num * channels * pooled_h * pooled_w;
@@ -364,6 +537,25 @@ cudaError_t lrn_backward(const __nv_bfloat16* x, const __nv_bfloat16* dy, __nv_b
                          int height, int width, int local_size, float alpha, float beta, float k,
                          cudaStream_t stream) {
   return lrn_backward_t(x, dy, dx, num, channels, height, width, local_size, alpha, beta, k, stream);
+}
+
+cudaError_t lrn_within_forward(const float* x, float* y, int num, int channels, int height, int width, int local_size,
+                               float alpha, float beta, cudaStream_t stream) {
+  return lrn_within_forward_t(x, y, num, channels, height, width, local_size, alpha, beta, stream);
+}
+cudaError_t lrn_within_forward(const __nv_bfloat16* x, __nv_bfloat16* y, int num, int channels, int height, int width,
+                               int local_size, float alpha, float beta, cudaStream_t stream) {
+  return lrn_within_forward_t(x, y, num, channels, height, width, local_size, alpha, beta, stream);
+}
+
+cudaError_t lrn_within_backward(const float* x, const float* dy, float* dx, int num, int channels, int height,
+                                int width, int local_size, float alpha, float beta, cudaStream_t stream) {
+  return lrn_within_backward_t(x, dy, dx, num, channels, height, width, local_size, alpha, beta, stream);
+}
+cudaError_t lrn_within_backward(const __nv_bfloat16* x, const __nv_bfloat16* dy, __nv_bfloat16* dx, int num,
+                                int channels, int height, int width, int local_size, float alpha, float beta,
+                                cudaStream_t stream) {
+  return lrn_within_backward_t(x, dy, dx, num, channels, height, width, local_size, alpha, beta, stream);
 }
 
 int pooled_size(int in, int kernel, int stride) {

@@ -25,6 +25,19 @@ cudaError_t lrn_backward(const __nv_bfloat16* x, const __nv_bfloat16* dy, __nv_b
                          int height, int width, int local_size, float alpha, float beta, float k,
                          cudaStream_t stream);
 
+// LRN within the channel (Caffe's WITHIN_CHANNEL), local_size odd and <= kLrnMaxLocalSize:
+// s = 1 + alpha/local_size^2 * sum of x^2 over the local_size x local_size window centred on the pixel, clipped to the
+// plane; y = x * s^-beta.  Caffe ignores k for this region, so there is none.  Not in place (x != y, dx != x, dy).
+cudaError_t lrn_within_forward(const float* x, float* y, int num, int channels, int height, int width, int local_size,
+                               float alpha, float beta, cudaStream_t stream);
+cudaError_t lrn_within_backward(const float* x, const float* dy, float* dx, int num, int channels, int height,
+                                int width, int local_size, float alpha, float beta, cudaStream_t stream);
+cudaError_t lrn_within_forward(const __nv_bfloat16* x, __nv_bfloat16* y, int num, int channels, int height, int width,
+                               int local_size, float alpha, float beta, cudaStream_t stream);
+cudaError_t lrn_within_backward(const __nv_bfloat16* x, const __nv_bfloat16* dy, __nv_bfloat16* dx, int num,
+                                int channels, int height, int width, int local_size, float alpha, float beta,
+                                cudaStream_t stream);
+
 // Window clipping of ceil-mode pooling with pad 0: the pooled size, or -1 when the shape is invalid.
 int pooled_size(int in, int kernel, int stride);
 

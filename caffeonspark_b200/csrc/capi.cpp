@@ -465,6 +465,20 @@ const char* lrn_args(const void* a, const void* b, const void* c, int num, int c
   if (!(k > 0.f) || !std::isfinite(beta)) return "LRN needs k > 0 and a finite beta";
   return nullptr;
 }
+// the within-channel kernels read a halo around every output, so no output may overlap an input (dy: NULL for the
+// forward, which has none)
+const char* lrn_within_args(const void* x, const void* dy, const void* out, size_t elem, int num, int channels,
+                            int height, int width, int local_size, float beta, bool backward) {
+  if (backward && !dy) return "NULL tensor";
+  if (const char* e = lrn_args(x, out, out, num, channels, height, width, local_size, beta, 1.f)) return e;
+  const size_t bytes = static_cast<size_t>(num) * channels * height * width * elem;
+  auto overlap = [&](const void* a) {
+    const char *p = static_cast<const char*>(a), *q = static_cast<const char*>(out);
+    return bytes > 0 && p < q + bytes && q < p + bytes;
+  };
+  if (overlap(x) || (backward && overlap(dy))) return "within-channel LRN cannot run in place";
+  return nullptr;
+}
 const char* pool_args(const void* a, const void* b, const void* c, int num, int channels, int height, int width,
                       int kernel, int stride, int pooled_height, int pooled_width) {
   if (!a || !b || !c) return "NULL tensor";
@@ -491,6 +505,25 @@ int cos_lrn_backward(const float* x, const float* dy, float* dx, int num, int ch
   return launched(cosb::lrn_backward(x, dy, dx, num, channels, height, width, local_size, alpha, beta, k,
                                      static_cast<cudaStream_t>(cuda_stream)),
                   "cos_lrn_backward");
+}
+
+int cos_lrn_within_forward(const float* x, float* y, int num, int channels, int height, int width, int local_size,
+                           float alpha, float beta, void* cuda_stream) {
+  if (const char* e = lrn_within_args(x, nullptr, y, sizeof(float), num, channels, height, width, local_size, beta,
+                                      false))
+    return fail(e);
+  return launched(cosb::lrn_within_forward(x, y, num, channels, height, width, local_size, alpha, beta,
+                                           static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_lrn_within_forward");
+}
+
+int cos_lrn_within_backward(const float* x, const float* dy, float* dx, int num, int channels, int height, int width,
+                            int local_size, float alpha, float beta, void* cuda_stream) {
+  if (const char* e = lrn_within_args(x, dy, dx, sizeof(float), num, channels, height, width, local_size, beta, true))
+    return fail(e);
+  return launched(cosb::lrn_within_backward(x, dy, dx, num, channels, height, width, local_size, alpha, beta,
+                                            static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_lrn_within_backward");
 }
 
 int cos_bias_relu_maxpool_forward(const float* x, const float* bias, float* y, uint8_t* index, int num, int channels,
@@ -538,6 +571,26 @@ int cos_lrn_backward_bf16(const uint16_t* x, const uint16_t* dy, uint16_t* dx, i
   return launched(cosb::lrn_backward(bf16_in(x), bf16_in(dy), bf16_out(dx), num, channels, height, width, local_size, alpha,
                                      beta, k, static_cast<cudaStream_t>(cuda_stream)),
                   "cos_lrn_backward_bf16");
+}
+
+int cos_lrn_within_forward_bf16(const uint16_t* x, uint16_t* y, int num, int channels, int height, int width,
+                                int local_size, float alpha, float beta, void* cuda_stream) {
+  if (const char* e = lrn_within_args(x, nullptr, y, sizeof(uint16_t), num, channels, height, width, local_size, beta,
+                                      false))
+    return fail(e);
+  return launched(cosb::lrn_within_forward(bf16_in(x), bf16_out(y), num, channels, height, width, local_size, alpha,
+                                           beta, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_lrn_within_forward_bf16");
+}
+
+int cos_lrn_within_backward_bf16(const uint16_t* x, const uint16_t* dy, uint16_t* dx, int num, int channels,
+                                 int height, int width, int local_size, float alpha, float beta, void* cuda_stream) {
+  if (const char* e = lrn_within_args(x, dy, dx, sizeof(uint16_t), num, channels, height, width, local_size, beta,
+                                      true))
+    return fail(e);
+  return launched(cosb::lrn_within_backward(bf16_in(x), bf16_in(dy), bf16_out(dx), num, channels, height, width,
+                                            local_size, alpha, beta, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_lrn_within_backward_bf16");
 }
 
 int cos_bias_relu_maxpool_forward_bf16(const uint16_t* x, const float* bias, uint16_t* y, uint8_t* index, int num,

@@ -1,8 +1,11 @@
 // native_producer.cpp -- the built-in producer's net plan (host only); see native_producer.hpp.
 #include "native_producer.hpp"
 
+#include <cmath>
 #include <map>
 #include <sstream>
+
+#include "caffe_layers.hpp"
 
 namespace cosb {
 namespace {
@@ -88,7 +91,8 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       return false;
     }
     const bool known = L.type == "Convolution" || L.type == "Pooling" || L.type == "InnerProduct" || L.type == "ReLU" ||
-                       L.type == "Sigmoid" || L.type == "BatchNorm" || L.type == "SoftmaxWithLoss";
+                       L.type == "Sigmoid" || L.type == "BatchNorm" || L.type == "SoftmaxWithLoss" ||
+                       (L.type == "LRN" && L.norm_region == "WITHIN_CHANNEL");  // ACROSS_CHANNELS has no engine op
     if (!known) {
       *err = why(L, "layer type not supported");
       return false;
@@ -213,6 +217,20 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.global_stats = L.use_global_stats;
       op.fraction = L.moving_average_fraction;
       op.eps = L.eps;
+    } else if (L.type == "LRN") {
+      if (L.local_size < 1 || L.local_size % 2 == 0 || L.local_size > kLrnMaxLocalSize) {
+        *err = why(L, "local_size " + std::to_string(L.local_size) + " is not odd and <= " +
+                          std::to_string(kLrnMaxLocalSize));
+        return false;
+      }
+      if (op.in_shape.size() != 4 || !std::isfinite(L.lrn_beta)) {
+        *err = why(L, "needs a 4-axis bottom and a finite beta");
+        return false;
+      }
+      op.kind = OpKind::kLRNWithin;  // separate top storage even when top == bottom: the kernels read a halo
+      op.lrn_size = static_cast<int>(L.local_size);
+      op.lrn_alpha = L.lrn_alpha;
+      op.lrn_beta = L.lrn_beta;
     } else {  // SoftmaxWithLoss
       if (++losses > 1) {
         *err = why(L, "a second loss layer is not supported");
@@ -258,7 +276,8 @@ bool plan_from_prototxt(const std::string& path, SolverSpec* spec, Plan* plan, s
 
 std::string Plan::text() const {
   static const char* kinds[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling", "InnerProduct",
-                                "ReLU",        "Sigmoid",             "BatchNorm", "SoftmaxWithLoss"};
+                                "ReLU",        "Sigmoid",             "BatchNorm", "SoftmaxWithLoss",
+                                "LRN(WITHIN_CHANNEL)"};
   std::ostringstream os;
   for (int i = 0; i < ninputs; ++i) os << "input " << i << " " << input_names[i] << " " << tensor_count[i] << "\n";
   for (size_t i = 0; i < ops.size(); ++i) {
@@ -270,6 +289,7 @@ std::string Plan::text() const {
       os << " k" << op.kh << "x" << op.kw << " s" << op.sh << "x" << op.sw << " p" << op.ph << "x" << op.pw;
     if (op.kind == OpKind::kConvBiasReluMaxPool) os << " pool" << op.pool_kernel << "/" << op.pool_stride;
     if (op.kind == OpKind::kReLU && op.slope != 0.f) os << " slope=" << op.slope;
+    if (op.kind == OpKind::kLRNWithin) os << " n=" << op.lrn_size << " alpha=" << op.lrn_alpha << " beta=" << op.lrn_beta;
     if (op.w_off >= 0 && op.kind != OpKind::kBatchNorm) os << " w=" << op.w_off << ":" << op.w_count;
     if (op.b_off >= 0) os << " b=" << op.b_off << ":" << op.b_count;
     if (op.kind == OpKind::kBatchNorm) os << " stats=" << op.w_off;

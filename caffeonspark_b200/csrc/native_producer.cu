@@ -660,6 +660,10 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, cudaStream_t 
       return batch_norm_forward(x, y, m, m + c, m + 2 * c, static_cast<float*>(op_aux_[i]), workspace_, bn, c, hw, 1,
                                 op.global_stats, op.fraction, op.eps, s);
     }
+    case OpKind::kLRNWithin:
+      return lrn_within_forward(x, y, static_cast<int>(op.in_shape[0]), static_cast<int>(op.in_shape[1]),
+                                static_cast<int>(op.in_shape[2]), static_cast<int>(op.in_shape[3]), op.lrn_size,
+                                op.lrn_alpha, op.lrn_beta, s);
     default:
       return cudaSuccess;
   }
@@ -718,6 +722,11 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
       return batch_norm_backward(x, dy, dx, static_cast<const float*>(op_aux_[i]), workspace_, bn, c, hw, 1,
                                  op.global_stats, op.eps, s);
     }
+    case OpKind::kLRNWithin:
+      if (!dx) return cudaSuccess;
+      return lrn_within_backward(x, dy, dx, static_cast<int>(op.in_shape[0]), static_cast<int>(op.in_shape[1]),
+                                 static_cast<int>(op.in_shape[2]), static_cast<int>(op.in_shape[3]), op.lrn_size,
+                                 op.lrn_alpha, op.lrn_beta, s);
     default:  // SoftmaxWithLoss wrote its bottom gradient in the forward pass
       return cudaSuccess;
   }

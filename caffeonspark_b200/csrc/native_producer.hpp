@@ -1,5 +1,5 @@
 // native_producer.hpp -- the built-in gradient producer (Net::ForwardBackward for the TRAIN phase of the LeNet,
-// CIFAR-10-quick and CIFAR-10-full-BN family of nets; DESIGN.md section 14).
+// CIFAR-10-quick, CIFAR-10-full and CIFAR-10-full-BN family of nets; DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -19,7 +19,9 @@
 
 namespace cosb {
 
-enum class OpKind { kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss };
+enum class OpKind {
+  kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin
+};
 
 struct Op {
   OpKind kind;
@@ -38,6 +40,8 @@ struct Op {
   float loss_weight = 1.f;             // SoftmaxWithLoss
   bool global_stats = false;           // BatchNorm
   float fraction = 0.999f, eps = 1e-5f;
+  int lrn_size = 0;                    // LRN (WITHIN_CHANNEL only)
+  float lrn_alpha = 1.f, lrn_beta = 0.75f;
 };
 
 struct Plan {

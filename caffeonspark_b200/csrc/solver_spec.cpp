@@ -478,6 +478,15 @@ bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, s
       if (!bottom_shape(0, &in)) return false;
       for (const std::string& t : tops) blobs[t] = in;
       if (const Node* p = L->first("relu_param")) rec.negative_slope = static_cast<float>(p->num("negative_slope", 0.0));
+      if (const Node* p = L->first("lrn_param")) {  // caffe.proto LRNParameter
+        rec.local_size = p->integer("local_size", 5);
+        rec.lrn_alpha = static_cast<float>(p->num("alpha", 1.0));
+        rec.lrn_beta = static_cast<float>(p->num("beta", 0.75));
+        rec.lrn_k = static_cast<float>(p->num("k", 1.0));
+        rec.norm_region = p->str("norm_region", "ACROSS_CHANNELS");
+        if (rec.norm_region == "0") rec.norm_region = "ACROSS_CHANNELS";  // the enum's numeric form
+        if (rec.norm_region == "1") rec.norm_region = "WITHIN_CHANNEL";
+      }
     } else if (type == "Flatten") {
       Shape in;
       if (!bottom_shape(0, &in) || in.empty()) return false;

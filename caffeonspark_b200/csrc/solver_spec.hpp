@@ -40,6 +40,10 @@ struct NetLayer {
   float moving_average_fraction = 0.999f, eps = 1e-5f;
   float loss_weight = 1.f;
   bool has_loss_param = false;
+  // LRN (caffe.proto LRNParameter defaults); norm_region is "ACROSS_CHANNELS" or "WITHIN_CHANNEL"
+  int64_t local_size = 5;
+  float lrn_alpha = 1.f, lrn_beta = 0.75f, lrn_k = 1.f;
+  std::string norm_region = "ACROSS_CHANNELS";
   FillerSpec weight_filler, bias_filler;
 };
 

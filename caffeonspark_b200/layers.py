@@ -1,4 +1,4 @@
-"""Native producer layers: autograd Functions and modules over the library's LRN and fused
+"""Native producer layers: autograd Functions and modules over the library's LRN (across and within channels) and fused
 conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10) and its
 BatchNorm entry points (csrc/batch_norm.cu, DESIGN.md section 13).
 
@@ -74,6 +74,36 @@ class LRNFunction(torch.autograd.Function):
         _call(_entry("cos_lrn_backward", x.dtype), x.data_ptr(), dy.data_ptr(), dx.data_ptr(), *x.shape, *ctx.hyper,
               _stream())
         return dx, None, None, None, None
+
+
+class LRNWithinFunction(torch.autograd.Function):
+    """Caffe's WITHIN_CHANNEL LRN on the native stencil kernels (no k: Caffe does not use it for this region)."""
+
+    @staticmethod
+    def forward(ctx, x, size, alpha, beta):
+        x = _check(x)
+        y = torch.empty_like(x)
+        _call(_entry("cos_lrn_within_forward", x.dtype), x.data_ptr(), y.data_ptr(), *x.shape, size, alpha, beta,
+              _stream())
+        ctx.save_for_backward(x)
+        ctx.hyper = (size, alpha, beta)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        dy = _grad(dy, x.dtype)
+        dx = torch.empty_like(x)
+        _call(_entry("cos_lrn_within_backward", x.dtype), x.data_ptr(), dy.data_ptr(), dx.data_ptr(), *x.shape,
+              *ctx.hyper, _stream())
+        return dx, None, None, None
+
+
+def lrn_within_composite(x, size, alpha, beta):
+    """Caffe's WITHIN_CHANNEL LRN as its own layer composition (lrn_layer.cpp): square, AVE pool size x size with pad
+    size // 2 and stride 1 (the divisor counts the pad cells), power (1 + alpha * a)^-beta, product with x."""
+    a = F.avg_pool2d(x * x, size, stride=1, padding=size // 2, count_include_pad=True)
+    return x * torch.pow(1 + alpha * a, -beta)
 
 
 class BiasReluMaxPoolFunction(torch.autograd.Function):
@@ -188,15 +218,25 @@ def batch_norm_composite(x, mean, variance, scale, use_global_stats=False, movin
 
 
 class LRN(nn.Module):
-    """Caffe's cross-channel LRN (nn.LocalResponseNorm's function) on the native kernels."""
+    """Caffe's LRN on the native kernels.  region ACROSS_CHANNELS (the default) is nn.LocalResponseNorm's function;
+    WITHIN_CHANNEL normalises over a size x size window of each plane and ignores k, as Caffe does.  CPU tensors take
+    the PyTorch composition that defines the region."""
 
-    def __init__(self, size, alpha=1e-4, beta=0.75, k=1.0):
+    REGIONS = ("ACROSS_CHANNELS", "WITHIN_CHANNEL")
+
+    def __init__(self, size, alpha=1e-4, beta=0.75, k=1.0, region="ACROSS_CHANNELS"):
         super().__init__()
         if size < 1 or size % 2 == 0:
             raise ValueError("LRN only supports odd values for local_size")
-        self.size, self.alpha, self.beta, self.k = size, alpha, beta, k
+        if region not in self.REGIONS:
+            raise ValueError(f"LRN region must be one of {self.REGIONS}, got {region!r}")
+        self.size, self.alpha, self.beta, self.k, self.region = size, alpha, beta, k, region
 
     def forward(self, x):
+        if self.region == "WITHIN_CHANNEL":
+            if not x.is_cuda:
+                return lrn_within_composite(x, self.size, self.alpha, self.beta)
+            return LRNWithinFunction.apply(x, self.size, self.alpha, self.beta)
         if not x.is_cuda:
             return F.local_response_norm(x, self.size, self.alpha, self.beta, self.k)
         return LRNFunction.apply(x, self.size, self.alpha, self.beta, self.k)

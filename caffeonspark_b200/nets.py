@@ -1,4 +1,4 @@
-"""The three BASELINE nets and the reference's BatchNorm example as layer lists -> (a) Caffe prototxt text for the C
+"""The three BASELINE nets and the reference's CIFAR-10-full examples (plain and BatchNorm) as layer lists -> (a) Caffe prototxt text for the C
 library's layout parser, (b) the learnable-blob layout, (c) a PyTorch module
 used ONLY as the gradient producer (Net::ForwardBackward is out of scope of
 the sync library; SURVEY.md section 8 row f1).
@@ -8,6 +8,7 @@ Architectures follow the reference's configuration files
   data/cifar10_quick_train_test.prototxt, data/cifar10_quick_solver.prototxt
   data/bvlc_reference_net.prototxt, data/bvlc_reference_solver.prototxt
   caffe-public/examples/cifar10/cifar10_full_sigmoid_train_test_bn.prototxt (+ _solver_bn)
+  caffe-public/examples/cifar10/cifar10_full_train_test.prototxt, cifar10_full_solver.prototxt
 (batch 256/device for CaffeNet per
  caffe-public/models/bvlc_reference_caffenet/train_val.prototxt:25).
 """
@@ -16,7 +17,8 @@ from .caffenet import SolverDesc
 # layer tuples:
 #   ("conv", name, cout, k, stride, pad, group, (lr_w, dm_w), (lr_b, dm_b) or None for bias_term: false)
 #   ("ip",   name, nout, (lr_w, dm_w), (lr_b, dm_b))
-#   ("pool", name, "MAX"|"AVE", k, stride)   ("relu", name)  ("lrn", name, size, alpha, beta)
+#   ("pool", name, "MAX"|"AVE", k, stride)   ("relu", name)
+#   ("lrn",  name, size, alpha, beta[, "ACROSS_CHANNELS"|"WITHIN_CHANNEL"]): norm_region, ACROSS_CHANNELS if absent
 #   ("drop", name, ratio)   ("sigmoid", name)
 #   ("bn",   name): Caffe BatchNorm, blobs mean [C], variance [C], scale factor [1], each lr_mult 0 decay_mult 1
 _W, _B = (1.0, 1.0), (2.0, 1.0)
@@ -65,10 +67,24 @@ NETS = {
                 ("ip", "ip1", 10, _W, (1.0, 0.0))],
         solver=dict(lr_policy="step", base_lr=0.001, gamma=1, stepsize=5000, momentum=0.9, max_iter=60000,
                     test_iter=10, test_interval=1000, snapshot_prefix="cifar10_full_sigmoid_bn")),
+    # caffe-public/examples/cifar10/cifar10_full_{train_test,solver}.prototxt: conv3 has no param specs (lr_mult 1 for
+    # its bias too); ip1's weight decays 250x.  fillers: gaussian std of each weight (biases constant 0).
+    "cifar10_full": dict(
+        input=(3, 32, 32), batch=100, classes=10,
+        layers=[("conv", "conv1", 32, 5, 1, 2, 1, _W, _B), ("pool", "pool1", "MAX", 3, 2), ("relu", "relu1"),
+                ("lrn", "norm1", 3, 5e-05, 0.75, "WITHIN_CHANNEL"),
+                ("conv", "conv2", 32, 5, 1, 2, 1, _W, _B), ("relu", "relu2"), ("pool", "pool2", "AVE", 3, 2),
+                ("lrn", "norm2", 3, 5e-05, 0.75, "WITHIN_CHANNEL"),
+                ("conv", "conv3", 64, 5, 1, 2, 1, _W, _W), ("relu", "relu3"), ("pool", "pool3", "AVE", 3, 2),
+                ("ip", "ip1", 10, (1.0, 250.0), (2.0, 0.0))],
+        fillers={"conv1": 0.0001, "conv2": 0.01, "conv3": 0.01, "ip1": 0.01},
+        solver=dict(lr_policy="fixed", base_lr=0.001, momentum=0.9, weight_decay=0.004, max_iter=60000,
+                    test_iter=100, test_interval=1000, snapshot_prefix="cifar10_full")),
 }
 
-# SURVEY.md App. D: expected flat sizes (checked by tests)
-EXPECTED_PARAM_COUNT = {"lenet": 431080, "cifar10_quick": 145578, "caffenet": 60965224}
+# SURVEY.md App. D: expected flat sizes (checked by tests); cifar10_full: conv1 2432, conv2 25632, conv3 51264,
+# ip1 10250
+EXPECTED_PARAM_COUNT = {"lenet": 431080, "cifar10_quick": 145578, "caffenet": 60965224, "cifar10_full": 89578}
 # Nets with BatchNorm statistics among their learnable blobs: the forward pass writes those, and no backward
 # gives them a gradient.  3x32x32 -> conv1 2400, bn1 65, conv2 25600, bn2 65, conv3 51200, bn3 129, ip1 10240 + 10
 STATS_NET_PARAM_COUNT = {"cifar10_full_bn": 89709}
@@ -136,6 +152,12 @@ def net_prototxt(name):
                    f'  memory_data_param {{ batch_size: {net["batch"]} channels: {c} height: {h} width: {w} '
                    f'share_in_parallel: false }} }}')
     bottom = "data"
+    fillers = net.get("fillers", {})
+
+    def filler(nm):  # gaussian weights, constant-0 biases; nothing for a net without fillers
+        return (f' weight_filler {{ type: "gaussian" std: {fillers[nm]:g} }} bias_filler {{ type: "constant" }}'
+                if nm in fillers else "")
+
     for L in net["layers"]:
         kind, nm = L[0], L[1]
         if kind == "conv":
@@ -146,7 +168,7 @@ def net_prototxt(name):
             out.append(f'layer {{ name: "{nm}" type: "Convolution" bottom: "{bottom}" top: "{nm}"\n'
                        f'  param {{ lr_mult: {pw[0]:g} decay_mult: {pw[1]:g} }}{bias}\n'
                        f'  convolution_param {{ num_output: {cout} kernel_size: {k} stride: {s}{pad}{grp}'
-                       f'{"" if pb is not None else " bias_term: false"} }} }}')
+                       f'{"" if pb is not None else " bias_term: false"}{filler(nm)} }} }}')
             bottom = nm
         elif kind == "pool":
             _, _, mode, k, s = L
@@ -158,14 +180,15 @@ def net_prototxt(name):
             out.append(f'layer {{ name: "{nm}" type: "InnerProduct" bottom: "{bottom}" top: "{nm}"\n'
                        f'  param {{ lr_mult: {pw[0]:g} decay_mult: {pw[1]:g} }} param {{ lr_mult: {pb[0]:g} '
                        f'decay_mult: {pb[1]:g} }}\n'
-                       f'  inner_product_param {{ num_output: {nout} }} }}')
+                       f'  inner_product_param {{ num_output: {nout}{filler(nm)} }} }}')
             bottom = nm
         elif kind == "relu":
             out.append(f'layer {{ name: "{nm}" type: "ReLU" bottom: "{bottom}" top: "{bottom}" }}')
         elif kind == "lrn":
-            _, _, size, alpha, beta = L
+            size, alpha, beta = L[2:5]
+            region = f" norm_region: {L[5]}" if len(L) > 5 else ""
             out.append(f'layer {{ name: "{nm}" type: "LRN" bottom: "{bottom}" top: "{nm}" '
-                       f'lrn_param {{ local_size: {size} alpha: {alpha:g} beta: {beta:g} }} }}')
+                       f'lrn_param {{ local_size: {size} alpha: {alpha:g} beta: {beta:g}{region} }} }}')
             bottom = nm
         elif kind == "drop":
             out.append(f'layer {{ name: "{nm}" type: "Dropout" bottom: "{bottom}" top: "{bottom}" '
@@ -259,7 +282,7 @@ def torch_module(name):
         elif kind == "relu":
             mods.append(nn.ReLU(inplace=True))
         elif kind == "lrn":
-            mods.append(LRN(L[2], alpha=L[3], beta=L[4], k=1.0))
+            mods.append(LRN(L[2], alpha=L[3], beta=L[4], k=1.0, region=L[5] if len(L) > 5 else "ACROSS_CHANNELS"))
         elif kind == "drop":
             mods.append(nn.Dropout(L[2]))
         elif kind == "bn":

@@ -304,6 +304,16 @@ COS_API int cos_lrn_forward(const float* x, float* y, int num, int channels, int
 COS_API int cos_lrn_backward(const float* x, const float* dy, float* dx, int num, int channels, int height, int width,
                              int local_size, float alpha, float beta, float k, void* cuda_stream);
 
+/* LRN within the channel (Caffe's WITHIN_CHANNEL: split, square, AVE pool local_size x local_size with pad
+ * local_size/2 and stride 1, power with shift 1, scale alpha and power -beta, product), local_size odd and <= 15:
+ * s = 1 + alpha/local_size^2 * sum of x^2 over the window centred on (h, w), clipped to the plane;  y = x * s^-beta.
+ * Caffe does not use k for this region, so there is none.  The backward recomputes s from x.  Not in place: y, and
+ * dx, must not overlap an input. */
+COS_API int cos_lrn_within_forward(const float* x, float* y, int num, int channels, int height, int width,
+                                   int local_size, float alpha, float beta, void* cuda_stream);
+COS_API int cos_lrn_within_backward(const float* x, const float* dy, float* dx, int num, int channels, int height,
+                                    int width, int local_size, float alpha, float beta, void* cuda_stream);
+
 /* conv bias + ReLU + MAX pooling (ceil mode, pad 0; either order of ReLU and pooling gives the same
  * result).  x is the conv output WITHOUT bias, bias has `channels` elements, y and index are
  * num x channels x pooled_height x pooled_width with pooled_* the ceil-mode sizes (checked).
@@ -328,6 +338,11 @@ COS_API int cos_lrn_forward_bf16(const uint16_t* x, uint16_t* y, int num, int ch
 COS_API int cos_lrn_backward_bf16(const uint16_t* x, const uint16_t* dy, uint16_t* dx, int num, int channels,
                                   int height, int width, int local_size, float alpha, float beta, float k,
                                   void* cuda_stream);
+COS_API int cos_lrn_within_forward_bf16(const uint16_t* x, uint16_t* y, int num, int channels, int height, int width,
+                                        int local_size, float alpha, float beta, void* cuda_stream);
+COS_API int cos_lrn_within_backward_bf16(const uint16_t* x, const uint16_t* dy, uint16_t* dx, int num, int channels,
+                                         int height, int width, int local_size, float alpha, float beta,
+                                         void* cuda_stream);
 COS_API int cos_bias_relu_maxpool_forward_bf16(const uint16_t* x, const float* bias, uint16_t* y, uint8_t* index,
                                                int num, int channels, int height, int width, int kernel, int stride,
                                                int pooled_height, int pooled_width, void* cuda_stream);
