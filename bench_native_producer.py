@@ -1,7 +1,8 @@
 """Forward/backward time of the built-in producer against the PyTorch fp32 producer (DESIGN.md section 14).
 
-Workloads: the four nets the engine runs, at their reference batch sizes (LeNet b64, CIFAR-10-quick b100,
-cifar10_full_bn b100, cifar10_full b100).  For each, one process times the native engine, the PyTorch module with TF32 off and with
+Workloads: the five nets the engine runs, at their reference batch sizes (LeNet b64, CIFAR-10-quick b100,
+cifar10_full_bn b100, cifar10_full b100, and the siamese MNIST example b64 of 2x28x28 pairs: its two LeNet trunks share
+their weights and end in a ContrastiveLoss, timed against the PyTorch module that runs one trunk twice).  For each, one process times the native engine, the PyTorch module with TF32 off and with
 TF32 on (cuDNN's default, here applied to matmuls too), alternating the three in every round; each sample is CUDA events around `--iters`
 back-to-back forward/backward calls on one stream after `--warmup` untimed ones.  Prints one JSON line per
 workload with median / min / max ms per call and images/s, and the card's name and power limit.
@@ -22,7 +23,7 @@ import tempfile
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full")
+WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full", "mnist_siamese")
 FP32_PEAK = 67e12  # H100 SXM data sheet, dense FP32, at up to 700 W
 
 
@@ -35,6 +36,22 @@ def card():
         return "unknown"
 
 
+def siamese_solver(directory):
+    """The reference's siamese example with its TRAIN Data layer swapped for MemoryData (batch 64, 2x28x28)."""
+    configs = os.path.join(ROOT, "tests", "golden", "configs")
+    net = open(os.path.join(configs, "mnist_siamese_train_test.prototxt")).read()
+    start, end = net.index("layer {"), net.index('layer {\n  name: "slice_pair"')
+    data = ('layer { name: "pair_data" type: "MemoryData" top: "pair_data" top: "sim" include { phase: TRAIN } '
+            'memory_data_param { batch_size: 64 channels: 2 height: 28 width: 28 } }\n')
+    with open(os.path.join(directory, "mnist_siamese_net.prototxt"), "w") as f:
+        f.write(net[:start] + data + net[end:])
+    solver = open(os.path.join(configs, "mnist_siamese_solver.prototxt")).read()
+    path = os.path.join(directory, "mnist_siamese_solver.prototxt")
+    with open(path, "w") as f:
+        f.write(solver.replace("examples/siamese/mnist_siamese_train_test.prototxt", "mnist_siamese_net.prototxt"))
+    return path
+
+
 def plan_gemms(text):
     """(label, flops) of every GEMM one forward/backward launches, in launch order (native_producer.cu)."""
     fwd, bwd = [], []
@@ -45,7 +62,8 @@ def plan_gemms(text):
         kind, name = f[2], f[3]
         ins = [int(v) for v in f[4].split("x")]
         w = int(re.search(r" w=\d+:(\d+)", line).group(1)) if " w=" in line else 0
-        need_dx = " staged-bottom" not in line  # the plan's rule: no data gradient into a staged input
+        # the plan's rule: no data gradient into a staged input, nor into a blob with no learnable blob before it
+        need_dx = " staged-bottom" not in line and " no-bottom-grad" not in line
         if kind in ("Convolution", "ConvBiasReLUMaxPool"):
             kh, kw = (int(v) for v in re.search(r" k(\d+)x(\d+)", line).groups())
             sh, sw = (int(v) for v in re.search(r" s(\d+)x(\d+)", line).groups())
@@ -93,15 +111,17 @@ def main():
     gpu = card()
     tmp = tempfile.mkdtemp(prefix="bench_native_producer_")
     for name in args.workloads.split(","):
-        solver = nets.write_prototxts(name, tmp)
+        siamese = name == "mnist_siamese"
+        solver = siamese_solver(tmp) if siamese else nets.write_prototxts(name, tmp)
         net = C.CaffeNet(solver, "", "", 1, 1, 0, True, C.CaffeNet.NONE, -1, 0)
         net.use_native_producer(fill_weights=False)
         net.fill("data", 1, 0, 0.05)
         torch.cuda.synchronize()
-        batch = nets.NETS[name]["batch"]
+        batch = 64 if siamese else nets.NETS[name]["batch"]
         rng = np.random.RandomState(0)
-        x = torch.from_numpy(rng.rand(batch, *nets.NETS[name]["input"]).astype(np.float32)).cuda()
-        y = torch.from_numpy(rng.randint(0, 10, batch).astype(np.float32)).cuda()
+        shape = (2, 28, 28) if siamese else nets.NETS[name]["input"]
+        x = torch.from_numpy(rng.rand(batch, *shape).astype(np.float32)).cuda()
+        y = torch.from_numpy(rng.randint(0, 2 if siamese else 10, batch).astype(np.float32)).cuda()
         loss = torch.zeros(1, device="cuda")
         # a stream of its own: the legacy default stream's handle is 0, which would send the engine to the net's
         # stream, outside the events
@@ -112,7 +132,7 @@ def main():
         def native():
             assert net.forward_backward([x, y], loss.data_ptr(), stream=stream.cuda_stream), net.last_error()
 
-        module = nets.torch_module(name).cuda()
+        module = (nets.siamese_module() if siamese else nets.torch_module(name)).cuda()
         with torch.no_grad():
             w, off = net.data().clone(), 0
             for p in module.parameters():
@@ -121,6 +141,10 @@ def main():
         ylong = y.long()
 
         def torch_fb():
+            if siamese:
+                a, b = module(x)
+                nets.contrastive_loss(a, b, y).backward()
+                return
             out = module(x)
             F.cross_entropy(out, ylong).backward()
 

@@ -9,6 +9,7 @@
 #include <string.h>
 #include <unistd.h>
 
+#include <map>
 #include <sstream>
 
 namespace cosb {
@@ -708,8 +709,28 @@ std::vector<BlobView> CaffeNet::blob_views(const float* flat) const {
     else b.shape.assign(1, spec_.counts[k]);
     b.count = static_cast<uint64_t>(spec_.counts[k]);
     b.data = flat + off;
+    if (k < spec_.param_index.size()) b.param_index = spec_.param_index[k];
     off += b.count;
     v.push_back(std::move(b));
+  }
+  return v;
+}
+
+std::vector<BlobView> CaffeNet::model_views(const float* flat, bool with_shared) const {
+  std::vector<BlobView> owners = blob_views(flat);
+  if (!with_shared || spec_.shared.empty()) return owners;
+  std::vector<BlobView> v;
+  size_t s = 0;
+  for (size_t k = 0; k <= owners.size(); ++k) {  // a shared param goes before the owners that follow it in net order
+    for (; s < spec_.shared.size() && spec_.shared[s].position == static_cast<int>(k); ++s) {
+      const SharedParam& sp = spec_.shared[s];
+      BlobView b = owners[sp.owner];
+      b.layer_name = sp.layer_name;
+      b.layer_type = sp.layer_type;
+      b.param_index = sp.param_index;
+      v.push_back(std::move(b));
+    }
+    if (k < owners.size()) v.push_back(owners[k]);
   }
   return v;
 }
@@ -752,11 +773,11 @@ int CaffeNet::snapshot(std::string* err) {
   }
   const std::string model = snapshot_filename(iter_, false), state = snapshot_filename(iter_, true);
   if (spec_.snapshot_hdf5) {  // solver.cpp:417-418 SnapshotToHDF5 + sgd_solver.cpp:251-252 (csrc/hdf5_io.cpp)
-    if (!write_caffemodel_h5(model, blob_views(w.data()), err)) return -1;
+    if (!write_caffemodel_h5(model, model_views(w.data(), false), err)) return -1;
     if (!write_solverstate_h5(state, iter_, current_step_, model, hv, err)) return -1;
     return iter_;
   }
-  if (!write_caffemodel(model, spec_.net_name, blob_views(w.data()), err)) return -1;
+  if (!write_caffemodel(model, spec_.net_name, model_views(w.data(), true), err)) return -1;
   if (!write_solverstate(state, iter_, current_step_, model, hv, err)) return -1;
   return iter_;
 }
@@ -803,24 +824,38 @@ bool CaffeNet::restore(const std::string& model_file, const std::string& state_f
     if (!read_caffemodel(model, &name, &layers, err)) return false;
     std::vector<float> flat(count_);
     COS_RT(cudaMemcpy(flat.data(), data_, count_ * sizeof(float), cudaMemcpyDeviceToHost));
+    // every use of a learnable blob by layer name: (param index within the layer, blob, shared)
+    struct Use { size_t j; size_t k; bool shared; };
+    std::map<std::string, std::vector<Use>> uses;
+    std::vector<uint64_t> offs(spec_.counts.size());
     uint64_t off = 0;
-    int matched = 0;
     for (size_t k = 0; k < spec_.counts.size(); ++k) {
-      const std::string& lname = k < spec_.layer_names.size() ? spec_.layer_names[k] : std::string();
+      const std::string lname = k < spec_.layer_names.size() ? spec_.layer_names[k] : std::string();
       size_t j = 0;  // index of blob k inside its layer
-      for (size_t q = k; q > 0 && q - 1 < spec_.layer_names.size() && spec_.layer_names[q - 1] == lname; --q) ++j;
-      for (const ParsedLayer& L : layers) {
-        if (L.name != lname) continue;
-        if (j >= L.blobs.size() || L.blobs[j].data.size() != static_cast<size_t>(spec_.counts[k])) {
-          *err = "'" + model + "' is not a matching snapshot of this net: layer '" + lname + "' blob " +
-                 std::to_string(j) + " does not have " + std::to_string(spec_.counts[k]) + " elements";
+      if (k < spec_.param_index.size()) j = static_cast<size_t>(spec_.param_index[k]);
+      else for (size_t q = k; q > 0 && q - 1 < spec_.layer_names.size() && spec_.layer_names[q - 1] == lname; --q) ++j;
+      uses[lname].push_back(Use{j, k, false});
+      offs[k] = off;
+      off += static_cast<uint64_t>(spec_.counts[k]);
+    }
+    for (const SharedParam& sp : spec_.shared)
+      uses[sp.layer_name].push_back(Use{static_cast<size_t>(sp.param_index), static_cast<size_t>(sp.owner), true});
+    int matched = 0;
+    for (const ParsedLayer& L : layers) {  // CopyTrainedLayersFrom: file order, layers matched by name
+      auto it = uses.find(L.name);
+      if (it == uses.end()) continue;
+      for (const Use& u : it->second) {
+        const bool absent = u.j >= L.blobs.size() || !L.blobs[u.j].present;
+        if (absent && u.shared) continue;  // its owner's blob holds it (net.cpp:838)
+        if (absent || L.blobs[u.j].data.size() != static_cast<size_t>(spec_.counts[u.k])) {
+          *err = "'" + model + "' is not a matching snapshot of this net: layer '" + L.name + "' blob " +
+                 std::to_string(u.j) + " does not have " + std::to_string(spec_.counts[u.k]) + " elements";
           return false;  // CopyTrainedLayersFrom CHECKs the shapes (net.cpp)
         }
-        memcpy(flat.data() + off, L.blobs[j].data.data(), L.blobs[j].data.size() * sizeof(float));
+        // a shared param writes its owner's memory
+        memcpy(flat.data() + offs[u.k], L.blobs[u.j].data.data(), L.blobs[u.j].data.size() * sizeof(float));
         ++matched;
-        break;
       }
-      off += static_cast<uint64_t>(spec_.counts[k]);
     }
     if (matched == 0 && !spec_.counts.empty()) {
       *err = "'" + model + "' is not a matching snapshot of this net: no layer name matches";

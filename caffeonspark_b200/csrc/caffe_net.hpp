@@ -60,7 +60,10 @@ class CaffeNet {
   bool train_accumulate(int solver_index, const cos_blob* data, int ndata, int passes, std::string* err);
   virtual int snapshot(std::string* err);
   std::string snapshot_filename(int iter, bool is_state) const;  // Solver::SnapshotFilename
-  std::vector<BlobView> blob_views(const float* flat) const;
+  std::vector<BlobView> blob_views(const float* flat) const;  // the learnable blobs (owners), in order
+  // A .caffemodel's blobs: every layer's, a shared param holding its owner's data (Net::ToProto), or with
+  // with_shared false the owners only (Net::ToHDF5 skips a param that does not own itself, net.cpp:901).
+  std::vector<BlobView> model_views(const float* flat, bool with_shared) const;
   // resume from snapshot files, ours or stock Caffe's (CaffeNet.cpp:198-205 restore path)
   virtual bool restore(const std::string& model_file, const std::string& state_file, std::string* err);
   int getInitIter(int solver_index) const { return solver_index == 0 ? spec_.init_iter : -1; }

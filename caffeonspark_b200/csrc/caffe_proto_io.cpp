@@ -4,7 +4,10 @@
 #include "hdf5_io.hpp"
 
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
+
+#include <algorithm>
 
 namespace cosb {
 namespace {
@@ -237,16 +240,33 @@ bool blob_from_h5(const H5Node& d, const std::string& path, ParsedBlob* b, std::
   b->data = d.f32;
   return true;
 }
-// datasets "0", "1", ... of a group, in numeric order (the B-tree returns them in strcmp order: "0","1","10","2")
-bool numbered_blobs(const H5Node& g, const std::string& path, std::vector<ParsedBlob>* out, std::string* err) {
-  for (size_t j = 0; j < g.children.size(); ++j) {
+// datasets "0", "1", ... of a group, in numeric order (the B-tree returns them in strcmp order: "0","1","10","2").
+// With gaps (a model's layer group), an index below the largest without a dataset is a blob marked absent:
+// Net::ToHDF5 skips a param a layer shares.  Without (the solverstate's history), every index must be there.
+bool numbered_blobs(const H5Node& g, const std::string& path, bool gaps, std::vector<ParsedBlob>* out,
+                    std::string* err) {
+  size_t n = g.children.size();
+  if (gaps) {
+    n = 0;
+    for (const auto& c : g.children) {
+      const bool index = !c->name.empty() && c->name.size() < 10 &&
+                         c->name.find_first_not_of("0123456789") == std::string::npos;
+      if (!index) {
+        *err = "'" + path + "': group '" + g.name + "' has dataset '" + c->name + "', which is not a blob index";
+        return false;
+      }
+      n = std::max(n, static_cast<size_t>(atol(c->name.c_str())) + 1);
+    }
+  }
+  for (size_t j = 0; j < n; ++j) {
+    ParsedBlob b;
     const H5Node* d = g.find(std::to_string(j));
-    if (!d) {
+    if (!d && !gaps) {
       *err = "'" + path + "': group '" + g.name + "' has no dataset '" + std::to_string(j) + "'";
       return false;
     }
-    ParsedBlob b;
-    if (!blob_from_h5(*d, path, &b, err)) return false;
+    if (!d) b.present = false;
+    else if (!blob_from_h5(*d, path, &b, err)) return false;
     out->push_back(std::move(b));
   }
   return true;
@@ -268,7 +288,7 @@ bool read_caffemodel(const std::string& path, std::string* net_name, std::vector
       if (L->kind != H5Node::kGroup) continue;
       ParsedLayer pl;
       pl.name = L->name;
-      if (!numbered_blobs(*L, path, &pl.blobs, err)) return false;
+      if (!numbered_blobs(*L, path, true, &pl.blobs, err)) return false;
       layers->push_back(std::move(pl));
     }
     return true;
@@ -358,7 +378,9 @@ bool write_caffemodel_h5(const std::string& path, const std::vector<BlobView>& b
     }
     std::vector<int64_t> shape = blobs[i].shape;
     if (shape.empty()) shape.assign(1, static_cast<int64_t>(blobs[i].count));
-    layer->add_float(std::to_string(j++), shape, blobs[i].data, blobs[i].count);
+    const int name = blobs[i].param_index >= 0 ? blobs[i].param_index : j;
+    ++j;
+    layer->add_float(std::to_string(name), shape, blobs[i].data, blobs[i].count);
   }
   return h5_write(path, root, err);
 }
@@ -394,7 +416,7 @@ bool read_solverstate(const std::string& path, int* iter, int* current_step, std
     if (iter) *iter = it->i32[0];
     if (current_step) *current_step = cs->i32[0];
     if (learned_net) *learned_net = (ln && ln->kind == H5Node::kString) ? ln->str : std::string();
-    return numbered_blobs(*h, path, history, err);
+    return numbered_blobs(*h, path, false, history, err);
   }
   std::vector<unsigned char> buf;
   if (!slurp(path, &buf, err)) return false;

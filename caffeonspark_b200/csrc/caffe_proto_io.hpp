@@ -31,11 +31,13 @@ struct BlobView {  // one learnable blob (or one history blob) to write
   std::vector<int64_t> shape;
   const float* data = nullptr;  // host pointer, prod(shape) elements
   uint64_t count = 0;
+  int param_index = -1;  // index within its layer (the HDF5 dataset name); -1: its place among the layer's views
 };
 
 struct ParsedBlob {
   std::vector<int64_t> shape;
   std::vector<float> data;
+  bool present = true;  // false: an HDF5 layer group without this index's dataset (a shared param Net::ToHDF5 skips)
 };
 
 struct ParsedLayer {

@@ -53,6 +53,17 @@ bool fusable_pool(const NetLayer& L) {
          L.tops.size() == 1 && L.bottom_shapes[0].size() == 4;
 }
 
+// The weight (and bias) of a Convolution or InnerProduct: a shared param uses its owner's offsets, and only the owner's
+// filler fills the blob.
+void set_params(const NetLayer& L, Op* op, Plan* P) {
+  op->w_off = P->blob_off[L.blobs[0]], op->w_count = P->blob_count[L.blobs[0]];
+  if (!L.shared[0]) P->blob_filler[L.blobs[0]] = L.weight_filler;
+  if (L.bias_term) {
+    op->b_off = P->blob_off[L.blobs[1]], op->b_count = P->blob_count[L.blobs[1]];
+    if (!L.shared[1]) P->blob_filler[L.blobs[1]] = L.bias_filler;
+  }
+}
+
 }  // namespace
 
 bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Plan* plan, std::string* err) {
@@ -68,10 +79,14 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
   P.param_count = off;
   std::map<std::string, int> cur;  // blob name -> tensor id it currently names
   std::vector<std::string> consumer;  // per tensor: the layer that reads it ("" = none yet)
+  // per tensor: whether anything before it has a learnable blob, so that its gradient is wanted (Caffe's
+  // bottom_need_backward).  Staged inputs want none.
+  std::vector<bool> wants_grad;
   auto new_tensor = [&](int64_t n, int storage) {
     P.tensor_count.push_back(n);
     P.storage.push_back(storage < 0 ? static_cast<int>(P.tensor_count.size()) - 1 : storage);
     consumer.emplace_back();
+    wants_grad.push_back(false);
     return static_cast<int>(P.tensor_count.size()) - 1;
   };
   for (const NetLayer& L : layers) {  // staged inputs first: tensors 0 .. ninputs-1
@@ -92,18 +107,22 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     }
     const bool known = L.type == "Convolution" || L.type == "Pooling" || L.type == "InnerProduct" || L.type == "ReLU" ||
                        L.type == "Sigmoid" || L.type == "BatchNorm" || L.type == "SoftmaxWithLoss" ||
+                       L.type == "Slice" || L.type == "ContrastiveLoss" ||
                        (L.type == "LRN" && L.norm_region == "WITHIN_CHANNEL");  // ACROSS_CHANNELS has no engine op
     if (!known) {
       *err = why(L, "layer type not supported");
       return false;
     }
-    const size_t want_bottoms = L.type == "SoftmaxWithLoss" ? 2 : 1;
-    if (L.bottoms.size() != want_bottoms || L.tops.size() != 1) {
+    // Slice is the one layer with several tops; ContrastiveLoss reads a, b and sim
+    const size_t want_bottoms = L.type == "SoftmaxWithLoss" ? 2 : L.type == "ContrastiveLoss" ? 3 : 1;
+    if (L.bottoms.size() != want_bottoms || (L.tops.size() != 1 && L.type != "Slice") || L.tops.empty()) {
       *err = why(L, "needs " + std::to_string(want_bottoms) + " bottom(s) and one top");
       return false;
     }
     Op op;
     op.name = L.name;
+    for (size_t j = 0; j < L.blobs.size(); ++j)
+      if (L.shared[j]) op.shares.push_back(L.blobs[j]);
     auto take = [&](const std::string& name, int* id) {
       auto it = cur.find(name);
       if (it == cur.end()) {
@@ -122,7 +141,20 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     if (!take(L.bottoms[0], &op.in)) return false;
     op.in_shape = L.bottom_shapes[0];
     op.out_shape = L.top_shapes[0];
-    op.need_dx = op.in >= P.ninputs;
+    op.need_dx = wants_grad[op.in];
+    if (L.type == "Slice") {  // one op per top, each copying its range of the bottom (and back, in the backward)
+      op.kind = OpKind::kSlice;
+      op.slice_axis = static_cast<int>(L.axis);
+      for (size_t t = 0; t < L.tops.size(); ++t) {
+        op.slice_begin = L.slice_begin[t];
+        op.out_shape = L.top_shapes[t];
+        op.out = new_tensor(count_of(op.out_shape), -1);
+        wants_grad[op.out] = op.need_dx;
+        cur[L.tops[t]] = op.out;
+        P.ops.push_back(op);
+      }
+      continue;
+    }
     int storage = -1;
     std::string reason;
     if (L.type == "Convolution") {
@@ -142,12 +174,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.kh = static_cast<int>(L.kernel_h), op.kw = static_cast<int>(L.kernel_w);
       op.sh = static_cast<int>(L.stride_h), op.sw = static_cast<int>(L.stride_w);
       op.ph = static_cast<int>(L.pad_h), op.pw = static_cast<int>(L.pad_w);
-      op.w_off = P.blob_off[L.first_blob], op.w_count = P.blob_count[L.first_blob];
-      P.blob_filler[L.first_blob] = L.weight_filler;
-      if (L.bias_term) {
-        op.b_off = P.blob_off[L.first_blob + 1], op.b_count = P.blob_count[L.first_blob + 1];
-        P.blob_filler[L.first_blob + 1] = L.bias_filler;
-      }
+      set_params(L, &op, &P);
       // conv + bias followed by ReLU and MAX pool in either order: the existing fused block (caffe_layers.cu)
       if (L.bias_term && i + 2 < layers.size()) {
         const NetLayer& a = layers[i + 1];
@@ -166,6 +193,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
             op.pool_stride = static_cast<int>(pool.stride_h);
             op.out_shape = b.top_shapes[0];
             const int out = new_tensor(count_of(op.out_shape), -1);
+            wants_grad[out] = true;  // the block has a weight and a bias
             cur[b.tops[0]] = out;
             op.out = out;
             P.ops.push_back(op);
@@ -198,12 +226,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         return false;
       }
       op.kind = OpKind::kInnerProduct;
-      op.w_off = P.blob_off[L.first_blob], op.w_count = P.blob_count[L.first_blob];
-      P.blob_filler[L.first_blob] = L.weight_filler;
-      if (L.bias_term) {
-        op.b_off = P.blob_off[L.first_blob + 1], op.b_count = P.blob_count[L.first_blob + 1];
-        P.blob_filler[L.first_blob + 1] = L.bias_filler;
-      }
+      set_params(L, &op, &P);
     } else if (L.type == "ReLU" || L.type == "Sigmoid") {
       op.kind = L.type == "ReLU" ? OpKind::kReLU : OpKind::kSigmoid;
       op.slope = L.negative_slope;
@@ -212,8 +235,12 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.in_place = L.tops[0] == L.bottoms[0] && op.in >= P.ninputs;
       if (op.in_place) storage = P.storage[op.in];
     } else if (L.type == "BatchNorm") {
+      if (!op.shares.empty()) {
+        *err = why(L, "shared BatchNorm statistics are not supported");
+        return false;
+      }
       op.kind = OpKind::kBatchNorm;  // separate top storage even when top == bottom: the kernels are not in place
-      op.w_off = P.blob_off[L.first_blob];
+      op.w_off = P.blob_off[L.blobs[0]];
       op.global_stats = L.use_global_stats;
       op.fraction = L.moving_average_fraction;
       op.eps = L.eps;
@@ -231,6 +258,23 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.lrn_size = static_cast<int>(L.local_size);
       op.lrn_alpha = L.lrn_alpha;
       op.lrn_beta = L.lrn_beta;
+    } else if (L.type == "ContrastiveLoss") {  // the parser checked the shapes: a, b N x C (x 1 x 1), sim N values
+      if (++losses > 1) {
+        *err = why(L, "a second loss layer is not supported");
+        return false;
+      }
+      op.kind = OpKind::kContrastiveLoss;
+      op.loss_weight = L.loss_weight;
+      op.margin = L.margin;
+      op.legacy = L.legacy_version;
+      if (!take(L.bottoms[1], &op.in2)) return false;
+      op.need_dx2 = wants_grad[op.in2];
+      auto it = cur.find(L.bottoms[2]);
+      if (it == cur.end()) {
+        *err = why(L, "sim bottom '" + L.bottoms[2] + "' is not produced by an earlier TRAIN layer");
+        return false;
+      }
+      op.label = it->second;
     } else {  // SoftmaxWithLoss
       if (++losses > 1) {
         *err = why(L, "a second loss layer is not supported");
@@ -252,11 +296,13 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       }
     }
     op.out = new_tensor(count_of(op.out_shape), storage);
+    // BatchNorm's blobs are statistics, with no gradient
+    wants_grad[op.out] = op.need_dx || (op.kind != OpKind::kBatchNorm && (op.w_off >= 0 || op.b_off >= 0));
     cur[L.tops[0]] = op.out;
     P.ops.push_back(op);
   }
   if (losses == 0) {
-    *err = "the net has no SoftmaxWithLoss layer in its TRAIN phase (native producer)";
+    *err = "the net has no SoftmaxWithLoss or ContrastiveLoss layer in its TRAIN phase (native producer)";
     return false;
   }
   for (size_t t = 0; t < P.tensor_count.size(); ++t) {
@@ -277,7 +323,7 @@ bool plan_from_prototxt(const std::string& path, SolverSpec* spec, Plan* plan, s
 std::string Plan::text() const {
   static const char* kinds[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling", "InnerProduct",
                                 "ReLU",        "Sigmoid",             "BatchNorm", "SoftmaxWithLoss",
-                                "LRN(WITHIN_CHANNEL)"};
+                                "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss"};
   std::ostringstream os;
   for (int i = 0; i < ninputs; ++i) os << "input " << i << " " << input_names[i] << " " << tensor_count[i] << "\n";
   for (size_t i = 0; i < ops.size(); ++i) {
@@ -293,9 +339,21 @@ std::string Plan::text() const {
     if (op.w_off >= 0 && op.kind != OpKind::kBatchNorm) os << " w=" << op.w_off << ":" << op.w_count;
     if (op.b_off >= 0) os << " b=" << op.b_off << ":" << op.b_count;
     if (op.kind == OpKind::kBatchNorm) os << " stats=" << op.w_off;
+    if (!op.shares.empty()) {
+      os << " shares=";
+      for (size_t j = 0; j < op.shares.size(); ++j) os << (j ? "," : "") << op.shares[j];
+    }
+    if (op.kind == OpKind::kSlice) os << " axis=" << op.slice_axis << " begin=" << op.slice_begin;
     if (op.kind == OpKind::kSoftmaxLoss) os << " label=" << op.label << " loss_weight=" << op.loss_weight;
+    if (op.kind == OpKind::kContrastiveLoss)
+      os << " second=" << op.in2 << " sim=" << op.label << " margin=" << op.margin << (op.legacy ? " legacy" : "")
+         << " loss_weight=" << op.loss_weight;
     if (op.in_place) os << " in-place";
-    if (!op.need_dx) os << " staged-bottom";  // no data gradient is propagated into a staged input
+    // no data gradient is propagated into a staged input, nor into a blob with no learnable blob before it
+    auto mark = [&](int in, bool need) { return need ? "" : in < ninputs ? " staged-bottom" : " no-bottom-grad"; };
+    const char* m = mark(op.in, op.need_dx);
+    if (!*m && op.kind == OpKind::kContrastiveLoss) m = mark(op.in2, op.need_dx2);
+    os << m;
     os << "\n";
   }
   os << "params " << param_count << " blobs " << blob_count.size() << "\n";

@@ -343,6 +343,72 @@ __global__ void __launch_bounds__(kThreads) softmax_loss_kernel(const float* x, 
   if (threadIdx.x == 0) *loss = __fmul_rn(loss_weight, __fdiv_rn(part, count));
 }
 
+// ------------------------------------------------------------------ Slice (slice_layer.cu semantics)
+// One top of a Slice: top[n, i, r] = bottom[n, begin + i, r] over outer n, top_axis i and inner r.  Forward copies the
+// top out of the bottom; backward (to_bottom) writes the top's gradient into its range of the bottom's gradient.
+__global__ void slice_copy_kernel(const float* src, float* dst, int64_t total, int64_t top_span, int64_t bottom_span,
+                                  int64_t offset, bool to_bottom) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t b = (i / top_span) * bottom_span + offset + i % top_span;
+    if (to_bottom) dst[b] = src[i];
+    else dst[i] = src[b];
+  }
+}
+
+// ------------------------------------------------------------------ ContrastiveLoss (contrastive_loss_layer.cpp)
+// One block.  Pair r: d = a_r - b_r, dist_sq = sum over c of d_c^2 in c order.  A similar pair (static_cast<int>(sim)
+// nonzero) adds dist_sq to the loss and gets da = alpha * d.  A dissimilar pair adds max(margin - dist_sq, 0)
+// (legacy_version) or max(margin - dist, 0)^2, and gets da = beta * d while mdist = margin - dist_sq (legacy) or
+// margin - dist is > 0, else 0, with beta = -alpha (legacy) or -alpha * mdist / (dist + 1e-4).  alpha = loss_weight / N
+// and db = -da.  Pairs are summed per thread in order, then by a fixed tree; *loss = loss_weight * (sum / N / 2).  A
+// non-finite sim sets *status and its pair contributes neither loss nor gradient.  da / db are null for a staged bottom.
+// Made for the narrow embeddings of siamese nets (C of a few to a few dozen: each thread walks its pairs' C channels
+// twice).  For wide embeddings and few pairs most threads idle and the row loads are not coalesced.
+__global__ void __launch_bounds__(kThreads) contrastive_loss_kernel(const float* a, const float* b, const float* sim,
+                                                                    float* da, float* db, float* loss, int N, int C,
+                                                                    float margin, bool legacy, float loss_weight,
+                                                                    int* status) {
+  __shared__ float sh[kThreads];
+  const float alpha = __fdiv_rn(loss_weight, static_cast<float>(N));
+  float part = 0.f;
+  for (int r = threadIdx.x; r < N; r += kThreads) {
+    const float* ar = a + (size_t)r * C;
+    const float* br = b + (size_t)r * C;
+    float dist_sq = 0.f;
+    for (int c = 0; c < C; ++c) {
+      const float d = __fsub_rn(ar[c], br[c]);
+      dist_sq = __fadd_rn(dist_sq, __fmul_rn(d, d));
+    }
+    const float s = sim[r];
+    float scale = 0.f;  // gradient of a = scale * d
+    if (!isfinite(s)) {
+      *reinterpret_cast<volatile int*>(status) = kStatusBadLabel;
+    } else if (static_cast<int>(s)) {
+      part = __fadd_rn(part, dist_sq);
+      scale = alpha;
+    } else if (legacy) {
+      const float mdist = __fsub_rn(margin, dist_sq);
+      part = __fadd_rn(part, fmaxf(mdist, 0.f));
+      if (mdist > 0.f) scale = -alpha;
+    } else {
+      const float dist = __fsqrt_rn(dist_sq);
+      const float mdist = __fsub_rn(margin, dist);
+      const float m = fmaxf(mdist, 0.f);
+      part = __fadd_rn(part, __fmul_rn(m, m));
+      if (mdist > 0.f) scale = __fdiv_rn(__fmul_rn(-alpha, mdist), __fadd_rn(dist, 1e-4f));
+    }
+    for (int c = 0; c < C; ++c) {
+      const float g = __fmul_rn(scale, __fsub_rn(ar[c], br[c]));
+      if (da) da[(size_t)r * C + c] = g;
+      if (db) db[(size_t)r * C + c] = -g;
+    }
+  }
+  part = block_sum(part, sh);
+  if (threadIdx.x == 0)
+    *loss = __fmul_rn(loss_weight, __fdiv_rn(__fdiv_rn(part, static_cast<float>(N)), 2.f));
+}
+
 // ------------------------------------------------------------------ fillers (u: the cos_net_fill value in [-1, 1))
 __global__ void constant_fill_kernel(float* p, int n, float v) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = v;
@@ -392,6 +458,13 @@ void bn_dims(const Op& op, int* n, int* c, int* hw) {
   *c = static_cast<int>(op.in_shape.size() > 1 ? op.in_shape[1] : 1);
   *hw = static_cast<int>(total / (static_cast<int64_t>(*n) * *c));
 }
+// Slice: elements after the slice axis, and the elements of one outer index of a blob (its axis times that)
+int64_t slice_inner(const Op& op) {
+  int64_t n = 1;
+  for (size_t a = op.slice_axis + 1; a < op.in_shape.size(); ++a) n *= op.in_shape[a];
+  return n;
+}
+int64_t slice_span(const Op& op, const std::vector<int64_t>& shape) { return shape[op.slice_axis] * slice_inner(op); }
 int ip_k(const Op& op) { return static_cast<int>(op.w_count / (op.w_count > 0 ? op.out_shape[1] : 1)); }
 
 // conv weight / bias gradients and the data gradient, from dy = the conv output's gradient
@@ -597,6 +670,17 @@ int NativeProducer::forward_backward(const cos_blob* inputs, int ninputs, float*
   }
   for (size_t i = 0; i < plan_.ops.size(); ++i) {
     const Op& op = plan_.ops[i];
+    if (op.kind == OpKind::kContrastiveLoss) {  // writes both bottoms' gradients here, as SoftmaxWithLoss does
+      const int N = static_cast<int>(op.in_shape[0]);
+      const int C = static_cast<int>(plan_.tensor_count[op.in] / N);
+      contrastive_loss_kernel<<<1, kThreads, 0, s>>>(act_[op.in], act_[op.in2], act_[op.label],
+                                                     op.need_dx ? grad_[op.in] : nullptr,
+                                                     op.need_dx2 ? grad_[op.in2] : nullptr, loss_dev, N, C, op.margin,
+                                                     op.legacy, op.loss_weight, status_);
+      cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) return e;
+      continue;
+    }
     if (op.kind == OpKind::kSoftmaxLoss) {
       const int C = static_cast<int>(op.in_shape[1]);
       const int rows = static_cast<int>(plan_.tensor_count[op.in] / C);
@@ -660,6 +744,10 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, cudaStream_t 
       return batch_norm_forward(x, y, m, m + c, m + 2 * c, static_cast<float*>(op_aux_[i]), workspace_, bn, c, hw, 1,
                                 op.global_stats, op.fraction, op.eps, s);
     }
+    case OpKind::kSlice:
+      slice_copy_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n, slice_span(op, op.out_shape), slice_span(op, op.in_shape),
+                                                         op.slice_begin * slice_inner(op), false);
+      return cudaGetLastError();
     case OpKind::kLRNWithin:
       return lrn_within_forward(x, y, static_cast<int>(op.in_shape[0]), static_cast<int>(op.in_shape[1]),
                                 static_cast<int>(op.in_shape[2]), static_cast<int>(op.in_shape[3]), op.lrn_size,
@@ -727,7 +815,15 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
       return lrn_within_backward(x, dy, dx, static_cast<int>(op.in_shape[0]), static_cast<int>(op.in_shape[1]),
                                  static_cast<int>(op.in_shape[2]), static_cast<int>(op.in_shape[3]), op.lrn_size,
                                  op.lrn_alpha, op.lrn_beta, s);
-    default:  // SoftmaxWithLoss wrote its bottom gradient in the forward pass
+    case OpKind::kSlice: {
+      if (!dx) return cudaSuccess;
+      const int64_t n = plan_.tensor_count[op.out];
+      slice_copy_kernel<<<grid_for(n), kThreads, 0, s>>>(dy, dx, n, slice_span(op, op.out_shape),
+                                                         slice_span(op, op.in_shape), op.slice_begin * slice_inner(op),
+                                                         true);
+      return cudaGetLastError();
+    }
+    default:  // SoftmaxWithLoss and ContrastiveLoss wrote their bottom gradients in the forward pass
       return cudaSuccess;
   }
 }

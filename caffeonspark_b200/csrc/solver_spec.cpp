@@ -291,6 +291,10 @@ bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, s
   spec->layer_names.clear();
   spec->layer_types.clear();
   spec->shapes.clear();
+  spec->param_index.clear();
+  spec->shared.clear();
+  std::map<std::string, int> param_owner;  // ParamSpec.name -> learnable blob that owns it
+  std::vector<bool> has_lr, has_decay;     // per learnable blob: lr_mult / decay_mult set explicitly
   spec->net_name = net.str("name");
   // legacy "input:" / "input_shape" / "input_dim" net-level inputs
   {
@@ -343,7 +347,10 @@ bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, s
     rec.bottoms = bottoms;
     rec.tops = tops;
     for (const std::string& b : bottoms) rec.bottom_shapes.push_back(blobs.count(b) ? to64(blobs[b]) : std::vector<int64_t>());
-    rec.first_blob = static_cast<int>(spec->counts.size());
+    auto refuse = [&](const std::string& reason) {
+      *err = "layer '" + name + "' (" + type + "): " + reason;
+      return false;
+    };
     rec.has_loss_param = L->first("loss_param") != nullptr;
     if (const Node* lw = L->first("loss_weight")) rec.loss_weight = static_cast<float>(atof(lw->value.c_str()));
     if (type == "MemoryData") {
@@ -521,25 +528,139 @@ bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, s
         rec.moving_average_fraction = static_cast<float>(p->num("moving_average_fraction", 0.999));
         rec.eps = static_cast<float>(p->num("eps", 1e-5));
       }
+    } else if (type == "Slice") {  // slice_layer.cpp Reshape
+      Shape in;
+      if (!bottom_shape(0, &in)) return false;
+      const Node* p = L->first("slice_param");
+      const long naxes = static_cast<long>(in.size());
+      long axis = 1;
+      if (p && p->first("axis") && p->first("slice_dim")) return refuse("either axis or slice_dim should be specified; not both");
+      if (p && p->first("slice_dim")) {
+        axis = p->integer("slice_dim", 1);
+      } else {
+        axis = p ? p->integer("axis", 1) : 1;
+        if (axis < 0) axis += naxes;
+      }
+      if (axis < 0 || axis >= naxes) return refuse("slice axis " + std::to_string(axis) + " is out of range for a " +
+                                                   std::to_string(naxes) + "-axis bottom");
+      if (tops.empty()) return refuse("needs at least one top");
+      const long A = in[axis], ntop = static_cast<long>(tops.size());
+      std::vector<long> bounds{0};
+      auto points = p ? p->all("slice_point") : std::vector<const Node*>();
+      if (!points.empty()) {
+        if (static_cast<long>(points.size()) != ntop - 1)
+          return refuse(std::to_string(points.size()) + " slice_point(s) for " + std::to_string(ntop) + " tops");
+        for (const Node* sp : points) {
+          const long v = atol(sp->value.c_str());
+          if (v <= bounds.back() || v >= A)
+            return refuse("slice_point " + std::to_string(v) + " is not increasing inside (0, " + std::to_string(A) + ")");
+          bounds.push_back(v);
+        }
+      } else {
+        if (A % ntop) return refuse(std::to_string(ntop) + " tops do not evenly divide slice axis " + std::to_string(A));
+        for (long t = 1; t < ntop; ++t) bounds.push_back(t * (A / ntop));
+      }
+      bounds.push_back(A);
+      rec.axis = axis;
+      for (long t = 0; t < ntop; ++t) {
+        Shape s = in;
+        s[axis] = bounds[t + 1] - bounds[t];
+        blobs[tops[t]] = s;
+        rec.slice_begin.push_back(bounds[t]);
+        rec.slice_end.push_back(bounds[t + 1]);
+      }
+    } else if (type == "ContrastiveLoss") {  // contrastive_loss_layer.cpp LayerSetUp and LossLayer::Reshape
+      Shape a, b, sim;
+      if (bottoms.size() != 3) return refuse("needs 3 bottoms (a, b, sim)");
+      if (!bottom_shape(0, &a) || !bottom_shape(1, &b) || !bottom_shape(2, &sim)) return false;
+      auto legacy = [](const Shape& s, size_t i) { return i < s.size() ? s[i] : 1L; };  // Blob::LegacyShape
+      if (a.empty() || a.size() > 4 || b.size() != a.size() || sim.empty() || sim.size() > 4)
+        return refuse("bottoms must have 1 to 4 axes, a and b as many");
+      if (b[0] != a[0] || sim[0] != a[0]) return refuse("a, b and sim must have the same first dimension");
+      if (legacy(a, 1) != legacy(b, 1)) return refuse("a and b must have the same channels");
+      if (legacy(a, 2) != 1 || legacy(a, 3) != 1 || legacy(b, 2) != 1 || legacy(b, 3) != 1)
+        return refuse("a and b must be N x C (x 1 x 1)");
+      if (legacy(sim, 1) != 1 || legacy(sim, 2) != 1 || legacy(sim, 3) != 1) return refuse("sim must hold one value per pair");
+      if (const Node* p = L->first("contrastive_loss_param")) {
+        rec.margin = static_cast<float>(p->num("margin", 1.0));
+        rec.legacy_version = p->boolean("legacy_version", false);
+      }
+      for (const std::string& t : tops) blobs[t] = Shape{};
     } else if (type == "Silence") {
     } else {
       *err = "layer '" + name + "' of type '" + type +
              "' is not understood by the layout parser; pass the layout with cos_net_allocate_desc";
       return false;
     }
+    // net.cpp AppendParam: an anonymous param, or the first use of a name, owns a learnable blob; a later use of the
+    // name shares the owner's
     auto pspecs = L->all("param");
     for (size_t i = 0; i < param_counts.size(); ++i) {
-      spec->counts.push_back(param_counts[i]);
-      // ParamSpec defaults lr_mult = 1, decay_mult = 1 (caffe.proto:297-304)
-      spec->lr_mult.push_back(i < pspecs.size() ? static_cast<float>(pspecs[i]->num("lr_mult", 1.0)) : 1.0f);
-      spec->decay_mult.push_back(i < pspecs.size() ? static_cast<float>(pspecs[i]->num("decay_mult", 1.0)) : 1.0f);
-      spec->blob_names.push_back(name + "." + std::to_string(i));
-      spec->layer_names.push_back(name);
-      spec->layer_types.push_back(type);
-      spec->shapes.push_back(param_shapes[i]);
+      const Node* ps = i < pspecs.size() ? pspecs[i] : nullptr;
+      const std::string pname = ps ? ps->str("name", "") : "";
+      auto owner = pname.empty() ? param_owner.end() : param_owner.find(pname);
+      if (owner == param_owner.end()) {
+        if (!pname.empty()) param_owner[pname] = static_cast<int>(spec->counts.size());
+        rec.blobs.push_back(static_cast<int>(spec->counts.size()));
+        rec.shared.push_back(false);
+        spec->counts.push_back(param_counts[i]);
+        // ParamSpec defaults lr_mult = 1, decay_mult = 1 (caffe.proto:297-304)
+        spec->lr_mult.push_back(ps ? static_cast<float>(ps->num("lr_mult", 1.0)) : 1.0f);
+        spec->decay_mult.push_back(ps ? static_cast<float>(ps->num("decay_mult", 1.0)) : 1.0f);
+        has_lr.push_back(ps && ps->first("lr_mult"));
+        has_decay.push_back(ps && ps->first("decay_mult"));
+        spec->blob_names.push_back(name + "." + std::to_string(i));
+        spec->layer_names.push_back(name);
+        spec->layer_types.push_back(type);
+        spec->shapes.push_back(param_shapes[i]);
+        spec->param_index.push_back(static_cast<int>(i));
+        continue;
+      }
+      const int k = owner->second;
+      auto shape_string = [](const std::vector<int64_t>& s) {  // Blob::shape_string
+        std::string t;
+        int64_t n = 1;
+        for (int64_t d : s) t += std::to_string(d) + " ", n *= d;
+        return t + "(" + std::to_string(n) + ")";
+      };
+      const std::string share = "Cannot share param '" + pname + "' owned by layer '" + spec->layer_names[k] +
+                                "' with layer '" + name + "'; ";
+      const std::string mode = ps->str("share_mode", "STRICT");
+      if (mode == "PERMISSIVE" || mode == "1") {
+        if (spec->counts[k] != param_counts[i]) {
+          *err = share + "count mismatch.  Owner layer param shape is " + shape_string(spec->shapes[k]) +
+                 "; sharing layer shape is " + shape_string(param_shapes[i]);
+          return false;
+        }
+      } else if (spec->shapes[k] != param_shapes[i]) {
+        *err = share + "shape mismatch.  Owner layer param shape is " + shape_string(spec->shapes[k]) +
+               "; sharing layer expects shape " + shape_string(param_shapes[i]);
+        return false;
+      }
+      // the first explicit lr_mult / decay_mult, by the owner or a sharer, is the blob's; a different later one is an
+      // error
+      struct Mult { const char* field; std::vector<float>* value; std::vector<bool>* set; };
+      for (const Mult& m : {Mult{"lr_mult", &spec->lr_mult, &has_lr}, Mult{"decay_mult", &spec->decay_mult, &has_decay}}) {
+        if (!ps->first(m.field)) continue;
+        const float v = static_cast<float>(ps->num(m.field, 1.0));
+        if ((*m.set)[k] && v != (*m.value)[k]) {
+          *err = "Shared param '" + pname + "' has mismatched " + m.field + ".";
+          return false;
+        }
+        (*m.set)[k] = true;
+        (*m.value)[k] = v;
+      }
+      rec.blobs.push_back(k);
+      rec.shared.push_back(true);
+      SharedParam sp;
+      sp.layer_name = name;
+      sp.layer_type = type;
+      sp.param_index = static_cast<int>(i);
+      sp.owner = k;
+      sp.position = static_cast<int>(spec->counts.size());
+      spec->shared.push_back(sp);
     }
     if (out) {
-      rec.nblobs = static_cast<int>(param_counts.size());
       for (const std::string& t : tops) rec.top_shapes.push_back(blobs.count(t) ? to64(blobs[t]) : std::vector<int64_t>());
       out->push_back(rec);
     }

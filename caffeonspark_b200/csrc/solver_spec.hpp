@@ -30,7 +30,10 @@ struct NetLayer {
   std::string name, type;
   std::vector<std::string> bottoms, tops;
   std::vector<std::vector<int64_t>> bottom_shapes, top_shapes;
-  int first_blob = 0, nblobs = 0;  // learnable blobs of this layer: SolverSpec index first_blob ..
+  // per param of this layer: the learnable blob it reads (SolverSpec index; the owner's for a shared param), and
+  // whether it is shared (a later use of a named param)
+  std::vector<int> blobs;
+  std::vector<bool> shared;
   int64_t num_output = 0, axis = 1, group = 1;
   int64_t kernel_h = 0, kernel_w = 0, stride_h = 1, stride_w = 1, pad_h = 0, pad_w = 0, dilation_h = 1, dilation_w = 1;
   bool bias_term = true, transpose = false, global_pooling = false;
@@ -44,7 +47,21 @@ struct NetLayer {
   int64_t local_size = 5;
   float lrn_alpha = 1.f, lrn_beta = 0.75f, lrn_k = 1.f;
   std::string norm_region = "ACROSS_CHANNELS";
+  // Slice (slice_layer.cpp): the canonical axis and every top's [begin, end) along it
+  std::vector<int64_t> slice_begin, slice_end;
+  // ContrastiveLoss (caffe.proto ContrastiveLossParameter)
+  float margin = 1.f;
+  bool legacy_version = false;
   FillerSpec weight_filler, bias_filler;
+};
+
+// A later use of a named param (net.cpp AppendParam): it reads the owner's data and adds its gradient into the owner's
+// diff, and has no learnable blob, lr_mult or history of its own.
+struct SharedParam {
+  std::string layer_name, layer_type;
+  int param_index = 0;  // index of the blob within its layer
+  int owner = 0;        // the learnable blob it shares
+  int position = 0;     // learnable blobs before it in net order: where Net::ToProto writes it among the owners
 };
 
 struct SolverSpec {
@@ -56,6 +73,8 @@ struct SolverSpec {
   std::string net_name;
   std::vector<std::string> layer_names, layer_types;  // per learnable blob: owning layer
   std::vector<std::vector<int64_t>> shapes;            // per learnable blob: Blob shape
+  std::vector<int> param_index;                        // per learnable blob: its index within its layer
+  std::vector<SharedParam> shared;                     // every shared use of a named param, in net order
   bool snapshot_hdf5 = false;                          // SolverParameter.snapshot_format (caffe.proto:194-198)
   // SolverParameter
   std::string lr_policy = "fixed";

@@ -246,9 +246,12 @@ def torch_module(name):
     """PyTorch gradient producer with parameters in learnable_params() order.  LRN and BatchNorm layers and every
     conv with a bias followed by ReLU + MAX pool (either order) run on the library's native kernels (layers.py); the
     rest is PyTorch."""
+    return _sequential(NETS[name])
+
+
+def _sequential(net):
     import torch.nn as nn
     from .layers import LRN, BatchNorm, ConvReluMaxPool
-    net = NETS[name]
     c, h, w = net["input"]
     layers = net["layers"]
     mods, flat, skip = [], None, 0
@@ -290,3 +293,63 @@ def torch_module(name):
         elif kind == "sigmoid":
             mods.append(nn.Sigmoid())
     return nn.Sequential(*mods)
+
+
+# caffe-public/examples/siamese/mnist_siamese_train_test.prototxt: a 2x28x28 pair sliced into two LeNet trunks with an
+# extra 2-output InnerProduct `feat`; every param of the second trunk (the `_p` layers) is named after the first's, so
+# the net has LeNet's blobs plus feat's: 431,102 parameters in 10 blobs.
+SIAMESE = dict(input=(1, 28, 28), layers=NETS["lenet"]["layers"] + [("ip", "feat", 2, _W, _B)])
+SIAMESE_PARAM_COUNT = 431102
+
+
+def siamese_module():
+    """The siamese net as one PyTorch module: both halves of a pair go through the same trunk, whose parameters are in
+    learnable_params() order.  forward(pair [N, 2, 28, 28]) -> (feat, feat_p)."""
+    import torch.nn as nn
+
+    class Siamese(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.trunk = _sequential(SIAMESE)
+
+        def forward(self, pair):
+            return self.trunk(pair[:, :1]), self.trunk(pair[:, 1:])
+
+    return Siamese()
+
+
+def contrastive_loss(a, b, sim, margin=1.0, legacy=False, loss_weight=1.0):
+    """Caffe's ContrastiveLoss (contrastive_loss_layer.cpp) with its backward: a similar pair (int(sim) != 0) costs
+    d^2, a dissimilar one max(margin - d^2, 0) (legacy) or max(margin - d, 0)^2, summed over N pairs / (2N).  The
+    gradient of a dissimilar pair divides by d + 1e-4 as Caffe does, so it is not autograd's derivative of the loss."""
+    import torch
+
+    class _Loss(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, a, b):
+            d = a.reshape(a.shape[0], -1) - b.reshape(b.shape[0], -1)
+            dist_sq = (d * d).sum(1)
+            similar = sim.to(torch.int64) != 0
+            if legacy:
+                mdist = margin - dist_sq
+                dissimilar = mdist.clamp(min=0)
+                beta = torch.full_like(dist_sq, -1.0)
+            else:
+                dist = dist_sq.sqrt()
+                mdist = margin - dist
+                dissimilar = mdist.clamp(min=0) ** 2
+                beta = -mdist / (dist + 1e-4)
+            per = torch.where(similar, dist_sq, dissimilar)
+            n = a.shape[0]
+            scale = torch.where(similar, torch.ones_like(beta), torch.where(mdist > 0, beta, torch.zeros_like(beta)))
+            ctx.save_for_backward(scale[:, None] * d)
+            ctx.shapes = (a.shape, b.shape)
+            return loss_weight * (per.sum() / n / 2)
+
+        @staticmethod
+        def backward(ctx, grad):
+            (g,) = ctx.saved_tensors
+            g = g * (grad * loss_weight / g.shape[0])
+            return g.reshape(ctx.shapes[0]), (-g).reshape(ctx.shapes[1])
+
+    return _Loss.apply(a, b)
