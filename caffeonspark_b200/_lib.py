@@ -107,6 +107,9 @@ SYMBOLS = [
     ("cos_lrn_within_backward_bf16", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
     ("cos_bias_relu_maxpool_forward_bf16", _i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     ("cos_bias_relu_maxpool_backward_bf16", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    ("cos_layers_set_reference_kernels", None, [_i]),
+    ("cos_layers_reference_kernels", _i, []),
+    ("cos_pool_fast_path", _i, [_i, _i, _i, _i, _i, _i]),
     ("cos_batch_norm_forward", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),
     ("cos_batch_norm_backward", _i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
     ("cos_batch_norm_forward_bf16", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp]),

@@ -17,6 +17,11 @@
 // output on the upcast inputs rounded once to bf16 (round to nearest even).  The bias, its gradient and the
 // gradient's partials are fp32 for both.
 #include <math.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include <algorithm>
+#include <atomic>
 
 #include "caffe_layers.hpp"
 
@@ -433,6 +438,268 @@ __global__ void bias_grad_kernel(const float* __restrict__ partials, float* __re
   dbias[c] = s;
 }
 
+// ---------------------------------------------------------------- staged bias + ReLU + MAX pool (the fast path)
+//
+// The kernels above gather straight from global memory, one element per thread: 9 x loads per pooled output, and up
+// to 4 index and 4 dy loads plus ~80 instructions of window arithmetic per dx element, which makes the backward
+// issue-bound.  The bias gradient's second pass walks N partials per channel with one thread each, so it waits on N
+// loads in turn.  The staged kernels give the same bits with less work:
+//
+//  * a block copies whole planes into shared memory first (x for the forward; dy and the 1-byte index for the
+//    backward) with 16-byte loads over the planes' aligned body and scalar loads for the head and tail;
+//  * the forward computes each output from shared memory with pool_forward_kernel's expressions;
+//  * the backward (compile-time geometry) computes dx per S x S cell of conv-output elements: the cell's at most
+//    ceil(K/S)^2 windows are read once, and each element adds the dy of the windows that point at it in (ph, pw)
+//    order from +0.f.  The reference adds +0.f for every other window of the element; g is never -0.f, so that leaves
+//    g's bits unchanged and skipping it gives the same g.  g goes to shared memory; then dx is stored coalesced while
+//    each warp re-runs the reduction of one warp of pool_backward_kernel's B-thread block (B depends on H * W only):
+//    the same elements per lane in the same order, the same butterfly, the plane's warp sums in the same order, so
+//    the partials keep their bits;
+//  * the bias gradient stages a 32-channel column of partials per block and sums each channel over n in order.
+//
+// Small planes share a block, so every block has enough elements for its threads.  Both paths' outputs are compared
+// bit for bit by tests/test_gpu_layers_fast_path.py.
+constexpr int kPoolSmemMax = 48 * 1024;  // dynamic + static shared memory a block may take without an opt-in attribute
+constexpr int kPoolFwdThreads = 256;
+constexpr int kPoolFwdSmem = 32 * 1024;  // the forward's target per block
+constexpr int kPoolFwdMaxPlanes = 16;
+constexpr int kPoolBwdThreads = 256;
+constexpr int kPoolBwdSmem = 32 * 1024;  // the backward's target per block
+constexpr int kPoolBwdMaxWarps = 256;    // the reference kernel's warps a staged backward block stands in for
+constexpr int kPoolBwdStatic = (int)sizeof(float) * kPoolBwdMaxWarps;  // warp_sums
+constexpr int kStageSlack = 16;  // elements before a staged region's aligned body (< 16 / sizeof(element))
+
+__device__ __forceinline__ float to_staged(float v) { return v; }
+__device__ __forceinline__ float to_staged(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ uint8_t to_staged(uint8_t v) { return v; }
+
+// 16 bytes of S, converted, to 16-byte aligned shared memory
+__device__ __forceinline__ void put16(uint4 u, float* d, const float*) { *reinterpret_cast<uint4*>(d) = u; }
+__device__ __forceinline__ void put16(uint4 u, uint8_t* d, const uint8_t*) { *reinterpret_cast<uint4*>(d) = u; }
+__device__ __forceinline__ void put16(uint4 u, float* d, const __nv_bfloat16*) {
+  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+  float4 a, b;
+  a.x = __low2float(h[0]), a.y = __high2float(h[0]), a.z = __low2float(h[1]), a.w = __high2float(h[1]);
+  b.x = __low2float(h[2]), b.y = __high2float(h[2]), b.z = __low2float(h[3]), b.w = __high2float(h[3]);
+  reinterpret_cast<float4*>(d)[0] = a;
+  reinterpret_cast<float4*>(d)[1] = b;
+}
+
+// dst[off + i] = src[i] for i < n, by the whole block, off = the number of S elements src lies past a 16-byte
+// boundary: the 16-byte aligned body of src lands on 16-byte aligned dst + off + head (dst must be 16-byte aligned and
+// hold n + kStageSlack elements).  Every global load is coalesced; the body's are 16 bytes wide.  Returns off.
+template <typename S, typename D>
+__device__ __forceinline__ int stage(const S* __restrict__ src, D* __restrict__ dst, int n) {
+  constexpr int V = 16 / (int)sizeof(S);
+  const int off = (int)((reinterpret_cast<uintptr_t>(src) / sizeof(S)) % V);
+  const int head = min(n, (V - off) % V), nv = (n - head) / V, nt = (int)blockDim.x;
+  for (int i = threadIdx.x; i < head; i += nt) dst[off + i] = to_staged(src[i]);
+  const uint4* sv = reinterpret_cast<const uint4*>(src + head);
+  D* dv = dst + off + head;
+  int i = threadIdx.x;
+  for (; i + nt < nv; i += 2 * nt) {  // two 16-byte loads in flight per thread
+    const uint4 a = sv[i], b = sv[i + nt];
+    put16(a, dv + i * V, src);
+    put16(b, dv + (i + nt) * V, src);
+  }
+  if (i < nv) put16(sv[i], dv + i * V, src);
+  for (int j = head + nv * V + threadIdx.x; j < n; j += nt) dst[off + j] = to_staged(src[j]);
+  return off;
+}
+
+__host__ __device__ constexpr int round4(int n) { return (n + 3) & ~3; }
+// shared memory of a staged forward block of G planes, and of a staged backward block (g, then dy, then index)
+int pool_fwd_smem(int G, int hw) { return (int)sizeof(float) * (G * hw + kStageSlack); }
+int pool_bwd_smem(int G, int hw, int phw) {
+  return (int)sizeof(float) * (round4(G * hw) + round4(G * phw + kStageSlack)) + G * phw + kStageSlack;
+}
+
+// One block per G consecutive (n, c) planes: x of the G planes in shared memory, then the G * PH * PW outputs, one
+// per thread in turn, stored coalesced.
+template <typename T, int KERNEL, int STRIDE>
+__global__ void __launch_bounds__(kPoolFwdThreads) pool_forward_staged_kernel(
+    const T* __restrict__ x, const float* __restrict__ bias, T* __restrict__ y, uint8_t* __restrict__ index,
+    unsigned planes, int G, FastDiv fd_pp, FastDiv fd_pw, FastDiv fd_c, int H, int W, int kernel_rt, int stride_rt) {
+  extern __shared__ __align__(16) float smem[];
+  const int kernel = KERNEL ? KERNEL : kernel_rt, stride = STRIDE ? STRIDE : stride_rt;
+  const unsigned plane0 = blockIdx.x * (unsigned)G;
+  const int np = (int)min((unsigned)G, planes - plane0);
+  const int HW = H * W, PHW = (int)fd_pp.d;
+  const float* xs = smem + stage(x + (size_t)plane0 * HW, smem, np * HW);
+  __syncthreads();
+  T* yb = y + (size_t)plane0 * PHW;
+  uint8_t* ib = index + (size_t)plane0 * PHW;
+  for (int o = threadIdx.x; o < np * PHW; o += blockDim.x) {
+    const int gp = (int)fd_pp.div(o), e = o - gp * PHW;
+    const int ph = (int)fd_pw.div(e), pw = e - ph * (int)fd_pw.d;
+    const unsigned plane = plane0 + gp;
+    const float b = bias[plane - fd_c.div(plane) * fd_c.d];
+    const float* xp = xs + gp * HW;
+    const int hs = ph * stride, ws = pw * stride;
+    float vmax = -INFINITY;
+    int pos = 0;
+#pragma unroll
+    for (int dh = 0; dh < (KERNEL ? KERNEL : 15); ++dh) {
+      if (dh >= kernel || hs + dh >= H) break;
+#pragma unroll
+      for (int dw = 0; dw < (KERNEL ? KERNEL : 15); ++dw) {
+        if (dw >= kernel || ws + dw >= W) break;
+        const float v = xp[(hs + dh) * W + ws + dw] + b;
+        if (v > vmax || isnan(v)) {  // as pool_forward_kernel
+          vmax = v;
+          pos = dh * kernel + dw;
+        }
+      }
+    }
+    const bool pass = vmax > 0.f || isnan(vmax);
+    yb[o] = from_f32<T>(pass ? vmax : 0.f);
+    ib[o] = pass ? (uint8_t)pos : kPoolNoGrad;
+  }
+}
+
+// One block per G consecutive planes (see above).  In the second phase each warp stands in for warps of
+// pool_backward_kernel's B-thread blocks in turn: lane l of reference warp vw of a plane sums the elements
+// vw * 32 + l + k * B, then the butterfly, then the plane's warp sums in order.  KERNEL/STRIDE 0: the runtime
+// geometry, whose first phase gathers per element as pool_backward_kernel does.
+template <typename T, int KERNEL, int STRIDE>
+__global__ void __launch_bounds__(kPoolBwdThreads) pool_backward_staged_kernel(
+    const T* __restrict__ dy, const uint8_t* __restrict__ index, T* __restrict__ dx, float* __restrict__ partials,
+    unsigned planes, int G, int B, FastDiv fd_w, FastDiv fd_cells, FastDiv fd_cw, int H, int kernel_rt,
+    int stride_rt, int PH, int PW) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ float warp_sums[kPoolBwdMaxWarps];
+  const int kernel = KERNEL ? KERNEL : kernel_rt, stride = STRIDE ? STRIDE : stride_rt;
+  const int W = (int)fd_w.d, HW = H * W, PHW = PH * PW;
+  float* gs = smem;                                  // g of the G planes
+  float* dys = gs + round4(G * HW);                  // dy of the G planes
+  uint8_t* ids = reinterpret_cast<uint8_t*>(dys + round4(G * PHW + kStageSlack));  // index of the G planes
+  const unsigned plane0 = blockIdx.x * (unsigned)G;
+  const int np = (int)min((unsigned)G, planes - plane0);
+  const float* dyb = dys + stage(dy + (size_t)plane0 * PHW, dys, np * PHW);
+  const uint8_t* ib = ids + stage(index + (size_t)plane0 * PHW, ids, np * PHW);
+  __syncthreads();
+  if (KERNEL) {
+    constexpr int S = STRIDE ? STRIDE : 1, K = KERNEL ? KERNEL : 1;
+    constexpr int NA = (K - 1) / S;  // windows that start before a cell's row (column) and still cover part of it
+    const int cells = (int)fd_cells.d, CW = (int)fd_cw.d;
+    for (int q = threadIdx.x; q < np * cells; q += blockDim.x) {
+      const int gp = (int)fd_cells.div(q), cq = q - gp * cells;
+      const int ci = (int)fd_cw.div(cq), cj = cq - ci * CW;
+      const float* dyp = dyb + gp * PHW;
+      const uint8_t* ip = ib + gp * PHW;
+      // the windows (ci - da, cj - db): index (kPoolNoGrad, which matches no position, outside the pooled plane), dy
+      unsigned id[NA + 1][NA + 1];
+      float v[NA + 1][NA + 1];
+#pragma unroll
+      for (int da = 0; da <= NA; ++da) {
+#pragma unroll
+        for (int db = 0; db <= NA; ++db) {
+          const int ph = ci - da, pw = cj - db;
+          const bool ok = ph >= 0 && pw >= 0 && ph < PH && pw < PW;
+          const int o = ok ? ph * PW + pw : 0;
+          id[da][db] = ok ? ip[o] : kPoolNoGrad;
+          v[da][db] = ok ? dyp[o] : 0.f;
+        }
+      }
+      float* gp_s = gs + gp * HW;
+#pragma unroll
+      for (int r = 0; r < S; ++r) {
+        const int h = ci * S + r;
+        if (h >= H) break;
+#pragma unroll
+        for (int c = 0; c < S; ++c) {
+          const int w = cj * S + c;
+          if (w >= W) break;
+          float g = 0.f;
+#pragma unroll
+          for (int da = NA; da >= 0; --da) {  // ph = ci - da ascending
+#pragma unroll
+            for (int db = NA; db >= 0; --db) {
+              if (r + da * S < K && c + db * S < K) {  // the window covers (h, w): compile-time
+                if (id[da][db] == (unsigned)((r + da * S) * K + c + db * S)) g += v[da][db];
+              }
+            }
+          }
+          gp_s[h * W + w] = g;
+        }
+      }
+    }
+  } else {
+    for (int q = threadIdx.x; q < np * HW; q += blockDim.x) {
+      const int gp = q / HW, e = q - gp * HW;
+      const float* dyp = dyb + gp * PHW;
+      const uint8_t* ip = ib + gp * PHW;
+      const int h = (int)fd_w.div(e), w = e - h * W;
+      const int phs = h < kernel ? 0 : (h - kernel) / stride + 1, phe = min(h / stride + 1, PH);
+      const int pws = w < kernel ? 0 : (w - kernel) / stride + 1, pwe = min(w / stride + 1, PW);
+      float g = 0.f;
+      for (int ph = phs; ph < phe; ++ph) {
+        for (int pw = pws; pw < pwe; ++pw) {
+          if (ip[ph * PW + pw] == (h - ph * stride) * kernel + (w - pw * stride)) g += dyp[ph * PW + pw];
+        }
+      }
+      gs[q] = g;
+    }
+  }
+  __syncthreads();
+  const int VW = B >> 5, lane = (int)threadIdx.x & 31;
+  for (int item = (int)threadIdx.x >> 5; item < np * VW; item += (int)blockDim.x >> 5) {
+    const int gp = item / VW, t = (item - gp * VW) * 32 + lane;
+    const float* g = gs + gp * HW;
+    T* dxp = dx + (size_t)(plane0 + gp) * HW;
+    float part = 0.f;
+    for (int e = t; e < HW; e += B) {
+      dxp[e] = from_f32<T>(g[e]);
+      part += g[e];  // the unrounded g: dbias does not depend on the storage type
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    if (lane == 0) warp_sums[item] = part;
+  }
+  __syncthreads();
+  for (int gp = threadIdx.x; gp < np; gp += blockDim.x) {
+    float s = 0.f;
+    for (int i = 0; i < VW; ++i) s += warp_sums[gp * VW + i];
+    partials[plane0 + gp] = s;
+  }
+}
+
+// dbias[c] = sum over n, in order, of partials[n * C + c], as bias_grad_kernel: each block stages kBiasRows x 32
+// partials at a time (all loads in flight at once) and its first warp adds them, one channel per thread.
+constexpr int kBiasThreads = 256, kBiasRows = 128;
+__global__ void __launch_bounds__(kBiasThreads) bias_grad_staged_kernel(const float* __restrict__ partials,
+                                                                        float* __restrict__ dbias, int N, int C) {
+  __shared__ float ps[kBiasRows][33];
+  const int c = blockIdx.x * 32 + (threadIdx.x & 31), row = threadIdx.x >> 5;
+  float s = 0.f;
+  for (int n0 = 0; n0 < N; n0 += kBiasRows) {
+    const int rows = min(kBiasRows, N - n0);
+#pragma unroll 4
+    for (int r = row; r < rows; r += kBiasThreads / 32)
+      ps[r][threadIdx.x & 31] = c < C ? partials[(size_t)(n0 + r) * C + c] : 0.f;
+    __syncthreads();
+    if (threadIdx.x < 32)
+      for (int r = 0; r < rows; ++r) s += ps[r][threadIdx.x];
+    __syncthreads();
+  }
+  if (threadIdx.x < 32 && c < C) dbias[c] = s;
+}
+
+// the backward's threads per plane (the reference kernel's block size): it depends on the shape only, so the
+// partials' summation order is fixed
+int pool_backward_block(int hw) { return hw >= 256 ? 256 : ((hw + 31) / 32) * 32; }
+
+struct PoolStaged {
+  int fwd_planes, fwd_smem, bwd_planes, bwd_smem;
+  PoolStaged(long long planes, int hw, int phw) {
+    fwd_planes = (int)std::max(1ll, std::min({(long long)kPoolFwdMaxPlanes, planes, kPoolFwdSmem / (hw * 4ll)}));
+    fwd_smem = pool_fwd_smem(fwd_planes, hw);
+    bwd_planes = (int)std::max(1ll, std::min((long long)(kPoolBwdMaxWarps / (pool_backward_block(hw) / 32)), planes));
+    while (bwd_planes > 1 && pool_bwd_smem(bwd_planes, hw, phw) > kPoolBwdSmem) --bwd_planes;
+    bwd_smem = pool_bwd_smem(bwd_planes, hw, phw);
+  }
+};
+
 template <typename T>
 cudaError_t lrn_forward_t(const T* x, T* y, int num, int channels, int height, int width, int local_size, float alpha,
                           float beta, float k, cudaStream_t stream) {
@@ -479,9 +746,21 @@ cudaError_t pool_forward_t(const T* x, const float* bias, T* y, uint8_t* index, 
   const long long total = (long long)num * channels * pooled_h * pooled_w;
   if (total == 0) return cudaSuccess;
   if (total >= (1ll << 31) || (long long)height * width >= (1ll << 31)) return cudaErrorInvalidValue;
+  const FastDiv fpp(pooled_h * pooled_w), fpw(pooled_w), fc(channels);
+  if (!reference_kernels() && pool_fast_path(num, channels, height, width, kernel, stride)) {
+    const long long planes = (long long)num * channels;
+    const PoolStaged p(planes, height * width, pooled_h * pooled_w);
+    const unsigned grid = (unsigned)((planes + p.fwd_planes - 1) / p.fwd_planes);
+    if (kernel == 3 && stride == 2)
+      pool_forward_staged_kernel<T, 3, 2><<<grid, kPoolFwdThreads, p.fwd_smem, stream>>>(
+          x, bias, y, index, (unsigned)planes, p.fwd_planes, fpp, fpw, fc, height, width, kernel, stride);
+    else
+      pool_forward_staged_kernel<T, 0, 0><<<grid, kPoolFwdThreads, p.fwd_smem, stream>>>(
+          x, bias, y, index, (unsigned)planes, p.fwd_planes, fpp, fpw, fc, height, width, kernel, stride);
+    return cudaGetLastError();
+  }
   const int block = 256;
   const unsigned grid = (unsigned)((total + block - 1) / block);
-  const FastDiv fpp(pooled_h * pooled_w), fpw(pooled_w), fc(channels);
   if (kernel == 3 && stride == 2)
     pool_forward_kernel<T, 3, 2><<<grid, block, 0, stream>>>(x, bias, y, index, (unsigned)total, fpp, fpw, fc,
                                                              height, width, kernel, stride);
@@ -499,11 +778,24 @@ cudaError_t pool_backward_t(const T* dy, const uint8_t* index, T* dx, float* dbi
   if (channels == 0) return cudaSuccess;
   if (planes > 0) {
     if (planes >= (1ll << 31) || (long long)height * width >= (1ll << 31)) return cudaErrorInvalidValue;
-    // the block size depends on the shape only, so the partials' summation order is fixed
     const int hw = height * width;
-    const int block = hw >= 256 ? 256 : ((hw + 31) / 32) * 32;
+    const int block = pool_backward_block(hw);
     const FastDiv fw(width);
-    if (kernel == 3 && stride == 2)
+    if (!reference_kernels() && pool_fast_path(num, channels, height, width, kernel, stride)) {
+      const PoolStaged p(planes, hw, pooled_h * pooled_w);
+      const unsigned grid = (unsigned)((planes + p.bwd_planes - 1) / p.bwd_planes);
+      // S x S cells of conv-output elements (compile-time geometry)
+      const int cw = (width + stride - 1) / stride, cells = cw * ((height + stride - 1) / stride);
+      const FastDiv fcells(cells), fcw(cw);
+      if (kernel == 3 && stride == 2)
+        pool_backward_staged_kernel<T, 3, 2><<<grid, kPoolBwdThreads, p.bwd_smem, stream>>>(
+            dy, index, dx, dbias_partials, (unsigned)planes, p.bwd_planes, block, fw, fcells, fcw, height, kernel, stride, pooled_h,
+            pooled_w);
+      else
+        pool_backward_staged_kernel<T, 0, 0><<<grid, kPoolBwdThreads, p.bwd_smem, stream>>>(
+            dy, index, dx, dbias_partials, (unsigned)planes, p.bwd_planes, block, fw, fcells, fcw, height, kernel, stride, pooled_h,
+            pooled_w);
+    } else if (kernel == 3 && stride == 2)
       pool_backward_kernel<T, 3, 2><<<(unsigned)planes, block, 0, stream>>>(dy, index, dx, dbias_partials, fw,
                                                                             height, kernel, stride, pooled_h,
                                                                             pooled_w);
@@ -513,6 +805,10 @@ cudaError_t pool_backward_t(const T* dy, const uint8_t* index, T* dx, float* dbi
                                                                             pooled_w);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
+  }
+  if (!reference_kernels()) {
+    bias_grad_staged_kernel<<<(channels + 31) / 32, kBiasThreads, 0, stream>>>(dbias_partials, dbias, num, channels);
+    return cudaGetLastError();
   }
   bias_grad_kernel<<<(channels + 127) / 128, 128, 0, stream>>>(dbias_partials, dbias, num, channels);
   return cudaGetLastError();
@@ -564,6 +860,33 @@ int pooled_size(int in, int kernel, int stride) {
   int out = (in - kernel + stride - 1) / stride + 1;
   if ((out - 1) * stride >= in) --out;
   return out;
+}
+
+namespace {
+bool reference_from_env() {
+  const char* v = getenv("COS_LAYERS_REFERENCE_KERNELS");
+  return v && *v && strcmp(v, "0") != 0;
+}
+std::atomic<bool> g_reference_kernels{reference_from_env()};
+}  // namespace
+
+void set_reference_kernels(bool on) { g_reference_kernels.store(on, std::memory_order_relaxed); }
+bool reference_kernels() { return g_reference_kernels.load(std::memory_order_relaxed); }
+
+bool pool_fast_path(int num, int channels, int height, int width, int kernel, int stride) {
+  // A 1-wide window shares nothing with its neighbours, so staging buys nothing.  Windows that overlap by more than
+  // two rows (k > s + 2) stay on the per-element kernels: no net here uses them and each element's gather grows as
+  // (k/s)^2.
+  if (num < 1 || channels < 1 || kernel < 2 || stride < 1 || kernel > stride + 2) return false;
+  const int ph = pooled_size(height, kernel, stride), pw = pooled_size(width, kernel, stride);
+  if (ph < 1 || pw < 1) return false;
+  const long long hw = (long long)height * width, phw = (long long)ph * pw, planes = (long long)num * channels;
+  // one plane of x (forward), and of dy and index (backward), must fit a block's shared memory
+  if (hw > kPoolSmemMax || pool_fwd_smem(1, (int)hw) > kPoolSmemMax ||
+      pool_bwd_smem(1, (int)hw, (int)phw) + kPoolBwdStatic > kPoolSmemMax)
+    return false;
+  // plane and output indices are 32-bit
+  return planes * phw < (1ll << 31);
 }
 
 cudaError_t bias_relu_maxpool_forward(const float* x, const float* bias, float* y, uint8_t* index, int num,

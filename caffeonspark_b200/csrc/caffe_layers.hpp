@@ -58,4 +58,13 @@ cudaError_t bias_relu_maxpool_backward(const __nv_bfloat16* dy, const uint8_t* i
                                        int width, int kernel, int stride, int pooled_h, int pooled_w,
                                        cudaStream_t stream);
 
+// The bias+ReLU+max-pool launchers run shared-memory staged kernels where pool_fast_path() holds and the per-element
+// kernels (the reference path) elsewhere; both give the same bits.  set_reference_kernels(true) forces the reference
+// path everywhere, for tests and benchmarks.  Its initial value is COS_LAYERS_REFERENCE_KERNELS (set and not "0":
+// on), read once when the library loads.  It is host state read at launch, so the launchers stay graph capturable.
+void set_reference_kernels(bool on);
+bool reference_kernels();
+// true when the staged pool kernels take this geometry (forward and backward alike); a pure host function
+bool pool_fast_path(int num, int channels, int height, int width, int kernel, int stride);
+
 }  // namespace cosb

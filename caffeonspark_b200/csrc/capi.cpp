@@ -618,6 +618,12 @@ int cos_bias_relu_maxpool_backward_bf16(const uint16_t* dy, const uint8_t* index
                   "cos_bias_relu_maxpool_backward_bf16");
 }
 
+void cos_layers_set_reference_kernels(int on) { cosb::set_reference_kernels(on != 0); }
+int cos_layers_reference_kernels(void) { return cosb::reference_kernels() ? 1 : 0; }
+int cos_pool_fast_path(int num, int channels, int height, int width, int kernel, int stride) {
+  return cosb::pool_fast_path(num, channels, height, width, kernel, stride) ? 1 : 0;
+}
+
 namespace {
 const char* bn_args(const void* a, const void* b, const void* c, const void* save, const void* workspace, int num,
                     int channels, int height, int width, float eps) {

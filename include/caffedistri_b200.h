@@ -353,6 +353,17 @@ COS_API int cos_bias_relu_maxpool_backward_bf16(const uint16_t* dy, const uint8_
                                                 int width, int kernel, int stride, int pooled_height,
                                                 int pooled_width, void* cuda_stream);
 
+/* The bias+ReLU+max-pool calls run shared-memory staged kernels where cos_pool_fast_path() returns 1 and
+ * per-element kernels (the reference path) elsewhere; both write the same bits.  For tests and benchmarks only:
+ * cos_layers_set_reference_kernels(1) makes every later launch in the process take the reference path, 0 (the
+ * default) restores the choice by geometry.  The initial value is COS_LAYERS_REFERENCE_KERNELS from the environment
+ * (set and not "0": on), read once when the library loads.  cos_layers_reference_kernels() returns the setting.
+ * cos_pool_fast_path() is a pure host function of the shape: 1 = staged kernels, 0 = reference path (whatever the
+ * switch says). */
+COS_API void cos_layers_set_reference_kernels(int on);
+COS_API int cos_layers_reference_kernels(void);
+COS_API int cos_pool_fast_path(int num, int channels, int height, int width, int kernel, int stride);
+
 /* Caffe's BatchNorm layer (batch_norm_layer.cpp; DESIGN.md section 13), x contiguous NCHW (a 2-axis
  * num x channels bottom passes height = width = 1).  mean_blob and var_blob have `channels` floats and
  * scale_blob one: the layer's three learnable blobs, usually pointers into data_.  save holds 2 * channels
