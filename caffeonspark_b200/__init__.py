@@ -6,9 +6,9 @@ reference's ``com.yahoo.ml.jcaffe.CaffeNet`` JNI class over the C ABI of
 in the CUDA library; there is no CPU fallback anywhere in this package.
 """
 from .caffenet import (CaffeNet, CosError, PeerAdapter, SolverDesc, chunk, learning_rate, parse_solver,  # noqa: F401
-                       native_producer_plan, read_caffemodel_blob, read_solverstate)
+                       input_transform_plan, native_producer_plan, read_caffemodel_blob, read_solverstate)
 from ._lib import build_library, library_path  # noqa: F401
 
 __all__ = ["CaffeNet", "CosError", "PeerAdapter", "SolverDesc", "chunk", "learning_rate", "parse_solver",
-           "native_producer_plan", "read_caffemodel_blob", "read_solverstate",
+           "input_transform_plan", "native_producer_plan", "read_caffemodel_blob", "read_solverstate",
            "build_library", "library_path"]

@@ -25,6 +25,11 @@ class cos_blob(ctypes.Structure):
                 ("height", ctypes.c_int), ("width", ctypes.c_int)]
 
 
+class cos_raw_blob(ctypes.Structure):
+    _fields_ = [("data", ctypes.c_void_p), ("format", ctypes.c_int), ("num", ctypes.c_int), ("channels", ctypes.c_int),
+                ("height", ctypes.c_int), ("width", ctypes.c_int)]
+
+
 class cos_solver_desc(ctypes.Structure):
     _fields_ = [("nblobs", ctypes.c_int), ("counts", ctypes.POINTER(ctypes.c_int64)),
                 ("lr_mult", ctypes.POINTER(ctypes.c_float)), ("decay_mult", ctypes.POINTER(ctypes.c_float)),
@@ -56,6 +61,9 @@ SYMBOLS = [
     ("cos_net_init", _i, [_vp, _i, _i]),
     ("cos_net_train", _i, [_vp, _i, _c.POINTER(cos_blob), _i]),
     ("cos_net_train_accumulate", _i, [_vp, _i, _c.POINTER(cos_blob), _i, _i]),
+    ("cos_net_train_raw", _i, [_vp, _i, _c.POINTER(cos_raw_blob), _i]),
+    ("cos_data_transform", _i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp, _c.POINTER(_f), _i, _f, _u64, _vp]),
+    ("cos_input_transform_plan", _i, [_cp, _cp, _i]),
     ("cos_net_predict", _i, [_vp, _i, _c.POINTER(cos_blob), _i, _pcp, _i, _c.POINTER(cos_blob)]),
     ("cos_net_validation", _i, [_vp, _c.POINTER(cos_blob), _i]),
     ("cos_net_aggregate_validation_outputs", _i, [_vp]),

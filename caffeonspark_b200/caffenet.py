@@ -9,7 +9,7 @@ the role ``CaffeProcessor`` plays on the Scala side.
 import ctypes
 
 from . import _lib
-from ._lib import FORWARD_BACKWARD_FN, cos_blob, cos_solver_desc
+from ._lib import FORWARD_BACKWARD_FN, cos_blob, cos_raw_blob, cos_solver_desc
 
 
 class CosError(RuntimeError):
@@ -141,6 +141,42 @@ def native_producer_plan(prototxt):
     return buf.value.decode()
 
 
+def input_transform_plan(prototxt):
+    """One line per staged input of a solver or net prototxt: its transform_param (scale, mirror, crop, mean source),
+    with mean files read and checked (host only).  Raises CosError naming the layer."""
+    L = _lib.lib()
+    n = L.cos_input_transform_plan(str(prototxt).encode(), None, 0)
+    if n < 0:
+        raise CosError(_err())
+    buf = ctypes.create_string_buffer(n + 1)
+    L.cos_input_transform_plan(str(prototxt).encode(), buf, n + 1)
+    return buf.value.decode()
+
+
+RAW_F32_NCHW, RAW_U8_NHWC = 0, 1  # COS_RAW_*
+
+
+def _raw_blob_array(data):
+    """list of numpy arrays (uint8 N x H x W x C images, or float32 N x C x H x W) -> cos_raw_blob[]"""
+    import numpy as np
+    blobs = (cos_raw_blob * max(1, len(data)))()
+    keep = []
+    for i, a in enumerate(data):
+        if not isinstance(a, np.ndarray) or a.dtype not in (np.uint8, np.float32):
+            raise CosError("train_raw(): blobs must be numpy uint8 (N x H x W x C) or float32 (N x C x H x W) arrays")
+        a = np.ascontiguousarray(a)
+        if a.dtype == np.uint8:
+            if a.ndim != 4:
+                raise CosError("train_raw(): a uint8 blob must be N x H x W x C")
+            fmt, (n, h, w, c) = RAW_U8_NHWC, a.shape
+        else:
+            fmt, (n, c, h, w) = RAW_F32_NCHW, tuple(a.shape) + (1,) * (4 - a.ndim)
+        keep.append(a)
+        blobs[i].data, blobs[i].format = a.ctypes.data, fmt
+        blobs[i].num, blobs[i].channels, blobs[i].height, blobs[i].width = int(n), int(c), int(h), int(w)
+    return blobs, keep
+
+
 def read_caffemodel_blob(path, layer_name, blob_index=0):
     """One blob of a Caffe .caffemodel (ours or stock Caffe's) as a flat float32 numpy array."""
     import numpy as np
@@ -233,6 +269,9 @@ class CaffeNet:
         if self._h:
             self._L.cos_net_deallocate(self._h)
             self._h = ctypes.c_void_p()
+        # the C side no longer calls the producer: drop it, so that a producer holding this net (and its CUDA
+        # graphs) is freed when its last user lets go, not by a later cyclic garbage collection
+        self._fb_keep = None
 
     def __del__(self):
         try:
@@ -282,6 +321,19 @@ class CaffeNet:
             raise CosError("train_accumulate(): every micro-batch must have the same number of blobs")
         blobs, keep = _blob_array([b for g in groups for b in g])
         ok = bool(self._L.cos_net_train_accumulate(self._h, solver_index, blobs, len(groups[0]), len(groups)))
+        del keep
+        return ok
+
+    def train_raw(self, solver_index, arrays):
+        """One Solver::Step on untransformed host arrays, one per staged input: each input's transform_param (crop,
+        mirror, mean, scale) runs on the device.  uint8 N x H x W x C images draw their crop and mirror per image,
+        a float32 N x C x H x W blob once per batch; an input without a transform_param (the label) is float32.
+        Raises CosError for a dtype other than uint8 / float32; returns False when the step is refused or fails."""
+        if arrays is None:
+            self._L.cos_net_train_raw(self._h, solver_index, None, 0)
+            raise CosError(_err())
+        blobs, keep = _raw_blob_array(list(arrays))
+        ok = bool(self._L.cos_net_train_raw(self._h, solver_index, blobs, len(keep)))
         del keep
         return ok
 

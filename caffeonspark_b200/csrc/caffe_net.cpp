@@ -96,11 +96,15 @@ CaffeNet::~CaffeNet() {
     for (InputStage& st : stage_) {
       for (void* p : st.dev)
         if (p) cudaFree(p);
+      for (void* p : st.raw)
+        if (p) cudaFree(p);
       if (st.copied) cudaEventDestroy(st.copied);
       if (st.consumed) cudaEventDestroy(st.consumed);
     }
     for (cudaEvent_t e : loss_ev_)
       if (e) cudaEventDestroy(e);
+    for (float* p : mean_dev_)
+      if (p) cudaFree(p);
     if (copy_stream_) cudaStreamDestroy(copy_stream_);
     if (seg_end_) cudaFree(seg_end_);
     if (seg_lr_) cudaFree(seg_lr_);
@@ -505,7 +509,7 @@ bool CaffeNet::train(int solver_index, const cos_blob* data, int ndata, std::str
     *err = "data is NULL";  // JniCaffeNet.cpp:391-395
     return false;
   }
-  return run_step(solver_index, data, ndata, 1, err);
+  return run_step(solver_index, data, ndata, 1, nullptr, err);
 }
 
 // Gradient accumulation over distinct micro-batches: pass i of the step reads data[i*ndata .. (i+1)*ndata).
@@ -527,10 +531,136 @@ bool CaffeNet::train_accumulate(int solver_index, const cos_blob* data, int ndat
            std::to_string(spec_.iter_size) + ")";
     return false;
   }
-  return run_step(solver_index, data, ndata, passes, err);
+  return run_step(solver_index, data, ndata, passes, nullptr, err);
 }
 
-bool CaffeNet::run_step(int solver_index, const cos_blob* data, int ndata, int groups, std::string* err) {
+bool CaffeNet::train_raw(int solver_index, const cos_raw_blob* data, int ndata, std::string* err) {
+  if (solver_index != 0) {
+    *err = "solver_index must be 0";
+    return false;
+  }
+  if (!data) {
+    *err = "data is NULL";
+    return false;
+  }
+  if (!check_raw(data, ndata, err)) return false;
+  return run_step(solver_index, nullptr, ndata, 1, data, err);
+}
+
+// DataTransformer's checks (data_transformer.cpp: Transform(cv::Mat) and Transform(Blob*)), once the first call has
+// read the mean files; then every call must have the first call's shapes, which size the raw staging sets.
+bool CaffeNet::check_raw(const cos_raw_blob* data, int ndata, std::string* err) {
+  if (spec_.solver_file.empty()) {
+    *err = "train_raw: this net was allocated from a layout descriptor, which has no data layer and no "
+           "transform_param; allocate it from a prototxt";
+    return false;
+  }
+  const bool first = raw_shapes_.empty();
+  std::vector<InputTransform> resolved;
+  if (first && !resolve_input_transforms(spec_, &resolved, err)) return false;
+  const std::vector<InputTransform>& tr = first ? resolved : transforms_;
+  if (ndata != static_cast<int>(tr.size())) {
+    *err = "train_raw: " + std::to_string(ndata) + " blobs for the net's " + std::to_string(tr.size()) +
+           " staged inputs";
+    return false;
+  }
+  for (int i = 0; i < ndata; ++i) {
+    const cos_raw_blob& b = data[i];
+    const InputTransform& t = tr[i];
+    const std::vector<int64_t>& top = t.input.shape;
+    auto refuse = [&](const std::string& why) {
+      *err = "train_raw: layer '" + t.input.layer + "' (" + t.input.type + "), top '" + t.input.top + "': " + why;
+      return false;
+    };
+    if (!b.data) return refuse("data[" + std::to_string(i) + "] is NULL");
+    if (b.format != kRawF32Nchw && b.format != kRawU8Nhwc)
+      return refuse("format " + std::to_string(b.format) + " is neither COS_RAW_F32_NCHW nor COS_RAW_U8_NHWC");
+    if (b.num < 1 || b.channels < 1 || b.height < 1 || b.width < 1)
+      return refuse("num, channels, height and width must be positive");
+    const int64_t count = static_cast<int64_t>(b.num) * b.channels * b.height * b.width;
+    if (!t.active()) {
+      int64_t want = 1;
+      for (int64_t d : top) want *= d;
+      if (b.format != kRawF32Nchw || count != want)
+        return refuse("an input without transform_param must be COS_RAW_F32_NCHW with the top's " +
+                      std::to_string(want) + " elements");
+    } else {
+      const TransformSpec& ts = t.input.transform;
+      if (b.num != top[0])
+        return refuse("raw num " + std::to_string(b.num) + " != the top's " + std::to_string(top[0]));
+      if (b.channels != top[1])
+        return refuse("Check failed: channels == img_channels (" + std::to_string(top[1]) + " vs. " +
+                      std::to_string(b.channels) + ")");
+      if (ts.crop_size) {
+        if (b.height < ts.crop_size || b.width < ts.crop_size)
+          return refuse("Check failed: img_height >= crop_size (" + std::to_string(b.height) + "x" +
+                        std::to_string(b.width) + " vs. " + std::to_string(ts.crop_size) + ")");
+      } else if (b.height != top[2] || b.width != top[3]) {
+        return refuse("Check failed: img_height == height (raw " + std::to_string(b.height) + "x" +
+                      std::to_string(b.width) + ", top " + std::to_string(top[2]) + "x" + std::to_string(top[3]) + ")");
+      }
+      if (!t.mean.empty() && (b.height != t.mean_shape[1] || b.width != t.mean_shape[2]))
+        return refuse("Check failed: img_height == data_mean_.height() (raw " + std::to_string(b.height) + "x" +
+                      std::to_string(b.width) + ", mean " + std::to_string(t.mean_shape[1]) + "x" +
+                      std::to_string(t.mean_shape[2]) + ")");
+      const int64_t wo = ts.crop_size ? ts.crop_size : b.width;
+      if (b.format == kRawU8Nhwc && wo * b.channels > kMaxTransformRowBytes)
+        return refuse("an 8-bit crop row of " + std::to_string(wo * b.channels) + " bytes exceeds " +
+                      std::to_string(kMaxTransformRowBytes));
+    }
+    if (!first) {
+      const cos_raw_blob& s = raw_shapes_[i];
+      if (b.format != s.format || b.num != s.num || b.channels != s.channels || b.height != s.height ||
+          b.width != s.width)
+        return refuse("raw shape " + std::to_string(b.num) + "x" + std::to_string(b.channels) + "x" +
+                      std::to_string(b.height) + "x" + std::to_string(b.width) + " (format " +
+                      std::to_string(b.format) + ") differs from the first call's " + std::to_string(s.num) + "x" +
+                      std::to_string(s.channels) + "x" + std::to_string(s.height) + "x" + std::to_string(s.width) +
+                      " (format " + std::to_string(s.format) + ")");
+    }
+  }
+  if (!first) return true;
+  // the means go to this net's device once; the first call's shapes are kept
+  COS_RT(cudaSetDevice(device_));
+  std::vector<float*> means(resolved.size(), nullptr);
+  for (size_t i = 0; i < resolved.size(); ++i) {
+    if (resolved[i].mean.empty()) continue;
+    const size_t n = resolved[i].mean.size() * sizeof(float);
+    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&means[i]), n);
+    if (e == cudaSuccess) e = cudaMemcpy(means[i], resolved[i].mean.data(), n, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+      for (float* p : means)
+        if (p) cudaFree(p);
+      *err = rt_err("train_raw: mean upload", e);
+      return false;
+    }
+  }
+  transforms_ = std::move(resolved);
+  mean_dev_ = std::move(means);
+  raw_shapes_.assign(data, data + ndata);
+  for (cos_raw_blob& s : raw_shapes_) s.data = nullptr;
+  return true;
+}
+
+// Pass `pass` of this step: every input with a transform_param, from stage `stage`'s raw set into its fp32 set.
+bool CaffeNet::transform_inputs(int stage, const cos_raw_blob* raw, int pass, std::string* err) {
+  InputStage& st = stage_[stage];
+  for (size_t i = 0; i < transforms_.size(); ++i) {
+    const InputTransform& t = transforms_[i];
+    if (!t.active()) continue;
+    const TransformSpec& ts = t.input.transform;
+    const cos_raw_blob& b = raw[i];
+    const uint64_t key = transform_key(spec_.random_seed, rank_, static_cast<int>(i), iter_, pass);
+    COS_RT(launch_data_transform(st.raw[i], b.format, b.num, b.channels, b.height, b.width,
+                                 static_cast<float*>(st.dev[i]), static_cast<int>(ts.crop_size), ts.mirror,
+                                 mean_dev_[i], ts.mean_values.data(), static_cast<int>(ts.mean_values.size()),
+                                 ts.scale, key, stream_));
+  }
+  return true;
+}
+
+bool CaffeNet::run_step(int solver_index, const cos_blob* data, int ndata, int groups, const cos_raw_blob* raw,
+                        std::string* err) {
   if (!fb_fn_) {
     *err = "train: no gradient producer registered (cos_net_set_forward_backward); Net::ForwardBackward is "
            "outside this library";
@@ -540,31 +670,52 @@ bool CaffeNet::run_step(int solver_index, const cos_blob* data, int ndata, int g
   if (!check_status(err)) return false;  // a device-side error of an earlier (pipelined) step surfaces here
   // MemoryInputAdapter::feed (MemoryInputAdapter.cpp:24-32) equivalent: stage the host blobs on the device.
   // Stage k was last read by step t-2: its H2D may only start once that step is done (device-side wait).
-  InputStage& st = stage_[stage_idx_];
+  const int stage = stage_idx_;
+  InputStage& st = stage_[stage];
   const int nblobs = ndata * groups;
   if (static_cast<int>(st.dev.size()) < nblobs) {
     st.dev.resize(nblobs, nullptr);
     st.bytes.resize(nblobs, 0);
+    st.raw.resize(nblobs, nullptr);
+    st.raw_bytes.resize(nblobs, 0);
   }
+  auto reserve = [&](void** buf, size_t* have, size_t n) {
+    if (n > *have) {
+      if (*buf) {
+        COS_RT(cudaStreamSynchronize(stream_));  // an earlier step may still read the old buffer
+        cudaFree(*buf);
+      }
+      *buf = nullptr;
+      COS_RT(cudaMalloc(buf, n));
+      *have = n;
+    }
+    return true;
+  };
   if (st.consumed_valid) COS_RT(cudaStreamWaitEvent(copy_stream_, st.consumed, 0));
   std::vector<cos_blob> dev_blobs(nblobs);
   for (int i = 0; i < nblobs; ++i) {
-    if (!data[i].data) {
+    // the producer sees the fp32 set; a raw input with a transform_param lands in the raw set, and each pass
+    // transforms it into the fp32 set (transform_inputs)
+    const bool transformed = raw && transforms_[i].active();
+    const void* host = raw ? raw[i].data : data[i].data;
+    cos_blob b = raw ? cos_blob{nullptr, raw[i].num, raw[i].channels, raw[i].height, raw[i].width} : data[i];
+    if (!host) {
       *err = "data[" + std::to_string(i) + "] is NULL";
       return false;
     }
-    size_t n = static_cast<size_t>(data[i].num) * data[i].channels * data[i].height * data[i].width * sizeof(float);
-    if (n > st.bytes[i]) {
-      if (st.dev[i]) {
-        COS_RT(cudaStreamSynchronize(stream_));  // an earlier step may still read the old buffer
-        cudaFree(st.dev[i]);
-      }
-      st.dev[i] = nullptr;
-      COS_RT(cudaMalloc(&st.dev[i], n));
-      st.bytes[i] = n;
+    const size_t elem = raw && raw[i].format == kRawU8Nhwc ? 1 : sizeof(float);
+    size_t n = static_cast<size_t>(b.num) * b.channels * b.height * b.width * elem;
+    if (transformed) {
+      const std::vector<int64_t>& top = transforms_[i].input.shape;
+      b.height = static_cast<int>(top[2]), b.width = static_cast<int>(top[3]);
+      if (!reserve(&st.dev[i], &st.bytes[i], static_cast<size_t>(b.num) * b.channels * b.height * b.width * 4))
+        return false;
+      if (!reserve(&st.raw[i], &st.raw_bytes[i], n)) return false;
+    } else if (!reserve(&st.dev[i], &st.bytes[i], n)) {
+      return false;
     }
-    COS_RT(cudaMemcpyAsync(st.dev[i], data[i].data, n, cudaMemcpyHostToDevice, copy_stream_));
-    dev_blobs[i] = data[i];
+    COS_RT(cudaMemcpyAsync(transformed ? st.raw[i] : st.dev[i], host, n, cudaMemcpyHostToDevice, copy_stream_));
+    dev_blobs[i] = b;
     dev_blobs[i].data = static_cast<const float*>(st.dev[i]);
   }
   COS_RT(cudaEventRecord(st.copied, copy_stream_));
@@ -572,6 +723,7 @@ bool CaffeNet::run_step(int solver_index, const cos_blob* data, int ndata, int g
   // solver.cpp:219-224: for i < iter_size: loss += ForwardBackward(); the producers accumulate into diff_
   const int passes = spec_.iter_size;
   for (int i = 0; i < passes; ++i) {
+    if (raw && !transform_inputs(stage, raw, i, err)) return false;
     const cos_blob* in = dev_blobs.data() + static_cast<size_t>(groups == 1 ? 0 : i) * ndata;
     float* loss = passes > 1 ? loss_slots_ + i : loss_dev_;
     int rc = fb_fn_(fb_user_, solver_index_, in, ndata, loss, stream_);

@@ -21,6 +21,7 @@
 
 #include "../../include/caffedistri_b200.h"
 #include "caffe_proto_io.hpp"
+#include "data_transform.hpp"
 #include "fused_sync_sgd.hpp"
 #include "peer_adapter.hpp"
 #include "peer_memory.hpp"
@@ -58,6 +59,8 @@ class CaffeNet {
   bool train(int solver_index, const cos_blob* data, int ndata, std::string* err);
   // one step over `passes` (== iter_size) groups of ndata blobs, one distinct micro-batch per pass
   bool train_accumulate(int solver_index, const cos_blob* data, int ndata, int passes, std::string* err);
+  // train() on untransformed blobs: each staged input's transform_param runs on the device (data_transform.hpp)
+  bool train_raw(int solver_index, const cos_raw_blob* data, int ndata, std::string* err);
   virtual int snapshot(std::string* err);
   std::string snapshot_filename(int iter, bool is_state) const;  // Solver::SnapshotFilename
   std::vector<BlobView> blob_views(const float* flat) const;  // the learnable blobs (owners), in order
@@ -112,8 +115,12 @@ class CaffeNet {
   bool launch(int mode, cudaStream_t stream, std::string* err);
   bool check_status(std::string* err);
   // Solver::Step: stage `groups` x ndata host blobs, run the producer iter_size times (pass i reads group i, or
-  // group 0 when groups == 1), the loss mean, then sync_step
-  bool run_step(int solver_index, const cos_blob* data, int ndata, int groups, std::string* err);
+  // group 0 when groups == 1), the loss mean, then sync_step.  With `raw` (train_raw, groups 1) the blobs come from
+  // there instead of `data`, and every pass first transforms the inputs that have a transform_param.
+  bool run_step(int solver_index, const cos_blob* data, int ndata, int groups, const cos_raw_blob* raw,
+                std::string* err);
+  bool check_raw(const cos_raw_blob* data, int ndata, std::string* err);  // train_raw's argument checks
+  bool transform_inputs(int stage, const cos_raw_blob* raw, int pass, std::string* err);
   int resolved_algo() const;
   int resolved_kernel() const;
 
@@ -199,8 +206,10 @@ class CaffeNet {
   // copy of batch t runs on its own copy stream while the compute stream still works on batch t-1; train()
   // returns as soon as ITS batch has left host memory (the caller recycles the blobs after train() returns).
   struct InputStage {
-    std::vector<void*> dev;
+    std::vector<void*> dev;            // the fp32 inputs the producer reads
     std::vector<size_t> bytes;
+    std::vector<void*> raw;            // train_raw: the untransformed inputs that have a transform_param
+    std::vector<size_t> raw_bytes;
     cudaEvent_t copied = nullptr;    // H2D of this stage finished
     cudaEvent_t consumed = nullptr;  // the step that read this stage finished
     bool consumed_valid = false;
@@ -212,6 +221,10 @@ class CaffeNet {
   bool loss_pending_[2] = {false, false};
   int loss_idx_ = 0;
   int opt_train_pipeline_ = 1;      // 0: train() returns only after the whole Step finished (reference behaviour)
+  // train_raw: the staged inputs' transforms with their means on this device, and the first call's raw shapes
+  std::vector<InputTransform> transforms_;
+  std::vector<float*> mean_dev_;
+  std::vector<cos_raw_blob> raw_shapes_;
   void harvest_losses(bool wait);
   std::vector<std::string> addr_store_;
   std::vector<const char*> addr_cstrs_;

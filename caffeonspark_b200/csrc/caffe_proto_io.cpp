@@ -452,4 +452,18 @@ bool read_solverstate(const std::string& path, int* iter, int* current_step, std
   return true;
 }
 
+bool read_blobproto(const std::string& path, ParsedBlob* blob, std::string* err) {
+  std::vector<unsigned char> buf;
+  if (!slurp(path, &buf, err)) return false;
+  *blob = ParsedBlob();
+  int64_t n = 1;
+  const bool parsed = parse_blob(Reader{buf.data(), buf.data() + buf.size(), true}, blob);
+  for (int64_t d : blob->shape) n = d < 0 ? -1 : n * d;
+  if (!parsed || blob->shape.empty() || n != static_cast<int64_t>(blob->data.size())) {
+    *err = "'" + path + "' is not a BlobProto with float data matching its shape";
+    return false;
+  }
+  return true;
+}
+
 }  // namespace cosb

@@ -63,6 +63,8 @@ bool write_solverstate_h5(const std::string& path, int iter, int current_step, c
                           const std::vector<BlobView>& history, std::string* err);
 bool read_solverstate(const std::string& path, int* iter, int* current_step, std::string* learned_net,
                       std::vector<ParsedBlob>* history, std::string* err);
+// A file holding one BlobProto (a mean.binaryproto): shape from `shape` or the legacy num/channels/height/width.
+bool read_blobproto(const std::string& path, ParsedBlob* blob, std::string* err);
 
 }  // namespace cosb
 #endif

@@ -238,6 +238,34 @@ int cos_net_train_accumulate(cos_net* net, int solver_index, const cos_blob* dat
   })
 }
 
+int cos_net_train_raw(cos_net* net, int solver_index, const cos_raw_blob* data, int ndata) {
+  COS_GUARD(0, {
+    if (!net) return fail("net is NULL");
+    if (solver_index < 0) return fail("invalid solver_index");
+    if (!data) return fail("data is NULL");
+    std::string err;
+    CaffeNet* r = R(net, solver_index);
+    if (!r) return fail("invalid solver_index");
+    if (!r->train_raw(0, data, ndata, &err)) return fail(err);
+    return 1;
+  })
+}
+
+int cos_input_transform_plan(const char* prototxt, char* buf, int cap) {
+  COS_GUARD(-1, {
+    if (!prototxt) return fail("prototxt is NULL", -1);
+    SolverSpec s;
+    std::vector<cosb::NetLayer> layers;
+    std::vector<cosb::InputTransform> inputs;
+    std::string err;
+    if (!cosb::parse_train_net(prototxt, &s, &layers, &err) || !cosb::resolve_input_transforms(s, &inputs, &err))
+      return fail(err, -1);
+    const std::string t = cosb::input_transform_plan_text(inputs);
+    if (buf && cap > static_cast<int>(t.size())) memcpy(buf, t.c_str(), t.size() + 1);
+    return static_cast<int>(t.size());
+  })
+}
+
 int cos_net_predict(cos_net*, int, const cos_blob*, int, const char* const*, int, cos_blob*) {
   return fail("predict: forward-only inference is not part of the gradient-sync library", -1);
 }
@@ -524,6 +552,20 @@ int cos_lrn_within_backward(const float* x, const float* dy, float* dx, int num,
   return launched(cosb::lrn_within_backward(x, dy, dx, num, channels, height, width, local_size, alpha, beta,
                                             static_cast<cudaStream_t>(cuda_stream)),
                   "cos_lrn_within_backward");
+}
+
+int cos_data_transform(const void* in, int format, int num, int channels, int height, int width, float* out,
+                       int crop_size, int mirror, const float* mean, const float* mean_values, int nmean, float scale,
+                       uint64_t key, void* cuda_stream) {
+  COS_GUARD(0, {
+    const std::string e = cosb::check_transform_args(in, format, num, channels, height, width, out, crop_size, mean,
+                                                     mean_values, nmean);
+    if (!e.empty()) return fail("cos_data_transform: " + e);
+    return launched(cosb::launch_data_transform(in, format, num, channels, height, width, out, crop_size, mirror != 0,
+                                                mean, mean_values, nmean, scale, key,
+                                                static_cast<cudaStream_t>(cuda_stream)),
+                    "cos_data_transform");
+  })
 }
 
 int cos_bias_relu_maxpool_forward(const float* x, const float* bias, float* y, uint8_t* index, int num, int channels,

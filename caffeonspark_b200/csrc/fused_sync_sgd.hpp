@@ -18,6 +18,13 @@ constexpr int kMaxCtas = 2048;
 // SMs of the target GPU (H100 SXM): fallback where the device cannot be queried, and the push kernel's grid cap,
 // which must be the same number on every rank.
 constexpr int kTargetSms = 132;
+
+// splitmix64 finaliser: the seeded device fill (cos_net_fill) and the input transform's draws hash counters with it
+__host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ULL;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebULL;
+  return z ^ (z >> 31);
+}
 // Flag region at the start of every rank's arena: three arrays [kMaxCtas][kMaxRanks]
 // of 32-bit words: epochs A = "gradients ready" and B = "reads done + weights landed", and C = per-CTA
 // progress of an owner's reduce phase (NVLS kernel: lets the peers zero diff_ behind the owner's reads).

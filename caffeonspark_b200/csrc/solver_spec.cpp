@@ -280,10 +280,34 @@ FillerSpec filler(const Node* f) {
 
 std::vector<int64_t> to64(const Shape& s) { return std::vector<int64_t>(s.begin(), s.end()); }
 
+// TransformationParameter; force_color / force_gray only matter for decoding, which happens before the library.
+TransformSpec transform(const Node* t, const std::string& net_file) {
+  TransformSpec s;
+  if (!t || !t->is_msg) return s;
+  s.present = true;
+  s.scale = static_cast<float>(t->num("scale", 1.0));
+  s.mirror = t->boolean("mirror", false);
+  s.crop_size = t->integer("crop_size", 0);
+  s.mean_file = t->str("mean_file", "");
+  s.net_file = net_file;
+  for (const Node* v : t->all("mean_value")) s.mean_values.push_back(static_cast<float>(atof(v->value.c_str())));
+  return s;
+}
+
 // `out` (optional) receives every TRAIN-phase layer with its blob shapes and the parameters the native producer reads.
-bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, std::string* err) {
+// `net_file` is the prototxt the net was read from ("" for text).
+bool net_layout(const Node& net, const std::string& net_file, SolverSpec* spec, std::vector<NetLayer>* out,
+                std::string* err) {
   std::map<std::string, Shape> blobs;
   if (out) out->clear();
+  spec->inputs.clear();
+  auto staged = [&](const std::string& layer, const std::string& type, const std::string& top, const Shape& s,
+                    const Node* t) {
+    StagedInput in;
+    in.layer = layer, in.type = type, in.top = top, in.shape = to64(s);
+    in.transform = transform(t, net_file);
+    spec->inputs.push_back(in);
+  };
   spec->counts.clear();
   spec->lr_mult.clear();
   spec->decay_mult.clear();
@@ -306,6 +330,7 @@ bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, s
       if (i < shapes.size()) for (const Node* d : shapes[i]->all("dim")) s.push_back(atol(d->value.c_str()));
       else for (size_t k = 4 * i; k < 4 * i + 4 && k < dims.size(); ++k) s.push_back(atol(dims[k]->value.c_str()));
       blobs[inputs[i]->value] = s;
+      staged("input", "Input", inputs[i]->value, s, nullptr);
     }
     if (out && !inputs.empty()) {
       NetLayer rec;
@@ -359,6 +384,8 @@ bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, s
       Shape s{p->integer("batch_size", 0), p->integer("channels", 0), p->integer("height", 0), p->integer("width", 0)};
       if (!tops.empty()) blobs[tops[0]] = s;
       if (tops.size() > 1) blobs[tops[1]] = Shape{s[0]};
+      for (size_t i = 0; i < tops.size(); ++i)  // the transform applies to the data, never to the label
+        staged(name, type, tops[i], blobs[tops[i]], i == 0 ? L->first("transform_param") : nullptr);
       if (first_data) { spec->batch_size = static_cast<int>(s[0]); spec->input_shape.assign(s.begin(), s.end()); first_data = false; }
     } else if (type == "CoSData") {
       const Node* p = L->first("cos_data_param");
@@ -377,6 +404,7 @@ bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, s
           for (long a = 0; a < axes && a < 3; ++a) s.push_back(full[a] ? full[a] : 1);
         }
         blobs[tops[i]] = s;
+        staged(name, type, tops[i], s, i < tb.size() ? tb[i]->first("transform_param") : nullptr);
         if (first_data && i == 0) { spec->batch_size = static_cast<int>(batch); spec->input_shape.assign(s.begin(), s.end()); first_data = false; }
       }
     } else if (type == "Input") {
@@ -387,6 +415,7 @@ bool net_layout(const Node& net, SolverSpec* spec, std::vector<NetLayer>* out, s
         const Node* sh = shapes.empty() ? nullptr : shapes[std::min(i, shapes.size() - 1)];
         if (sh) for (const Node* d : sh->all("dim")) s.push_back(atol(d->value.c_str()));
         blobs[tops[i]] = s;
+        staged(name, type, tops[i], s, nullptr);
         if (first_data && i == 0 && !s.empty()) { spec->batch_size = static_cast<int>(s[0]); spec->input_shape.assign(s.begin(), s.end()); first_data = false; }
       }
     } else if (type == "Convolution" || type == "Deconvolution") {
@@ -676,7 +705,18 @@ bool parse_net_prototxt_text(const std::string& text, SolverSpec* spec, std::str
   Node net;
   TextParser tp(text);
   if (!tp.parse(&net, err)) return false;
-  return net_layout(net, spec, nullptr, err);
+  return net_layout(net, "", spec, nullptr, err);
+}
+
+std::string find_relative_file(const std::string& path, const std::string& relative_to) {
+  auto opens = [](const std::string& p) { return static_cast<bool>(std::ifstream(p.c_str(), std::ios::binary)); };
+  if (opens(path)) return path;
+  size_t slash = relative_to.find_last_of('/');
+  std::string dir = slash == std::string::npos ? "." : relative_to.substr(0, slash);
+  if (opens(dir + "/" + path)) return dir + "/" + path;
+  size_t s2 = path.find_last_of('/');
+  if (s2 != std::string::npos && opens(dir + "/" + path.substr(s2 + 1))) return dir + "/" + path.substr(s2 + 1);
+  return "";
 }
 
 bool parse_train_net(const std::string& path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err) {
@@ -689,7 +729,7 @@ bool parse_train_net(const std::string& path, SolverSpec* spec, std::vector<NetL
   TextParser tp(text);
   if (!tp.parse(&top, err)) return false;
   if (!top.all("layer").empty() || !top.all("layers").empty() || !top.all("input").empty())
-    return net_layout(top, spec, layers, err);
+    return net_layout(top, path, spec, layers, err);
   return parse_solver(path, spec, layers, err);
 }
 
@@ -767,7 +807,7 @@ bool parse_solver(const std::string& solver_path, SolverSpec* spec, std::vector<
   }
   // locate the net definition
   if (const Node* inl = s.first("net_param") ? s.first("net_param") : s.first("train_net_param")) {
-    return net_layout(*inl, spec, layers, err) && check_solver_layout(*spec, err);
+    return net_layout(*inl, solver_path, spec, layers, err) && check_solver_layout(*spec, err);
   }
   std::string net_path = s.str("net", "");
   if (net_path.empty()) net_path = s.str("train_net", "");
@@ -775,25 +815,17 @@ bool parse_solver(const std::string& solver_path, SolverSpec* spec, std::vector<
     *err = "solver file names no net (net / train_net / net_param)";
     return false;
   }
+  // as given, then relative to the solver file's directory, then by basename there
+  const std::string net_file = find_relative_file(net_path, solver_path);
   std::string net_text;
-  bool ok = read_file(net_path, &net_text);
-  if (!ok) {  // relative to the solver file's directory, then by basename there
-    size_t slash = solver_path.find_last_of('/');
-    std::string dir = slash == std::string::npos ? "." : solver_path.substr(0, slash);
-    ok = read_file(dir + "/" + net_path, &net_text);
-    if (!ok) {
-      size_t s2 = net_path.find_last_of('/');
-      if (s2 != std::string::npos) ok = read_file(dir + "/" + net_path.substr(s2 + 1), &net_text);
-    }
-  }
-  if (!ok) {
+  if (net_file.empty() || !read_file(net_file, &net_text)) {
     *err = "cannot read net file '" + net_path + "' named by '" + solver_path + "'";
     return false;
   }
   Node net;
   TextParser np(net_text);
   if (!np.parse(&net, err)) return false;
-  return net_layout(net, spec, layers, err) && check_solver_layout(*spec, err);
+  return net_layout(net, net_file, spec, layers, err) && check_solver_layout(*spec, err);
 }
 }  // namespace
 

@@ -64,6 +64,25 @@ struct SharedParam {
   int position = 0;     // learnable blobs before it in net order: where Net::ToProto writes it among the owners
 };
 
+// TransformationParameter (caffe.proto) of one staged input: what Caffe's DataTransformer applies in TRAIN.  Only the
+// path of a mean file is recorded here; data_transform.hpp reads it.
+struct TransformSpec {
+  bool present = false;  // the top has a transform_param
+  float scale = 1.f;
+  bool mirror = false;
+  int64_t crop_size = 0;
+  std::string mean_file;  // as written in the prototxt ("" = none)
+  std::string net_file;   // the prototxt it was written in: a relative mean_file is also looked for next to it
+  std::vector<float> mean_values;
+};
+
+// One staged input: a top of a data layer (MemoryData, CoSData, Input), in the order the producer receives them.
+struct StagedInput {
+  std::string layer, type, top;
+  std::vector<int64_t> shape;
+  TransformSpec transform;  // MemoryData: top 0 only; CoSData: each top's own
+};
+
 struct SolverSpec {
   // learnable blobs in learnable_params() order
   std::vector<int64_t> counts;
@@ -97,6 +116,7 @@ struct SolverSpec {
   // training input layer
   int batch_size = 0;
   std::vector<int> input_shape;  // N,C,H,W of the first top of the data layer
+  std::vector<StagedInput> inputs;  // every staged input with its transform_param (empty for a descriptor)
   // this library's extensions
   int grad_dtype = 0;  // COS_GRAD_FP32 / COS_GRAD_BF16
   int init_iter = 0;
@@ -130,6 +150,9 @@ bool parse_net_prototxt_text(const std::string& text, SolverSpec* spec, std::str
 // A solver prototxt (its net is read as parse_solver_prototxt reads it) or a net prototxt, told apart by whether the
 // file has top-level layers: fills spec (solver fields only for a solver file) and the TRAIN-phase layer list.
 bool parse_train_net(const std::string& path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err);
+// The file `path` names, looked for as the solver's net: path is: as given, then relative to the directory of
+// `relative_to`, then by its basename in that directory.  "" when none can be opened.
+std::string find_relative_file(const std::string& path, const std::string& relative_to);
 
 }  // namespace cosb
 #endif

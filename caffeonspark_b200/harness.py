@@ -13,6 +13,7 @@ caffe-public solver.cpp:221-223), reduced to what the benchmark needs.
 PyTorch here is plumbing (device tensors, streams, process group); the sync
 path itself is entirely inside libcaffedistri_b200.so.
 """
+import gc
 import os
 
 import torch
@@ -99,9 +100,18 @@ class TorchProducer:
                 try:
                     ext.synchronize()
                     g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g, stream=self._capture_stream, capture_error_mode="thread_local"):
-                        loss = self.forward_backward(st["x"], st["lab"].long())
-                        st["loss"].copy_(loss.reshape(1))
+                    # Destroying a CUDA graph is not permitted while a stream captures: it invalidates the capture.
+                    # A dead producer's graphs are freed here, and no cyclic garbage collection runs inside.
+                    gc.collect()
+                    gc_was_enabled = gc.isenabled()
+                    gc.disable()
+                    try:
+                        with torch.cuda.graph(g, stream=self._capture_stream, capture_error_mode="thread_local"):
+                            loss = self.forward_backward(st["x"], st["lab"].long())
+                            st["loss"].copy_(loss.reshape(1))
+                    finally:
+                        if gc_was_enabled:
+                            gc.enable()
                     # the capture itself did not execute anything: run this step through the graph
                     g.replay()
                     st["graph"] = g

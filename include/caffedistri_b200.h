@@ -157,6 +157,35 @@ COS_API int cos_net_train(cos_net* net, int solver_index, const cos_blob* data, 
  * 1/0 with the reason in cos_last_error(). */
 COS_API int cos_net_train_accumulate(cos_net* net, int solver_index, const cos_blob* data, int ndata, int passes);
 
+/* Untransformed input formats of cos_net_train_raw / cos_data_transform: what the JVM hands Caffe's
+ * DataTransformer.  F32_NCHW is a FloatBlob (Transform(Blob*, Blob*): one mirror / crop draw per batch);
+ * U8_NHWC is a vector of 8-bit images, each height x width x channels interleaved (Transform(cv::Mat):
+ * one draw per image). */
+#define COS_RAW_F32_NCHW 0
+#define COS_RAW_U8_NHWC 1
+typedef struct cos_raw_blob {
+  const void* data; /* host memory, owned by the caller for the duration of the call */
+  int format;       /* COS_RAW_* */
+  int num, channels, height, width;
+} cos_raw_blob;
+/* train() on untransformed host blobs, one per staged input (data-layer top) in order: stage them, apply each input's
+ * transform_param on the device, then run the registered producer and the fused sync exactly as train() does.  An
+ * input without a transform_param (the label) must be F32_NCHW with its top's element count; it is copied.  The net
+ * must have been allocated from a prototxt; mean files are read by the first call.  With iter_size k every pass
+ * transforms again with its own draws.  Returns when the caller's memory has been read.  1/0 + cos_last_error(). */
+COS_API int cos_net_train_raw(cos_net* net, int solver_index, const cos_raw_blob* data, int ndata);
+/* The transform kernel alone, only enqueued on cuda_stream: in, out and mean are device pointers, mean_values a host
+ * array of nmean floats (1 or channels; at most 64).  mean (channels x height x width of the input) and mean_values
+ * exclusive; neither: x * scale.  out is num x channels x crop x crop fp32 (x height x width when crop_size is 0).
+ * key seeds the draws (DESIGN.md, "Input transform on the device").  1/0 + cos_last_error(). */
+COS_API int cos_data_transform(const void* in, int format, int num, int channels, int height, int width, float* out,
+                               int crop_size, int mirror, const float* mean, const float* mean_values, int nmean,
+                               float scale, uint64_t key, void* cuda_stream);
+/* Host only: one line per staged input of a solver or net prototxt, with its name, shape, scale, mirror, crop and
+ * mean source (mean files are read and checked).  Returns the text length and copies it with its NUL when cap exceeds
+ * it (buf may be NULL), or -1 + error naming the layer. */
+COS_API int cos_input_transform_plan(const char* prototxt, char* buf, int cap);
+
 /* J:110 predict / JN:277-376: forward-only; not on the sync path -> always
  * fails with "predict: not supported" (returns -1).  Kept for symbol parity. */
 COS_API int cos_net_predict(cos_net* net, int solver_index, const cos_blob* data, int ndata,
