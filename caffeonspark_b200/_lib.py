@@ -30,6 +30,14 @@ class cos_raw_blob(ctypes.Structure):
                 ("height", ctypes.c_int), ("width", ctypes.c_int)]
 
 
+class cos_raw_image(ctypes.Structure):
+    _fields_ = [("data", ctypes.c_void_p), ("height", ctypes.c_int), ("width", ctypes.c_int)]
+
+
+class cos_image_geometry(ctypes.Structure):
+    _fields_ = [("offset", ctypes.c_int64), ("height", ctypes.c_int), ("width", ctypes.c_int)]
+
+
 class cos_solver_desc(ctypes.Structure):
     _fields_ = [("nblobs", ctypes.c_int), ("counts", ctypes.POINTER(ctypes.c_int64)),
                 ("lr_mult", ctypes.POINTER(ctypes.c_float)), ("decay_mult", ctypes.POINTER(ctypes.c_float)),
@@ -63,6 +71,8 @@ SYMBOLS = [
     ("cos_net_train_accumulate", _i, [_vp, _i, _c.POINTER(cos_blob), _i, _i]),
     ("cos_net_train_raw", _i, [_vp, _i, _c.POINTER(cos_raw_blob), _i]),
     ("cos_data_transform", _i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp, _c.POINTER(_f), _i, _f, _u64, _vp]),
+    ("cos_image_transform", _i, [_vp, _c.POINTER(cos_image_geometry), _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _i,
+                                 _i, _c.POINTER(_f), _i, _f, _u64, _vp]),
     ("cos_input_transform_plan", _i, [_cp, _cp, _i]),
     ("cos_net_predict", _i, [_vp, _i, _c.POINTER(cos_blob), _i, _pcp, _i, _c.POINTER(cos_blob)]),
     ("cos_net_validation", _i, [_vp, _c.POINTER(cos_blob), _i]),

@@ -9,7 +9,7 @@ the role ``CaffeProcessor`` plays on the Scala side.
 import ctypes
 
 from . import _lib
-from ._lib import FORWARD_BACKWARD_FN, cos_blob, cos_raw_blob, cos_solver_desc
+from ._lib import FORWARD_BACKWARD_FN, cos_blob, cos_raw_blob, cos_raw_image, cos_solver_desc
 
 
 class CosError(RuntimeError):
@@ -153,15 +153,41 @@ def input_transform_plan(prototxt):
     return buf.value.decode()
 
 
-RAW_F32_NCHW, RAW_U8_NHWC = 0, 1  # COS_RAW_*
+RAW_F32_NCHW, RAW_U8_NHWC, RAW_U8_IMAGES = 0, 1, 2  # COS_RAW_*
 
 
-def _raw_blob_array(data):
-    """list of numpy arrays (uint8 N x H x W x C images, or float32 N x C x H x W) -> cos_raw_blob[]"""
+def _image_list(images):
+    """list of uint8 H x W x C (or H x W) arrays of any size -> (cos_raw_image[], kept arrays, channels)"""
+    import numpy as np
+    arr = (cos_raw_image * max(1, len(images)))()
+    keep, channels = [], None
+    for k, a in enumerate(images):
+        if not isinstance(a, np.ndarray) or a.dtype != np.uint8 or a.ndim not in (2, 3):
+            raise CosError("train_raw(): an image list holds numpy uint8 H x W x C (or H x W) arrays")
+        a = np.ascontiguousarray(a)
+        c = a.shape[2] if a.ndim == 3 else 1
+        if channels is not None and c != channels:
+            raise CosError(f"train_raw(): image {k} has {c} channels, image 0 {channels}")
+        channels = c
+        keep.append(a)
+        arr[k].data, arr[k].height, arr[k].width = a.ctypes.data, int(a.shape[0]), int(a.shape[1])
+    return arr, keep, channels or 0
+
+
+def _raw_blob_array(data, resize=None):
+    """list of numpy arrays (uint8 N x H x W x C images, or float32 N x C x H x W) or lists of uint8 images of any
+    size (COS_RAW_U8_IMAGES, resized to `resize` when given) -> cos_raw_blob[]"""
     import numpy as np
     blobs = (cos_raw_blob * max(1, len(data)))()
     keep = []
+    rh, rw = (0, 0) if resize is None else (int(resize[0]), int(resize[1]))
     for i, a in enumerate(data):
+        if isinstance(a, (list, tuple)):
+            arr, imgs, c = _image_list(a)
+            keep.append((arr, imgs))
+            blobs[i].data, blobs[i].format = ctypes.addressof(arr), RAW_U8_IMAGES
+            blobs[i].num, blobs[i].channels, blobs[i].height, blobs[i].width = len(imgs), c, rh, rw
+            continue
         if not isinstance(a, np.ndarray) or a.dtype not in (np.uint8, np.float32):
             raise CosError("train_raw(): blobs must be numpy uint8 (N x H x W x C) or float32 (N x C x H x W) arrays")
         a = np.ascontiguousarray(a)
@@ -324,15 +350,23 @@ class CaffeNet:
         del keep
         return ok
 
-    def train_raw(self, solver_index, arrays):
+    def train_raw(self, solver_index, arrays, resize=None):
         """One Solver::Step on untransformed host arrays, one per staged input: each input's transform_param (crop,
         mirror, mean, scale) runs on the device.  uint8 N x H x W x C images draw their crop and mirror per image,
         a float32 N x C x H x W blob once per batch; an input without a transform_param (the label) is float32.
+        An input given as a Python list of uint8 H x W x C arrays of any sizes is a ragged batch (COS_RAW_U8_IMAGES):
+        with resize=(h, w) each image is first resized to h x w with OpenCV's 8-bit INTER_LINEAR, on the device.
         Raises CosError for a dtype other than uint8 / float32; returns False when the step is refused or fails."""
         if arrays is None:
             self._L.cos_net_train_raw(self._h, solver_index, None, 0)
             raise CosError(_err())
-        blobs, keep = _raw_blob_array(list(arrays))
+        arrays = list(arrays)
+        if resize is not None:
+            if len(tuple(resize)) != 2:
+                raise CosError("train_raw(): resize is (height, width)")
+            if not any(isinstance(a, (list, tuple)) for a in arrays):
+                raise CosError("train_raw(): resize needs an input given as a list of images")
+        blobs, keep = _raw_blob_array(arrays, resize)
         ok = bool(self._L.cos_net_train_raw(self._h, solver_index, blobs, len(keep)))
         del keep
         return ok

@@ -98,6 +98,10 @@ CaffeNet::~CaffeNet() {
         if (p) cudaFree(p);
       for (void* p : st.raw)
         if (p) cudaFree(p);
+      for (void* p : st.geom)
+        if (p) cudaFree(p);
+      for (void* p : st.geom_host)
+        if (p) cudaFreeHost(p);
       if (st.copied) cudaEventDestroy(st.copied);
       if (st.consumed) cudaEventDestroy(st.consumed);
     }
@@ -573,12 +577,18 @@ bool CaffeNet::check_raw(const cos_raw_blob* data, int ndata, std::string* err) 
       return false;
     };
     if (!b.data) return refuse("data[" + std::to_string(i) + "] is NULL");
-    if (b.format != kRawF32Nchw && b.format != kRawU8Nhwc)
-      return refuse("format " + std::to_string(b.format) + " is neither COS_RAW_F32_NCHW nor COS_RAW_U8_NHWC");
-    if (b.num < 1 || b.channels < 1 || b.height < 1 || b.width < 1)
+    if (b.format != kRawF32Nchw && b.format != kRawU8Nhwc && b.format != kRawU8Images)
+      return refuse("format " + std::to_string(b.format) +
+                    " is not COS_RAW_F32_NCHW, COS_RAW_U8_NHWC or COS_RAW_U8_IMAGES");
+    if (b.format == kRawU8Images) {
+      if (!check_raw_images(b, t, refuse)) return false;
+    } else if (b.num < 1 || b.channels < 1 || b.height < 1 || b.width < 1) {
       return refuse("num, channels, height and width must be positive");
+    }
     const int64_t count = static_cast<int64_t>(b.num) * b.channels * b.height * b.width;
-    if (!t.active()) {
+    if (b.format == kRawU8Images) {
+      // checked image by image above
+    } else if (!t.active()) {
       int64_t want = 1;
       for (int64_t d : top) want *= d;
       if (b.format != kRawF32Nchw || count != want)
@@ -642,6 +652,57 @@ bool CaffeNet::check_raw(const cos_raw_blob* data, int ndata, std::string* err) 
   return true;
 }
 
+// COS_RAW_U8_IMAGES: Transform(const cv::Mat&)'s checks image by image, on each image's post-resize size.  Reads
+// num entries of the caller's image array only once num is the top's batch.
+bool CaffeNet::check_raw_images(const cos_raw_blob& b, const InputTransform& t,
+                                const std::function<bool(const std::string&)>& refuse) {
+  const std::vector<int64_t>& top = t.input.shape;
+  if (!t.active()) {
+    int64_t want = 1;
+    for (int64_t d : top) want *= d;
+    return refuse("an input without transform_param must be COS_RAW_F32_NCHW with the top's " + std::to_string(want) +
+                  " elements");
+  }
+  const TransformSpec& ts = t.input.transform;
+  if (b.num != top[0]) return refuse("raw num " + std::to_string(b.num) + " != the top's " + std::to_string(top[0]));
+  if (b.channels != top[1])
+    return refuse("Check failed: channels == img_channels (" + std::to_string(top[1]) + " vs. " +
+                  std::to_string(b.channels) + ")");
+  if (b.height < 0 || b.width < 0 || (b.height == 0) != (b.width == 0))
+    return refuse("resize target " + std::to_string(b.height) + "x" + std::to_string(b.width) +
+                  ": give both sides, or 0x0 for no resize");
+  const int64_t wo = ts.crop_size ? ts.crop_size : top[3];
+  if (wo > kMaxImageOutWidth)
+    return refuse("an output width of " + std::to_string(wo) + " exceeds " + std::to_string(kMaxImageOutWidth));
+  const cos_raw_image* img = static_cast<const cos_raw_image*>(b.data);
+  int64_t total = 0;
+  for (int k = 0; k < b.num; ++k) {
+    const std::string which = "image " + std::to_string(k) + ": ";
+    if (!img[k].data) return refuse(which + "data is NULL");
+    const int h = img[k].height, w = img[k].width;
+    if (h < 1 || w < 1)
+      return refuse(which + "height and width must be positive (" + std::to_string(h) + "x" + std::to_string(w) + ")");
+    const int hr = b.height ? b.height : h, wr = b.height ? b.width : w;  // the post-resize size
+    const std::string size = std::to_string(hr) + "x" + std::to_string(wr);
+    if (ts.crop_size) {
+      if (hr < ts.crop_size || wr < ts.crop_size)
+        return refuse(which + "Check failed: img_height >= crop_size (" + size + " vs. " +
+                      std::to_string(ts.crop_size) + ")");
+    } else if (hr != top[2] || wr != top[3]) {
+      return refuse(which + "Check failed: img_height == height (image " + size + ", top " + std::to_string(top[2]) +
+                    "x" + std::to_string(top[3]) + ")");
+    }
+    if (!t.mean.empty() && (hr != t.mean_shape[1] || wr != t.mean_shape[2]))
+      return refuse(which + "Check failed: img_height == data_mean_.height() (image " + size + ", mean " +
+                    std::to_string(t.mean_shape[1]) + "x" + std::to_string(t.mean_shape[2]) + ")");
+    int64_t bytes = 0;
+    if (__builtin_mul_overflow(static_cast<int64_t>(h) * w, static_cast<int64_t>(b.channels), &bytes) ||
+        __builtin_add_overflow(total, bytes, &total))
+      return refuse("the images' total byte count overflows");
+  }
+  return true;
+}
+
 // Pass `pass` of this step: every input with a transform_param, from stage `stage`'s raw set into its fp32 set.
 bool CaffeNet::transform_inputs(int stage, const cos_raw_blob* raw, int pass, std::string* err) {
   InputStage& st = stage_[stage];
@@ -651,6 +712,18 @@ bool CaffeNet::transform_inputs(int stage, const cos_raw_blob* raw, int pass, st
     const TransformSpec& ts = t.input.transform;
     const cos_raw_blob& b = raw[i];
     const uint64_t key = transform_key(spec_.random_seed, rank_, static_cast<int>(i), iter_, pass);
+    if (b.format == kRawU8Images) {
+      const std::vector<int64_t>& top = t.input.shape;
+      const bool file = mean_dev_[i] != nullptr;
+      COS_RT(launch_image_transform(static_cast<const uint8_t*>(st.raw[i]),
+                                    static_cast<const ImageGeometry*>(st.geom[i]), b.num, b.channels, b.height,
+                                    b.width, static_cast<float*>(st.dev[i]), static_cast<int>(top[2]),
+                                    static_cast<int>(top[3]), static_cast<int>(ts.crop_size), ts.mirror,
+                                    mean_dev_[i], file ? static_cast<int>(t.mean_shape[1]) : 0,
+                                    file ? static_cast<int>(t.mean_shape[2]) : 0, ts.mean_values.data(),
+                                    static_cast<int>(ts.mean_values.size()), ts.scale, key, stream_));
+      continue;
+    }
     COS_RT(launch_data_transform(st.raw[i], b.format, b.num, b.channels, b.height, b.width,
                                  static_cast<float*>(st.dev[i]), static_cast<int>(ts.crop_size), ts.mirror,
                                  mean_dev_[i], ts.mean_values.data(), static_cast<int>(ts.mean_values.size()),
@@ -678,6 +751,10 @@ bool CaffeNet::run_step(int solver_index, const cos_blob* data, int ndata, int g
     st.bytes.resize(nblobs, 0);
     st.raw.resize(nblobs, nullptr);
     st.raw_bytes.resize(nblobs, 0);
+    st.geom.resize(nblobs, nullptr);
+    st.geom_bytes.resize(nblobs, 0);
+    st.geom_host.resize(nblobs, nullptr);
+    st.geom_host_bytes.resize(nblobs, 0);
   }
   auto reserve = [&](void** buf, size_t* have, size_t n) {
     if (n > *have) {
@@ -702,6 +779,39 @@ bool CaffeNet::run_step(int solver_index, const cos_blob* data, int ndata, int g
     if (!host) {
       *err = "data[" + std::to_string(i) + "] is NULL";
       return false;
+    }
+    if (raw && raw[i].format == kRawU8Images) {
+      // a ragged batch: each image to its offset in the arena, and the geometry table from pinned memory, all on
+      // the copy stream (the table of this stage was last copied by step t-2, whose copy train_raw waited for)
+      const cos_raw_image* img = static_cast<const cos_raw_image*>(host);
+      const size_t table = static_cast<size_t>(b.num) * sizeof(ImageGeometry);
+      if (st.geom_host_bytes[i] < table) {
+        if (st.geom_host[i]) COS_RT(cudaFreeHost(st.geom_host[i]));
+        st.geom_host[i] = nullptr;
+        st.geom_host_bytes[i] = 0;
+        COS_RT(cudaMallocHost(&st.geom_host[i], table));
+        st.geom_host_bytes[i] = table;
+      }
+      COS_RT(cudaEventSynchronize(st.copied));
+      ImageGeometry* geom = static_cast<ImageGeometry*>(st.geom_host[i]);
+      size_t total = 0;
+      for (int k = 0; k < b.num; ++k) {
+        geom[k] = ImageGeometry{static_cast<int64_t>(total), img[k].height, img[k].width};
+        total += static_cast<size_t>(img[k].height) * img[k].width * b.channels;
+      }
+      const std::vector<int64_t>& top = transforms_[i].input.shape;
+      b.height = static_cast<int>(top[2]), b.width = static_cast<int>(top[3]);
+      if (!reserve(&st.dev[i], &st.bytes[i], static_cast<size_t>(b.num) * b.channels * b.height * b.width * 4) ||
+          !reserve(&st.raw[i], &st.raw_bytes[i], total) || !reserve(&st.geom[i], &st.geom_bytes[i], table))
+        return false;
+      for (int k = 0; k < b.num; ++k)
+        COS_RT(cudaMemcpyAsync(static_cast<uint8_t*>(st.raw[i]) + geom[k].offset, img[k].data,
+                               static_cast<size_t>(img[k].height) * img[k].width * b.channels,
+                               cudaMemcpyHostToDevice, copy_stream_));
+      COS_RT(cudaMemcpyAsync(st.geom[i], geom, table, cudaMemcpyHostToDevice, copy_stream_));
+      dev_blobs[i] = b;
+      dev_blobs[i].data = static_cast<const float*>(st.dev[i]);
+      continue;
     }
     const size_t elem = raw && raw[i].format == kRawU8Nhwc ? 1 : sizeof(float);
     size_t n = static_cast<size_t>(b.num) * b.channels * b.height * b.width * elem;

@@ -14,6 +14,7 @@
 
 #include <cuda_runtime_api.h>
 
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -120,6 +121,8 @@ class CaffeNet {
   bool run_step(int solver_index, const cos_blob* data, int ndata, int groups, const cos_raw_blob* raw,
                 std::string* err);
   bool check_raw(const cos_raw_blob* data, int ndata, std::string* err);  // train_raw's argument checks
+  bool check_raw_images(const cos_raw_blob& b, const InputTransform& t,
+                        const std::function<bool(const std::string&)>& refuse);
   bool transform_inputs(int stage, const cos_raw_blob* raw, int pass, std::string* err);
   int resolved_algo() const;
   int resolved_kernel() const;
@@ -209,7 +212,11 @@ class CaffeNet {
     std::vector<void*> dev;            // the fp32 inputs the producer reads
     std::vector<size_t> bytes;
     std::vector<void*> raw;            // train_raw: the untransformed inputs that have a transform_param
-    std::vector<size_t> raw_bytes;
+    std::vector<size_t> raw_bytes;     // (COS_RAW_U8_IMAGES: a ragged arena, grown to the largest batch seen)
+    std::vector<void*> geom;           // COS_RAW_U8_IMAGES: the call's ImageGeometry table on the device
+    std::vector<size_t> geom_bytes;
+    std::vector<void*> geom_host;      // ... and in pinned host memory, the source of its copy
+    std::vector<size_t> geom_host_bytes;
     cudaEvent_t copied = nullptr;    // H2D of this stage finished
     cudaEvent_t consumed = nullptr;  // the step that read this stage finished
     bool consumed_valid = false;

@@ -7,6 +7,7 @@
 #include <string.h>
 
 #include <cmath>
+#include <cstddef>
 #include <exception>
 #include <string>
 #include <vector>
@@ -565,6 +566,28 @@ int cos_data_transform(const void* in, int format, int num, int channels, int he
                                                 mean, mean_values, nmean, scale, key,
                                                 static_cast<cudaStream_t>(cuda_stream)),
                     "cos_data_transform");
+  })
+}
+
+static_assert(sizeof(cos_image_geometry) == sizeof(cosb::ImageGeometry) &&
+                  offsetof(cos_image_geometry, height) == offsetof(cosb::ImageGeometry, height),
+              "cos_image_geometry and cosb::ImageGeometry share one layout");
+
+int cos_image_transform(const void* in, const cos_image_geometry* geometry, int num, int channels, int resize_height,
+                        int resize_width, float* out, int out_height, int out_width, int crop_size, int mirror,
+                        const float* mean, int mean_height, int mean_width, const float* mean_values, int nmean,
+                        float scale, uint64_t key, void* cuda_stream) {
+  COS_GUARD(0, {
+    const std::string e =
+        cosb::check_image_transform_args(in, geometry, num, channels, resize_height, resize_width, out, out_height,
+                                         out_width, crop_size, mean, mean_height, mean_width, mean_values, nmean);
+    if (!e.empty()) return fail("cos_image_transform: " + e);
+    return launched(cosb::launch_image_transform(static_cast<const uint8_t*>(in),
+                                                 reinterpret_cast<const cosb::ImageGeometry*>(geometry), num,
+                                                 channels, resize_height, resize_width, out, out_height, out_width,
+                                                 crop_size, mirror != 0, mean, mean_height, mean_width, mean_values,
+                                                 nmean, scale, key, static_cast<cudaStream_t>(cuda_stream)),
+                    "cos_image_transform");
   })
 }
 

@@ -93,6 +93,117 @@ __global__ void __launch_bounds__(kThreads) data_transform_kernel(const Transfor
   }
 }
 
+struct ImageArgs {
+  const uint8_t* in;
+  const ImageGeometry* geom;
+  float* out;
+  const float* mean;  // C x mh x mw, or null
+  int C, Ho, Wo;
+  int rh, rw;  // resize target, or 0, 0
+  int mh, mw;
+  int crop, mirror, nmean;
+  float scale;
+  uint64_t key;
+  float mean_values[kMaxMeanValues];
+};
+
+// OpenCV's INTER_LINEAR source position of output index d: (d + 0.5) * (src / dst) - 0.5 in double, unfused, then
+// float; -> floor and the fraction
+__device__ __forceinline__ int resize_tap(int d, double scale, float* frac) {
+  const float f = __double2float_rn(__dadd_rn(__dmul_rn(__dadd_rn(static_cast<double>(d), 0.5), scale), -0.5));
+  const float i = floorf(f);
+  *frac = __fsub_rn(f, i);
+  return static_cast<int>(i);
+}
+// the first 11-bit fixed-point coefficient, rint(float(1 - f) * 2048); the second is 2048 minus it
+__device__ __forceinline__ int resize_coef(float frac) { return __float2int_rn(__fmul_rn(__fsub_rn(1.f, frac), 2048.f)); }
+
+// COS_RAW_U8_IMAGES: one block per kRowsPerBlock output rows of one image of a ragged batch.  Each image is resized to
+// the target (when there is one) and transformed as data_transform_kernel<true> does, with its draws taken on the
+// post-resize size.  Only the pixels inside the crop window are resized, each from its 2x2 source taps with OpenCV's
+// integer arithmetic, so the fusion changes no bit.  The block first tabulates each output column's source column and
+// horizontal coefficient in shared memory; each thread then makes all channels of one output column, so the fp32
+// stores of each channel are coalesced.  An image whose size the call cannot take comes out as NaN.
+__global__ void __launch_bounds__(kThreads) image_transform_kernel(const ImageArgs a) {
+  extern __shared__ int2 cols[];  // per output column: source column, horizontal coefficient cx0
+  const int row_blocks = (a.Ho + kRowsPerBlock - 1) / kRowsPerBlock;
+  const int n = blockIdx.x / row_blocks, h0 = (blockIdx.x % row_blocks) * kRowsPerBlock;
+  const int h_end = h0 + kRowsPerBlock < a.Ho ? h0 + kRowsPerBlock : a.Ho;
+  const ImageGeometry g = a.geom[n];
+  const bool resize = a.rh > 0;
+  const int H = g.height, W = g.width, Hr = resize ? a.rh : H, Wr = resize ? a.rw : W;
+  // src / dst per axis.  Divided here, while few registers are live: the division's slow-path call then saves none
+  // to the stack (ptxas reports no spill).
+  const double sx = __ddiv_rn(static_cast<double>(W), static_cast<double>(Wr));
+  const double sy = __ddiv_rn(static_cast<double>(H), static_cast<double>(Hr));
+  const bool fits = H > 0 && W > 0 && (a.crop ? Hr >= a.crop && Wr >= a.crop : Hr == a.Ho && Wr == a.Wo) &&
+                    (!a.mean || (Hr == a.mh && Wr == a.mw));
+  float* out = a.out + static_cast<int64_t>(n) * a.C * a.Ho * a.Wo;
+  if (!fits) {
+    for (int c = 0; c < a.C; ++c)
+      for (int h = h0; h < h_end; ++h)
+        for (int w = threadIdx.x; w < a.Wo; w += blockDim.x)
+          out[(static_cast<int64_t>(c) * a.Ho + h) * a.Wo + w] = __int_as_float(0x7fc00000);
+    return;
+  }
+  const bool mirror = a.mirror && draw(a.key, n, 0, 2);
+  const int h_off = a.crop ? static_cast<int>(draw(a.key, n, 1, static_cast<uint32_t>(Hr - a.crop + 1))) : 0;
+  const int w_off = a.crop ? static_cast<int>(draw(a.key, n, 2, static_cast<uint32_t>(Wr - a.crop + 1))) : 0;
+  for (int w = threadIdx.x; w < a.Wo; w += blockDim.x) {
+    // mirrored: output column w holds column Wo-1-w of the crop (Caffe writes width-1-w from w)
+    const int xr = w_off + (mirror ? a.Wo - 1 - w : w);
+    int ix = xr, cx0 = 2048;
+    if (resize) {
+      float fx;
+      ix = resize_tap(xr, sx, &fx);
+      if (ix < 0) ix = 0, fx = 0.f;  // horizontally the fraction is clamped with the index
+      if (ix >= W - 1) ix = W - 1, fx = 0.f;
+      cx0 = resize_coef(fx);
+    }
+    cols[w] = make_int2(ix, cx0);
+  }
+  __syncthreads();
+  const uint8_t* img = a.in + g.offset;
+  for (int h = h0; h < h_end; ++h) {
+    const int yr = h_off + h;  // row of the resized image
+    int r0 = yr, r1 = yr, cy0 = 2048;
+    if (resize) {
+      float fy;
+      const int iy = resize_tap(yr, sy, &fy);  // vertically only the rows are clamped, not the coefficients
+      cy0 = resize_coef(fy);
+      r0 = min(max(iy, 0), H - 1), r1 = min(max(iy + 1, 0), H - 1);
+    }
+    const uint8_t* row0 = img + static_cast<int64_t>(r0) * W * a.C;
+    const uint8_t* row1 = img + static_cast<int64_t>(r1) * W * a.C;
+    for (int w = threadIdx.x; w < a.Wo; w += blockDim.x) {
+      const int2 t = cols[w];
+      const int x0 = t.x * a.C, x1 = min(t.x + 1, W - 1) * a.C, cx1 = 2048 - t.y;
+      const int xr = w_off + (mirror ? a.Wo - 1 - w : w);
+      for (int c = 0; c < a.C; ++c) {
+        int p;
+        if (resize) {
+          const int s0 = __ldg(row0 + x0 + c) * t.y + __ldg(row0 + x1 + c) * cx1;
+          const int s1 = __ldg(row1 + x0 + c) * t.y + __ldg(row1 + x1 + c) * cx1;
+          p = (((cy0 * (s0 >> 4)) >> 16) + (((2048 - cy0) * (s1 >> 4)) >> 16) + 2) >> 2;
+          p = min(max(p, 0), 255);
+        } else {
+          p = __ldg(row0 + x0 + c);
+        }
+        const float x = static_cast<float>(p);
+        float v;
+        if (a.mean) {
+          v = __fmul_rn(__fsub_rn(x, __ldg(a.mean + (static_cast<int64_t>(c) * a.mh + yr) * a.mw + xr)), a.scale);
+        } else if (a.nmean) {
+          v = __fmul_rn(__fsub_rn(x, a.mean_values[a.nmean == 1 ? 0 : c]), a.scale);
+        } else {
+          v = __fmul_rn(x, a.scale);
+        }
+        out[(static_cast<int64_t>(c) * a.Ho + h) * a.Wo + w] = v;
+      }
+    }
+  }
+}
+
 std::string shape_str(const std::vector<int64_t>& s) {
   std::ostringstream os;
   for (size_t i = 0; i < s.size(); ++i) os << (i ? "x" : "") << s[i];
@@ -158,6 +269,61 @@ cudaError_t launch_data_transform(const void* in, int format, int num, int chann
   } else {
     data_transform_kernel<false><<<grid, kThreads, 0, stream>>>(a);
   }
+  return cudaGetLastError();
+}
+
+std::string check_image_transform_args(const void* in, const void* geometry, int num, int channels, int resize_height,
+                                       int resize_width, const float* out, int out_height, int out_width,
+                                       int crop_size, const float* mean, int mean_height, int mean_width,
+                                       const float* mean_values, int nmean) {
+  if (!in || !geometry || !out) return "in, geometry and out must not be NULL";
+  if (num < 1 || channels < 1 || out_height < 1 || out_width < 1)
+    return "num, channels, out_height and out_width must be positive";
+  if (resize_height < 0 || resize_width < 0 || (resize_height == 0) != (resize_width == 0))
+    return "resize " + std::to_string(resize_height) + "x" + std::to_string(resize_width) +
+           ": give both sides, or 0x0 for no resize";
+  if (crop_size < 0) return "crop_size " + std::to_string(crop_size) + " is negative";
+  if (crop_size && (out_height != crop_size || out_width != crop_size))
+    return "out " + std::to_string(out_height) + "x" + std::to_string(out_width) + " must be crop x crop (" +
+           std::to_string(crop_size) + ")";
+  if (resize_height && crop_size && (resize_height < crop_size || resize_width < crop_size))
+    return "Check failed: img_height >= crop_size (resize " + std::to_string(resize_height) + "x" +
+           std::to_string(resize_width) + " vs. " + std::to_string(crop_size) + ")";
+  if (resize_height && !crop_size && (resize_height != out_height || resize_width != out_width))
+    return "Check failed: img_height == height (resize " + std::to_string(resize_height) + "x" +
+           std::to_string(resize_width) + ", out " + std::to_string(out_height) + "x" + std::to_string(out_width) + ")";
+  if (mean && nmean) return "Cannot specify mean_file and mean_value at the same time";
+  if (mean && (mean_height < 1 || mean_width < 1)) return "mean_height and mean_width must be positive";
+  if (mean && resize_height && (mean_height != resize_height || mean_width != resize_width))
+    return "Check failed: img_height == data_mean_.height() (resize " + std::to_string(resize_height) + "x" +
+           std::to_string(resize_width) + ", mean " + std::to_string(mean_height) + "x" + std::to_string(mean_width) +
+           ")";
+  if (nmean < 0 || (nmean && !mean_values)) return "mean_values is NULL";
+  if (nmean && nmean != 1 && nmean != channels)
+    return "Specify either 1 mean_value or as many as channels: " + std::to_string(channels);
+  if (nmean > kMaxMeanValues) return "at most " + std::to_string(kMaxMeanValues) + " mean values";
+  if (out_width > kMaxImageOutWidth)
+    return "an output width of " + std::to_string(out_width) + " exceeds " + std::to_string(kMaxImageOutWidth);
+  if (static_cast<int64_t>(num) * out_height > 0x7fffffff) return "num x output height exceeds the grid";
+  return "";
+}
+
+cudaError_t launch_image_transform(const uint8_t* in, const ImageGeometry* geometry, int num, int channels,
+                                   int resize_height, int resize_width, float* out, int out_height, int out_width,
+                                   int crop_size, bool mirror, const float* mean, int mean_height, int mean_width,
+                                   const float* mean_values, int nmean, float scale, uint64_t key,
+                                   cudaStream_t stream) {
+  ImageArgs a;
+  a.in = in, a.geom = geometry, a.out = out, a.mean = mean;
+  a.C = channels, a.Ho = out_height, a.Wo = out_width;
+  a.rh = resize_height, a.rw = resize_width;
+  a.mh = mean ? mean_height : 0, a.mw = mean ? mean_width : 0;
+  a.crop = crop_size, a.mirror = mirror ? 1 : 0, a.nmean = mean ? 0 : nmean;
+  a.scale = scale, a.key = key;
+  for (int i = 0; i < kMaxMeanValues; ++i) a.mean_values[i] = i < a.nmean ? mean_values[i] : 0.f;
+  const int row_blocks = (a.Ho + kRowsPerBlock - 1) / kRowsPerBlock;
+  const unsigned grid = static_cast<unsigned>(static_cast<int64_t>(num) * row_blocks);
+  image_transform_kernel<<<grid, kThreads, static_cast<size_t>(a.Wo) * sizeof(int2), stream>>>(a);
   return cudaGetLastError();
 }
 

@@ -181,6 +181,32 @@ COS_API int cos_net_train_raw(cos_net* net, int solver_index, const cos_raw_blob
 COS_API int cos_data_transform(const void* in, int format, int num, int channels, int height, int width, float* out,
                                int crop_size, int mirror, const float* mean, const float* mean_values, int nmean,
                                float scale, uint64_t key, void* cuda_stream);
+/* Decoded 8-bit images of any size, one cv::Mat each (format COS_RAW_U8_IMAGES of cos_net_train_raw).  For this
+ * format the cos_raw_blob fields mean: data points to num cos_raw_image, each with its own size; channels is shared by
+ * all images; height and width are the resize target (OpenCV's 8-bit INTER_LINEAR, as the reference's -resize), or
+ * 0, 0 for no resize.  Each image is then transformed as a U8_NHWC image is, with its draws taken on its post-resize
+ * size; Caffe's per-image checks (crop, top size, mean size) apply to that size.  Every call must repeat the first
+ * call's num, channels and target; the images' own sizes may change from call to call. */
+#define COS_RAW_U8_IMAGES 2
+typedef struct cos_raw_image {
+  const void* data; /* host, height x width x channels uint8, interleaved (a decoded cv::Mat) */
+  int height, width;
+} cos_raw_image;
+/* One image of a ragged batch on the device: byte offset into the arena, its height and width. */
+typedef struct cos_image_geometry {
+  int64_t offset;
+  int height, width;
+} cos_image_geometry;
+/* The COS_RAW_U8_IMAGES kernel alone, only enqueued on cuda_stream.  in (the images, each at its geometry's offset),
+ * geometry (num entries), out and mean are device pointers; mean_values is a host array as for cos_data_transform.
+ * resize_height x resize_width is the target, or 0 x 0.  out is num x channels x out_height x out_width fp32: crop x crop
+ * with a crop, else every image's post-resize size.  mean is channels x mean_height x mean_width, every image's
+ * post-resize size.  Geometry the host cannot see is checked by the kernel: an image it cannot take (a side below 1,
+ * below the crop, or off the output or mean size) comes out as NaN.  1/0 + cos_last_error(). */
+COS_API int cos_image_transform(const void* in, const cos_image_geometry* geometry, int num, int channels,
+                                int resize_height, int resize_width, float* out, int out_height, int out_width,
+                                int crop_size, int mirror, const float* mean, int mean_height, int mean_width,
+                                const float* mean_values, int nmean, float scale, uint64_t key, void* cuda_stream);
 /* Host only: one line per staged input of a solver or net prototxt, with its name, shape, scale, mirror, crop and
  * mean source (mean files are read and checked).  Returns the text length and copies it with its NUL when cap exceeds
  * it (buf may be NULL), or -1 + error naming the layer. */
