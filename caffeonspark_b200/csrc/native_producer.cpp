@@ -107,16 +107,24 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     }
     const bool known = L.type == "Convolution" || L.type == "Pooling" || L.type == "InnerProduct" || L.type == "ReLU" ||
                        L.type == "Sigmoid" || L.type == "BatchNorm" || L.type == "SoftmaxWithLoss" ||
-                       L.type == "Slice" || L.type == "ContrastiveLoss" ||
+                       L.type == "Slice" || L.type == "ContrastiveLoss" || L.type == "Concat" ||
+                       L.type == "EuclideanLoss" ||
                        (L.type == "LRN" && L.norm_region == "WITHIN_CHANNEL");  // ACROSS_CHANNELS has no engine op
     if (!known) {
       *err = why(L, "layer type not supported");
       return false;
     }
-    // Slice is the one layer with several tops; ContrastiveLoss reads a, b and sim
-    const size_t want_bottoms = L.type == "SoftmaxWithLoss" ? 2 : L.type == "ContrastiveLoss" ? 3 : 1;
-    if (L.bottoms.size() != want_bottoms || (L.tops.size() != 1 && L.type != "Slice") || L.tops.empty()) {
-      *err = why(L, "needs " + std::to_string(want_bottoms) + " bottom(s) and one top");
+    // Slice is the one layer with several tops and Concat the one with any number of bottoms; ContrastiveLoss reads
+    // a, b and sim.  EuclideanLoss may leave its top out, as Caffe's solver tests write it (a loss layer's
+    // AutoTopBlobs): the engine writes the loss to loss_dev either way.
+    const size_t want_bottoms = L.type == "SoftmaxWithLoss" || L.type == "EuclideanLoss" ? 2
+                                : L.type == "ContrastiveLoss"                             ? 3
+                                                                                          : 1;
+    const bool auto_top = L.type == "EuclideanLoss" && L.tops.empty();
+    const bool tops_ok = L.type == "Slice" ? !L.tops.empty() : L.tops.size() == 1 || auto_top;
+    if ((L.type == "Concat" ? L.bottoms.empty() : L.bottoms.size() != want_bottoms) || !tops_ok) {
+      *err = why(L, (L.type == "Concat" ? std::string("needs at least 1") : std::to_string(want_bottoms)) +
+                        " bottom(s) and one top");
       return false;
     }
     Op op;
@@ -140,7 +148,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     };
     if (!take(L.bottoms[0], &op.in)) return false;
     op.in_shape = L.bottom_shapes[0];
-    op.out_shape = L.top_shapes[0];
+    if (!auto_top) op.out_shape = L.top_shapes[0];  // else the scalar loss
     op.need_dx = wants_grad[op.in];
     if (L.type == "Slice") {  // one op per top, each copying its range of the bottom (and back, in the backward)
       op.kind = OpKind::kSlice;
@@ -153,6 +161,25 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         cur[L.tops[t]] = op.out;
         P.ops.push_back(op);
       }
+      continue;
+    }
+    if (L.type == "Concat") {  // one op per bottom, each copying its bottom into its range of the one top (and back)
+      op.kind = OpKind::kConcat;
+      op.slice_axis = static_cast<int>(L.axis);  // the parser checked the axis and the bottoms' shapes
+      op.out = new_tensor(count_of(op.out_shape), -1);
+      int64_t begin = 0;
+      for (size_t b = 0; b < L.bottoms.size(); ++b) {
+        if (b > 0) {
+          if (!take(L.bottoms[b], &op.in)) return false;
+          op.in_shape = L.bottom_shapes[b];
+          op.need_dx = wants_grad[op.in];
+        }
+        op.slice_begin = begin;
+        begin += op.in_shape[op.slice_axis];
+        wants_grad[op.out] = wants_grad[op.out] || op.need_dx;
+        P.ops.push_back(op);
+      }
+      cur[L.tops[0]] = op.out;
       continue;
     }
     int storage = -1;
@@ -275,6 +302,26 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         return false;
       }
       op.label = it->second;
+    } else if (L.type == "EuclideanLoss") {  // euclidean_loss_layer.cpp, after LossLayer::Reshape's check
+      if (++losses > 1) {
+        *err = why(L, "a second loss layer is not supported");
+        return false;
+      }
+      const std::vector<int64_t>& a = L.bottom_shapes[0];
+      const std::vector<int64_t>& b = L.bottom_shapes[1];
+      if (a.empty() || b.empty() || a[0] != b[0]) {
+        *err = why(L, "The data and label should have the same number.");
+        return false;
+      }
+      if (count_of(std::vector<int64_t>(a.begin() + 1, a.end())) !=
+          count_of(std::vector<int64_t>(b.begin() + 1, b.end()))) {  // Blob::count(1)
+        *err = why(L, "Inputs must have the same dimension.");
+        return false;
+      }
+      op.kind = OpKind::kEuclideanLoss;
+      op.loss_weight = L.loss_weight;
+      if (!take(L.bottoms[1], &op.in2)) return false;
+      op.need_dx2 = wants_grad[op.in2];
     } else {  // SoftmaxWithLoss
       if (++losses > 1) {
         *err = why(L, "a second loss layer is not supported");
@@ -298,11 +345,11 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     op.out = new_tensor(count_of(op.out_shape), storage);
     // BatchNorm's blobs are statistics, with no gradient
     wants_grad[op.out] = op.need_dx || (op.kind != OpKind::kBatchNorm && (op.w_off >= 0 || op.b_off >= 0));
-    cur[L.tops[0]] = op.out;
+    if (!auto_top) cur[L.tops[0]] = op.out;
     P.ops.push_back(op);
   }
   if (losses == 0) {
-    *err = "the net has no SoftmaxWithLoss or ContrastiveLoss layer in its TRAIN phase (native producer)";
+    *err = "the net has no SoftmaxWithLoss, ContrastiveLoss or EuclideanLoss layer in its TRAIN phase (native producer)";
     return false;
   }
   for (size_t t = 0; t < P.tensor_count.size(); ++t) {
@@ -323,7 +370,7 @@ bool plan_from_prototxt(const std::string& path, SolverSpec* spec, Plan* plan, s
 std::string Plan::text() const {
   static const char* kinds[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling", "InnerProduct",
                                 "ReLU",        "Sigmoid",             "BatchNorm", "SoftmaxWithLoss",
-                                "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss"};
+                                "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss", "Concat", "EuclideanLoss"};
   std::ostringstream os;
   for (int i = 0; i < ninputs; ++i) os << "input " << i << " " << input_names[i] << " " << tensor_count[i] << "\n";
   for (size_t i = 0; i < ops.size(); ++i) {
@@ -343,16 +390,18 @@ std::string Plan::text() const {
       os << " shares=";
       for (size_t j = 0; j < op.shares.size(); ++j) os << (j ? "," : "") << op.shares[j];
     }
-    if (op.kind == OpKind::kSlice) os << " axis=" << op.slice_axis << " begin=" << op.slice_begin;
+    if (op.kind == OpKind::kSlice || op.kind == OpKind::kConcat)
+      os << " axis=" << op.slice_axis << " begin=" << op.slice_begin;
     if (op.kind == OpKind::kSoftmaxLoss) os << " label=" << op.label << " loss_weight=" << op.loss_weight;
     if (op.kind == OpKind::kContrastiveLoss)
       os << " second=" << op.in2 << " sim=" << op.label << " margin=" << op.margin << (op.legacy ? " legacy" : "")
          << " loss_weight=" << op.loss_weight;
+    if (op.kind == OpKind::kEuclideanLoss) os << " second=" << op.in2 << " loss_weight=" << op.loss_weight;
     if (op.in_place) os << " in-place";
     // no data gradient is propagated into a staged input, nor into a blob with no learnable blob before it
     auto mark = [&](int in, bool need) { return need ? "" : in < ninputs ? " staged-bottom" : " no-bottom-grad"; };
     const char* m = mark(op.in, op.need_dx);
-    if (!*m && op.kind == OpKind::kContrastiveLoss) m = mark(op.in2, op.need_dx2);
+    if (!*m && (op.kind == OpKind::kContrastiveLoss || op.kind == OpKind::kEuclideanLoss)) m = mark(op.in2, op.need_dx2);
     os << m;
     os << "\n";
   }

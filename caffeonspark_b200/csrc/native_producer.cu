@@ -343,15 +343,17 @@ __global__ void __launch_bounds__(kThreads) softmax_loss_kernel(const float* x, 
   if (threadIdx.x == 0) *loss = __fmul_rn(loss_weight, __fdiv_rn(part, count));
 }
 
-// ------------------------------------------------------------------ Slice (slice_layer.cu semantics)
-// One top of a Slice: top[n, i, r] = bottom[n, begin + i, r] over outer n, top_axis i and inner r.  Forward copies the
-// top out of the bottom; backward (to_bottom) writes the top's gradient into its range of the bottom's gradient.
-__global__ void slice_copy_kernel(const float* src, float* dst, int64_t total, int64_t top_span, int64_t bottom_span,
-                                  int64_t offset, bool to_bottom) {
+// ------------------------------------------------------------------ Slice and Concat (slice_layer.cu, concat_layer.cu)
+// One range of a blob split along an axis: part[n, i, r] = whole[n, begin + i, r] over outer n, part_axis i and inner
+// r.  Without into_whole it copies the range out of the whole (the forward of a Slice top, the backward of a Concat
+// bottom); with into_whole it writes the part into its range (the backward of a Slice top, the forward of a Concat
+// bottom).
+__global__ void slice_copy_kernel(const float* src, float* dst, int64_t total, int64_t part_span, int64_t whole_span,
+                                  int64_t offset, bool into_whole) {
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    const int64_t b = (i / top_span) * bottom_span + offset + i % top_span;
-    if (to_bottom) dst[b] = src[i];
+    const int64_t b = (i / part_span) * whole_span + offset + i % part_span;
+    if (into_whole) dst[b] = src[i];
     else dst[i] = src[b];
   }
 }
@@ -409,6 +411,28 @@ __global__ void __launch_bounds__(kThreads) contrastive_loss_kernel(const float*
     *loss = __fmul_rn(loss_weight, __fdiv_rn(__fdiv_rn(part, static_cast<float>(N)), 2.f));
 }
 
+// ------------------------------------------------------------------ EuclideanLoss (euclidean_loss_layer.cpp)
+// One block.  d = a - b over the `count` elements of each bottom; each thread sums d^2 over its elements in index order,
+// then a fixed tree adds the threads: *loss = loss_weight * (dot / num / 2), each operation rounded once in float as
+// Caffe computes it.  The gradients are alpha * d with alpha = loss_weight / num into a and -loss_weight / num into b,
+// one rounding each; da / db are null for a bottom that wants none.  A NaN reaches the loss, as in Caffe.  Made for
+// regression targets of a few values per row: on large blobs one block leaves most of the GPU idle.
+__global__ void __launch_bounds__(kThreads) euclidean_loss_kernel(const float* a, const float* b, float* da, float* db,
+                                                                  float* loss, int count, int num, float loss_weight) {
+  __shared__ float sh[kThreads];
+  const float alpha = __fdiv_rn(loss_weight, static_cast<float>(num));
+  float part = 0.f;
+  for (int i = threadIdx.x; i < count; i += kThreads) {
+    const float d = __fsub_rn(a[i], b[i]);
+    part = __fadd_rn(part, __fmul_rn(d, d));
+    if (da) da[i] = __fmul_rn(alpha, d);
+    if (db) db[i] = __fmul_rn(-alpha, d);
+  }
+  part = block_sum(part, sh);
+  if (threadIdx.x == 0)
+    *loss = __fmul_rn(loss_weight, __fdiv_rn(__fdiv_rn(part, static_cast<float>(num)), 2.f));
+}
+
 // ------------------------------------------------------------------ fillers (u: the cos_net_fill value in [-1, 1))
 __global__ void constant_fill_kernel(float* p, int n, float v) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = v;
@@ -458,7 +482,8 @@ void bn_dims(const Op& op, int* n, int* c, int* hw) {
   *c = static_cast<int>(op.in_shape.size() > 1 ? op.in_shape[1] : 1);
   *hw = static_cast<int>(total / (static_cast<int64_t>(*n) * *c));
 }
-// Slice: elements after the slice axis, and the elements of one outer index of a blob (its axis times that)
+// Slice, Concat: elements after the axis (the same in the bottom and the top), and the elements of one outer index of a
+// blob (its axis times that)
 int64_t slice_inner(const Op& op) {
   int64_t n = 1;
   for (size_t a = op.slice_axis + 1; a < op.in_shape.size(); ++a) n *= op.in_shape[a];
@@ -681,6 +706,15 @@ int NativeProducer::forward_backward(const cos_blob* inputs, int ninputs, float*
       if (e != cudaSuccess) return e;
       continue;
     }
+    if (op.kind == OpKind::kEuclideanLoss) {  // writes both bottoms' gradients here, as SoftmaxWithLoss does
+      euclidean_loss_kernel<<<1, kThreads, 0, s>>>(act_[op.in], act_[op.in2], op.need_dx ? grad_[op.in] : nullptr,
+                                                   op.need_dx2 ? grad_[op.in2] : nullptr, loss_dev,
+                                                   static_cast<int>(plan_.tensor_count[op.in]),
+                                                   static_cast<int>(op.in_shape[0]), op.loss_weight);
+      cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) return e;
+      continue;
+    }
     if (op.kind == OpKind::kSoftmaxLoss) {
       const int C = static_cast<int>(op.in_shape[1]);
       const int rows = static_cast<int>(plan_.tensor_count[op.in] / C);
@@ -748,6 +782,13 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, cudaStream_t 
       slice_copy_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n, slice_span(op, op.out_shape), slice_span(op, op.in_shape),
                                                          op.slice_begin * slice_inner(op), false);
       return cudaGetLastError();
+    case OpKind::kConcat: {
+      const int64_t nin = plan_.tensor_count[op.in];
+      slice_copy_kernel<<<grid_for(nin), kThreads, 0, s>>>(x, y, nin, slice_span(op, op.in_shape),
+                                                           slice_span(op, op.out_shape),
+                                                           op.slice_begin * slice_inner(op), true);
+      return cudaGetLastError();
+    }
     case OpKind::kLRNWithin:
       return lrn_within_forward(x, y, static_cast<int>(op.in_shape[0]), static_cast<int>(op.in_shape[1]),
                                 static_cast<int>(op.in_shape[2]), static_cast<int>(op.in_shape[3]), op.lrn_size,
@@ -823,7 +864,13 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
                                                          true);
       return cudaGetLastError();
     }
-    default:  // SoftmaxWithLoss and ContrastiveLoss wrote their bottom gradients in the forward pass
+    case OpKind::kConcat:
+      if (!dx) return cudaSuccess;
+      slice_copy_kernel<<<grid_for(nin), kThreads, 0, s>>>(dy, dx, nin, slice_span(op, op.in_shape),
+                                                           slice_span(op, op.out_shape),
+                                                           op.slice_begin * slice_inner(op), false);
+      return cudaGetLastError();
+    default:  // SoftmaxWithLoss, ContrastiveLoss and EuclideanLoss wrote their bottom gradients in the forward pass
       return cudaSuccess;
   }
 }

@@ -1,5 +1,6 @@
 // native_producer.hpp -- the built-in gradient producer (Net::ForwardBackward for the TRAIN phase of the LeNet,
-// CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets; DESIGN.md section 14).
+// CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, and least-squares regression nets;
+// DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -21,14 +22,14 @@ namespace cosb {
 
 enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
-  kContrastiveLoss
+  kContrastiveLoss, kConcat, kEuclideanLoss
 };
 
 struct Op {
   OpKind kind;
   std::string name;                    // layer name (the fused block: "conv1+relu1+pool1")
   int in = -1, out = -1, label = -1;   // tensor ids (label: SoftmaxWithLoss's label, ContrastiveLoss's sim)
-  int in2 = -1;                        // ContrastiveLoss: the second feature bottom
+  int in2 = -1;                        // ContrastiveLoss, EuclideanLoss: the second bottom
   std::vector<int64_t> in_shape, out_shape;
   bool need_dx = true;                 // false when the bottom is a staged input or follows no learnable blob
   bool need_dx2 = true;                // the same for in2
@@ -41,12 +42,13 @@ struct Op {
   int64_t w_off = -1, w_count = 0, b_off = -1, b_count = 0;  // flat offsets into data_ / diff_
   std::vector<int> shares;             // learnable blobs this op uses as a sharer of a named param (owned elsewhere)
   float slope = 0.f;                   // ReLU negative_slope
-  float loss_weight = 1.f;             // SoftmaxWithLoss
+  float loss_weight = 1.f;             // SoftmaxWithLoss, ContrastiveLoss, EuclideanLoss
   bool global_stats = false;           // BatchNorm
   float fraction = 0.999f, eps = 1e-5f;
   int lrn_size = 0;                    // LRN (WITHIN_CHANNEL only)
   float lrn_alpha = 1.f, lrn_beta = 0.75f;
-  // Slice: this op copies bottom[.., slice_begin .. slice_begin + out_shape[slice_axis], ..] to its one top
+  // Slice: this op copies bottom[.., slice_begin .. slice_begin + out_shape[slice_axis], ..] to its one top.
+  // Concat, the inverse: this op copies its one bottom to top[.., slice_begin .. slice_begin + in_shape[slice_axis], ..]
   int slice_axis = 0;
   int64_t slice_begin = 0;
   float margin = 1.f;                  // ContrastiveLoss
@@ -66,7 +68,8 @@ struct Plan {
   std::string text() const;  // one op per line (cos_native_producer_plan)
 };
 
-// Builds the plan of a parsed TRAIN net (a Slice layer becomes one kSlice op per top); false with
+// Builds the plan of a parsed TRAIN net (a Slice layer becomes one kSlice op per top, a Concat layer one kConcat op
+// per bottom); false with
 // "layer '<name>' (<type>): <reason>" when it cannot be run.
 bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Plan* plan, std::string* err);
 // parse_train_net + build_plan.

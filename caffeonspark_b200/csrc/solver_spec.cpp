@@ -527,17 +527,33 @@ bool net_layout(const Node& net, const std::string& net_file, SolverSpec* spec, 
       Shape in;
       if (!bottom_shape(0, &in) || in.empty()) return false;
       if (!tops.empty()) blobs[tops[0]] = Shape{in[0], prod(in, 1)};
-    } else if (type == "Concat") {
+    } else if (type == "Concat") {  // concat_layer.cpp LayerSetUp and Reshape, with its CHECK messages
       Shape out;
       if (!bottom_shape(0, &out)) return false;
       const Node* p = L->first("concat_param");
-      long axis = p ? p->integer("axis", 1) : 1;
-      if (axis < 0) axis += static_cast<long>(out.size());
+      const long naxes = static_cast<long>(out.size());
+      long axis = 1;
+      if (p && p->first("axis") && p->first("concat_dim"))
+        return refuse("Either axis or concat_dim should be specified; not both.");
+      if (p && p->first("concat_dim")) {  // a uint32: never counted from the end
+        axis = p->integer("concat_dim", 1);
+        if (axis < 0 || axis >= naxes) return refuse("concat_dim out of range.");
+      } else {
+        const long given = p ? p->integer("axis", 1) : 1;
+        axis = given < 0 ? given + naxes : given;
+        if (axis < 0 || axis >= naxes)  // Blob::CanonicalAxisIndex
+          return refuse("axis " + std::to_string(given) + " out of range for " + std::to_string(naxes) +
+                        "-D Blob");
+      }
       for (size_t i = 1; i < bottoms.size(); ++i) {
         Shape s;
-        if (!bottom_shape(i, &s) || s.size() != out.size()) return false;
+        if (!bottom_shape(i, &s)) return false;
+        if (s.size() != out.size()) return refuse("All inputs must have the same #axes.");
+        for (long j = 0; j < naxes; ++j)
+          if (j != axis && s[j] != out[j]) return refuse("All inputs must have the same shape, except at concat_axis.");
         out[axis] += s[axis];
       }
+      rec.axis = axis;
       if (!tops.empty()) blobs[tops[0]] = out;
     } else if (type == "SoftmaxWithLoss" || type == "Accuracy" || type == "EuclideanLoss" ||
                type == "SigmoidCrossEntropyLoss" || type == "HingeLoss" || type == "MultinomialLogisticLoss") {
