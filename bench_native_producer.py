@@ -1,8 +1,9 @@
 """Forward/backward time of the built-in producer against the PyTorch fp32 producer (DESIGN.md section 14).
 
-Workloads: the five nets the engine runs, at their reference batch sizes (LeNet b64, CIFAR-10-quick b100,
-cifar10_full_bn b100, cifar10_full b100, and the siamese MNIST example b64 of 2x28x28 pairs: its two LeNet trunks share
-their weights and end in a ContrastiveLoss, timed against the PyTorch module that runs one trunk twice).  For each, one process times the native engine, the PyTorch module with TF32 off and with
+Workloads: the six nets the engine runs, at their reference batch sizes (LeNet b64, CIFAR-10-quick b100,
+cifar10_full_bn b100, cifar10_full b100, the siamese MNIST example b64 of 2x28x28 pairs: its two LeNet trunks share
+their weights and end in a ContrastiveLoss, timed against the PyTorch module that runs one trunk twice; and the
+ResNet-20 fixture b100, timed against nets.resnet20_module, whose BatchNorms run the same native kernels).  For each, one process times the native engine, the PyTorch module with TF32 off and with
 TF32 on (cuDNN's default, here applied to matmuls too), alternating the three in every round; each sample is CUDA events around `--iters`
 back-to-back forward/backward calls on one stream after `--warmup` untimed ones.  Prints one JSON line per
 workload with median / min / max ms per call and images/s, and the card's name and power limit.
@@ -23,7 +24,7 @@ import tempfile
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full", "mnist_siamese")
+WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full", "mnist_siamese", "cifar10_resnet20")
 FP32_PEAK = 67e12  # H100 SXM data sheet, dense FP32, at up to 700 W
 
 
@@ -49,6 +50,17 @@ def siamese_solver(directory):
     path = os.path.join(directory, "mnist_siamese_solver.prototxt")
     with open(path, "w") as f:
         f.write(solver.replace("examples/siamese/mnist_siamese_train_test.prototxt", "mnist_siamese_net.prototxt"))
+    return path
+
+
+def resnet20_solver(directory):
+    """The ResNet-20 fixture's solver, pointed at the fixture's net wherever this runs from."""
+    configs = os.path.join(ROOT, "tests", "golden", "configs")
+    solver = open(os.path.join(configs, "cifar10_resnet20_solver.prototxt")).read()
+    path = os.path.join(directory, "cifar10_resnet20_solver.prototxt")
+    with open(path, "w") as f:
+        f.write(solver.replace('net: "cifar10_resnet20_train_test.prototxt"',
+                               f'net: "{os.path.join(configs, "cifar10_resnet20_train_test.prototxt")}"'))
     return path
 
 
@@ -111,15 +123,16 @@ def main():
     gpu = card()
     tmp = tempfile.mkdtemp(prefix="bench_native_producer_")
     for name in args.workloads.split(","):
-        siamese = name == "mnist_siamese"
-        solver = siamese_solver(tmp) if siamese else nets.write_prototxts(name, tmp)
+        siamese, resnet = name == "mnist_siamese", name == "cifar10_resnet20"
+        solver = siamese_solver(tmp) if siamese else resnet20_solver(tmp) if resnet else nets.write_prototxts(name, tmp)
         net = C.CaffeNet(solver, "", "", 1, 1, 0, True, C.CaffeNet.NONE, -1, 0)
         net.use_native_producer(fill_weights=False)
         net.fill("data", 1, 0, 0.05)
         torch.cuda.synchronize()
-        batch = 64 if siamese else nets.NETS[name]["batch"]
+        spec = nets.RESNET20 if resnet else None if siamese else nets.NETS[name]
+        batch = 64 if siamese else spec["batch"]
         rng = np.random.RandomState(0)
-        shape = (2, 28, 28) if siamese else nets.NETS[name]["input"]
+        shape = (2, 28, 28) if siamese else spec["input"]
         x = torch.from_numpy(rng.rand(batch, *shape).astype(np.float32)).cuda()
         y = torch.from_numpy(rng.randint(0, 2 if siamese else 10, batch).astype(np.float32)).cuda()
         loss = torch.zeros(1, device="cuda")
@@ -132,7 +145,7 @@ def main():
         def native():
             assert net.forward_backward([x, y], loss.data_ptr(), stream=stream.cuda_stream), net.last_error()
 
-        module = (nets.siamese_module() if siamese else nets.torch_module(name)).cuda()
+        module = (nets.siamese_module() if siamese else nets.resnet20_module() if resnet else nets.torch_module(name)).cuda()
         with torch.no_grad():
             w, off = net.data().clone(), 0
             for p in module.parameters():

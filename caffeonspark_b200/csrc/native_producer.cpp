@@ -85,6 +85,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
   auto new_tensor = [&](int64_t n, int storage) {
     P.tensor_count.push_back(n);
     P.storage.push_back(storage < 0 ? static_cast<int>(P.tensor_count.size()) - 1 : storage);
+    P.data_alias.push_back(false);
     consumer.emplace_back();
     wants_grad.push_back(false);
     return static_cast<int>(P.tensor_count.size()) - 1;
@@ -108,22 +109,27 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     const bool known = L.type == "Convolution" || L.type == "Pooling" || L.type == "InnerProduct" || L.type == "ReLU" ||
                        L.type == "Sigmoid" || L.type == "BatchNorm" || L.type == "SoftmaxWithLoss" ||
                        L.type == "Slice" || L.type == "ContrastiveLoss" || L.type == "Concat" ||
-                       L.type == "EuclideanLoss" ||
+                       L.type == "EuclideanLoss" || L.type == "Split" || L.type == "Eltwise" || L.type == "Scale" ||
                        (L.type == "LRN" && L.norm_region == "WITHIN_CHANNEL");  // ACROSS_CHANNELS has no engine op
     if (!known) {
       *err = why(L, "layer type not supported");
       return false;
     }
-    // Slice is the one layer with several tops and Concat the one with any number of bottoms; ContrastiveLoss reads
-    // a, b and sim.  EuclideanLoss may leave its top out, as Caffe's solver tests write it (a loss layer's
-    // AutoTopBlobs): the engine writes the loss to loss_dev either way.
+    if (L.type == "Scale" && L.bottoms.size() == 2) {
+      *err = why(L, "the two-bottom form (the scale read from bottom[1]) is not supported");
+      return false;
+    }
+    // Slice and Split are the layers with several tops, Concat and Eltwise the ones with any number of bottoms (the
+    // parser checked Eltwise's at least 2); ContrastiveLoss reads a, b and sim.  EuclideanLoss may leave its top out,
+    // as Caffe's solver tests write it (a loss layer's AutoTopBlobs): the engine writes the loss to loss_dev either way.
     const size_t want_bottoms = L.type == "SoftmaxWithLoss" || L.type == "EuclideanLoss" ? 2
                                 : L.type == "ContrastiveLoss"                             ? 3
                                                                                           : 1;
+    const bool any_bottoms = L.type == "Concat" || L.type == "Eltwise";
     const bool auto_top = L.type == "EuclideanLoss" && L.tops.empty();
-    const bool tops_ok = L.type == "Slice" ? !L.tops.empty() : L.tops.size() == 1 || auto_top;
-    if ((L.type == "Concat" ? L.bottoms.empty() : L.bottoms.size() != want_bottoms) || !tops_ok) {
-      *err = why(L, (L.type == "Concat" ? std::string("needs at least 1") : std::to_string(want_bottoms)) +
+    const bool tops_ok = L.type == "Slice" || L.type == "Split" ? !L.tops.empty() : L.tops.size() == 1 || auto_top;
+    if ((any_bottoms ? L.bottoms.empty() : L.bottoms.size() != want_bottoms) || !tops_ok) {
+      *err = why(L, (any_bottoms ? std::string("needs at least 1") : std::to_string(want_bottoms)) +
                         " bottom(s) and one top");
       return false;
     }
@@ -161,6 +167,37 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         cur[L.tops[t]] = op.out;
         P.ops.push_back(op);
       }
+      continue;
+    }
+    if (L.type == "Split") {  // one op per top; each top reads the bottom's activation (split_layer.cpp ShareData)
+      op.kind = OpKind::kSplit;
+      for (size_t t = 0; t < L.tops.size(); ++t) {
+        op.split_top = static_cast<int>(t);
+        op.out = new_tensor(count_of(op.out_shape), -1);
+        P.data_alias[op.out] = true;
+        wants_grad[op.out] = op.need_dx;
+        cur[L.tops[t]] = op.out;
+        P.ops.push_back(op);
+      }
+      continue;
+    }
+    if (L.type == "Eltwise") {  // eltwise_layer.cpp: every bottom is consumed, the top has storage of its own
+      op.kind = OpKind::kEltwise;
+      op.eltwise_op = L.eltwise_op == "PROD" ? kEltwiseProd : L.eltwise_op == "MAX" ? kEltwiseMax : kEltwiseSum;
+      op.coeffs = L.coeffs;
+      op.stable_prod_grad = L.stable_prod_grad;
+      op.ins = {op.in};
+      op.ins_need_dx = {op.need_dx};
+      for (size_t b = 1; b < L.bottoms.size(); ++b) {
+        int id;
+        if (!take(L.bottoms[b], &id)) return false;
+        op.ins.push_back(id);
+        op.ins_need_dx.push_back(wants_grad[id]);
+      }
+      op.out = new_tensor(count_of(op.out_shape), -1);
+      for (bool need : op.ins_need_dx) wants_grad[op.out] = wants_grad[op.out] || need;
+      cur[L.tops[0]] = op.out;
+      P.ops.push_back(op);
       continue;
     }
     if (L.type == "Concat") {  // one op per bottom, each copying its bottom into its range of the one top (and back)
@@ -258,8 +295,9 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.kind = L.type == "ReLU" ? OpKind::kReLU : OpKind::kSigmoid;
       op.slope = L.negative_slope;
       // top == bottom shares the bottom's memory, except on a staged input: that is never written (every pass of an
-      // iter_size step reads it again), so the top gets storage of its own
-      op.in_place = L.tops[0] == L.bottoms[0] && op.in >= P.ninputs;
+      // iter_size step reads it again), so the top gets storage of its own.  So does a Split top: its memory is the
+      // Split's bottom, which the sibling tops read too.
+      op.in_place = L.tops[0] == L.bottoms[0] && op.in >= P.ninputs && !P.data_alias[op.in];
       if (op.in_place) storage = P.storage[op.in];
     } else if (L.type == "BatchNorm") {
       if (!op.shares.empty()) {
@@ -271,6 +309,17 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.global_stats = L.use_global_stats;
       op.fraction = L.moving_average_fraction;
       op.eps = L.eps;
+    } else if (L.type == "Scale") {  // scale_layer.cpp, one-bottom form; the parser resolved axis and num_axes
+      if (!filler_ok(L.weight_filler, &reason) || (L.bias_term && !filler_ok(L.bias_filler, &reason))) {
+        *err = why(L, reason);
+        return false;
+      }
+      op.kind = OpKind::kScale;  // separate top storage even when top == bottom: the scale's gradient reads x
+      set_params(L, &op, &P);
+      const size_t first = static_cast<size_t>(L.axis), end = first + static_cast<size_t>(L.num_axes);
+      op.scale_outer = count_of(std::vector<int64_t>(op.in_shape.begin(), op.in_shape.begin() + first));
+      op.scale_dim = count_of(std::vector<int64_t>(op.in_shape.begin() + first, op.in_shape.begin() + end));
+      op.scale_inner = count_of(std::vector<int64_t>(op.in_shape.begin() + end, op.in_shape.end()));
     } else if (L.type == "LRN") {
       if (L.local_size < 1 || L.local_size % 2 == 0 || L.local_size > kLrnMaxLocalSize) {
         *err = why(L, "local_size " + std::to_string(L.local_size) + " is not odd and <= " +
@@ -348,6 +397,15 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     if (!auto_top) cur[L.tops[0]] = op.out;
     P.ops.push_back(op);
   }
+  // the op of each Split's top 0 sums the gradients of the tops some layer reads (consumer[] is complete now)
+  for (size_t i = 0; i < P.ops.size(); ++i) {
+    if (P.ops[i].kind != OpKind::kSplit || P.ops[i].split_top != 0) continue;
+    for (size_t j = i; j < P.ops.size() && P.ops[j].kind == OpKind::kSplit && P.ops[j].in == P.ops[i].in; ++j) {
+      if (j > i && P.ops[j].split_top == 0) break;  // the next Split of the same bottom
+      if (consumer[P.ops[j].out].empty()) P.ops[j].split_unread = true;
+      else P.ops[i].split_sum.push_back(P.ops[j].out);
+    }
+  }
   if (losses == 0) {
     *err = "the net has no SoftmaxWithLoss, ContrastiveLoss or EuclideanLoss layer in its TRAIN phase (native producer)";
     return false;
@@ -370,13 +428,16 @@ bool plan_from_prototxt(const std::string& path, SolverSpec* spec, Plan* plan, s
 std::string Plan::text() const {
   static const char* kinds[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling", "InnerProduct",
                                 "ReLU",        "Sigmoid",             "BatchNorm", "SoftmaxWithLoss",
-                                "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss", "Concat", "EuclideanLoss"};
+                                "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss", "Concat", "EuclideanLoss",
+                                "Split", "Eltwise", "Scale"};
+  static const char* eltwise_ops[] = {"PROD", "SUM", "MAX"};
   std::ostringstream os;
   for (int i = 0; i < ninputs; ++i) os << "input " << i << " " << input_names[i] << " " << tensor_count[i] << "\n";
   for (size_t i = 0; i < ops.size(); ++i) {
     const Op& op = ops[i];
     os << "op " << i << " " << kinds[static_cast<int>(op.kind)];
     if (op.kind == OpKind::kPool) os << "(" << (op.max_pool ? "MAX" : "AVE") << ")";
+    if (op.kind == OpKind::kEltwise) os << "(" << eltwise_ops[op.eltwise_op] << ")";
     os << " " << op.name << " " << shape_str(op.in_shape) << " -> " << shape_str(op.out_shape);
     if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kPool)
       os << " k" << op.kh << "x" << op.kw << " s" << op.sh << "x" << op.sw << " p" << op.ph << "x" << op.pw;
@@ -397,11 +458,23 @@ std::string Plan::text() const {
       os << " second=" << op.in2 << " sim=" << op.label << " margin=" << op.margin << (op.legacy ? " legacy" : "")
          << " loss_weight=" << op.loss_weight;
     if (op.kind == OpKind::kEuclideanLoss) os << " second=" << op.in2 << " loss_weight=" << op.loss_weight;
+    if (op.kind == OpKind::kSplit) os << " top=" << op.split_top << " data=bottom" << (op.split_unread ? " unread" : "");
+    if (op.kind == OpKind::kEltwise) {
+      os << " bottoms=" << op.ins.size();
+      if (op.eltwise_op == kEltwiseSum) {
+        os << " coeff=";
+        for (size_t j = 0; j < op.coeffs.size(); ++j) os << (j ? "," : "") << op.coeffs[j];
+      }
+      if (op.eltwise_op == kEltwiseProd) os << (op.stable_prod_grad ? " stable_prod_grad" : " top/bottom_grad");
+    }
+    if (op.kind == OpKind::kScale)
+      os << " outer=" << op.scale_outer << " dim=" << op.scale_dim << " inner=" << op.scale_inner;
     if (op.in_place) os << " in-place";
     // no data gradient is propagated into a staged input, nor into a blob with no learnable blob before it
     auto mark = [&](int in, bool need) { return need ? "" : in < ninputs ? " staged-bottom" : " no-bottom-grad"; };
     const char* m = mark(op.in, op.need_dx);
     if (!*m && (op.kind == OpKind::kContrastiveLoss || op.kind == OpKind::kEuclideanLoss)) m = mark(op.in2, op.need_dx2);
+    for (size_t j = 1; j < op.ins.size() && !*m; ++j) m = mark(op.ins[j], op.ins_need_dx[j]);  // Eltwise
     os << m;
     os << "\n";
   }

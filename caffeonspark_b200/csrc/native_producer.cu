@@ -433,6 +433,74 @@ __global__ void __launch_bounds__(kThreads) euclidean_loss_kernel(const float* a
     *loss = __fmul_rn(loss_weight, __fdiv_rn(__fdiv_rn(part, static_cast<float>(num)), 2.f));
 }
 
+// ------------------------------------------------------------------ Split, Eltwise (split_layer.cpp, eltwise_layer.cpp)
+// dst = a + b: the Split backward's first two read tops (later ones go through accumulate_kernel, in top order)
+__global__ void add_kernel(const float* a, const float* b, float* dst, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] = __fadd_rn(a[i], b[i]);
+}
+// SUM, one bottom at a time in bottom order: y = c * x for the first (caffe_set(0) + axpy), then y = fma(c, x, y)
+__global__ void eltwise_axpy_kernel(const float* x, float c, float* y, int n, bool first) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    y[i] = first ? __fmul_rn(c, x[i]) : __fmaf_rn(c, x[i], y[i]);
+}
+// dst = c * src: SUM's backward for a coefficient other than 1
+__global__ void scale_copy_kernel(const float* src, float c, float* dst, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] = __fmul_rn(c, src[i]);
+}
+// dst = a * b: PROD's forward (y = b0 * b1, then y = y * b_i) and the stable backward's running product
+__global__ void mul_kernel(const float* a, const float* b, float* dst, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] = __fmul_rn(a[i], b[i]);
+}
+// PROD's backward without stable_prod_grad: dx = (y / x) * dy, two roundings (caffe_div, then caffe_mul)
+__global__ void prod_div_backward_kernel(const float* y, const float* x, const float* dy, float* dx, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    dx[i] = __fmul_rn(__fdiv_rn(y[i], x[i]), dy[i]);
+}
+// MAX, one bottom at a time (eltwise_layer.cpp Forward_cpu).  The first call (a non-null) compares bottoms 0 and 1:
+// bottom 0 wins only when strictly greater.  Every later bottom b takes over only when strictly greater than y.
+__global__ void eltwise_max_kernel(const float* a, const float* b, int b_index, float* y, int* idx, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = b[i];
+    if (a) {
+      const float u = a[i];
+      y[i] = u > v ? u : v;
+      idx[i] = u > v ? 0 : 1;
+    } else if (v > y[i]) {
+      y[i] = v;
+      idx[i] = b_index;
+    }
+  }
+}
+// dx = dy where bottom `which` won, else 0
+__global__ void eltwise_max_backward_kernel(const float* dy, const int* idx, int which, float* dx, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    dx[i] = idx[i] == which ? dy[i] : 0.f;
+}
+
+// ------------------------------------------------------------------ Scale (scale_layer.cu)
+// y[o, d, i] = x[o, d, i] * s[d] (+ b[d], one fused rounding); also the data gradient dx = dy * s with b null
+__global__ void scale_forward_kernel(const float* x, const float* s, const float* b, float* y, int n, int dim,
+                                     int inner) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const int d = (i / inner) % dim;
+    y[i] = b ? __fmaf_rn(x[i], __ldg(s + d), __ldg(b + d)) : __fmul_rn(x[i], __ldg(s + d));
+  }
+}
+// dst[d] += sum over (o, i) of dy[o, d, i] * x[o, d, i]: one block per scale element, each thread's products summed
+// in index order, then a fixed tree (bias_grad_kernel's order, with the product fused into each addition)
+__global__ void __launch_bounds__(kThreads) scale_grad_kernel(const float* dy, const float* x, int outer, int dim,
+                                                              int inner, float* dst) {
+  __shared__ float sh[kThreads];
+  const int d = blockIdx.x;
+  float s = 0.f;
+  for (int i = threadIdx.x; i < outer * inner; i += kThreads) {
+    const size_t j = ((size_t)(i / inner) * dim + d) * inner + i % inner;
+    s = __fmaf_rn(dy[j], x[j], s);
+  }
+  s = block_sum(s, sh);
+  if (threadIdx.x == 0) dst[d] = __fadd_rn(dst[d], s);
+}
+
 // ------------------------------------------------------------------ fillers (u: the cos_net_fill value in [-1, 1))
 __global__ void constant_fill_kernel(float* p, int n, float v) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = v;
@@ -571,7 +639,8 @@ bool NativeProducer::allocate(std::string* err) {
       return false;
     }
     grad_[t] = static_cast<float*>(g);
-    if (static_cast<int>(t) < plan_.ninputs) continue;
+    // a Split top's activation is its bottom's, set when the forward reaches it
+    if (static_cast<int>(t) < plan_.ninputs || plan_.data_alias[t]) continue;
     void* a;
     if (!alloc(bytes, &a)) return false;
     act_[t] = static_cast<float*>(a);
@@ -585,7 +654,7 @@ bool NativeProducer::allocate(std::string* err) {
     }
     grad_[t] = grad_[st];
     if (static_cast<int>(t) >= plan_.ninputs) act_[t] = act_[st];
-    if (!grad_[t] || (static_cast<int>(t) >= plan_.ninputs && !act_[t])) {
+    if (!grad_[t] || (static_cast<int>(t) >= plan_.ninputs && !plan_.data_alias[t] && !act_[t])) {
       *err = "native producer: tensor " + std::to_string(t) + " has no device storage";
       return false;
     }
@@ -608,7 +677,8 @@ bool NativeProducer::allocate(std::string* err) {
         op_z_[i] = static_cast<float*>(z), op_dz_[i] = static_cast<float*>(dz), op_aux_[i] = idx;
         ws = std::max(ws, static_cast<size_t>(d.N + 1) * d.Cout);  // bias partials + dbias
       }
-    } else if (op.kind == OpKind::kPool && op.max_pool) {
+    } else if ((op.kind == OpKind::kPool && op.max_pool) ||
+               (op.kind == OpKind::kEltwise && op.eltwise_op == kEltwiseMax)) {
       if (!alloc(out * sizeof(int), &op_aux_[i])) return false;
     } else if (op.kind == OpKind::kInnerProduct) {
       ws = std::max(ws, static_cast<size_t>(splits_of(static_cast<int>(op.in_shape[0]))) * op.w_count);
@@ -649,7 +719,7 @@ bool NativeProducer::fill(uint64_t seed, cudaStream_t s, std::string* err) {
     float* p = data_ + plan_.blob_off[k];
     const std::vector<int64_t>& sh = plan_.blob_shape[k];
     // filler.hpp: fan_in = count / shape(0), fan_out = count / shape(1) (count for a 1-axis blob)
-    const int fan_in = static_cast<int>(n / sh[0]);
+    const int fan_in = sh.empty() ? n : static_cast<int>(n / sh[0]);  // a 0-axis (scalar) blob: its one element
     const int fan_out = sh.size() > 1 ? static_cast<int>(n / sh[1]) : n;
     const float norm = f.variance_norm == "FAN_OUT" ? static_cast<float>(fan_out)
                        : f.variance_norm == "AVERAGE" ? static_cast<float>(fan_in + fan_out) / 2.0f
@@ -789,6 +859,30 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, cudaStream_t 
                                                            op.slice_begin * slice_inner(op), true);
       return cudaGetLastError();
     }
+    case OpKind::kSplit:  // no copy: the top reads the bottom's memory
+      act_[op.out] = act_[op.in];
+      return cudaSuccess;
+    case OpKind::kEltwise: {
+      const size_t nb = op.ins.size();
+      if (op.eltwise_op == kEltwiseSum) {
+        for (size_t b = 0; b < nb; ++b)
+          eltwise_axpy_kernel<<<grid_for(n), kThreads, 0, s>>>(act_[op.ins[b]], op.coeffs[b], y, n, b == 0);
+      } else if (op.eltwise_op == kEltwiseProd) {
+        mul_kernel<<<grid_for(n), kThreads, 0, s>>>(act_[op.ins[0]], act_[op.ins[1]], y, n);
+        for (size_t b = 2; b < nb; ++b) mul_kernel<<<grid_for(n), kThreads, 0, s>>>(y, act_[op.ins[b]], y, n);
+      } else {
+        int* idx = static_cast<int*>(op_aux_[i]);
+        eltwise_max_kernel<<<grid_for(n), kThreads, 0, s>>>(act_[op.ins[0]], act_[op.ins[1]], 1, y, idx, n);
+        for (size_t b = 2; b < nb; ++b)
+          eltwise_max_kernel<<<grid_for(n), kThreads, 0, s>>>(nullptr, act_[op.ins[b]], static_cast<int>(b), y, idx, n);
+      }
+      return cudaGetLastError();
+    }
+    case OpKind::kScale:
+      scale_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, data_ + op.w_off, op.b_off >= 0 ? data_ + op.b_off : nullptr,
+                                                            y, n, static_cast<int>(op.scale_dim),
+                                                            static_cast<int>(op.scale_inner));
+      return cudaGetLastError();
     case OpKind::kLRNWithin:
       return lrn_within_forward(x, y, static_cast<int>(op.in_shape[0]), static_cast<int>(op.in_shape[1]),
                                 static_cast<int>(op.in_shape[2]), static_cast<int>(op.in_shape[3]), op.lrn_size,
@@ -870,6 +964,54 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
                                                            slice_span(op, op.out_shape),
                                                            op.slice_begin * slice_inner(op), false);
       return cudaGetLastError();
+    case OpKind::kSplit: {  // top 0's op: dx = the read tops' gradients summed in top order; the other tops' do nothing
+      if (!dx || op.split_top != 0) return cudaSuccess;
+      const std::vector<int>& g = op.split_sum;
+      const size_t bytes = static_cast<size_t>(nin) * sizeof(float);
+      if (g.empty()) return cudaMemsetAsync(dx, 0, bytes, s);
+      if (g.size() == 1) return cudaMemcpyAsync(dx, grad_[g[0]], bytes, cudaMemcpyDeviceToDevice, s);
+      add_kernel<<<grid_for(nin), kThreads, 0, s>>>(grad_[g[0]], grad_[g[1]], dx, nin);
+      for (size_t k = 2; k < g.size(); ++k) accumulate_kernel<<<grid_for(nin), kThreads, 0, s>>>(dx, grad_[g[k]], nin);
+      return cudaGetLastError();
+    }
+    case OpKind::kEltwise: {  // eltwise_layer.cpp Backward_cpu, bottom by bottom
+      const size_t nb = op.ins.size();
+      const size_t bytes = static_cast<size_t>(nin) * sizeof(float);
+      for (size_t b = 0; b < nb; ++b) {
+        if (!op.ins_need_dx[b]) continue;
+        float* db = grad_[op.ins[b]];
+        cudaError_t e = cudaSuccess;
+        if (op.eltwise_op == kEltwiseSum) {
+          if (op.coeffs[b] == 1.f) e = cudaMemcpyAsync(db, dy, bytes, cudaMemcpyDeviceToDevice, s);
+          else scale_copy_kernel<<<grid_for(nin), kThreads, 0, s>>>(dy, op.coeffs[b], db, nin);
+        } else if (op.eltwise_op == kEltwiseMax) {
+          eltwise_max_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(dy, static_cast<const int*>(op_aux_[i]),
+                                                                         static_cast<int>(b), db, nin);
+        } else if (op.stable_prod_grad) {  // the product of the other bottoms in bottom order, then times dy
+          bool first = true;
+          for (size_t j = 0; j < nb && e == cudaSuccess; ++j) {
+            if (j == b) continue;
+            if (first) e = cudaMemcpyAsync(db, act_[op.ins[j]], bytes, cudaMemcpyDeviceToDevice, s);
+            else mul_kernel<<<grid_for(nin), kThreads, 0, s>>>(act_[op.ins[j]], db, db, nin);
+            first = false;
+          }
+          if (e == cudaSuccess) mul_kernel<<<grid_for(nin), kThreads, 0, s>>>(db, dy, db, nin);
+        } else {
+          prod_div_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(act_[op.out], act_[op.ins[b]], dy, db, nin);
+        }
+        if (e == cudaSuccess) e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+      }
+      return cudaSuccess;
+    }
+    case OpKind::kScale: {
+      const int outer = static_cast<int>(op.scale_outer), dim = static_cast<int>(op.scale_dim);
+      const int inner = static_cast<int>(op.scale_inner);
+      scale_grad_kernel<<<dim, kThreads, 0, s>>>(dy, x, outer, dim, inner, diff_ + op.w_off);
+      if (op.b_off >= 0) bias_grad_kernel<<<dim, kThreads, 0, s>>>(dy, outer, dim, inner, diff_ + op.b_off);
+      if (dx) scale_forward_kernel<<<grid_for(nin), kThreads, 0, s>>>(dy, data_ + op.w_off, nullptr, dx, nin, dim, inner);
+      return cudaGetLastError();
+    }
     default:  // SoftmaxWithLoss, ContrastiveLoss and EuclideanLoss wrote their bottom gradients in the forward pass
       return cudaSuccess;
   }

@@ -1,6 +1,6 @@
 // native_producer.hpp -- the built-in gradient producer (Net::ForwardBackward for the TRAIN phase of the LeNet,
-// CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, and least-squares regression nets;
-// DESIGN.md section 14).
+// CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, least-squares regression nets and
+// residual nets built of Split, Eltwise and Scale; DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -22,8 +22,10 @@ namespace cosb {
 
 enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
-  kContrastiveLoss, kConcat, kEuclideanLoss
+  kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale
 };
+
+enum EltwiseOp { kEltwiseProd = 0, kEltwiseSum = 1, kEltwiseMax = 2 };  // caffe.proto EltwiseParameter numbering
 
 struct Op {
   OpKind kind;
@@ -53,12 +55,28 @@ struct Op {
   int64_t slice_begin = 0;
   float margin = 1.f;                  // ContrastiveLoss
   bool legacy = false;
+  // Split: this op's top index.  Its top's activation is the bottom's (Plan::data_alias); the op of top 0 sums the
+  // gradients of split_sum (the tops some layer reads, in top order) into the bottom's, and the others do nothing.
+  int split_top = 0;
+  std::vector<int> split_sum;
+  bool split_unread = false;           // no layer reads this top: it adds nothing to the bottom's gradient
+  // Eltwise: every bottom (ins[0] == in) and whether it wants a gradient; coeffs for SUM
+  std::vector<int> ins;
+  std::vector<bool> ins_need_dx;
+  int eltwise_op = kEltwiseSum;
+  std::vector<float> coeffs;
+  bool stable_prod_grad = true;
+  // Scale: y[o, d, i] = x[o, d, i] * s[d] (+ b[d]) over outer o, scale_dim d and inner i; w_off / b_off are s and b
+  int64_t scale_outer = 1, scale_dim = 1, scale_inner = 1;
 };
 
 struct Plan {
   std::vector<Op> ops;
   std::vector<int64_t> tensor_count;   // elements per tensor id
   std::vector<int> storage;            // tensor id -> tensor id that owns its memory (itself unless in place)
+  // per tensor id: its activation is another tensor's memory, set when the forward reaches it (a Split top reads its
+  // bottom's, as Caffe's ShareData); its gradient is still its own
+  std::vector<bool> data_alias;
   int ninputs = 0;                     // tensors 0 .. ninputs-1 are the staged inputs, in data-layer top order
   std::vector<std::string> input_names;
   std::vector<int64_t> blob_off, blob_count;  // every learnable blob, learnable_params() order
@@ -68,7 +86,7 @@ struct Plan {
   std::string text() const;  // one op per line (cos_native_producer_plan)
 };
 
-// Builds the plan of a parsed TRAIN net (a Slice layer becomes one kSlice op per top, a Concat layer one kConcat op
+// Builds the plan of a parsed TRAIN net (a Slice or Split layer becomes one op per top, a Concat layer one kConcat op
 // per bottom); false with
 // "layer '<name>' (<type>): <reason>" when it cannot be run.
 bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Plan* plan, std::string* err);
@@ -105,7 +123,8 @@ class NativeProducer {
   float* diff_;
   int* status_;
   std::vector<float*> act_, grad_;        // per tensor id (staged inputs: act_ is the caller's buffer, set per call)
-  std::vector<void*> op_aux_;             // per op: MAX pool argmax (int32), fused block index (uint8), BN save
+  std::vector<void*> op_aux_;             // per op: MAX pool / Eltwise MAX argmax (int32), fused block index (uint8),
+                                          // BN save
   std::vector<float*> op_z_, op_dz_;      // fused block: conv output without bias and its gradient
   cudaEvent_t done_ = nullptr;            // recorded at the end of every call: the destructor waits for it
   float* workspace_ = nullptr;            // split-K partials, bias partials, BatchNorm scratch (ops run in order)

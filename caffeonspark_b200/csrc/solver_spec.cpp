@@ -252,6 +252,12 @@ long prod(const Shape& s, size_t from = 0) {
   return p;
 }
 
+std::string shape_text(const Shape& s) {  // "2x3x4", "scalar"
+  std::string t;
+  for (size_t i = 0; i < s.size(); ++i) t += (i ? "x" : "") + std::to_string(s[i]);
+  return s.empty() ? "scalar" : t;
+}
+
 struct HW { long h, w; };
 
 // kernel_size / kernel_h,kernel_w style repeated-or-pair fields
@@ -509,7 +515,7 @@ bool net_layout(const Node& net, const std::string& net_file, SolverSpec* spec, 
       rec.bias_filler = filler(p->first("bias_filler"));
     } else if (type == "ReLU" || type == "LRN" || type == "Dropout" || type == "Sigmoid" || type == "TanH" ||
                type == "Softmax" || type == "Power" || type == "AbsVal" || type == "BNLL" || type == "ELU" ||
-               type == "Exp" || type == "Log" || type == "Threshold" || type == "Split" || type == "Eltwise") {
+               type == "Exp" || type == "Log" || type == "Threshold") {
       Shape in;
       if (!bottom_shape(0, &in)) return false;
       for (const std::string& t : tops) blobs[t] = in;
@@ -523,6 +529,84 @@ bool net_layout(const Node& net, const std::string& net_file, SolverSpec* spec, 
         if (rec.norm_region == "0") rec.norm_region = "ACROSS_CHANNELS";  // the enum's numeric form
         if (rec.norm_region == "1") rec.norm_region = "WITHIN_CHANNEL";
       }
+    } else if (type == "Split") {  // split_layer.cpp Reshape
+      Shape in;
+      if (!bottom_shape(0, &in)) return false;
+      for (const std::string& t : tops) {
+        if (t == bottoms[0]) return refuse("Split Layer does not allow in-place computation.");
+        blobs[t] = in;
+      }
+    } else if (type == "Eltwise") {  // eltwise_layer.cpp LayerSetUp and Reshape, after Layer::CheckBlobCounts
+      if (bottoms.size() < 2) return refuse("Eltwise Layer takes at least 2 bottom blob(s) as input.");
+      Shape in;
+      if (!bottom_shape(0, &in)) return false;
+      const Node* p = L->first("eltwise_param");
+      auto coeffs = p ? p->all("coeff") : std::vector<const Node*>();
+      if (!coeffs.empty() && coeffs.size() != bottoms.size())
+        return refuse("Eltwise Layer takes one coefficient per bottom blob.");
+      std::string op = p ? p->str("operation", "SUM") : "SUM";
+      if (op == "0") op = "PROD";  // the enum's numeric form
+      if (op == "1") op = "SUM";
+      if (op == "2") op = "MAX";
+      if (op != "PROD" && op != "SUM" && op != "MAX") return refuse("Unknown elementwise operation.");
+      if (op == "PROD" && !coeffs.empty()) return refuse("Eltwise layer only takes coefficients for summation.");
+      rec.eltwise_op = op;
+      rec.coeffs.assign(bottoms.size(), 1.f);
+      for (size_t i = 0; i < coeffs.size(); ++i) rec.coeffs[i] = static_cast<float>(atof(coeffs[i]->value.c_str()));
+      rec.stable_prod_grad = !p || p->boolean("stable_prod_grad", true);
+      for (size_t i = 1; i < bottoms.size(); ++i) {
+        Shape s;
+        if (!bottom_shape(i, &s)) return false;
+        if (s != in)
+          return refuse("bottom " + std::to_string(i) + " is " + shape_text(s) + ", bottom 0 " + shape_text(in) +
+                        " (Check failed: bottom[i]->shape() == bottom[0]->shape())");
+      }
+      for (const std::string& t : tops) blobs[t] = in;
+    } else if (type == "Scale") {  // scale_layer.cpp LayerSetUp and Reshape; the bias as bias_layer.cpp sets it up
+      if (bottoms.size() > 2) return refuse("Scale Layer takes at most 2 bottom blob(s) as input.");
+      Shape in;
+      if (!bottom_shape(0, &in)) return false;
+      const Node* p = L->first("scale_param");
+      const long naxes = static_cast<long>(in.size());
+      const long given = p ? p->integer("axis", 1) : 1;
+      const long axis = given < 0 ? given + naxes : given;
+      if (axis < 0 || axis >= naxes)  // Blob::CanonicalAxisIndex
+        return refuse("axis " + std::to_string(given) + " out of range for " + std::to_string(naxes) + "-D Blob");
+      Shape scale;  // the scale blob's shape, or bottom[1]'s
+      if (bottoms.size() == 1) {
+        const long num_axes = p ? p->integer("num_axes", 1) : 1;
+        if (num_axes < -1) return refuse("num_axes must be non-negative, or -1 to extend to the end of bottom[0]");
+        if (num_axes >= 0 && naxes < axis + num_axes)
+          return refuse("scale blob's shape extends past bottom[0]'s shape when applied starting with bottom[0] axis = " +
+                        std::to_string(axis));
+        scale.assign(in.begin() + axis, num_axes == -1 ? in.end() : in.begin() + axis + num_axes);
+        param_counts.push_back(prod(scale));
+        param_shapes.push_back(to64(scale));
+      } else if (!bottom_shape(1, &scale)) {
+        return false;
+      }
+      const long first = scale.empty() ? 0 : axis;  // Reshape: a scalar scale applies from axis 0
+      if (naxes < first + static_cast<long>(scale.size()))
+        return refuse("scale blob's shape extends past bottom[0]'s shape when applied starting with bottom[0] axis = " +
+                      std::to_string(first));
+      for (size_t i = 0; i < scale.size(); ++i)
+        if (in[first + i] != scale[i])
+          return refuse("dimension mismatch between bottom[0]->shape(" + std::to_string(first + i) +
+                        ") and scale->shape(" + std::to_string(i) + ")");
+      rec.bias_term = p && p->boolean("bias_term", false);
+      if (rec.bias_term) {  // the Bias layer's blob: the scale's shape (bottom[1]'s in the two-bottom form)
+        param_counts.push_back(prod(scale));
+        param_shapes.push_back(to64(scale));
+      }
+      rec.axis = first;
+      rec.num_axes = static_cast<int64_t>(scale.size());
+      if (p && p->first("filler")) {
+        rec.weight_filler = filler(p->first("filler"));
+      } else {
+        rec.weight_filler.value = 1.f;  // unit scale: a constant 1 filler
+      }
+      rec.bias_filler = filler(p ? p->first("bias_filler") : nullptr);
+      for (const std::string& t : tops) blobs[t] = in;
     } else if (type == "Flatten") {
       Shape in;
       if (!bottom_shape(0, &in) || in.empty()) return false;

@@ -52,6 +52,14 @@ struct NetLayer {
   // ContrastiveLoss (caffe.proto ContrastiveLossParameter)
   float margin = 1.f;
   bool legacy_version = false;
+  // Scale (scale_layer.cpp): `axis` is the first scaled axis (0 when the scale is a scalar, as Reshape sets it) and
+  // num_axes the scale's number of axes (-1 resolved); bias_term defaults to false here.  weight_filler is the scale's
+  // filler (constant 1 when the prototxt gives none), bias_filler the bias's.
+  int64_t num_axes = 1;
+  // Eltwise (caffe.proto EltwiseParameter): "PROD", "SUM" or "MAX"; one coeff per bottom (all 1 when none are given)
+  std::string eltwise_op = "SUM";
+  std::vector<float> coeffs;
+  bool stable_prod_grad = true;
   FillerSpec weight_filler, bias_filler;
 };
 

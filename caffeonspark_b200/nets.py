@@ -353,3 +353,65 @@ def contrastive_loss(a, b, sim, margin=1.0, legacy=False, loss_weight=1.0):
             return g.reshape(ctx.shapes[0]), (-g).reshape(ctx.shapes[1])
 
     return _Loss.apply(a, b)
+
+
+# He et al.'s CIFAR-10 ResNet-20 (tests/golden/configs/cifar10_resnet20_train_test.prototxt): conv1 and three stages of
+# three basic blocks, every convolution bias-free and followed by BatchNorm + Scale (with bias), explicit Splits,
+# Eltwise SUM shortcuts with a 1x1 stride-2 projection where the shape changes, global AVE pooling and a 10-way
+# InnerProduct.  Batch 100 of 3x32x32.
+RESNET20 = dict(input=(3, 32, 32), batch=100, classes=10, stages=(16, 32, 64), blocks=3)
+
+
+def resnet20_module():
+    """ResNet-20 as one PyTorch module with its parameters in learnable_params() order: per convolution its weight, the
+    BatchNorm's three statistics and the Scale's scale and bias; per block branch2a, branch2b, then the projection
+    (branch1) where there is one; the InnerProduct last.  forward(x [N, 3, 32, 32]) -> scores [N, 10]."""
+    import torch
+    import torch.nn as nn
+    from .layers import BatchNorm
+
+    class Scale(nn.Module):
+        """Caffe's Scale with bias_term over axis 1: y = x * s[c] + b[c] (scale_layer.cpp), s filled with 1, b with 0."""
+
+        def __init__(self, channels):
+            super().__init__()
+            self.weight = nn.Parameter(torch.ones(channels))
+            self.bias = nn.Parameter(torch.zeros(channels))
+
+        def forward(self, x):
+            shape = (1, -1) + (1,) * (x.dim() - 2)
+            return x * self.weight.view(shape) + self.bias.view(shape)
+
+    def unit(cin, cout, k, stride):  # conv (no bias) + BatchNorm + Scale
+        return nn.Sequential(nn.Conv2d(cin, cout, k, stride=stride, padding=k // 2, bias=False), BatchNorm(cout),
+                             Scale(cout))
+
+    class Block(nn.Module):
+        def __init__(self, cin, cout):
+            super().__init__()
+            stride = 1 if cin == cout else 2
+            self.branch2a = unit(cin, cout, 3, stride)
+            self.branch2b = unit(cout, cout, 3, 1)
+            self.branch1 = unit(cin, cout, 1, 2) if cin != cout else None
+
+        def forward(self, x):
+            y = self.branch2b(self.branch2a(x).relu())
+            return (y + (self.branch1(x) if self.branch1 is not None else x)).relu()
+
+    class ResNet20(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.conv1 = unit(3, 16, 3, 1)
+            blocks, cin = [], 16
+            for cout in RESNET20["stages"]:
+                for _ in range(RESNET20["blocks"]):
+                    blocks.append(Block(cin, cout))
+                    cin = cout
+            self.blocks = nn.Sequential(*blocks)
+            self.fc10 = nn.Linear(cin, RESNET20["classes"])
+
+        def forward(self, x):
+            y = self.blocks(self.conv1(x).relu())
+            return self.fc10(y.mean(dim=(2, 3)))
+
+    return ResNet20()
