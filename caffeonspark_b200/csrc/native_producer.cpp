@@ -2,6 +2,7 @@
 #include "native_producer.hpp"
 
 #include <cmath>
+#include <iterator>
 #include <map>
 #include <sstream>
 
@@ -53,16 +54,74 @@ bool fusable_pool(const NetLayer& L) {
          L.tops.size() == 1 && L.bottom_shapes[0].size() == 4;
 }
 
-// The weight (and bias) of a Convolution or InnerProduct: a shared param uses its owner's offsets, and only the owner's
-// filler fills the blob.
-void set_params(const NetLayer& L, Op* op, Plan* P) {
+// The weight (and bias) of a Convolution, InnerProduct or Scale: a shared param uses its owner's offsets, and only the
+// owner's filler fills the blob.  False when a filler is one the engine cannot draw.
+bool set_params(const NetLayer& L, Op* op, Plan* P, std::string* err) {
+  std::string reason;
+  if (!filler_ok(L.weight_filler, &reason) || (L.bias_term && !filler_ok(L.bias_filler, &reason))) {
+    *err = why(L, reason);
+    return false;
+  }
   op->w_off = P->blob_off[L.blobs[0]], op->w_count = P->blob_count[L.blobs[0]];
   if (!L.shared[0]) P->blob_filler[L.blobs[0]] = L.weight_filler;
   if (L.bias_term) {
     op->b_off = P->blob_off[L.blobs[1]], op->b_count = P->blob_count[L.blobs[1]];
     if (!L.shared[1]) P->blob_filler[L.blobs[1]] = L.bias_filler;
   }
+  return true;
 }
+
+// euclidean_loss_layer.cpp, after LossLayer::Reshape's check
+bool euclidean_shapes_ok(const NetLayer& L, std::string* err) {
+  const std::vector<int64_t>& a = L.bottom_shapes[0];
+  const std::vector<int64_t>& b = L.bottom_shapes[1];
+  if (a.empty() || b.empty() || a[0] != b[0]) {
+    *err = why(L, "The data and label should have the same number.");
+    return false;
+  }
+  if (count_of(std::vector<int64_t>(a.begin() + 1, a.end())) !=
+      count_of(std::vector<int64_t>(b.begin() + 1, b.end()))) {  // Blob::count(1)
+    *err = why(L, "Inputs must have the same dimension.");
+    return false;
+  }
+  return true;
+}
+
+// The layer types the engine runs.  bottoms: the exact count, or -1 for any number from 1 (the parser checked
+// Eltwise's at least 2).  several_tops: one op per top.  label: the label-like bottom (read, never differentiated and
+// not counted as its blob's reader), called `role` in refusals, or -1.  loss: a net has one loss layer.
+struct LayerType {
+  const char* type;
+  OpKind kind;
+  int bottoms = 1;
+  bool several_tops = false;
+  int label = -1;
+  const char* role = nullptr;
+  bool loss = false;
+};
+const LayerType kLayerTypes[] = {
+    {"Convolution", OpKind::kConv},
+    {"Pooling", OpKind::kPool},
+    {"InnerProduct", OpKind::kInnerProduct},
+    {"ReLU", OpKind::kReLU},
+    {"Sigmoid", OpKind::kSigmoid},
+    {"BatchNorm", OpKind::kBatchNorm},
+    {"LRN", OpKind::kLRNWithin},  // WITHIN_CHANNEL only: ACROSS_CHANNELS has no engine op
+    {"Slice", OpKind::kSlice, 1, true},
+    {"Split", OpKind::kSplit, 1, true},
+    {"Concat", OpKind::kConcat, -1},
+    {"Eltwise", OpKind::kEltwise, -1},
+    {"Scale", OpKind::kScale},  // the one-bottom form
+    {"SoftmaxWithLoss", OpKind::kSoftmaxLoss, 2, false, 1, "label", true},
+    {"ContrastiveLoss", OpKind::kContrastiveLoss, 3, false, 2, "sim", true},  // a, b, sim
+    {"EuclideanLoss", OpKind::kEuclideanLoss, 2, false, -1, nullptr, true},
+};
+
+// Plan::text's name of each OpKind
+const char* const kKindNames[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling", "InnerProduct", "ReLU", "Sigmoid",
+                                  "BatchNorm", "SoftmaxWithLoss", "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss",
+                                  "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale"};
+static_assert(std::size(kKindNames) == static_cast<size_t>(OpKind::kCount), "one name per OpKind");
 
 }  // namespace
 
@@ -99,6 +158,8 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
   }
   P.ninputs = static_cast<int>(P.tensor_count.size());
   int losses = 0;
+  int loss_top = -1;  // the loss layer's top: never written, the loss goes to loss_dev
+  std::string loss_layer;
   for (size_t i = 0; i < layers.size(); ++i) {
     const NetLayer& L = layers[i];
     if (is_data_layer(L.type) || L.type == "Accuracy" || L.type == "Silence") continue;  // no TRAIN work
@@ -106,122 +167,113 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       *err = why(L, "loss_param is not supported (only the default VALID normalisation without ignore_label is)");
       return false;
     }
-    const bool known = L.type == "Convolution" || L.type == "Pooling" || L.type == "InnerProduct" || L.type == "ReLU" ||
-                       L.type == "Sigmoid" || L.type == "BatchNorm" || L.type == "SoftmaxWithLoss" ||
-                       L.type == "Slice" || L.type == "ContrastiveLoss" || L.type == "Concat" ||
-                       L.type == "EuclideanLoss" || L.type == "Split" || L.type == "Eltwise" || L.type == "Scale" ||
-                       (L.type == "LRN" && L.norm_region == "WITHIN_CHANNEL");  // ACROSS_CHANNELS has no engine op
-    if (!known) {
+    const LayerType* row = nullptr;
+    for (const LayerType& r : kLayerTypes)
+      if (L.type == r.type) row = &r;
+    if (!row || (row->kind == OpKind::kLRNWithin && L.norm_region != "WITHIN_CHANNEL")) {
       *err = why(L, "layer type not supported");
       return false;
     }
-    if (L.type == "Scale" && L.bottoms.size() == 2) {
+    if (row->kind == OpKind::kScale && L.bottoms.size() == 2) {
       *err = why(L, "the two-bottom form (the scale read from bottom[1]) is not supported");
       return false;
     }
-    // Slice and Split are the layers with several tops, Concat and Eltwise the ones with any number of bottoms (the
-    // parser checked Eltwise's at least 2); ContrastiveLoss reads a, b and sim.  EuclideanLoss may leave its top out,
-    // as Caffe's solver tests write it (a loss layer's AutoTopBlobs): the engine writes the loss to loss_dev either way.
-    const size_t want_bottoms = L.type == "SoftmaxWithLoss" || L.type == "EuclideanLoss" ? 2
-                                : L.type == "ContrastiveLoss"                             ? 3
-                                                                                          : 1;
-    const bool any_bottoms = L.type == "Concat" || L.type == "Eltwise";
-    const bool auto_top = L.type == "EuclideanLoss" && L.tops.empty();
-    const bool tops_ok = L.type == "Slice" || L.type == "Split" ? !L.tops.empty() : L.tops.size() == 1 || auto_top;
-    if ((any_bottoms ? L.bottoms.empty() : L.bottoms.size() != want_bottoms) || !tops_ok) {
-      *err = why(L, (any_bottoms ? std::string("needs at least 1") : std::to_string(want_bottoms)) +
+    // EuclideanLoss may leave its top out, as Caffe's solver tests write it (a loss layer's AutoTopBlobs): the engine
+    // writes the loss to loss_dev either way.
+    const bool auto_top = row->kind == OpKind::kEuclideanLoss && L.tops.empty();
+    const bool tops_ok = row->several_tops ? !L.tops.empty() : L.tops.size() == 1 || auto_top;
+    if ((row->bottoms < 0 ? L.bottoms.empty() : L.bottoms.size() != static_cast<size_t>(row->bottoms)) || !tops_ok) {
+      *err = why(L, (row->bottoms < 0 ? std::string("needs at least 1") : std::to_string(row->bottoms)) +
                         " bottom(s) and one top");
       return false;
     }
     Op op;
+    op.kind = row->kind;
     op.name = L.name;
-    for (size_t j = 0; j < L.blobs.size(); ++j)
-      if (L.shared[j]) op.shares.push_back(L.blobs[j]);
-    auto take = [&](const std::string& name, int* id) {
-      auto it = cur.find(name);
-      if (it == cur.end()) {
-        *err = why(L, "bottom '" + name + "' is not produced by an earlier TRAIN layer");
-        return false;
-      }
-      if (!consumer[it->second].empty()) {
-        *err = why(L, "bottom '" + name + "' already feeds layer '" + consumer[it->second] +
-                          "'; a blob read by two layers needs a Split");
-        return false;
-      }
-      consumer[it->second] = L.name;
-      *id = it->second;
-      return true;
-    };
-    if (!take(L.bottoms[0], &op.in)) return false;
+    op.label_bottom = row->label;
     op.in_shape = L.bottom_shapes[0];
     if (!auto_top) op.out_shape = L.top_shapes[0];  // else the scalar loss
-    op.need_dx = wants_grad[op.in];
-    if (L.type == "Slice") {  // one op per top, each copying its range of the bottom (and back, in the backward)
-      op.kind = OpKind::kSlice;
+    if (row->loss) op.loss_weight = L.loss_weight;
+    for (size_t j = 0; j < L.blobs.size(); ++j)
+      if (L.shared[j]) op.shares.push_back(L.blobs[j]);
+    bool top_grad = false;  // the top wants a gradient when a bottom does (or, below, when the op has a weight or bias)
+    for (size_t b = 0; b < L.bottoms.size(); ++b) {
+      const std::string& name = L.bottoms[b];
+      const bool label = static_cast<int>(b) == row->label;
+      auto it = cur.find(name);
+      if (it == cur.end()) {
+        *err = why(L, (label ? std::string(row->role) + " " : std::string()) + "bottom '" + name +
+                          "' is not produced by an earlier TRAIN layer");
+        return false;
+      }
+      const int id = it->second;
+      if (id == loss_top) {
+        *err = why(L, "bottom '" + name + "' is the top of loss layer '" + loss_layer +
+                          "'; reading a loss layer's top is not supported");
+        return false;
+      }
+      if (!label) {
+        if (!consumer[id].empty()) {
+          *err = why(L, "bottom '" + name + "' already feeds layer '" + consumer[id] +
+                            "'; a blob read by two layers needs a Split");
+          return false;
+        }
+        consumer[id] = L.name;
+      }
+      op.bottoms.push_back(id);
+      op.bottom_grad.push_back(!label && wants_grad[id]);
+      top_grad = top_grad || op.bottom_grad.back();
+      if (b > 0 || !row->loss) continue;
+      // a loss layer's own checks come after its first bottom, before the others
+      if (++losses > 1) {
+        *err = why(L, "a second loss layer is not supported");
+        return false;
+      }
+      if (row->kind == OpKind::kEuclideanLoss && !euclidean_shapes_ok(L, err)) return false;
+    }
+    if (op.kind == OpKind::kSlice) {  // one op per top, each copying its range of the bottom (and back, in the backward)
       op.slice_axis = static_cast<int>(L.axis);
       for (size_t t = 0; t < L.tops.size(); ++t) {
         op.slice_begin = L.slice_begin[t];
         op.out_shape = L.top_shapes[t];
         op.out = new_tensor(count_of(op.out_shape), -1);
-        wants_grad[op.out] = op.need_dx;
+        wants_grad[op.out] = top_grad;
         cur[L.tops[t]] = op.out;
         P.ops.push_back(op);
       }
       continue;
     }
-    if (L.type == "Split") {  // one op per top; each top reads the bottom's activation (split_layer.cpp ShareData)
-      op.kind = OpKind::kSplit;
+    if (op.kind == OpKind::kSplit) {  // one op per top; each top reads the bottom's activation (split_layer.cpp ShareData)
       for (size_t t = 0; t < L.tops.size(); ++t) {
         op.split_top = static_cast<int>(t);
         op.out = new_tensor(count_of(op.out_shape), -1);
         P.data_alias[op.out] = true;
-        wants_grad[op.out] = op.need_dx;
+        wants_grad[op.out] = top_grad;
         cur[L.tops[t]] = op.out;
         P.ops.push_back(op);
       }
       continue;
     }
-    if (L.type == "Eltwise") {  // eltwise_layer.cpp: every bottom is consumed, the top has storage of its own
-      op.kind = OpKind::kEltwise;
-      op.eltwise_op = L.eltwise_op == "PROD" ? kEltwiseProd : L.eltwise_op == "MAX" ? kEltwiseMax : kEltwiseSum;
-      op.coeffs = L.coeffs;
-      op.stable_prod_grad = L.stable_prod_grad;
-      op.ins = {op.in};
-      op.ins_need_dx = {op.need_dx};
-      for (size_t b = 1; b < L.bottoms.size(); ++b) {
-        int id;
-        if (!take(L.bottoms[b], &id)) return false;
-        op.ins.push_back(id);
-        op.ins_need_dx.push_back(wants_grad[id]);
-      }
-      op.out = new_tensor(count_of(op.out_shape), -1);
-      for (bool need : op.ins_need_dx) wants_grad[op.out] = wants_grad[op.out] || need;
-      cur[L.tops[0]] = op.out;
-      P.ops.push_back(op);
-      continue;
-    }
-    if (L.type == "Concat") {  // one op per bottom, each copying its bottom into its range of the one top (and back)
-      op.kind = OpKind::kConcat;
+    if (op.kind == OpKind::kConcat) {  // one op per bottom, each copying its bottom into its range of the one top (and back)
       op.slice_axis = static_cast<int>(L.axis);  // the parser checked the axis and the bottoms' shapes
       op.out = new_tensor(count_of(op.out_shape), -1);
+      wants_grad[op.out] = top_grad;
       int64_t begin = 0;
       for (size_t b = 0; b < L.bottoms.size(); ++b) {
-        if (b > 0) {
-          if (!take(L.bottoms[b], &op.in)) return false;
-          op.in_shape = L.bottom_shapes[b];
-          op.need_dx = wants_grad[op.in];
-        }
-        op.slice_begin = begin;
-        begin += op.in_shape[op.slice_axis];
-        wants_grad[op.out] = wants_grad[op.out] || op.need_dx;
-        P.ops.push_back(op);
+        Op part = op;
+        part.bottoms = {op.bottoms[b]};
+        part.bottom_grad = {op.bottom_grad[b]};
+        part.in_shape = L.bottom_shapes[b];
+        part.slice_begin = begin;
+        begin += part.in_shape[op.slice_axis];
+        P.ops.push_back(part);
       }
       cur[L.tops[0]] = op.out;
       continue;
     }
     int storage = -1;
-    std::string reason;
-    if (L.type == "Convolution") {
+    const std::string* top = auto_top ? nullptr : &L.tops[0];
+    if (op.kind == OpKind::kConv) {
       if (L.group != 1) {
         *err = why(L, "group " + std::to_string(L.group) + " > 1 is not supported");
         return false;
@@ -230,15 +282,10 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         *err = why(L, "dilation other than 1 is not supported");
         return false;
       }
-      if (!filler_ok(L.weight_filler, &reason) || (L.bias_term && !filler_ok(L.bias_filler, &reason))) {
-        *err = why(L, reason);
-        return false;
-      }
-      op.kind = OpKind::kConv;
+      if (!set_params(L, &op, &P, err)) return false;
       op.kh = static_cast<int>(L.kernel_h), op.kw = static_cast<int>(L.kernel_w);
       op.sh = static_cast<int>(L.stride_h), op.sw = static_cast<int>(L.stride_w);
       op.ph = static_cast<int>(L.pad_h), op.pw = static_cast<int>(L.pad_w);
-      set_params(L, &op, &P);
       // conv + bias followed by ReLU and MAX pool in either order: the existing fused block (caffe_layers.cu)
       if (L.bias_term && i + 2 < layers.size()) {
         const NetLayer& a = layers[i + 1];
@@ -256,27 +303,21 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
             op.pool_kernel = static_cast<int>(pool.kernel_h);
             op.pool_stride = static_cast<int>(pool.stride_h);
             op.out_shape = b.top_shapes[0];
-            const int out = new_tensor(count_of(op.out_shape), -1);
-            wants_grad[out] = true;  // the block has a weight and a bias
-            cur[b.tops[0]] = out;
-            op.out = out;
-            P.ops.push_back(op);
+            top = &b.tops[0];
             i += 2;
-            continue;
           }
         }
       }
-    } else if (L.type == "Pooling") {
+    } else if (op.kind == OpKind::kPool) {
       if (L.pool != "MAX" && L.pool != "AVE") {
         *err = why(L, "pool method " + L.pool + " is not supported (MAX and AVE are)");
         return false;
       }
-      op.kind = OpKind::kPool;
       op.max_pool = L.pool == "MAX";
       op.kh = static_cast<int>(L.kernel_h), op.kw = static_cast<int>(L.kernel_w);
       op.sh = static_cast<int>(L.stride_h), op.sw = static_cast<int>(L.stride_w);
       op.ph = static_cast<int>(L.pad_h), op.pw = static_cast<int>(L.pad_w);
-    } else if (L.type == "InnerProduct") {
+    } else if (op.kind == OpKind::kInnerProduct) {
       if (L.transpose) {
         *err = why(L, "transpose: true is not supported");
         return false;
@@ -285,42 +326,37 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         *err = why(L, "axis other than 1 is not supported");
         return false;
       }
-      if (!filler_ok(L.weight_filler, &reason) || (L.bias_term && !filler_ok(L.bias_filler, &reason))) {
-        *err = why(L, reason);
-        return false;
-      }
-      op.kind = OpKind::kInnerProduct;
-      set_params(L, &op, &P);
-    } else if (L.type == "ReLU" || L.type == "Sigmoid") {
-      op.kind = L.type == "ReLU" ? OpKind::kReLU : OpKind::kSigmoid;
+      if (!set_params(L, &op, &P, err)) return false;
+    } else if (op.kind == OpKind::kReLU || op.kind == OpKind::kSigmoid) {
       op.slope = L.negative_slope;
       // top == bottom shares the bottom's memory, except on a staged input: that is never written (every pass of an
       // iter_size step reads it again), so the top gets storage of its own.  So does a Split top: its memory is the
       // Split's bottom, which the sibling tops read too.
-      op.in_place = L.tops[0] == L.bottoms[0] && op.in >= P.ninputs && !P.data_alias[op.in];
-      if (op.in_place) storage = P.storage[op.in];
-    } else if (L.type == "BatchNorm") {
+      const int in = op.bottoms[0];
+      op.in_place = L.tops[0] == L.bottoms[0] && in >= P.ninputs && !P.data_alias[in];
+      if (op.in_place) storage = P.storage[in];
+    } else if (op.kind == OpKind::kBatchNorm) {
       if (!op.shares.empty()) {
         *err = why(L, "shared BatchNorm statistics are not supported");
         return false;
       }
-      op.kind = OpKind::kBatchNorm;  // separate top storage even when top == bottom: the kernels are not in place
+      // separate top storage even when top == bottom: the kernels are not in place
       op.w_off = P.blob_off[L.blobs[0]];
       op.global_stats = L.use_global_stats;
       op.fraction = L.moving_average_fraction;
       op.eps = L.eps;
-    } else if (L.type == "Scale") {  // scale_layer.cpp, one-bottom form; the parser resolved axis and num_axes
-      if (!filler_ok(L.weight_filler, &reason) || (L.bias_term && !filler_ok(L.bias_filler, &reason))) {
-        *err = why(L, reason);
-        return false;
-      }
-      op.kind = OpKind::kScale;  // separate top storage even when top == bottom: the scale's gradient reads x
-      set_params(L, &op, &P);
+    } else if (op.kind == OpKind::kEltwise) {  // eltwise_layer.cpp: the top has storage of its own
+      op.eltwise_op = L.eltwise_op == "PROD" ? kEltwiseProd : L.eltwise_op == "MAX" ? kEltwiseMax : kEltwiseSum;
+      op.coeffs = L.coeffs;
+      op.stable_prod_grad = L.stable_prod_grad;
+    } else if (op.kind == OpKind::kScale) {  // scale_layer.cpp, one-bottom form; the parser resolved axis and num_axes
+      // separate top storage even when top == bottom: the scale's gradient reads x
+      if (!set_params(L, &op, &P, err)) return false;
       const size_t first = static_cast<size_t>(L.axis), end = first + static_cast<size_t>(L.num_axes);
       op.scale_outer = count_of(std::vector<int64_t>(op.in_shape.begin(), op.in_shape.begin() + first));
       op.scale_dim = count_of(std::vector<int64_t>(op.in_shape.begin() + first, op.in_shape.begin() + end));
       op.scale_inner = count_of(std::vector<int64_t>(op.in_shape.begin() + end, op.in_shape.end()));
-    } else if (L.type == "LRN") {
+    } else if (op.kind == OpKind::kLRNWithin) {
       if (L.local_size < 1 || L.local_size % 2 == 0 || L.local_size > kLrnMaxLocalSize) {
         *err = why(L, "local_size " + std::to_string(L.local_size) + " is not odd and <= " +
                           std::to_string(kLrnMaxLocalSize));
@@ -330,77 +366,34 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         *err = why(L, "needs a 4-axis bottom and a finite beta");
         return false;
       }
-      op.kind = OpKind::kLRNWithin;  // separate top storage even when top == bottom: the kernels read a halo
+      // separate top storage even when top == bottom: the kernels read a halo
       op.lrn_size = static_cast<int>(L.local_size);
       op.lrn_alpha = L.lrn_alpha;
       op.lrn_beta = L.lrn_beta;
-    } else if (L.type == "ContrastiveLoss") {  // the parser checked the shapes: a, b N x C (x 1 x 1), sim N values
-      if (++losses > 1) {
-        *err = why(L, "a second loss layer is not supported");
-        return false;
-      }
-      op.kind = OpKind::kContrastiveLoss;
-      op.loss_weight = L.loss_weight;
+    } else if (op.kind == OpKind::kContrastiveLoss) {  // the parser checked the shapes: a, b N x C (x 1 x 1), sim N values
       op.margin = L.margin;
       op.legacy = L.legacy_version;
-      if (!take(L.bottoms[1], &op.in2)) return false;
-      op.need_dx2 = wants_grad[op.in2];
-      auto it = cur.find(L.bottoms[2]);
-      if (it == cur.end()) {
-        *err = why(L, "sim bottom '" + L.bottoms[2] + "' is not produced by an earlier TRAIN layer");
-        return false;
-      }
-      op.label = it->second;
-    } else if (L.type == "EuclideanLoss") {  // euclidean_loss_layer.cpp, after LossLayer::Reshape's check
-      if (++losses > 1) {
-        *err = why(L, "a second loss layer is not supported");
-        return false;
-      }
-      const std::vector<int64_t>& a = L.bottom_shapes[0];
-      const std::vector<int64_t>& b = L.bottom_shapes[1];
-      if (a.empty() || b.empty() || a[0] != b[0]) {
-        *err = why(L, "The data and label should have the same number.");
-        return false;
-      }
-      if (count_of(std::vector<int64_t>(a.begin() + 1, a.end())) !=
-          count_of(std::vector<int64_t>(b.begin() + 1, b.end()))) {  // Blob::count(1)
-        *err = why(L, "Inputs must have the same dimension.");
-        return false;
-      }
-      op.kind = OpKind::kEuclideanLoss;
-      op.loss_weight = L.loss_weight;
-      if (!take(L.bottoms[1], &op.in2)) return false;
-      op.need_dx2 = wants_grad[op.in2];
-    } else {  // SoftmaxWithLoss
-      if (++losses > 1) {
-        *err = why(L, "a second loss layer is not supported");
-        return false;
-      }
-      op.kind = OpKind::kSoftmaxLoss;
-      op.loss_weight = L.loss_weight;
-      auto it = cur.find(L.bottoms[1]);
-      if (it == cur.end()) {
-        *err = why(L, "label bottom '" + L.bottoms[1] + "' is not produced by an earlier TRAIN layer");
-        return false;
-      }
-      op.label = it->second;
+    } else if (op.kind == OpKind::kSoftmaxLoss) {
+      const int64_t labels = P.tensor_count[op.bottoms[1]];
       const int64_t rows = op.in_shape.empty() ? 0 : count_of(op.in_shape) / (op.in_shape.size() > 1 ? op.in_shape[1] : 1);
-      if (op.in_shape.size() < 2 || P.tensor_count[op.label] != rows) {
-        *err = why(L, "label count " + std::to_string(P.tensor_count[op.label]) + " does not match the " +
-                          std::to_string(rows) + " rows of the scores");
+      if (op.in_shape.size() < 2 || labels != rows) {
+        *err = why(L, "label count " + std::to_string(labels) + " does not match the " + std::to_string(rows) +
+                          " rows of the scores");
         return false;
       }
     }
     op.out = new_tensor(count_of(op.out_shape), storage);
     // BatchNorm's blobs are statistics, with no gradient
-    wants_grad[op.out] = op.need_dx || (op.kind != OpKind::kBatchNorm && (op.w_off >= 0 || op.b_off >= 0));
-    if (!auto_top) cur[L.tops[0]] = op.out;
+    wants_grad[op.out] = top_grad || (op.kind != OpKind::kBatchNorm && (op.w_off >= 0 || op.b_off >= 0));
+    if (top) cur[*top] = op.out;
+    if (row->loss) loss_top = op.out, loss_layer = L.name;
     P.ops.push_back(op);
   }
   // the op of each Split's top 0 sums the gradients of the tops some layer reads (consumer[] is complete now)
   for (size_t i = 0; i < P.ops.size(); ++i) {
     if (P.ops[i].kind != OpKind::kSplit || P.ops[i].split_top != 0) continue;
-    for (size_t j = i; j < P.ops.size() && P.ops[j].kind == OpKind::kSplit && P.ops[j].in == P.ops[i].in; ++j) {
+    for (size_t j = i; j < P.ops.size() && P.ops[j].kind == OpKind::kSplit && P.ops[j].bottoms[0] == P.ops[i].bottoms[0];
+         ++j) {
       if (j > i && P.ops[j].split_top == 0) break;  // the next Split of the same bottom
       if (consumer[P.ops[j].out].empty()) P.ops[j].split_unread = true;
       else P.ops[i].split_sum.push_back(P.ops[j].out);
@@ -426,16 +419,12 @@ bool plan_from_prototxt(const std::string& path, SolverSpec* spec, Plan* plan, s
 }
 
 std::string Plan::text() const {
-  static const char* kinds[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling", "InnerProduct",
-                                "ReLU",        "Sigmoid",             "BatchNorm", "SoftmaxWithLoss",
-                                "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss", "Concat", "EuclideanLoss",
-                                "Split", "Eltwise", "Scale"};
   static const char* eltwise_ops[] = {"PROD", "SUM", "MAX"};
   std::ostringstream os;
   for (int i = 0; i < ninputs; ++i) os << "input " << i << " " << input_names[i] << " " << tensor_count[i] << "\n";
   for (size_t i = 0; i < ops.size(); ++i) {
     const Op& op = ops[i];
-    os << "op " << i << " " << kinds[static_cast<int>(op.kind)];
+    os << "op " << i << " " << kKindNames[static_cast<int>(op.kind)];
     if (op.kind == OpKind::kPool) os << "(" << (op.max_pool ? "MAX" : "AVE") << ")";
     if (op.kind == OpKind::kEltwise) os << "(" << eltwise_ops[op.eltwise_op] << ")";
     os << " " << op.name << " " << shape_str(op.in_shape) << " -> " << shape_str(op.out_shape);
@@ -453,14 +442,14 @@ std::string Plan::text() const {
     }
     if (op.kind == OpKind::kSlice || op.kind == OpKind::kConcat)
       os << " axis=" << op.slice_axis << " begin=" << op.slice_begin;
-    if (op.kind == OpKind::kSoftmaxLoss) os << " label=" << op.label << " loss_weight=" << op.loss_weight;
+    if (op.kind == OpKind::kSoftmaxLoss) os << " label=" << op.bottoms[1] << " loss_weight=" << op.loss_weight;
     if (op.kind == OpKind::kContrastiveLoss)
-      os << " second=" << op.in2 << " sim=" << op.label << " margin=" << op.margin << (op.legacy ? " legacy" : "")
-         << " loss_weight=" << op.loss_weight;
-    if (op.kind == OpKind::kEuclideanLoss) os << " second=" << op.in2 << " loss_weight=" << op.loss_weight;
+      os << " second=" << op.bottoms[1] << " sim=" << op.bottoms[2] << " margin=" << op.margin
+         << (op.legacy ? " legacy" : "") << " loss_weight=" << op.loss_weight;
+    if (op.kind == OpKind::kEuclideanLoss) os << " second=" << op.bottoms[1] << " loss_weight=" << op.loss_weight;
     if (op.kind == OpKind::kSplit) os << " top=" << op.split_top << " data=bottom" << (op.split_unread ? " unread" : "");
     if (op.kind == OpKind::kEltwise) {
-      os << " bottoms=" << op.ins.size();
+      os << " bottoms=" << op.bottoms.size();
       if (op.eltwise_op == kEltwiseSum) {
         os << " coeff=";
         for (size_t j = 0; j < op.coeffs.size(); ++j) os << (j ? "," : "") << op.coeffs[j];
@@ -470,12 +459,12 @@ std::string Plan::text() const {
     if (op.kind == OpKind::kScale)
       os << " outer=" << op.scale_outer << " dim=" << op.scale_dim << " inner=" << op.scale_inner;
     if (op.in_place) os << " in-place";
-    // no data gradient is propagated into a staged input, nor into a blob with no learnable blob before it
-    auto mark = [&](int in, bool need) { return need ? "" : in < ninputs ? " staged-bottom" : " no-bottom-grad"; };
-    const char* m = mark(op.in, op.need_dx);
-    if (!*m && (op.kind == OpKind::kContrastiveLoss || op.kind == OpKind::kEuclideanLoss)) m = mark(op.in2, op.need_dx2);
-    for (size_t j = 1; j < op.ins.size() && !*m; ++j) m = mark(op.ins[j], op.ins_need_dx[j]);  // Eltwise
-    os << m;
+    // the first bottom that gets no data gradient: a staged input, or a blob with no learnable blob before it
+    for (size_t j = 0; j < op.bottoms.size(); ++j) {
+      if (op.bottom_grad[j] || static_cast<int>(j) == op.label_bottom) continue;
+      os << (op.bottoms[j] < ninputs ? " staged-bottom" : " no-bottom-grad");
+      break;
+    }
     os << "\n";
   }
   os << "params " << param_count << " blobs " << blob_count.size() << "\n";

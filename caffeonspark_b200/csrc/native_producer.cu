@@ -764,38 +764,7 @@ int NativeProducer::forward_backward(const cos_blob* inputs, int ninputs, float*
     act_[i] = const_cast<float*>(b.data);
   }
   for (size_t i = 0; i < plan_.ops.size(); ++i) {
-    const Op& op = plan_.ops[i];
-    if (op.kind == OpKind::kContrastiveLoss) {  // writes both bottoms' gradients here, as SoftmaxWithLoss does
-      const int N = static_cast<int>(op.in_shape[0]);
-      const int C = static_cast<int>(plan_.tensor_count[op.in] / N);
-      contrastive_loss_kernel<<<1, kThreads, 0, s>>>(act_[op.in], act_[op.in2], act_[op.label],
-                                                     op.need_dx ? grad_[op.in] : nullptr,
-                                                     op.need_dx2 ? grad_[op.in2] : nullptr, loss_dev, N, C, op.margin,
-                                                     op.legacy, op.loss_weight, status_);
-      cudaError_t e = cudaGetLastError();
-      if (e != cudaSuccess) return e;
-      continue;
-    }
-    if (op.kind == OpKind::kEuclideanLoss) {  // writes both bottoms' gradients here, as SoftmaxWithLoss does
-      euclidean_loss_kernel<<<1, kThreads, 0, s>>>(act_[op.in], act_[op.in2], op.need_dx ? grad_[op.in] : nullptr,
-                                                   op.need_dx2 ? grad_[op.in2] : nullptr, loss_dev,
-                                                   static_cast<int>(plan_.tensor_count[op.in]),
-                                                   static_cast<int>(op.in_shape[0]), op.loss_weight);
-      cudaError_t e = cudaGetLastError();
-      if (e != cudaSuccess) return e;
-      continue;
-    }
-    if (op.kind == OpKind::kSoftmaxLoss) {
-      const int C = static_cast<int>(op.in_shape[1]);
-      const int rows = static_cast<int>(plan_.tensor_count[op.in] / C);
-      const int inner = static_cast<int>(rows / op.in_shape[0]);
-      softmax_loss_kernel<<<1, kThreads, 0, s>>>(act_[op.in], act_[op.label], grad_[op.in], loss_dev, rows, C, inner,
-                                                 op.loss_weight, status_);
-      cudaError_t e = cudaGetLastError();
-      if (e != cudaSuccess) return e;
-      continue;
-    }
-    cudaError_t e = run_op_forward(op, i, s);
+    cudaError_t e = run_op_forward(plan_.ops[i], i, loss_dev, s);
     if (e != cudaSuccess) return e;
   }
   for (size_t i = plan_.ops.size(); i-- > 0;) {
@@ -805,8 +774,8 @@ int NativeProducer::forward_backward(const cos_blob* inputs, int ninputs, float*
   return cudaEventRecord(done_, s);
 }
 
-cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, cudaStream_t s) {
-  const float* x = act_[op.in];
+cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_dev, cudaStream_t s) {
+  const float* x = act_[op.bottoms[0]];
   float* y = act_[op.out];
   const int n = static_cast<int>(plan_.tensor_count[op.out]);
   switch (op.kind) {
@@ -853,28 +822,29 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, cudaStream_t 
                                                          op.slice_begin * slice_inner(op), false);
       return cudaGetLastError();
     case OpKind::kConcat: {
-      const int64_t nin = plan_.tensor_count[op.in];
+      const int64_t nin = plan_.tensor_count[op.bottoms[0]];
       slice_copy_kernel<<<grid_for(nin), kThreads, 0, s>>>(x, y, nin, slice_span(op, op.in_shape),
                                                            slice_span(op, op.out_shape),
                                                            op.slice_begin * slice_inner(op), true);
       return cudaGetLastError();
     }
     case OpKind::kSplit:  // no copy: the top reads the bottom's memory
-      act_[op.out] = act_[op.in];
+      act_[op.out] = act_[op.bottoms[0]];
       return cudaSuccess;
     case OpKind::kEltwise: {
-      const size_t nb = op.ins.size();
+      const size_t nb = op.bottoms.size();
       if (op.eltwise_op == kEltwiseSum) {
         for (size_t b = 0; b < nb; ++b)
-          eltwise_axpy_kernel<<<grid_for(n), kThreads, 0, s>>>(act_[op.ins[b]], op.coeffs[b], y, n, b == 0);
+          eltwise_axpy_kernel<<<grid_for(n), kThreads, 0, s>>>(act_[op.bottoms[b]], op.coeffs[b], y, n, b == 0);
       } else if (op.eltwise_op == kEltwiseProd) {
-        mul_kernel<<<grid_for(n), kThreads, 0, s>>>(act_[op.ins[0]], act_[op.ins[1]], y, n);
-        for (size_t b = 2; b < nb; ++b) mul_kernel<<<grid_for(n), kThreads, 0, s>>>(y, act_[op.ins[b]], y, n);
+        mul_kernel<<<grid_for(n), kThreads, 0, s>>>(act_[op.bottoms[0]], act_[op.bottoms[1]], y, n);
+        for (size_t b = 2; b < nb; ++b) mul_kernel<<<grid_for(n), kThreads, 0, s>>>(y, act_[op.bottoms[b]], y, n);
       } else {
         int* idx = static_cast<int*>(op_aux_[i]);
-        eltwise_max_kernel<<<grid_for(n), kThreads, 0, s>>>(act_[op.ins[0]], act_[op.ins[1]], 1, y, idx, n);
+        eltwise_max_kernel<<<grid_for(n), kThreads, 0, s>>>(act_[op.bottoms[0]], act_[op.bottoms[1]], 1, y, idx, n);
         for (size_t b = 2; b < nb; ++b)
-          eltwise_max_kernel<<<grid_for(n), kThreads, 0, s>>>(nullptr, act_[op.ins[b]], static_cast<int>(b), y, idx, n);
+          eltwise_max_kernel<<<grid_for(n), kThreads, 0, s>>>(nullptr, act_[op.bottoms[b]], static_cast<int>(b), y, idx,
+                                                              n);
       }
       return cudaGetLastError();
     }
@@ -887,16 +857,42 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, cudaStream_t 
       return lrn_within_forward(x, y, static_cast<int>(op.in_shape[0]), static_cast<int>(op.in_shape[1]),
                                 static_cast<int>(op.in_shape[2]), static_cast<int>(op.in_shape[3]), op.lrn_size,
                                 op.lrn_alpha, op.lrn_beta, s);
+    // The loss kernels also write their bottoms' gradients.  SoftmaxWithLoss writes its bottom's whatever bottom_grad
+    // says (a staged input's too: every tensor has a gradient buffer).
+    case OpKind::kSoftmaxLoss: {
+      const int C = static_cast<int>(op.in_shape[1]);
+      const int rows = static_cast<int>(plan_.tensor_count[op.bottoms[0]] / C);
+      const int inner = static_cast<int>(rows / op.in_shape[0]);
+      softmax_loss_kernel<<<1, kThreads, 0, s>>>(x, act_[op.bottoms[1]], grad_[op.bottoms[0]], loss_dev, rows, C, inner,
+                                                 op.loss_weight, status_);
+      return cudaGetLastError();
+    }
+    case OpKind::kContrastiveLoss: {
+      const int N = static_cast<int>(op.in_shape[0]);
+      const int C = static_cast<int>(plan_.tensor_count[op.bottoms[0]] / N);
+      contrastive_loss_kernel<<<1, kThreads, 0, s>>>(x, act_[op.bottoms[1]], act_[op.bottoms[2]],
+                                                     op.bottom_grad[0] ? grad_[op.bottoms[0]] : nullptr,
+                                                     op.bottom_grad[1] ? grad_[op.bottoms[1]] : nullptr, loss_dev, N, C,
+                                                     op.margin, op.legacy, op.loss_weight, status_);
+      return cudaGetLastError();
+    }
+    case OpKind::kEuclideanLoss:
+      euclidean_loss_kernel<<<1, kThreads, 0, s>>>(x, act_[op.bottoms[1]],
+                                                   op.bottom_grad[0] ? grad_[op.bottoms[0]] : nullptr,
+                                                   op.bottom_grad[1] ? grad_[op.bottoms[1]] : nullptr, loss_dev,
+                                                   static_cast<int>(plan_.tensor_count[op.bottoms[0]]),
+                                                   static_cast<int>(op.in_shape[0]), op.loss_weight);
+      return cudaGetLastError();
     default:
-      return cudaSuccess;
+      return cudaErrorInvalidValue;
   }
 }
 
 cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t s) {
-  const float* x = act_[op.in];
+  const float* x = act_[op.bottoms[0]];
   const float* dy = grad_[op.out];
-  float* dx = op.need_dx ? grad_[op.in] : nullptr;
-  const int nin = static_cast<int>(plan_.tensor_count[op.in]);
+  float* dx = op.bottom_grad[0] ? grad_[op.bottoms[0]] : nullptr;
+  const int nin = static_cast<int>(plan_.tensor_count[op.bottoms[0]]);
   switch (op.kind) {
     case OpKind::kConv:
       return conv_backward(op, x, dy, dx, data_ + op.w_off, diff_, workspace_, op.b_off >= 0, s);
@@ -975,11 +971,11 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
       return cudaGetLastError();
     }
     case OpKind::kEltwise: {  // eltwise_layer.cpp Backward_cpu, bottom by bottom
-      const size_t nb = op.ins.size();
+      const size_t nb = op.bottoms.size();
       const size_t bytes = static_cast<size_t>(nin) * sizeof(float);
       for (size_t b = 0; b < nb; ++b) {
-        if (!op.ins_need_dx[b]) continue;
-        float* db = grad_[op.ins[b]];
+        if (!op.bottom_grad[b]) continue;
+        float* db = grad_[op.bottoms[b]];
         cudaError_t e = cudaSuccess;
         if (op.eltwise_op == kEltwiseSum) {
           if (op.coeffs[b] == 1.f) e = cudaMemcpyAsync(db, dy, bytes, cudaMemcpyDeviceToDevice, s);
@@ -991,13 +987,13 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
           bool first = true;
           for (size_t j = 0; j < nb && e == cudaSuccess; ++j) {
             if (j == b) continue;
-            if (first) e = cudaMemcpyAsync(db, act_[op.ins[j]], bytes, cudaMemcpyDeviceToDevice, s);
-            else mul_kernel<<<grid_for(nin), kThreads, 0, s>>>(act_[op.ins[j]], db, db, nin);
+            if (first) e = cudaMemcpyAsync(db, act_[op.bottoms[j]], bytes, cudaMemcpyDeviceToDevice, s);
+            else mul_kernel<<<grid_for(nin), kThreads, 0, s>>>(act_[op.bottoms[j]], db, db, nin);
             first = false;
           }
           if (e == cudaSuccess) mul_kernel<<<grid_for(nin), kThreads, 0, s>>>(db, dy, db, nin);
         } else {
-          prod_div_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(act_[op.out], act_[op.ins[b]], dy, db, nin);
+          prod_div_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(act_[op.out], act_[op.bottoms[b]], dy, db, nin);
         }
         if (e == cudaSuccess) e = cudaGetLastError();
         if (e != cudaSuccess) return e;
@@ -1012,8 +1008,12 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
       if (dx) scale_forward_kernel<<<grid_for(nin), kThreads, 0, s>>>(dy, data_ + op.w_off, nullptr, dx, nin, dim, inner);
       return cudaGetLastError();
     }
-    default:  // SoftmaxWithLoss, ContrastiveLoss and EuclideanLoss wrote their bottom gradients in the forward pass
+    case OpKind::kSoftmaxLoss:  // the loss kernels wrote their bottoms' gradients in the forward pass
+    case OpKind::kContrastiveLoss:
+    case OpKind::kEuclideanLoss:
       return cudaSuccess;
+    default:
+      return cudaErrorInvalidValue;
   }
 }
 

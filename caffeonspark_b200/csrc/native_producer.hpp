@@ -22,7 +22,8 @@ namespace cosb {
 
 enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
-  kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale
+  kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale,
+  kCount  // the number of kinds (Plan::text names each)
 };
 
 enum EltwiseOp { kEltwiseProd = 0, kEltwiseSum = 1, kEltwiseMax = 2 };  // caffe.proto EltwiseParameter numbering
@@ -30,13 +31,18 @@ enum EltwiseOp { kEltwiseProd = 0, kEltwiseSum = 1, kEltwiseMax = 2 };  // caffe
 struct Op {
   OpKind kind;
   std::string name;                    // layer name (the fused block: "conv1+relu1+pool1")
-  int in = -1, out = -1, label = -1;   // tensor ids (label: SoftmaxWithLoss's label, ContrastiveLoss's sim)
-  int in2 = -1;                        // ContrastiveLoss, EuclideanLoss: the second bottom
-  std::vector<int64_t> in_shape, out_shape;
-  bool need_dx = true;                 // false when the bottom is a staged input or follows no learnable blob
-  bool need_dx2 = true;                // the same for in2
-  bool in_place = false;               // ReLU / Sigmoid with top == bottom: out shares in's storage (never a staged
-                                       // input's: those are not written)
+  // tensor ids of the bottoms, in the layer's bottom order, and whether each gets a data gradient: not a staged input,
+  // nor a blob that no learnable blob precedes (Caffe's bottom_need_backward), nor the label-like bottom.
+  // SoftmaxWithLoss writes its bottom's gradient whatever the flag says.
+  std::vector<int> bottoms;
+  std::vector<bool> bottom_grad;
+  // the label-like bottom (SoftmaxWithLoss's label, ContrastiveLoss's sim), or -1: read, never differentiated, and not
+  // counted as its blob's reader
+  int label_bottom = -1;
+  int out = -1;                        // tensor id of the top
+  std::vector<int64_t> in_shape, out_shape;  // in_shape: bottoms[0]'s
+  bool in_place = false;               // ReLU / Sigmoid with top == bottom: out shares bottoms[0]'s storage (never a
+                                       // staged input's: those are not written)
   // Convolution, Pooling, the fused block's convolution
   int kh = 0, kw = 0, sh = 1, sw = 1, ph = 0, pw = 0;
   bool max_pool = true;
@@ -60,9 +66,7 @@ struct Op {
   int split_top = 0;
   std::vector<int> split_sum;
   bool split_unread = false;           // no layer reads this top: it adds nothing to the bottom's gradient
-  // Eltwise: every bottom (ins[0] == in) and whether it wants a gradient; coeffs for SUM
-  std::vector<int> ins;
-  std::vector<bool> ins_need_dx;
+  // Eltwise: coeffs for SUM, one per bottom
   int eltwise_op = kEltwiseSum;
   std::vector<float> coeffs;
   bool stable_prod_grad = true;
@@ -87,8 +91,7 @@ struct Plan {
 };
 
 // Builds the plan of a parsed TRAIN net (a Slice or Split layer becomes one op per top, a Concat layer one kConcat op
-// per bottom); false with
-// "layer '<name>' (<type>): <reason>" when it cannot be run.
+// per bottom, each with one bottom); false with "layer '<name>' (<type>): <reason>" when it cannot be run.
 bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Plan* plan, std::string* err);
 // parse_train_net + build_plan.
 bool plan_from_prototxt(const std::string& path, SolverSpec* spec, Plan* plan, std::string* err);
@@ -114,7 +117,7 @@ class NativeProducer {
   NativeProducer(const Plan& plan, int device, float* data, float* diff, int* status)
       : plan_(plan), device_(device), data_(data), diff_(diff), status_(status) {}
   bool allocate(std::string* err);
-  cudaError_t run_op_forward(const Op& op, size_t i, cudaStream_t s);
+  cudaError_t run_op_forward(const Op& op, size_t i, float* loss_dev, cudaStream_t s);
   cudaError_t run_op_backward(const Op& op, size_t i, cudaStream_t s);
 
   Plan plan_;

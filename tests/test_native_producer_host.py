@@ -93,6 +93,17 @@ def _net(tmp_path, body):
 IP = 'layer { name: "ip" type: "InnerProduct" bottom: "%s" top: "ip" inner_product_param { num_output: 4 } }'
 
 
+def _ip(name, bottom, top):
+    return (f'layer {{ name: "{name}" type: "InnerProduct" bottom: "{bottom}" top: "{top}" '
+            'inner_product_param { num_output: 4 } }')
+
+
+# the data's three channels sliced apart; a and b, 2x4 each, come out of the first two
+SLICE3 = 'layer { name: "sl" type: "Slice" bottom: "data" top: "d1" top: "d2" top: "d3" slice_param { axis: 1 } }'
+PAIR = SLICE3 + _ip("ipa", "d1", "a") + _ip("ipb", "d2", "b")
+CONTRASTIVE = 'layer { name: "cl" type: "ContrastiveLoss" bottom: "a" bottom: "b" bottom: "label" top: "cl" }'
+
+
 @pytest.mark.parametrize("body,match", [
     ('layer { name: "drop" type: "Dropout" bottom: "data" top: "data" }' + IP % "data",
      r"layer 'drop' \(Dropout\): layer type not supported"),
@@ -108,6 +119,22 @@ IP = 'layer { name: "ip" type: "InnerProduct" bottom: "%s" top: "ip" inner_produ
      + IP % "p", r"layer 'p' \(Pooling\): pool method STOCHASTIC"),
     ('layer { name: "r" type: "ReLU" bottom: "data" top: "r" }' + IP % "data",
      r"layer 'ip' \(InnerProduct\): bottom 'data' already feeds layer 'r'"),
+    ('layer { name: "s" type: "SoftmaxWithLoss" bottom: "data" top: "s" }' + IP % "data",
+     r"layer 's' \(SoftmaxWithLoss\): 2 bottom\(s\) and one top"),
+    (IP % "data" + 'layer { name: "e" type: "Eltwise" bottom: "ip" bottom: "ip" }',
+     r"layer 'e' \(Eltwise\): needs at least 1 bottom\(s\) and one top"),
+    (SLICE3 + _ip("ipa", "d1", "a") + 'layer { name: "l0" type: "SoftmaxWithLoss" bottom: "a" bottom: "label" top: "l0" }'
+     + _ip("ip", "d3", "ip"), r"layer 'loss' \(SoftmaxWithLoss\): a second loss layer is not supported"),
+    (PAIR + CONTRASTIVE + _ip("ip", "d3", "ip"),
+     r"layer 'loss' \(SoftmaxWithLoss\): a second loss layer is not supported"),
+    (PAIR + _ip("ipc", "d3", "c") + 'layer { name: "l0" type: "SoftmaxWithLoss" bottom: "c" bottom: "label" top: "l0" }'
+     + CONTRASTIVE, r"layer 'cl' \(ContrastiveLoss\): a second loss layer is not supported"),
+    (IP % "data" + 'layer { name: "acc" type: "Accuracy" bottom: "ip" bottom: "label" top: "acc" }'
+     'layer { name: "l0" type: "SoftmaxWithLoss" bottom: "ip" bottom: "acc" top: "l0" }',
+     r"layer 'l0' \(SoftmaxWithLoss\): label bottom 'acc' is not produced by an earlier TRAIN layer"),
+    ('layer { name: "sc" type: "Scale" bottom: "data" top: "sc" scale_param { bias_term: true '
+     'bias_filler { type: "positive_unitball" } } }' + IP % "sc",
+     r"layer 'sc' \(Scale\): filler type 'positive_unitball' is not supported"),
 ])
 def test_refusals_name_the_layer(cos, tmp_path, body, match):
     with pytest.raises(cos.CosError, match=match):
@@ -164,3 +191,14 @@ def test_staged_inputs_are_never_written(cos, tmp_path):
                  'layer { name: "loss" type: "SoftmaxWithLoss" bottom: "scores" bottom: "label" top: "loss" }\n')
     text = cos.native_producer_plan(str(p))
     assert _ops(text) == ["SoftmaxWithLoss loss 4x5 -> scalar"] and "staged-bottom" in text
+
+
+def test_a_loss_layers_top_is_not_read(cos, tmp_path):
+    # the engine writes the loss to the solver's loss word, never into the loss layer's top
+    p = tmp_path / "net.prototxt"
+    p.write_text('name: "t" layer { name: "in" type: "Input" top: "x" top: "y" input_param { shape { dim: 4 dim: 3 } '
+                 'shape { dim: 4 dim: 5 } } }\n' + _ip("ip", "y", "t").replace("num_output: 4", "num_output: 3") +
+                 '\nlayer { name: "euc" type: "EuclideanLoss" bottom: "x" bottom: "t" top: "loss" }\n'
+                 'layer { name: "r" type: "ReLU" bottom: "loss" top: "loss" }\n')
+    with pytest.raises(cos.CosError, match=r"^layer 'r' \(ReLU\): bottom 'loss' is the top of loss layer 'euc'"):
+        cos.native_producer_plan(str(p))
