@@ -17,18 +17,6 @@ std::string why(const NetLayer& L, const std::string& reason) {
   return "layer '" + L.name + "' (" + L.type + "): " + reason + " (native producer)";
 }
 
-int64_t count_of(const std::vector<int64_t>& s) {
-  int64_t n = 1;
-  for (int64_t d : s) n *= d;
-  return n;
-}
-
-std::string shape_str(const std::vector<int64_t>& s) {
-  std::ostringstream os;
-  for (size_t i = 0; i < s.size(); ++i) os << (i ? "x" : "") << s[i];
-  return s.empty() ? "scalar" : os.str();
-}
-
 bool filler_ok(const FillerSpec& f, std::string* reason) {
   static const char* types[] = {"constant", "uniform", "gaussian", "xavier", "msra"};
   bool known = false;
@@ -79,8 +67,7 @@ bool euclidean_shapes_ok(const NetLayer& L, std::string* err) {
     *err = why(L, "The data and label should have the same number.");
     return false;
   }
-  if (count_of(std::vector<int64_t>(a.begin() + 1, a.end())) !=
-      count_of(std::vector<int64_t>(b.begin() + 1, b.end()))) {  // Blob::count(1)
+  if (shape_count(a, 1) != shape_count(b, 1)) {
     *err = why(L, "Inputs must have the same dimension.");
     return false;
   }
@@ -152,7 +139,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
   for (const NetLayer& L : layers) {  // staged inputs first: tensors 0 .. ninputs-1
     if (!is_data_layer(L.type)) continue;
     for (size_t t = 0; t < L.tops.size(); ++t) {
-      cur[L.tops[t]] = new_tensor(count_of(L.top_shapes[t]), -1);
+      cur[L.tops[t]] = new_tensor(shape_count(L.top_shapes[t]), -1);
       P.input_names.push_back(L.tops[t]);
     }
   }
@@ -236,7 +223,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       for (size_t t = 0; t < L.tops.size(); ++t) {
         op.slice_begin = L.slice_begin[t];
         op.out_shape = L.top_shapes[t];
-        op.out = new_tensor(count_of(op.out_shape), -1);
+        op.out = new_tensor(shape_count(op.out_shape), -1);
         wants_grad[op.out] = top_grad;
         cur[L.tops[t]] = op.out;
         P.ops.push_back(op);
@@ -246,7 +233,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     if (op.kind == OpKind::kSplit) {  // one op per top; each top reads the bottom's activation (split_layer.cpp ShareData)
       for (size_t t = 0; t < L.tops.size(); ++t) {
         op.split_top = static_cast<int>(t);
-        op.out = new_tensor(count_of(op.out_shape), -1);
+        op.out = new_tensor(shape_count(op.out_shape), -1);
         P.data_alias[op.out] = true;
         wants_grad[op.out] = top_grad;
         cur[L.tops[t]] = op.out;
@@ -256,7 +243,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     }
     if (op.kind == OpKind::kConcat) {  // one op per bottom, each copying its bottom into its range of the one top (and back)
       op.slice_axis = static_cast<int>(L.axis);  // the parser checked the axis and the bottoms' shapes
-      op.out = new_tensor(count_of(op.out_shape), -1);
+      op.out = new_tensor(shape_count(op.out_shape), -1);
       wants_grad[op.out] = top_grad;
       int64_t begin = 0;
       for (size_t b = 0; b < L.bottoms.size(); ++b) {
@@ -353,9 +340,9 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       // separate top storage even when top == bottom: the scale's gradient reads x
       if (!set_params(L, &op, &P, err)) return false;
       const size_t first = static_cast<size_t>(L.axis), end = first + static_cast<size_t>(L.num_axes);
-      op.scale_outer = count_of(std::vector<int64_t>(op.in_shape.begin(), op.in_shape.begin() + first));
-      op.scale_dim = count_of(std::vector<int64_t>(op.in_shape.begin() + first, op.in_shape.begin() + end));
-      op.scale_inner = count_of(std::vector<int64_t>(op.in_shape.begin() + end, op.in_shape.end()));
+      op.scale_outer = shape_count(std::vector<int64_t>(op.in_shape.begin(), op.in_shape.begin() + first));
+      op.scale_dim = shape_count(std::vector<int64_t>(op.in_shape.begin() + first, op.in_shape.begin() + end));
+      op.scale_inner = shape_count(op.in_shape, end);
     } else if (op.kind == OpKind::kLRNWithin) {
       if (L.local_size < 1 || L.local_size % 2 == 0 || L.local_size > kLrnMaxLocalSize) {
         *err = why(L, "local_size " + std::to_string(L.local_size) + " is not odd and <= " +
@@ -375,14 +362,14 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.legacy = L.legacy_version;
     } else if (op.kind == OpKind::kSoftmaxLoss) {
       const int64_t labels = P.tensor_count[op.bottoms[1]];
-      const int64_t rows = op.in_shape.empty() ? 0 : count_of(op.in_shape) / (op.in_shape.size() > 1 ? op.in_shape[1] : 1);
+      const int64_t rows = op.in_shape.empty() ? 0 : shape_count(op.in_shape) / (op.in_shape.size() > 1 ? op.in_shape[1] : 1);
       if (op.in_shape.size() < 2 || labels != rows) {
         *err = why(L, "label count " + std::to_string(labels) + " does not match the " + std::to_string(rows) +
                           " rows of the scores");
         return false;
       }
     }
-    op.out = new_tensor(count_of(op.out_shape), storage);
+    op.out = new_tensor(shape_count(op.out_shape), storage);
     // BatchNorm's blobs are statistics, with no gradient
     wants_grad[op.out] = top_grad || (op.kind != OpKind::kBatchNorm && (op.w_off >= 0 || op.b_off >= 0));
     if (top) cur[*top] = op.out;
@@ -427,7 +414,7 @@ std::string Plan::text() const {
     os << "op " << i << " " << kKindNames[static_cast<int>(op.kind)];
     if (op.kind == OpKind::kPool) os << "(" << (op.max_pool ? "MAX" : "AVE") << ")";
     if (op.kind == OpKind::kEltwise) os << "(" << eltwise_ops[op.eltwise_op] << ")";
-    os << " " << op.name << " " << shape_str(op.in_shape) << " -> " << shape_str(op.out_shape);
+    os << " " << op.name << " " << shape_text(op.in_shape) << " -> " << shape_text(op.out_shape);
     if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kPool)
       os << " k" << op.kh << "x" << op.kw << " s" << op.sh << "x" << op.sw << " p" << op.ph << "x" << op.pw;
     if (op.kind == OpKind::kConvBiasReluMaxPool) os << " pool" << op.pool_kernel << "/" << op.pool_stride;
@@ -469,7 +456,7 @@ std::string Plan::text() const {
   }
   os << "params " << param_count << " blobs " << blob_count.size() << "\n";
   for (size_t k = 0; k < blob_off.size(); ++k)
-    os << "blob " << k << " " << blob_off[k] << ":" << blob_count[k] << " " << shape_str(blob_shape[k]) << " "
+    os << "blob " << k << " " << blob_off[k] << ":" << blob_count[k] << " " << shape_text(blob_shape[k]) << " "
        << blob_filler[k].type << "\n";
   return os.str();
 }

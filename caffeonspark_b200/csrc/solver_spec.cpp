@@ -70,9 +70,29 @@ bool learning_rate(const std::string& policy, float base_lr, float gamma, float 
   return true;
 }
 
-// ------------------------------------------------- protobuf text-format reader
+int64_t shape_count(const std::vector<int64_t>& s, size_t from) {
+  int64_t n = 1;
+  for (size_t i = from; i < s.size(); ++i) n *= s[i];
+  return n;
+}
+
+std::string shape_text(const std::vector<int64_t>& s) {
+  std::string t;
+  for (size_t i = 0; i < s.size(); ++i) t += (i ? "x" : "") + std::to_string(s[i]);
+  return s.empty() ? "scalar" : t;
+}
+
 namespace {
 
+typedef std::vector<int64_t> Shape;
+
+std::string shape_string(const Shape& s) {  // Blob::shape_string: "2 3 4 (24)"
+  std::string t;
+  for (int64_t d : s) t += std::to_string(d) + " ";
+  return t + "(" + std::to_string(shape_count(s)) + ")";
+}
+
+// ------------------------------------------------- protobuf text-format reader
 struct Node {
   bool is_msg = false;
   std::string value;                                             // scalar
@@ -244,24 +264,10 @@ bool in_train_phase(const Node& layer) {
   return own.empty() || own == "TRAIN";
 }
 
-typedef std::vector<long> Shape;
-
-long prod(const Shape& s, size_t from = 0) {
-  long p = 1;
-  for (size_t i = from; i < s.size(); ++i) p *= s[i];
-  return p;
-}
-
-std::string shape_text(const Shape& s) {  // "2x3x4", "scalar"
-  std::string t;
-  for (size_t i = 0; i < s.size(); ++i) t += (i ? "x" : "") + std::to_string(s[i]);
-  return s.empty() ? "scalar" : t;
-}
-
-struct HW { long h, w; };
+struct HW { int64_t h, w; };
 
 // kernel_size / kernel_h,kernel_w style repeated-or-pair fields
-HW pair_field(const Node& p, const std::string& rep, const std::string& h, const std::string& w, long dflt) {
+HW pair_field(const Node& p, const std::string& rep, const std::string& h, const std::string& w, int64_t dflt) {
   HW r{dflt, dflt};
   auto reps = p.all(rep);
   if (reps.size() == 1) r.h = r.w = atol(reps[0]->value.c_str());
@@ -284,8 +290,6 @@ FillerSpec filler(const Node* f) {
   return s;
 }
 
-std::vector<int64_t> to64(const Shape& s) { return std::vector<int64_t>(s.begin(), s.end()); }
-
 // TransformationParameter; force_color / force_gray only matter for decoding, which happens before the library.
 TransformSpec transform(const Node* t, const std::string& net_file) {
   TransformSpec s;
@@ -300,555 +304,511 @@ TransformSpec transform(const Node* t, const std::string& net_file) {
   return s;
 }
 
+// What a rule works with: `rec` arrives with the common fields set; spec, net_file and first_data serve data layers.
+struct Layer {
+  const Node& node;
+  NetLayer& rec;
+  std::map<std::string, Shape>& blobs;  // every blob so far, by name
+  std::string* err;
+  SolverSpec* spec;
+  const std::string& net_file;
+  bool& first_data;  // no data layer has given the net its batch_size and input_shape yet
+  bool bottom(size_t i, Shape* s) const {
+    if (i >= rec.bottoms.size() || !blobs.count(rec.bottoms[i])) return refuse("unknown bottom blob");
+    *s = blobs.at(rec.bottoms[i]);
+    return true;
+  }
+  void set_top(size_t i, const Shape& s) { if (i < rec.tops.size()) blobs[rec.tops[i]] = s; }
+  void set_tops(const Shape& s) { for (const std::string& t : rec.tops) blobs[t] = s; }
+  bool refuse(const std::string& reason) const { *err = "layer '" + rec.name + "' (" + rec.type + "): " + reason; return false; }
+  // the older wording, without the type ("layer 'c': bad Convolution"); an unknown bottom reported first stands
+  bool bad(const std::string& what) const { if (err->empty()) *err = "layer '" + rec.name + "': bad " + what; return false; }
+};
+
+// A rule infers the layer's top shapes, refuses what Caffe would refuse, and appends the shapes of the learnable blobs
+// the layer owns to `params`, in Caffe's order.
+typedef bool (*Rule)(Layer& L, std::vector<Shape>* params);
+
+bool canonical_axis(const Layer& L, int64_t given, int64_t naxes, int64_t* axis) {  // Blob::CanonicalAxisIndex
+  *axis = given < 0 ? given + naxes : given;
+  if (*axis < 0 || *axis >= naxes)
+    return L.refuse("axis " + std::to_string(given) + " out of range for " + std::to_string(naxes) + "-D Blob");
+  return true;
+}
+
+// Top i of a data layer, of shape s, as a staged input with `transform_param`.
+void data_top(Layer& L, size_t i, Shape s, const Node* transform_param) {
+  L.set_top(i, s);
+  StagedInput in;
+  in.layer = L.rec.name, in.type = L.rec.type, in.top = L.rec.tops[i], in.shape = s;
+  in.transform = transform(transform_param, L.net_file);
+  L.spec->inputs.push_back(in);
+}
+
+void data_input(Layer& L, const Shape& s) {  // the first data layer to call it gives the net's batch and input shape
+  if (!L.first_data) return;
+  L.spec->batch_size = static_cast<int>(s[0]);
+  L.spec->input_shape.assign(s.begin(), s.end());
+  L.first_data = false;
+}
+
+bool memory_data(Layer& L, std::vector<Shape>*) {
+  const Node* p = L.node.first("memory_data_param");
+  if (!p) { *L.err = "MemoryData layer without memory_data_param"; return false; }
+  Shape s{p->integer("batch_size", 0), p->integer("channels", 0), p->integer("height", 0), p->integer("width", 0)};
+  L.set_top(0, s), L.set_top(1, Shape{s[0]});  // data and label, both set before a top is staged with its name's shape
+  for (size_t i = 0; i < L.rec.tops.size(); ++i)  // the transform applies to the data, never to the label
+    data_top(L, i, L.blobs[L.rec.tops[i]], i == 0 ? L.node.first("transform_param") : nullptr);
+  data_input(L, s);  // even without a top
+  return true;
+}
+
+bool cos_data(Layer& L, std::vector<Shape>*) {
+  const Node* p = L.node.first("cos_data_param");
+  if (!p) { *L.err = "CoSData layer without cos_data_param"; return false; }
+  auto tb = p->all("top");
+  for (size_t i = 0; i < L.rec.tops.size(); ++i) {
+    Shape s{p->integer("batch_size", 0)};
+    if (i < tb.size()) {
+      int64_t c = tb[i]->integer("out_channels", 0), h = tb[i]->integer("out_height", 0), w = tb[i]->integer("out_width", 0);
+      if (!c) c = tb[i]->integer("channels", 0);
+      if (!h) h = tb[i]->integer("height", 0);
+      if (!w) w = tb[i]->integer("width", 0);
+      Shape full{c, h, w};
+      for (int64_t a = 0; a < tb[i]->integer("sample_num_axes", 3) && a < 3; ++a) s.push_back(full[a] ? full[a] : 1);
+    }
+    data_top(L, i, s, i < tb.size() ? tb[i]->first("transform_param") : nullptr);
+    if (i == 0) data_input(L, s);
+  }
+  return true;
+}
+
+bool input(Layer& L, std::vector<Shape>*) {
+  const Node* p = L.node.first("input_param");
+  auto shapes = p ? p->all("shape") : std::vector<const Node*>();
+  for (size_t i = 0; i < L.rec.tops.size(); ++i) {
+    Shape s;
+    if (!shapes.empty()) for (const Node* d : shapes[std::min(i, shapes.size() - 1)]->all("dim")) s.push_back(atol(d->value.c_str()));
+    data_top(L, i, s, nullptr);
+    if (i == 0 && !s.empty()) data_input(L, s);
+  }
+  return true;
+}
+
+bool convolution(Layer& L, std::vector<Shape>* params) {  // and Deconvolution; weight shapes of base_conv_layer.cpp
+  const Node* p = L.node.first("convolution_param");
+  Shape in;
+  if (!p || !L.bottom(0, &in) || in.size() != 4) return L.bad("Convolution");
+  const int64_t nout = p->integer("num_output", 0), group = p->integer("group", 1);
+  HW k = pair_field(*p, "kernel_size", "kernel_h", "kernel_w", 0), st = pair_field(*p, "stride", "stride_h", "stride_w", 1);
+  HW pad = pair_field(*p, "pad", "pad_h", "pad_w", 0), dil = pair_field(*p, "dilation", "dilation_h", "dilation_w", 1);
+  if (nout <= 0 || k.h <= 0 || k.w <= 0 || group <= 0 || in[1] % group || nout % group || st.h <= 0 || st.w <= 0 ||
+      dil.h <= 0 || dil.w <= 0 || pad.h < 0 || pad.w < 0)
+    return L.bad("convolution_param");
+  NetLayer& r = L.rec;
+  r.num_output = nout, r.group = group;
+  r.kernel_h = k.h, r.kernel_w = k.w, r.stride_h = st.h, r.stride_w = st.w;
+  r.pad_h = pad.h, r.pad_w = pad.w, r.dilation_h = dil.h, r.dilation_w = dil.w;
+  r.bias_term = p->boolean("bias_term", true);
+  r.weight_filler = filler(p->first("weight_filler")), r.bias_filler = filler(p->first("bias_filler"));
+  const int64_t kh = dil.h * (k.h - 1) + 1, kw = dil.w * (k.w - 1) + 1;  // the dilated kernel
+  if (r.type == "Convolution") {
+    params->push_back({nout, in[1] / group, k.h, k.w});
+    L.set_top(0, {in[0], nout, (in[2] + 2 * pad.h - kh) / st.h + 1, (in[3] + 2 * pad.w - kw) / st.w + 1});
+  } else {
+    params->push_back({in[1], nout / group, k.h, k.w});
+    L.set_top(0, {in[0], nout, st.h * (in[2] - 1) + kh - 2 * pad.h, st.w * (in[3] - 1) + kw - 2 * pad.w});
+  }
+  if (r.bias_term) params->push_back({nout});
+  return true;
+}
+
+bool pooling(Layer& L, std::vector<Shape>*) {
+  const Node* p = L.node.first("pooling_param");
+  Shape in;
+  if (!p || !L.bottom(0, &in) || in.size() != 4) return L.bad("Pooling");
+  HW k = pair_field(*p, "kernel_size", "kernel_h", "kernel_w", 0), st = pair_field(*p, "stride", "stride_h", "stride_w", 1);
+  HW pad = pair_field(*p, "pad", "pad_h", "pad_w", 0);
+  if (p->boolean("global_pooling", false)) { k.h = in[2]; k.w = in[3]; }
+  if (k.h <= 0 || k.w <= 0 || st.h <= 0 || st.w <= 0 || pad.h < 0 || pad.w < 0) return L.bad("pooling_param");
+  // pooling_layer.cpp: ceil((H + 2p - k) / s) + 1, clipped so the last window starts inside
+  int64_t oh = static_cast<int64_t>(ceil(static_cast<float>(in[2] + 2 * pad.h - k.h) / st.h)) + 1;
+  int64_t ow = static_cast<int64_t>(ceil(static_cast<float>(in[3] + 2 * pad.w - k.w) / st.w)) + 1;
+  if (pad.h || pad.w) {
+    if ((oh - 1) * st.h >= in[2] + pad.h) --oh;
+    if ((ow - 1) * st.w >= in[3] + pad.w) --ow;
+  }
+  NetLayer& r = L.rec;
+  r.kernel_h = k.h, r.kernel_w = k.w, r.stride_h = st.h, r.stride_w = st.w, r.pad_h = pad.h, r.pad_w = pad.w;
+  r.pool = p->str("pool", "MAX"), r.global_pooling = p->boolean("global_pooling", false);
+  L.set_tops({in[0], in[1], oh, ow});
+  return true;
+}
+
+bool inner_product(Layer& L, std::vector<Shape>* params) {
+  const Node* p = L.node.first("inner_product_param");
+  Shape in;
+  if (!p || !L.bottom(0, &in)) return L.bad("InnerProduct");
+  const int64_t nout = p->integer("num_output", 0), naxes = static_cast<int64_t>(in.size());
+  int64_t axis = p->integer("axis", 1);
+  if (axis < 0) axis += naxes;
+  if (nout <= 0 || axis < 0 || axis > naxes) return L.bad("inner_product_param");
+  NetLayer& r = L.rec;
+  r.num_output = nout, r.axis = axis;
+  r.bias_term = p->boolean("bias_term", true), r.transpose = p->boolean("transpose", false);
+  r.weight_filler = filler(p->first("weight_filler")), r.bias_filler = filler(p->first("bias_filler"));
+  params->push_back({nout, shape_count(in, static_cast<size_t>(axis))});  // inner_product_layer.cpp: N x K
+  if (r.bias_term) params->push_back({nout});
+  Shape out(in.begin(), in.begin() + axis);
+  out.push_back(nout);
+  L.set_top(0, out);
+  return true;
+}
+
+bool same_shape(Layer& L, std::vector<Shape>*) {  // ReLU, LRN, Dropout, Sigmoid, ...
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  L.set_tops(in);
+  NetLayer& r = L.rec;
+  if (const Node* p = L.node.first("relu_param")) r.negative_slope = static_cast<float>(p->num("negative_slope", 0.0));
+  if (const Node* p = L.node.first("lrn_param")) {  // caffe.proto LRNParameter
+    r.local_size = p->integer("local_size", 5);
+    r.lrn_alpha = static_cast<float>(p->num("alpha", 1.0));
+    r.lrn_beta = static_cast<float>(p->num("beta", 0.75));
+    r.lrn_k = static_cast<float>(p->num("k", 1.0));
+    r.norm_region = p->str("norm_region", "ACROSS_CHANNELS");
+    if (r.norm_region == "0") r.norm_region = "ACROSS_CHANNELS";  // the enum's numeric form
+    if (r.norm_region == "1") r.norm_region = "WITHIN_CHANNEL";
+  }
+  return true;
+}
+
+bool split(Layer& L, std::vector<Shape>*) {  // split_layer.cpp Reshape
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  for (const std::string& t : L.rec.tops) {
+    if (t == L.rec.bottoms[0]) return L.refuse("Split Layer does not allow in-place computation.");
+    L.blobs[t] = in;
+  }
+  return true;
+}
+
+bool eltwise(Layer& L, std::vector<Shape>*) {  // eltwise_layer.cpp LayerSetUp and Reshape, after Layer::CheckBlobCounts
+  const size_t n = L.rec.bottoms.size();
+  if (n < 2) return L.refuse("Eltwise Layer takes at least 2 bottom blob(s) as input.");
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  const Node* p = L.node.first("eltwise_param");
+  auto coeffs = p ? p->all("coeff") : std::vector<const Node*>();
+  if (!coeffs.empty() && coeffs.size() != n) return L.refuse("Eltwise Layer takes one coefficient per bottom blob.");
+  std::string op = p ? p->str("operation", "SUM") : "SUM";
+  if (op == "0") op = "PROD";  // the enum's numeric form
+  if (op == "1") op = "SUM";
+  if (op == "2") op = "MAX";
+  if (op != "PROD" && op != "SUM" && op != "MAX") return L.refuse("Unknown elementwise operation.");
+  if (op == "PROD" && !coeffs.empty()) return L.refuse("Eltwise layer only takes coefficients for summation.");
+  L.rec.eltwise_op = op, L.rec.coeffs.assign(n, 1.f);
+  for (size_t i = 0; i < coeffs.size(); ++i) L.rec.coeffs[i] = static_cast<float>(atof(coeffs[i]->value.c_str()));
+  L.rec.stable_prod_grad = !p || p->boolean("stable_prod_grad", true);
+  for (size_t i = 1; i < n; ++i) {
+    Shape s;
+    if (!L.bottom(i, &s)) return false;
+    if (s != in)
+      return L.refuse("bottom " + std::to_string(i) + " is " + shape_text(s) + ", bottom 0 " + shape_text(in) +
+                      " (Check failed: bottom[i]->shape() == bottom[0]->shape())");
+  }
+  L.set_tops(in);
+  return true;
+}
+
+bool scale(Layer& L, std::vector<Shape>* params) {  // scale_layer.cpp LayerSetUp and Reshape; the bias as bias_layer.cpp
+  if (L.rec.bottoms.size() > 2) return L.refuse("Scale Layer takes at most 2 bottom blob(s) as input.");
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  const Node* p = L.node.first("scale_param");
+  const int64_t naxes = static_cast<int64_t>(in.size());
+  int64_t axis;
+  if (!canonical_axis(L, p ? p->integer("axis", 1) : 1, naxes, &axis)) return false;
+  const std::string past = "scale blob's shape extends past bottom[0]'s shape when applied starting with bottom[0] axis = ";
+  Shape scale;  // the scale blob's shape, or bottom[1]'s
+  if (L.rec.bottoms.size() == 1) {
+    const int64_t num_axes = p ? p->integer("num_axes", 1) : 1;
+    if (num_axes < -1) return L.refuse("num_axes must be non-negative, or -1 to extend to the end of bottom[0]");
+    if (num_axes >= 0 && naxes < axis + num_axes) return L.refuse(past + std::to_string(axis));
+    scale.assign(in.begin() + axis, num_axes == -1 ? in.end() : in.begin() + axis + num_axes);
+    params->push_back(scale);
+  } else if (!L.bottom(1, &scale)) {
+    return false;
+  }
+  const int64_t first = scale.empty() ? 0 : axis;  // Reshape: a scalar scale applies from axis 0
+  if (naxes < first + static_cast<int64_t>(scale.size())) return L.refuse(past + std::to_string(first));
+  for (size_t i = 0; i < scale.size(); ++i)
+    if (in[first + i] != scale[i])
+      return L.refuse("dimension mismatch between bottom[0]->shape(" + std::to_string(first + i) + ") and scale->shape(" +
+                      std::to_string(i) + ")");
+  NetLayer& r = L.rec;
+  r.bias_term = p && p->boolean("bias_term", false);
+  if (r.bias_term) params->push_back(scale);  // the Bias layer's blob, of the scale's (or bottom[1]'s) shape
+  r.axis = first, r.num_axes = static_cast<int64_t>(scale.size());
+  if (p && p->first("filler")) r.weight_filler = filler(p->first("filler"));
+  else r.weight_filler.value = 1.f;  // unit scale: a constant 1 filler
+  r.bias_filler = filler(p ? p->first("bias_filler") : nullptr);
+  L.set_tops(in);
+  return true;
+}
+
+bool flatten(Layer& L, std::vector<Shape>*) {  // flatten_layer.cpp with its default axis 1 and end_axis -1
+  Shape in;
+  int64_t axis;  // CanonicalAxisIndex(1) refuses a 0-axis bottom; a 1-axis one, which Caffe refuses too, gives N x 1
+  if (!L.bottom(0, &in) || (in.empty() && !canonical_axis(L, 1, 0, &axis))) return false;
+  L.set_top(0, {in[0], shape_count(in, 1)});
+  return true;
+}
+
+bool concat(Layer& L, std::vector<Shape>*) {  // concat_layer.cpp LayerSetUp and Reshape, with its CHECK messages
+  Shape out;
+  if (!L.bottom(0, &out)) return false;
+  const Node* p = L.node.first("concat_param");
+  const int64_t naxes = static_cast<int64_t>(out.size());
+  int64_t axis = 1;
+  if (p && p->first("axis") && p->first("concat_dim")) return L.refuse("Either axis or concat_dim should be specified; not both.");
+  if (p && p->first("concat_dim")) {  // a uint32: never counted from the end
+    axis = p->integer("concat_dim", 1);
+    if (axis < 0 || axis >= naxes) return L.refuse("concat_dim out of range.");
+  } else if (!canonical_axis(L, p ? p->integer("axis", 1) : 1, naxes, &axis)) {
+    return false;
+  }
+  for (size_t i = 1; i < L.rec.bottoms.size(); ++i) {
+    Shape s;
+    if (!L.bottom(i, &s)) return false;
+    if (s.size() != out.size()) return L.refuse("All inputs must have the same #axes.");
+    for (int64_t j = 0; j < naxes; ++j)
+      if (j != axis && s[j] != out[j]) return L.refuse("All inputs must have the same shape, except at concat_axis.");
+    out[axis] += s[axis];
+  }
+  L.rec.axis = axis;
+  L.set_top(0, out);
+  return true;
+}
+
+bool batch_norm(Layer& L, std::vector<Shape>* params) {
+  // batch_norm_layer.cpp:17-36: mean [C], variance [C], moving-average scale factor [1]; C = shape(1), or 1
+  // for a 1-axis bottom.  The forward pass rewrites them; their lr_mult is whatever the prototxt says.
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  if (in.empty()) return L.bad("BatchNorm bottom");
+  const int64_t C = in.size() == 1 ? 1 : in[1];
+  *params = {{C}, {C}, {1}};
+  L.set_tops(in);
+  if (const Node* p = L.node.first("batch_norm_param")) {  // caffe.proto BatchNormParameter
+    L.rec.use_global_stats = p->boolean("use_global_stats", false);
+    L.rec.moving_average_fraction = static_cast<float>(p->num("moving_average_fraction", 0.999));
+    L.rec.eps = static_cast<float>(p->num("eps", 1e-5));
+  }
+  return true;
+}
+
+bool slice(Layer& L, std::vector<Shape>*) {  // slice_layer.cpp Reshape
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  const Node* p = L.node.first("slice_param");
+  const int64_t naxes = static_cast<int64_t>(in.size());
+  if (p && p->first("axis") && p->first("slice_dim")) return L.refuse("either axis or slice_dim should be specified; not both");
+  const bool dim = p && p->first("slice_dim");  // slice_dim is never counted from the end
+  int64_t axis = dim ? p->integer("slice_dim", 1) : p ? p->integer("axis", 1) : 1;
+  if (!dim && axis < 0) axis += naxes;
+  if (axis < 0 || axis >= naxes)
+    return L.refuse("slice axis " + std::to_string(axis) + " is out of range for a " + std::to_string(naxes) + "-axis bottom");
+  if (L.rec.tops.empty()) return L.refuse("needs at least one top");
+  const int64_t A = in[axis], ntop = static_cast<int64_t>(L.rec.tops.size());
+  std::vector<int64_t> bounds{0};
+  auto points = p ? p->all("slice_point") : std::vector<const Node*>();
+  if (!points.empty()) {
+    if (static_cast<int64_t>(points.size()) != ntop - 1)
+      return L.refuse(std::to_string(points.size()) + " slice_point(s) for " + std::to_string(ntop) + " tops");
+    for (const Node* sp : points) {
+      const int64_t v = atol(sp->value.c_str());
+      if (v <= bounds.back() || v >= A)
+        return L.refuse("slice_point " + std::to_string(v) + " is not increasing inside (0, " + std::to_string(A) + ")");
+      bounds.push_back(v);
+    }
+  } else {
+    if (A % ntop) return L.refuse(std::to_string(ntop) + " tops do not evenly divide slice axis " + std::to_string(A));
+    for (int64_t t = 1; t < ntop; ++t) bounds.push_back(t * (A / ntop));
+  }
+  bounds.push_back(A);
+  L.rec.axis = axis;
+  for (int64_t t = 0; t < ntop; ++t) {
+    Shape s = in;
+    s[axis] = bounds[t + 1] - bounds[t];
+    L.set_top(t, s);
+    L.rec.slice_begin.push_back(bounds[t]);
+    L.rec.slice_end.push_back(bounds[t + 1]);
+  }
+  return true;
+}
+
+bool contrastive_loss(Layer& L, std::vector<Shape>*) {  // contrastive_loss_layer.cpp LayerSetUp and LossLayer::Reshape
+  Shape a, b, sim;
+  if (L.rec.bottoms.size() != 3) return L.refuse("needs 3 bottoms (a, b, sim)");
+  if (!L.bottom(0, &a) || !L.bottom(1, &b) || !L.bottom(2, &sim)) return false;
+  auto legacy = [](const Shape& s, size_t i) { return i < s.size() ? s[i] : int64_t{1}; };  // Blob::LegacyShape
+  if (a.empty() || a.size() > 4 || b.size() != a.size() || sim.empty() || sim.size() > 4)
+    return L.refuse("bottoms must have 1 to 4 axes, a and b as many");
+  if (b[0] != a[0] || sim[0] != a[0]) return L.refuse("a, b and sim must have the same first dimension");
+  if (legacy(a, 1) != legacy(b, 1)) return L.refuse("a and b must have the same channels");
+  if (legacy(a, 2) != 1 || legacy(a, 3) != 1 || legacy(b, 2) != 1 || legacy(b, 3) != 1)
+    return L.refuse("a and b must be N x C (x 1 x 1)");
+  if (legacy(sim, 1) != 1 || legacy(sim, 2) != 1 || legacy(sim, 3) != 1) return L.refuse("sim must hold one value per pair");
+  if (const Node* p = L.node.first("contrastive_loss_param")) {
+    L.rec.margin = static_cast<float>(p->num("margin", 1.0));
+    L.rec.legacy_version = p->boolean("legacy_version", false);
+  }
+  L.set_tops(Shape{});
+  return true;
+}
+
+bool loss(Layer& L, std::vector<Shape>*) { L.set_tops(Shape{}); return true; }  // and Accuracy: scalar tops
+bool silence(Layer&, std::vector<Shape>*) { return true; }
+
+// The layer types the parser understands.  A new type needs a rule and a row here, and a row in native_producer.cpp's
+// table if the built-in engine runs it.
+const struct { const char* type; Rule rule; } kRules[] = {
+    {"MemoryData", memory_data}, {"CoSData", cos_data}, {"Input", input},
+    {"Convolution", convolution}, {"Deconvolution", convolution}, {"Pooling", pooling}, {"InnerProduct", inner_product},
+    {"ReLU", same_shape}, {"LRN", same_shape}, {"Dropout", same_shape}, {"Sigmoid", same_shape}, {"TanH", same_shape},
+    {"Softmax", same_shape}, {"Power", same_shape}, {"AbsVal", same_shape}, {"BNLL", same_shape}, {"ELU", same_shape},
+    {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape},
+    {"Split", split}, {"Eltwise", eltwise}, {"Scale", scale}, {"Flatten", flatten}, {"Concat", concat},
+    {"SoftmaxWithLoss", loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
+    {"HingeLoss", loss}, {"MultinomialLogisticLoss", loss},
+    {"BatchNorm", batch_norm}, {"Slice", slice}, {"ContrastiveLoss", contrastive_loss}, {"Silence", silence},
+};
+
+struct ParamOwners {
+  std::map<std::string, int> by_name;  // ParamSpec.name -> the learnable blob that owns it
+  std::vector<bool> has_lr, has_decay;  // per learnable blob: lr_mult / decay_mult set explicitly
+};
+
+// net.cpp AppendParam for the learnable blobs of one layer, of shapes `params`: an anonymous param, or the first use of
+// a name, owns a learnable blob; a later use of the name shares the owner's.
+bool append_params(const Node& layer, const std::vector<Shape>& params, ParamOwners* owners, SolverSpec* spec,
+                   NetLayer* rec, std::string* err) {
+  auto pspecs = layer.all("param");
+  for (size_t i = 0; i < params.size(); ++i) {
+    const Node* ps = i < pspecs.size() ? pspecs[i] : nullptr;
+    const std::string pname = ps ? ps->str("name", "") : "";
+    auto owner = pname.empty() ? owners->by_name.end() : owners->by_name.find(pname);
+    if (owner == owners->by_name.end()) {
+      if (!pname.empty()) owners->by_name[pname] = static_cast<int>(spec->counts.size());
+      rec->blobs.push_back(static_cast<int>(spec->counts.size())), rec->shared.push_back(false);
+      spec->counts.push_back(shape_count(params[i]));
+      // ParamSpec defaults lr_mult = 1, decay_mult = 1 (caffe.proto:297-304)
+      spec->lr_mult.push_back(ps ? static_cast<float>(ps->num("lr_mult", 1.0)) : 1.0f);
+      spec->decay_mult.push_back(ps ? static_cast<float>(ps->num("decay_mult", 1.0)) : 1.0f);
+      owners->has_lr.push_back(ps && ps->first("lr_mult")), owners->has_decay.push_back(ps && ps->first("decay_mult"));
+      spec->blob_names.push_back(rec->name + "." + std::to_string(i));
+      spec->layer_names.push_back(rec->name);
+      spec->layer_types.push_back(rec->type);
+      spec->shapes.push_back(params[i]);
+      spec->param_index.push_back(static_cast<int>(i));
+      continue;
+    }
+    const int k = owner->second;
+    const std::string share = "Cannot share param '" + pname + "' owned by layer '" + spec->layer_names[k] +
+                              "' with layer '" + rec->name + "'; ";
+    const std::string mode = ps->str("share_mode", "STRICT");
+    if (mode == "PERMISSIVE" || mode == "1") {
+      if (spec->counts[k] != shape_count(params[i])) {
+        *err = share + "count mismatch.  Owner layer param shape is " + shape_string(spec->shapes[k]) +
+               "; sharing layer shape is " + shape_string(params[i]);
+        return false;
+      }
+    } else if (spec->shapes[k] != params[i]) {
+      *err = share + "shape mismatch.  Owner layer param shape is " + shape_string(spec->shapes[k]) +
+             "; sharing layer expects shape " + shape_string(params[i]);
+      return false;
+    }
+    // the first explicit lr_mult / decay_mult, by the owner or a sharer, is the blob's; a different later one is an error
+    struct Mult { const char* field; std::vector<float>* value; std::vector<bool>* set; };
+    for (const Mult& m : {Mult{"lr_mult", &spec->lr_mult, &owners->has_lr},
+                          Mult{"decay_mult", &spec->decay_mult, &owners->has_decay}}) {
+      if (!ps->first(m.field)) continue;
+      const float v = static_cast<float>(ps->num(m.field, 1.0));
+      if ((*m.set)[k] && v != (*m.value)[k]) {
+        *err = "Shared param '" + pname + "' has mismatched " + m.field + ".";
+        return false;
+      }
+      (*m.set)[k] = true;
+      (*m.value)[k] = v;
+    }
+    rec->blobs.push_back(k);
+    rec->shared.push_back(true);
+    spec->shared.push_back(SharedParam{rec->name, rec->type, static_cast<int>(i), k, static_cast<int>(spec->counts.size())});
+  }
+  return true;
+}
+
 // `out` (optional) receives every TRAIN-phase layer with its blob shapes and the parameters the native producer reads.
 // `net_file` is the prototxt the net was read from ("" for text).
 bool net_layout(const Node& net, const std::string& net_file, SolverSpec* spec, std::vector<NetLayer>* out,
                 std::string* err) {
   std::map<std::string, Shape> blobs;
-  if (out) out->clear();
-  spec->inputs.clear();
-  auto staged = [&](const std::string& layer, const std::string& type, const std::string& top, const Shape& s,
-                    const Node* t) {
-    StagedInput in;
-    in.layer = layer, in.type = type, in.top = top, in.shape = to64(s);
-    in.transform = transform(t, net_file);
-    spec->inputs.push_back(in);
+  ParamOwners owners;
+  bool first_data = true;
+  auto record = [&](NetLayer& rec) {
+    if (!out) return;
+    for (const std::string& t : rec.tops) rec.top_shapes.push_back(blobs.count(t) ? blobs[t] : Shape());
+    out->push_back(rec);
   };
-  spec->counts.clear();
-  spec->lr_mult.clear();
-  spec->decay_mult.clear();
-  spec->blob_names.clear();
-  spec->layer_names.clear();
-  spec->layer_types.clear();
-  spec->shapes.clear();
-  spec->param_index.clear();
-  spec->shared.clear();
-  std::map<std::string, int> param_owner;  // ParamSpec.name -> learnable blob that owns it
-  std::vector<bool> has_lr, has_decay;     // per learnable blob: lr_mult / decay_mult set explicitly
+  if (out) out->clear();
+  spec->inputs.clear(), spec->counts.clear(), spec->lr_mult.clear(), spec->decay_mult.clear(), spec->shared.clear();
+  spec->blob_names.clear(), spec->layer_names.clear(), spec->layer_types.clear(), spec->shapes.clear(), spec->param_index.clear();
   spec->net_name = net.str("name");
-  // legacy "input:" / "input_shape" / "input_dim" net-level inputs
-  {
-    auto inputs = net.all("input");
-    auto shapes = net.all("input_shape");
-    auto dims = net.all("input_dim");
+  {  // the legacy net-level "input:" blobs, each with an "input_shape" or four "input_dim"s, as one Input layer
+    NetLayer rec;
+    rec.name = "input", rec.type = "Input";
+    Layer L{net, rec, blobs, err, spec, net_file, first_data};
+    auto inputs = net.all("input"), shapes = net.all("input_shape"), dims = net.all("input_dim");
     for (size_t i = 0; i < inputs.size(); ++i) {
       Shape s;
       if (i < shapes.size()) for (const Node* d : shapes[i]->all("dim")) s.push_back(atol(d->value.c_str()));
       else for (size_t k = 4 * i; k < 4 * i + 4 && k < dims.size(); ++k) s.push_back(atol(dims[k]->value.c_str()));
-      blobs[inputs[i]->value] = s;
-      staged("input", "Input", inputs[i]->value, s, nullptr);
+      rec.tops.push_back(inputs[i]->value);
+      data_top(L, i, s, nullptr);
     }
-    if (out && !inputs.empty()) {
-      NetLayer rec;
-      rec.name = "input";
-      rec.type = "Input";
-      for (const Node* in : inputs) {
-        rec.tops.push_back(in->value);
-        rec.top_shapes.push_back(to64(blobs[in->value]));
-      }
-      out->push_back(rec);
-    }
+    if (!inputs.empty()) record(rec);
   }
   auto layers = net.all("layer");
   if (layers.empty() && !net.all("layers").empty()) {
     *err = "V1 'layers' net definitions are not supported";
     return false;
   }
-  bool first_data = true;
-  for (const Node* L : layers) {
-    if (!in_train_phase(*L)) continue;
-    const std::string type = L->str("type");
-    const std::string name = L->str("name");
-    std::vector<std::string> bottoms, tops;
-    for (const Node* b : L->all("bottom")) bottoms.push_back(b->value);
-    for (const Node* t : L->all("top")) tops.push_back(t->value);
-    auto bottom_shape = [&](size_t i, Shape* s) -> bool {
-      if (i >= bottoms.size() || !blobs.count(bottoms[i])) {
-        *err = "layer '" + name + "' (" + type + "): unknown bottom blob";
-        return false;
-      }
-      *s = blobs[bottoms[i]];
-      return true;
-    };
-    std::vector<long> param_counts;  // learnable blobs this layer owns, in order
-    std::vector<std::vector<int64_t>> param_shapes;
+  for (const Node* node : layers) {
+    if (!in_train_phase(*node)) continue;
     NetLayer rec;
-    rec.name = name;
-    rec.type = type;
-    rec.bottoms = bottoms;
-    rec.tops = tops;
-    for (const std::string& b : bottoms) rec.bottom_shapes.push_back(blobs.count(b) ? to64(blobs[b]) : std::vector<int64_t>());
-    auto refuse = [&](const std::string& reason) {
-      *err = "layer '" + name + "' (" + type + "): " + reason;
-      return false;
-    };
-    rec.has_loss_param = L->first("loss_param") != nullptr;
-    if (const Node* lw = L->first("loss_weight")) rec.loss_weight = static_cast<float>(atof(lw->value.c_str()));
-    if (type == "MemoryData") {
-      const Node* p = L->first("memory_data_param");
-      if (!p) { *err = "MemoryData layer without memory_data_param"; return false; }
-      Shape s{p->integer("batch_size", 0), p->integer("channels", 0), p->integer("height", 0), p->integer("width", 0)};
-      if (!tops.empty()) blobs[tops[0]] = s;
-      if (tops.size() > 1) blobs[tops[1]] = Shape{s[0]};
-      for (size_t i = 0; i < tops.size(); ++i)  // the transform applies to the data, never to the label
-        staged(name, type, tops[i], blobs[tops[i]], i == 0 ? L->first("transform_param") : nullptr);
-      if (first_data) { spec->batch_size = static_cast<int>(s[0]); spec->input_shape.assign(s.begin(), s.end()); first_data = false; }
-    } else if (type == "CoSData") {
-      const Node* p = L->first("cos_data_param");
-      if (!p) { *err = "CoSData layer without cos_data_param"; return false; }
-      long batch = p->integer("batch_size", 0);
-      auto tb = p->all("top");
-      for (size_t i = 0; i < tops.size(); ++i) {
-        Shape s{batch};
-        if (i < tb.size()) {
-          long c = tb[i]->integer("out_channels", 0), h = tb[i]->integer("out_height", 0), w = tb[i]->integer("out_width", 0);
-          if (!c) c = tb[i]->integer("channels", 0);
-          if (!h) h = tb[i]->integer("height", 0);
-          if (!w) w = tb[i]->integer("width", 0);
-          long axes = tb[i]->integer("sample_num_axes", 3);
-          Shape full{c, h, w};
-          for (long a = 0; a < axes && a < 3; ++a) s.push_back(full[a] ? full[a] : 1);
-        }
-        blobs[tops[i]] = s;
-        staged(name, type, tops[i], s, i < tb.size() ? tb[i]->first("transform_param") : nullptr);
-        if (first_data && i == 0) { spec->batch_size = static_cast<int>(batch); spec->input_shape.assign(s.begin(), s.end()); first_data = false; }
-      }
-    } else if (type == "Input") {
-      const Node* p = L->first("input_param");
-      auto shapes = p ? p->all("shape") : std::vector<const Node*>();
-      for (size_t i = 0; i < tops.size(); ++i) {
-        Shape s;
-        const Node* sh = shapes.empty() ? nullptr : shapes[std::min(i, shapes.size() - 1)];
-        if (sh) for (const Node* d : sh->all("dim")) s.push_back(atol(d->value.c_str()));
-        blobs[tops[i]] = s;
-        staged(name, type, tops[i], s, nullptr);
-        if (first_data && i == 0 && !s.empty()) { spec->batch_size = static_cast<int>(s[0]); spec->input_shape.assign(s.begin(), s.end()); first_data = false; }
-      }
-    } else if (type == "Convolution" || type == "Deconvolution") {
-      const Node* p = L->first("convolution_param");
-      Shape in;
-      if (!p || !bottom_shape(0, &in) || in.size() != 4) { if (err->empty()) *err = "layer '" + name + "': bad Convolution"; return false; }
-      long nout = p->integer("num_output", 0), group = p->integer("group", 1);
-      HW k = pair_field(*p, "kernel_size", "kernel_h", "kernel_w", 0);
-      HW st = pair_field(*p, "stride", "stride_h", "stride_w", 1);
-      HW pad = pair_field(*p, "pad", "pad_h", "pad_w", 0);
-      HW dil = pair_field(*p, "dilation", "dilation_h", "dilation_w", 1);
-      bool bias = p->boolean("bias_term", true);
-      if (nout <= 0 || k.h <= 0 || k.w <= 0 || group <= 0 || in[1] % group || nout % group || st.h <= 0 || st.w <= 0 ||
-          dil.h <= 0 || dil.w <= 0 || pad.h < 0 || pad.w < 0) {
-        *err = "layer '" + name + "': bad convolution_param";
-        return false;
-      }
-      rec.num_output = nout;
-      rec.group = group;
-      rec.kernel_h = k.h, rec.kernel_w = k.w, rec.stride_h = st.h, rec.stride_w = st.w;
-      rec.pad_h = pad.h, rec.pad_w = pad.w, rec.dilation_h = dil.h, rec.dilation_w = dil.w;
-      rec.bias_term = bias;
-      rec.weight_filler = filler(p->first("weight_filler"));
-      rec.bias_filler = filler(p->first("bias_filler"));
-      Shape out(4);
-      out[0] = in[0];
-      if (type == "Convolution") {
-        param_counts.push_back(nout * (in[1] / group) * k.h * k.w);  // conv_layer / base_conv_layer.cpp weight shape
-        param_shapes.push_back({nout, in[1] / group, k.h, k.w});
-        out[1] = nout;
-        out[2] = (in[2] + 2 * pad.h - (dil.h * (k.h - 1) + 1)) / st.h + 1;
-        out[3] = (in[3] + 2 * pad.w - (dil.w * (k.w - 1) + 1)) / st.w + 1;
-      } else {
-        param_counts.push_back(in[1] * (nout / group) * k.h * k.w);
-        param_shapes.push_back({in[1], nout / group, k.h, k.w});
-        out[1] = nout;
-        out[2] = st.h * (in[2] - 1) + (dil.h * (k.h - 1) + 1) - 2 * pad.h;
-        out[3] = st.w * (in[3] - 1) + (dil.w * (k.w - 1) + 1) - 2 * pad.w;
-      }
-      if (bias) {
-        param_counts.push_back(nout);
-        param_shapes.push_back({nout});
-      }
-      if (!tops.empty()) blobs[tops[0]] = out;
-    } else if (type == "Pooling") {
-      const Node* p = L->first("pooling_param");
-      Shape in;
-      if (!p || !bottom_shape(0, &in) || in.size() != 4) { if (err->empty()) *err = "layer '" + name + "': bad Pooling"; return false; }
-      HW k = pair_field(*p, "kernel_size", "kernel_h", "kernel_w", 0);
-      HW st = pair_field(*p, "stride", "stride_h", "stride_w", 1);
-      HW pad = pair_field(*p, "pad", "pad_h", "pad_w", 0);
-      if (p->boolean("global_pooling", false)) { k.h = in[2]; k.w = in[3]; }
-      if (k.h <= 0 || k.w <= 0 || st.h <= 0 || st.w <= 0 || pad.h < 0 || pad.w < 0) {
-        *err = "layer '" + name + "': bad pooling_param";
-        return false;
-      }
-      // pooling_layer.cpp: ceil((H + 2p - k) / s) + 1, clipped so the last window starts inside
-      long oh = static_cast<long>(ceil(static_cast<float>(in[2] + 2 * pad.h - k.h) / st.h)) + 1;
-      long ow = static_cast<long>(ceil(static_cast<float>(in[3] + 2 * pad.w - k.w) / st.w)) + 1;
-      if (pad.h || pad.w) {
-        if ((oh - 1) * st.h >= in[2] + pad.h) --oh;
-        if ((ow - 1) * st.w >= in[3] + pad.w) --ow;
-      }
-      rec.kernel_h = k.h, rec.kernel_w = k.w, rec.stride_h = st.h, rec.stride_w = st.w;
-      rec.pad_h = pad.h, rec.pad_w = pad.w;
-      rec.pool = p->str("pool", "MAX");
-      rec.global_pooling = p->boolean("global_pooling", false);
-      for (const std::string& t : tops) blobs[t] = Shape{in[0], in[1], oh, ow};
-    } else if (type == "InnerProduct") {
-      const Node* p = L->first("inner_product_param");
-      Shape in;
-      if (!p || !bottom_shape(0, &in)) { if (err->empty()) *err = "layer '" + name + "': bad InnerProduct"; return false; }
-      long nout = p->integer("num_output", 0);
-      long axis = p->integer("axis", 1);
-      if (axis < 0) axis += static_cast<long>(in.size());
-      if (nout <= 0 || axis < 0 || axis > static_cast<long>(in.size())) { *err = "layer '" + name + "': bad inner_product_param"; return false; }
-      param_counts.push_back(nout * prod(in, static_cast<size_t>(axis)));
-      param_shapes.push_back({nout, prod(in, static_cast<size_t>(axis))});  // inner_product_layer.cpp: N x K
-      if (p->boolean("bias_term", true)) {
-        param_counts.push_back(nout);
-        param_shapes.push_back({nout});
-      }
-      Shape out(in.begin(), in.begin() + axis);
-      out.push_back(nout);
-      if (!tops.empty()) blobs[tops[0]] = out;
-      rec.num_output = nout;
-      rec.axis = axis;
-      rec.bias_term = p->boolean("bias_term", true);
-      rec.transpose = p->boolean("transpose", false);
-      rec.weight_filler = filler(p->first("weight_filler"));
-      rec.bias_filler = filler(p->first("bias_filler"));
-    } else if (type == "ReLU" || type == "LRN" || type == "Dropout" || type == "Sigmoid" || type == "TanH" ||
-               type == "Softmax" || type == "Power" || type == "AbsVal" || type == "BNLL" || type == "ELU" ||
-               type == "Exp" || type == "Log" || type == "Threshold") {
-      Shape in;
-      if (!bottom_shape(0, &in)) return false;
-      for (const std::string& t : tops) blobs[t] = in;
-      if (const Node* p = L->first("relu_param")) rec.negative_slope = static_cast<float>(p->num("negative_slope", 0.0));
-      if (const Node* p = L->first("lrn_param")) {  // caffe.proto LRNParameter
-        rec.local_size = p->integer("local_size", 5);
-        rec.lrn_alpha = static_cast<float>(p->num("alpha", 1.0));
-        rec.lrn_beta = static_cast<float>(p->num("beta", 0.75));
-        rec.lrn_k = static_cast<float>(p->num("k", 1.0));
-        rec.norm_region = p->str("norm_region", "ACROSS_CHANNELS");
-        if (rec.norm_region == "0") rec.norm_region = "ACROSS_CHANNELS";  // the enum's numeric form
-        if (rec.norm_region == "1") rec.norm_region = "WITHIN_CHANNEL";
-      }
-    } else if (type == "Split") {  // split_layer.cpp Reshape
-      Shape in;
-      if (!bottom_shape(0, &in)) return false;
-      for (const std::string& t : tops) {
-        if (t == bottoms[0]) return refuse("Split Layer does not allow in-place computation.");
-        blobs[t] = in;
-      }
-    } else if (type == "Eltwise") {  // eltwise_layer.cpp LayerSetUp and Reshape, after Layer::CheckBlobCounts
-      if (bottoms.size() < 2) return refuse("Eltwise Layer takes at least 2 bottom blob(s) as input.");
-      Shape in;
-      if (!bottom_shape(0, &in)) return false;
-      const Node* p = L->first("eltwise_param");
-      auto coeffs = p ? p->all("coeff") : std::vector<const Node*>();
-      if (!coeffs.empty() && coeffs.size() != bottoms.size())
-        return refuse("Eltwise Layer takes one coefficient per bottom blob.");
-      std::string op = p ? p->str("operation", "SUM") : "SUM";
-      if (op == "0") op = "PROD";  // the enum's numeric form
-      if (op == "1") op = "SUM";
-      if (op == "2") op = "MAX";
-      if (op != "PROD" && op != "SUM" && op != "MAX") return refuse("Unknown elementwise operation.");
-      if (op == "PROD" && !coeffs.empty()) return refuse("Eltwise layer only takes coefficients for summation.");
-      rec.eltwise_op = op;
-      rec.coeffs.assign(bottoms.size(), 1.f);
-      for (size_t i = 0; i < coeffs.size(); ++i) rec.coeffs[i] = static_cast<float>(atof(coeffs[i]->value.c_str()));
-      rec.stable_prod_grad = !p || p->boolean("stable_prod_grad", true);
-      for (size_t i = 1; i < bottoms.size(); ++i) {
-        Shape s;
-        if (!bottom_shape(i, &s)) return false;
-        if (s != in)
-          return refuse("bottom " + std::to_string(i) + " is " + shape_text(s) + ", bottom 0 " + shape_text(in) +
-                        " (Check failed: bottom[i]->shape() == bottom[0]->shape())");
-      }
-      for (const std::string& t : tops) blobs[t] = in;
-    } else if (type == "Scale") {  // scale_layer.cpp LayerSetUp and Reshape; the bias as bias_layer.cpp sets it up
-      if (bottoms.size() > 2) return refuse("Scale Layer takes at most 2 bottom blob(s) as input.");
-      Shape in;
-      if (!bottom_shape(0, &in)) return false;
-      const Node* p = L->first("scale_param");
-      const long naxes = static_cast<long>(in.size());
-      const long given = p ? p->integer("axis", 1) : 1;
-      const long axis = given < 0 ? given + naxes : given;
-      if (axis < 0 || axis >= naxes)  // Blob::CanonicalAxisIndex
-        return refuse("axis " + std::to_string(given) + " out of range for " + std::to_string(naxes) + "-D Blob");
-      Shape scale;  // the scale blob's shape, or bottom[1]'s
-      if (bottoms.size() == 1) {
-        const long num_axes = p ? p->integer("num_axes", 1) : 1;
-        if (num_axes < -1) return refuse("num_axes must be non-negative, or -1 to extend to the end of bottom[0]");
-        if (num_axes >= 0 && naxes < axis + num_axes)
-          return refuse("scale blob's shape extends past bottom[0]'s shape when applied starting with bottom[0] axis = " +
-                        std::to_string(axis));
-        scale.assign(in.begin() + axis, num_axes == -1 ? in.end() : in.begin() + axis + num_axes);
-        param_counts.push_back(prod(scale));
-        param_shapes.push_back(to64(scale));
-      } else if (!bottom_shape(1, &scale)) {
-        return false;
-      }
-      const long first = scale.empty() ? 0 : axis;  // Reshape: a scalar scale applies from axis 0
-      if (naxes < first + static_cast<long>(scale.size()))
-        return refuse("scale blob's shape extends past bottom[0]'s shape when applied starting with bottom[0] axis = " +
-                      std::to_string(first));
-      for (size_t i = 0; i < scale.size(); ++i)
-        if (in[first + i] != scale[i])
-          return refuse("dimension mismatch between bottom[0]->shape(" + std::to_string(first + i) +
-                        ") and scale->shape(" + std::to_string(i) + ")");
-      rec.bias_term = p && p->boolean("bias_term", false);
-      if (rec.bias_term) {  // the Bias layer's blob: the scale's shape (bottom[1]'s in the two-bottom form)
-        param_counts.push_back(prod(scale));
-        param_shapes.push_back(to64(scale));
-      }
-      rec.axis = first;
-      rec.num_axes = static_cast<int64_t>(scale.size());
-      if (p && p->first("filler")) {
-        rec.weight_filler = filler(p->first("filler"));
-      } else {
-        rec.weight_filler.value = 1.f;  // unit scale: a constant 1 filler
-      }
-      rec.bias_filler = filler(p ? p->first("bias_filler") : nullptr);
-      for (const std::string& t : tops) blobs[t] = in;
-    } else if (type == "Flatten") {
-      Shape in;
-      if (!bottom_shape(0, &in) || in.empty()) return false;
-      if (!tops.empty()) blobs[tops[0]] = Shape{in[0], prod(in, 1)};
-    } else if (type == "Concat") {  // concat_layer.cpp LayerSetUp and Reshape, with its CHECK messages
-      Shape out;
-      if (!bottom_shape(0, &out)) return false;
-      const Node* p = L->first("concat_param");
-      const long naxes = static_cast<long>(out.size());
-      long axis = 1;
-      if (p && p->first("axis") && p->first("concat_dim"))
-        return refuse("Either axis or concat_dim should be specified; not both.");
-      if (p && p->first("concat_dim")) {  // a uint32: never counted from the end
-        axis = p->integer("concat_dim", 1);
-        if (axis < 0 || axis >= naxes) return refuse("concat_dim out of range.");
-      } else {
-        const long given = p ? p->integer("axis", 1) : 1;
-        axis = given < 0 ? given + naxes : given;
-        if (axis < 0 || axis >= naxes)  // Blob::CanonicalAxisIndex
-          return refuse("axis " + std::to_string(given) + " out of range for " + std::to_string(naxes) +
-                        "-D Blob");
-      }
-      for (size_t i = 1; i < bottoms.size(); ++i) {
-        Shape s;
-        if (!bottom_shape(i, &s)) return false;
-        if (s.size() != out.size()) return refuse("All inputs must have the same #axes.");
-        for (long j = 0; j < naxes; ++j)
-          if (j != axis && s[j] != out[j]) return refuse("All inputs must have the same shape, except at concat_axis.");
-        out[axis] += s[axis];
-      }
-      rec.axis = axis;
-      if (!tops.empty()) blobs[tops[0]] = out;
-    } else if (type == "SoftmaxWithLoss" || type == "Accuracy" || type == "EuclideanLoss" ||
-               type == "SigmoidCrossEntropyLoss" || type == "HingeLoss" || type == "MultinomialLogisticLoss") {
-      for (const std::string& t : tops) blobs[t] = Shape{};
-    } else if (type == "BatchNorm") {
-      // batch_norm_layer.cpp:17-36: mean [C], variance [C], moving-average scale factor [1]; C = shape(1), or 1
-      // for a 1-axis bottom.  The forward pass rewrites them; their lr_mult is whatever the prototxt says.
-      Shape in;
-      if (!bottom_shape(0, &in)) return false;
-      if (in.empty()) { *err = "layer '" + name + "': bad BatchNorm bottom"; return false; }
-      const long C = in.size() == 1 ? 1 : in[1];
-      param_counts = {C, C, 1};
-      param_shapes = {{C}, {C}, {1}};
-      for (const std::string& t : tops) blobs[t] = in;
-      if (const Node* p = L->first("batch_norm_param")) {  // caffe.proto BatchNormParameter
-        rec.use_global_stats = p->boolean("use_global_stats", false);
-        rec.moving_average_fraction = static_cast<float>(p->num("moving_average_fraction", 0.999));
-        rec.eps = static_cast<float>(p->num("eps", 1e-5));
-      }
-    } else if (type == "Slice") {  // slice_layer.cpp Reshape
-      Shape in;
-      if (!bottom_shape(0, &in)) return false;
-      const Node* p = L->first("slice_param");
-      const long naxes = static_cast<long>(in.size());
-      long axis = 1;
-      if (p && p->first("axis") && p->first("slice_dim")) return refuse("either axis or slice_dim should be specified; not both");
-      if (p && p->first("slice_dim")) {
-        axis = p->integer("slice_dim", 1);
-      } else {
-        axis = p ? p->integer("axis", 1) : 1;
-        if (axis < 0) axis += naxes;
-      }
-      if (axis < 0 || axis >= naxes) return refuse("slice axis " + std::to_string(axis) + " is out of range for a " +
-                                                   std::to_string(naxes) + "-axis bottom");
-      if (tops.empty()) return refuse("needs at least one top");
-      const long A = in[axis], ntop = static_cast<long>(tops.size());
-      std::vector<long> bounds{0};
-      auto points = p ? p->all("slice_point") : std::vector<const Node*>();
-      if (!points.empty()) {
-        if (static_cast<long>(points.size()) != ntop - 1)
-          return refuse(std::to_string(points.size()) + " slice_point(s) for " + std::to_string(ntop) + " tops");
-        for (const Node* sp : points) {
-          const long v = atol(sp->value.c_str());
-          if (v <= bounds.back() || v >= A)
-            return refuse("slice_point " + std::to_string(v) + " is not increasing inside (0, " + std::to_string(A) + ")");
-          bounds.push_back(v);
-        }
-      } else {
-        if (A % ntop) return refuse(std::to_string(ntop) + " tops do not evenly divide slice axis " + std::to_string(A));
-        for (long t = 1; t < ntop; ++t) bounds.push_back(t * (A / ntop));
-      }
-      bounds.push_back(A);
-      rec.axis = axis;
-      for (long t = 0; t < ntop; ++t) {
-        Shape s = in;
-        s[axis] = bounds[t + 1] - bounds[t];
-        blobs[tops[t]] = s;
-        rec.slice_begin.push_back(bounds[t]);
-        rec.slice_end.push_back(bounds[t + 1]);
-      }
-    } else if (type == "ContrastiveLoss") {  // contrastive_loss_layer.cpp LayerSetUp and LossLayer::Reshape
-      Shape a, b, sim;
-      if (bottoms.size() != 3) return refuse("needs 3 bottoms (a, b, sim)");
-      if (!bottom_shape(0, &a) || !bottom_shape(1, &b) || !bottom_shape(2, &sim)) return false;
-      auto legacy = [](const Shape& s, size_t i) { return i < s.size() ? s[i] : 1L; };  // Blob::LegacyShape
-      if (a.empty() || a.size() > 4 || b.size() != a.size() || sim.empty() || sim.size() > 4)
-        return refuse("bottoms must have 1 to 4 axes, a and b as many");
-      if (b[0] != a[0] || sim[0] != a[0]) return refuse("a, b and sim must have the same first dimension");
-      if (legacy(a, 1) != legacy(b, 1)) return refuse("a and b must have the same channels");
-      if (legacy(a, 2) != 1 || legacy(a, 3) != 1 || legacy(b, 2) != 1 || legacy(b, 3) != 1)
-        return refuse("a and b must be N x C (x 1 x 1)");
-      if (legacy(sim, 1) != 1 || legacy(sim, 2) != 1 || legacy(sim, 3) != 1) return refuse("sim must hold one value per pair");
-      if (const Node* p = L->first("contrastive_loss_param")) {
-        rec.margin = static_cast<float>(p->num("margin", 1.0));
-        rec.legacy_version = p->boolean("legacy_version", false);
-      }
-      for (const std::string& t : tops) blobs[t] = Shape{};
-    } else if (type == "Silence") {
-    } else {
-      *err = "layer '" + name + "' of type '" + type +
+    rec.name = node->str("name"), rec.type = node->str("type");
+    for (const Node* b : node->all("bottom")) rec.bottoms.push_back(b->value);
+    for (const Node* t : node->all("top")) rec.tops.push_back(t->value);
+    for (const std::string& b : rec.bottoms) rec.bottom_shapes.push_back(blobs.count(b) ? blobs[b] : Shape());
+    rec.has_loss_param = node->first("loss_param") != nullptr;
+    if (const Node* lw = node->first("loss_weight")) rec.loss_weight = static_cast<float>(atof(lw->value.c_str()));
+    Rule rule = nullptr;
+    for (const auto& row : kRules)
+      if (rec.type == row.type) rule = row.rule;
+    if (!rule) {
+      *err = "layer '" + rec.name + "' of type '" + rec.type +
              "' is not understood by the layout parser; pass the layout with cos_net_allocate_desc";
       return false;
     }
-    // net.cpp AppendParam: an anonymous param, or the first use of a name, owns a learnable blob; a later use of the
-    // name shares the owner's
-    auto pspecs = L->all("param");
-    for (size_t i = 0; i < param_counts.size(); ++i) {
-      const Node* ps = i < pspecs.size() ? pspecs[i] : nullptr;
-      const std::string pname = ps ? ps->str("name", "") : "";
-      auto owner = pname.empty() ? param_owner.end() : param_owner.find(pname);
-      if (owner == param_owner.end()) {
-        if (!pname.empty()) param_owner[pname] = static_cast<int>(spec->counts.size());
-        rec.blobs.push_back(static_cast<int>(spec->counts.size()));
-        rec.shared.push_back(false);
-        spec->counts.push_back(param_counts[i]);
-        // ParamSpec defaults lr_mult = 1, decay_mult = 1 (caffe.proto:297-304)
-        spec->lr_mult.push_back(ps ? static_cast<float>(ps->num("lr_mult", 1.0)) : 1.0f);
-        spec->decay_mult.push_back(ps ? static_cast<float>(ps->num("decay_mult", 1.0)) : 1.0f);
-        has_lr.push_back(ps && ps->first("lr_mult"));
-        has_decay.push_back(ps && ps->first("decay_mult"));
-        spec->blob_names.push_back(name + "." + std::to_string(i));
-        spec->layer_names.push_back(name);
-        spec->layer_types.push_back(type);
-        spec->shapes.push_back(param_shapes[i]);
-        spec->param_index.push_back(static_cast<int>(i));
-        continue;
-      }
-      const int k = owner->second;
-      auto shape_string = [](const std::vector<int64_t>& s) {  // Blob::shape_string
-        std::string t;
-        int64_t n = 1;
-        for (int64_t d : s) t += std::to_string(d) + " ", n *= d;
-        return t + "(" + std::to_string(n) + ")";
-      };
-      const std::string share = "Cannot share param '" + pname + "' owned by layer '" + spec->layer_names[k] +
-                                "' with layer '" + name + "'; ";
-      const std::string mode = ps->str("share_mode", "STRICT");
-      if (mode == "PERMISSIVE" || mode == "1") {
-        if (spec->counts[k] != param_counts[i]) {
-          *err = share + "count mismatch.  Owner layer param shape is " + shape_string(spec->shapes[k]) +
-                 "; sharing layer shape is " + shape_string(param_shapes[i]);
-          return false;
-        }
-      } else if (spec->shapes[k] != param_shapes[i]) {
-        *err = share + "shape mismatch.  Owner layer param shape is " + shape_string(spec->shapes[k]) +
-               "; sharing layer expects shape " + shape_string(param_shapes[i]);
-        return false;
-      }
-      // the first explicit lr_mult / decay_mult, by the owner or a sharer, is the blob's; a different later one is an
-      // error
-      struct Mult { const char* field; std::vector<float>* value; std::vector<bool>* set; };
-      for (const Mult& m : {Mult{"lr_mult", &spec->lr_mult, &has_lr}, Mult{"decay_mult", &spec->decay_mult, &has_decay}}) {
-        if (!ps->first(m.field)) continue;
-        const float v = static_cast<float>(ps->num(m.field, 1.0));
-        if ((*m.set)[k] && v != (*m.value)[k]) {
-          *err = "Shared param '" + pname + "' has mismatched " + m.field + ".";
-          return false;
-        }
-        (*m.set)[k] = true;
-        (*m.value)[k] = v;
-      }
-      rec.blobs.push_back(k);
-      rec.shared.push_back(true);
-      SharedParam sp;
-      sp.layer_name = name;
-      sp.layer_type = type;
-      sp.param_index = static_cast<int>(i);
-      sp.owner = k;
-      sp.position = static_cast<int>(spec->counts.size());
-      spec->shared.push_back(sp);
-    }
-    if (out) {
-      for (const std::string& t : tops) rec.top_shapes.push_back(blobs.count(t) ? to64(blobs[t]) : std::vector<int64_t>());
-      out->push_back(rec);
-    }
+    Layer L{*node, rec, blobs, err, spec, net_file, first_data};
+    std::vector<Shape> params;
+    if (!rule(L, &params) || !append_params(*node, params, &owners, spec, &rec, err)) return false;
+    record(rec);
   }
   return true;
 }
 
-bool parse_solver(const std::string& solver_path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err);
-
-}  // namespace
-
-bool parse_net_prototxt_text(const std::string& text, SolverSpec* spec, std::string* err) {
-  Node net;
-  TextParser tp(text);
-  if (!tp.parse(&net, err)) return false;
-  return net_layout(net, "", spec, nullptr, err);
-}
-
-std::string find_relative_file(const std::string& path, const std::string& relative_to) {
-  auto opens = [](const std::string& p) { return static_cast<bool>(std::ifstream(p.c_str(), std::ios::binary)); };
-  if (opens(path)) return path;
-  size_t slash = relative_to.find_last_of('/');
-  std::string dir = slash == std::string::npos ? "." : relative_to.substr(0, slash);
-  if (opens(dir + "/" + path)) return dir + "/" + path;
-  size_t s2 = path.find_last_of('/');
-  if (s2 != std::string::npos && opens(dir + "/" + path.substr(s2 + 1))) return dir + "/" + path.substr(s2 + 1);
-  return "";
-}
-
-bool parse_train_net(const std::string& path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err) {
-  std::string text;
-  if (!read_file(path, &text)) {
-    *err = "cannot read prototxt '" + path + "'";
-    return false;
-  }
-  Node top;
-  TextParser tp(text);
-  if (!tp.parse(&top, err)) return false;
-  if (!top.all("layer").empty() || !top.all("layers").empty() || !top.all("input").empty())
-    return net_layout(top, path, spec, layers, err);
-  return parse_solver(path, spec, layers, err);
-}
-
-bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std::string* err) {
-  return parse_solver(solver_path, spec, nullptr, err);
-}
-
-bool check_solver_layout(const SolverSpec& spec, std::string* err) {
-  uint64_t n = 0;
-  for (int64_t c : spec.counts) n += static_cast<uint64_t>(c);
-  if (spec.solver_type == 1 && n == 0) {
-    *err = "solver type 'Adam' needs learnable parameters; for a net without any, only SGD is on the accelerated "
-           "path (with no history blobs, its Adam and SGD solver states could not be told apart)";
-    return false;
-  }
-  return true;
-}
-
-namespace {
 bool parse_solver(const std::string& solver_path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err) {
   std::string text;
   if (!read_file(solver_path, &text)) {
@@ -879,12 +839,8 @@ bool parse_solver(const std::string& solver_path, SolverSpec* spec, std::vector<
   spec->snapshot_hdf5 = s.str("snapshot_format", "BINARYPROTO") == "HDF5";
   spec->random_seed = s.integer("random_seed", -1);
   spec->solver_file = solver_path;
-  std::string type = s.str("type", "");
-  if (type.empty()) {
-    std::string st = s.str("solver_type", "SGD");  // deprecated enum field
-    type = st;
-  }
-  spec->type = type;
+  spec->type = s.str("type", "");
+  if (spec->type.empty()) spec->type = s.str("solver_type", "SGD");  // deprecated enum field
   if (spec->type != "SGD" && spec->type != "Adam" && spec->type != "ADAM") {
     *err = "solver type '" + spec->type + "' is not on the accelerated path (only SGD with momentum is)";
     return false;
@@ -927,6 +883,47 @@ bool parse_solver(const std::string& solver_path, SolverSpec* spec, std::vector<
   if (!np.parse(&net, err)) return false;
   return net_layout(net, net_file, spec, layers, err) && check_solver_layout(*spec, err);
 }
+
 }  // namespace
+
+std::string find_relative_file(const std::string& path, const std::string& relative_to) {
+  auto opens = [](const std::string& p) { return static_cast<bool>(std::ifstream(p.c_str(), std::ios::binary)); };
+  if (opens(path)) return path;
+  size_t slash = relative_to.find_last_of('/');
+  std::string dir = slash == std::string::npos ? "." : relative_to.substr(0, slash);
+  if (opens(dir + "/" + path)) return dir + "/" + path;
+  size_t s2 = path.find_last_of('/');
+  if (s2 != std::string::npos && opens(dir + "/" + path.substr(s2 + 1))) return dir + "/" + path.substr(s2 + 1);
+  return "";
+}
+
+bool parse_train_net(const std::string& path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err) {
+  std::string text;
+  if (!read_file(path, &text)) {
+    *err = "cannot read prototxt '" + path + "'";
+    return false;
+  }
+  Node top;
+  TextParser tp(text);
+  if (!tp.parse(&top, err)) return false;
+  if (!top.all("layer").empty() || !top.all("layers").empty() || !top.all("input").empty())
+    return net_layout(top, path, spec, layers, err);
+  return parse_solver(path, spec, layers, err);
+}
+
+bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std::string* err) {
+  return parse_solver(solver_path, spec, nullptr, err);
+}
+
+bool check_solver_layout(const SolverSpec& spec, std::string* err) {
+  uint64_t n = 0;
+  for (int64_t c : spec.counts) n += static_cast<uint64_t>(c);
+  if (spec.solver_type == 1 && n == 0) {
+    *err = "solver type 'Adam' needs learnable parameters; for a net without any, only SGD is on the accelerated "
+           "path (with no history blobs, its Adam and SGD solver states could not be told apart)";
+    return false;
+  }
+  return true;
+}
 
 }  // namespace cosb

@@ -134,6 +134,11 @@ struct SolverSpec {
   int history_sets() const { return solver_type == 1 ? 2 : 1; }
 };
 
+// Blob::count(from): the product of the axes from `from` on (1 for none).
+int64_t shape_count(const std::vector<int64_t>& s, size_t from = 0);
+// "2x3x4", or "scalar" for a shape without axes.
+std::string shape_text(const std::vector<int64_t>& s);
+
 // SocketSync::chunk (socket_sync_cpu.cpp:46-54).
 void chunk(uint64_t param_count, int cluster_size, int peer, uint64_t* offs, uint64_t* size);
 
@@ -153,8 +158,6 @@ bool parse_solver_prototxt(const std::string& solver_path, SolverSpec* spec, std
 // Checks that apply once the layout is known: an Adam solver needs at least one learnable element (a snapshot of a
 // net without any holds no history blobs, so restore could not refuse a state of the other solver kind).
 bool check_solver_layout(const SolverSpec& spec, std::string* err);
-// Parses only a net prototxt text (TRAIN phase) into the layout part of spec.
-bool parse_net_prototxt_text(const std::string& text, SolverSpec* spec, std::string* err);
 // A solver prototxt (its net is read as parse_solver_prototxt reads it) or a net prototxt, told apart by whether the
 // file has top-level layers: fills spec (solver fields only for a solver file) and the TRAIN-phase layer list.
 bool parse_train_net(const std::string& path, SolverSpec* spec, std::vector<NetLayer>* layers, std::string* err);
