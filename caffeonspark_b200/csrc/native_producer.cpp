@@ -32,14 +32,21 @@ bool filler_ok(const FillerSpec& f, std::string* reason) {
   return true;
 }
 
-// Caffe's ReLU and MAX pool as the existing fused block accepts them: slope 0; square window, pad 0, kernel <= 15.
+// Caffe's ReLU and MAX pool as the existing fused block accepts them: slope 0; square window, pad 0, kernel <= 15, and
+// no empty window.  Caffe's pooled size ceil((H - k) / s) + 1 (pad 0: no clip) counts a last window that starts at or
+// past the edge when s >= k + r (H - k = q * s + r, 0 < r < s); ReLU then MAX pool writes -FLT_MAX there, while the
+// fused block pools only the pooled_size() windows, which all start inside.  So it fuses only when the two sizes agree.
 bool fusable_relu(const NetLayer& L) {
   return L.type == "ReLU" && L.negative_slope == 0.f && L.bottoms.size() == 1 && L.tops.size() == 1;
 }
 bool fusable_pool(const NetLayer& L) {
-  return L.type == "Pooling" && L.pool == "MAX" && !L.global_pooling && L.pad_h == 0 && L.pad_w == 0 &&
-         L.kernel_h == L.kernel_w && L.stride_h == L.stride_w && L.kernel_h <= 15 && L.bottoms.size() == 1 &&
-         L.tops.size() == 1 && L.bottom_shapes[0].size() == 4;
+  if (L.type != "Pooling" || L.pool != "MAX" || L.global_pooling || L.pad_h != 0 || L.pad_w != 0 ||
+      L.kernel_h != L.kernel_w || L.stride_h != L.stride_w || L.kernel_h > 15 || L.bottoms.size() != 1 ||
+      L.tops.size() != 1 || L.bottom_shapes[0].size() != 4 || L.top_shapes[0].size() != 4)
+    return false;
+  const int k = static_cast<int>(L.kernel_h), s = static_cast<int>(L.stride_h);
+  return L.top_shapes[0][2] == pooled_size(static_cast<int>(L.bottom_shapes[0][2]), k, s) &&
+         L.top_shapes[0][3] == pooled_size(static_cast<int>(L.bottom_shapes[0][3]), k, s);
 }
 
 // The weight (and bias) of a Convolution, InnerProduct or Scale: a shared param uses its owner's offsets, and only the
@@ -360,12 +367,20 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     } else if (op.kind == OpKind::kContrastiveLoss) {  // the parser checked the shapes: a, b N x C (x 1 x 1), sim N values
       op.margin = L.margin;
       op.legacy = L.legacy_version;
-    } else if (op.kind == OpKind::kSoftmaxLoss) {
+    } else if (op.kind == OpKind::kSoftmaxLoss) {  // the parser made the axis canonical for the scores' shape
+      const size_t axis = static_cast<size_t>(L.axis);
+      if (L.axis < 0 || axis >= op.in_shape.size()) {
+        *err = why(L, "axis " + std::to_string(L.axis) + " is not an axis of the " + shape_text(op.in_shape) + " scores");
+        return false;
+      }
+      op.softmax_axis = static_cast<int>(axis);
+      op.classes = op.in_shape[axis];
+      op.inner = shape_count(op.in_shape, axis + 1);
+      op.rows = shape_count(std::vector<int64_t>(op.in_shape.begin(), op.in_shape.begin() + axis)) * op.inner;
       const int64_t labels = P.tensor_count[op.bottoms[1]];
-      const int64_t rows = op.in_shape.empty() ? 0 : shape_count(op.in_shape) / (op.in_shape.size() > 1 ? op.in_shape[1] : 1);
-      if (op.in_shape.size() < 2 || labels != rows) {
-        *err = why(L, "label count " + std::to_string(labels) + " does not match the " + std::to_string(rows) +
-                          " rows of the scores");
+      if (labels != op.rows) {
+        *err = why(L, "label count " + std::to_string(labels) + " does not match the " + std::to_string(op.rows) +
+                          " rows of the scores along axis " + std::to_string(axis));
         return false;
       }
     }
@@ -429,7 +444,8 @@ std::string Plan::text() const {
     }
     if (op.kind == OpKind::kSlice || op.kind == OpKind::kConcat)
       os << " axis=" << op.slice_axis << " begin=" << op.slice_begin;
-    if (op.kind == OpKind::kSoftmaxLoss) os << " label=" << op.bottoms[1] << " loss_weight=" << op.loss_weight;
+    if (op.kind == OpKind::kSoftmaxLoss)
+      os << " axis=" << op.softmax_axis << " label=" << op.bottoms[1] << " loss_weight=" << op.loss_weight;
     if (op.kind == OpKind::kContrastiveLoss)
       os << " second=" << op.bottoms[1] << " sim=" << op.bottoms[2] << " margin=" << op.margin
          << (op.legacy ? " legacy" : "") << " loss_weight=" << op.loss_weight;

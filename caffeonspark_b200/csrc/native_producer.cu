@@ -308,8 +308,8 @@ __global__ void sigmoid_backward_kernel(const float* y, const float* dy, float* 
 }
 
 // ------------------------------------------------------------------ SoftmaxWithLoss
-// One block.  Row r = (n, s) of the scores x[n, c, s]: p = softmax over c, loss_r = -log(max(p[label], FLT_MIN)),
-// dx = (p - onehot) * loss_weight / count.  Rows are summed per thread in order, then by a fixed tree, so the loss is
+// One block.  Row r = (o, s) of the scores x[o, c, s] (outer o, class c along the softmax axis, inner s): p = softmax
+// over c, loss_r = -log(max(p[label], FLT_MIN)), dx = (p - onehot) * loss_weight / count.  Rows are summed per thread in order, then by a fixed tree, so the loss is
 // reproducible; *loss = loss_weight * (sum / count).  A label outside [0, C) (or NaN) sets *status and contributes
 // neither loss nor gradient; nothing outside the row is read.
 __global__ void __launch_bounds__(kThreads) softmax_loss_kernel(const float* x, const float* label, float* dx,
@@ -859,14 +859,11 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
                                 op.lrn_alpha, op.lrn_beta, s);
     // The loss kernels also write their bottoms' gradients.  SoftmaxWithLoss writes its bottom's whatever bottom_grad
     // says (a staged input's too: every tensor has a gradient buffer).
-    case OpKind::kSoftmaxLoss: {
-      const int C = static_cast<int>(op.in_shape[1]);
-      const int rows = static_cast<int>(plan_.tensor_count[op.bottoms[0]] / C);
-      const int inner = static_cast<int>(rows / op.in_shape[0]);
-      softmax_loss_kernel<<<1, kThreads, 0, s>>>(x, act_[op.bottoms[1]], grad_[op.bottoms[0]], loss_dev, rows, C, inner,
-                                                 op.loss_weight, status_);
+    case OpKind::kSoftmaxLoss:
+      softmax_loss_kernel<<<1, kThreads, 0, s>>>(x, act_[op.bottoms[1]], grad_[op.bottoms[0]], loss_dev,
+                                                 static_cast<int>(op.rows), static_cast<int>(op.classes),
+                                                 static_cast<int>(op.inner), op.loss_weight, status_);
       return cudaGetLastError();
-    }
     case OpKind::kContrastiveLoss: {
       const int N = static_cast<int>(op.in_shape[0]);
       const int C = static_cast<int>(plan_.tensor_count[op.bottoms[0]] / N);

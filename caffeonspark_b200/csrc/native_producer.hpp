@@ -51,6 +51,10 @@ struct Op {
   std::vector<int> shares;             // learnable blobs this op uses as a sharer of a named param (owned elsewhere)
   float slope = 0.f;                   // ReLU negative_slope
   float loss_weight = 1.f;             // SoftmaxWithLoss, ContrastiveLoss, EuclideanLoss
+  // SoftmaxWithLoss (softmax_loss_layer.cpp Reshape): the class axis and its C classes; rows = count(0, axis) *
+  // inner, one label each, with inner = count(axis + 1)
+  int softmax_axis = 1;
+  int64_t classes = 0, rows = 0, inner = 1;
   bool global_stats = false;           // BatchNorm
   float fraction = 0.999f, eps = 1e-5f;
   int lrn_size = 0;                    // LRN (WITHIN_CHANNEL only)

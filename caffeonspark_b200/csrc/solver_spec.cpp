@@ -429,8 +429,20 @@ bool pooling(Layer& L, std::vector<Shape>*) {
   if (!p || !L.bottom(0, &in) || in.size() != 4) return L.bad("Pooling");
   HW k = pair_field(*p, "kernel_size", "kernel_h", "kernel_w", 0), st = pair_field(*p, "stride", "stride_h", "stride_w", 1);
   HW pad = pair_field(*p, "pad", "pad_h", "pad_w", 0);
-  if (p->boolean("global_pooling", false)) { k.h = in[2]; k.w = in[3]; }
+  const bool global = p->boolean("global_pooling", false);
+  if (global) {  // pooling_layer.cpp LayerSetUp's checks, in its order
+    if (p->first("kernel_size") || p->first("kernel_h") || p->first("kernel_w"))
+      return L.refuse("With Global_pooling: true Filter size cannot specified");
+    k.h = in[2], k.w = in[3];
+  }
   if (k.h <= 0 || k.w <= 0 || st.h <= 0 || st.w <= 0 || pad.h < 0 || pad.w < 0) return L.bad("pooling_param");
+  if (global && (pad.h || pad.w || st.h != 1 || st.w != 1))
+    return L.refuse("With Global_pooling: true; only pad = 0 and stride = 1");
+  // a window that lay entirely in the padding would pool nothing
+  if (pad.h >= k.h)
+    return L.refuse("Check failed: pad_h_ < kernel_h_ (" + std::to_string(pad.h) + " vs. " + std::to_string(k.h) + ")");
+  if (pad.w >= k.w)
+    return L.refuse("Check failed: pad_w_ < kernel_w_ (" + std::to_string(pad.w) + " vs. " + std::to_string(k.w) + ")");
   // pooling_layer.cpp: ceil((H + 2p - k) / s) + 1, clipped so the last window starts inside
   int64_t oh = static_cast<int64_t>(ceil(static_cast<float>(in[2] + 2 * pad.h - k.h) / st.h)) + 1;
   int64_t ow = static_cast<int64_t>(ceil(static_cast<float>(in[3] + 2 * pad.w - k.w) / st.w)) + 1;
@@ -440,7 +452,7 @@ bool pooling(Layer& L, std::vector<Shape>*) {
   }
   NetLayer& r = L.rec;
   r.kernel_h = k.h, r.kernel_w = k.w, r.stride_h = st.h, r.stride_w = st.w, r.pad_h = pad.h, r.pad_w = pad.w;
-  r.pool = p->str("pool", "MAX"), r.global_pooling = p->boolean("global_pooling", false);
+  r.pool = p->str("pool", "MAX"), r.global_pooling = global;
   L.set_tops({in[0], in[1], oh, ow});
   return true;
 }
@@ -669,6 +681,15 @@ bool contrastive_loss(Layer& L, std::vector<Shape>*) {  // contrastive_loss_laye
 }
 
 bool loss(Layer& L, std::vector<Shape>*) { L.set_tops(Shape{}); return true; }  // and Accuracy: scalar tops
+
+bool softmax_loss(Layer& L, std::vector<Shape>* params) {  // softmax_loss_layer.cpp Reshape: the class axis
+  Shape in;
+  const Node* p = L.node.first("softmax_param");
+  if (!L.rec.bottoms.empty() && L.blobs.count(L.rec.bottoms[0]) && L.bottom(0, &in) &&
+      !canonical_axis(L, p ? p->integer("axis", 1) : 1, static_cast<int64_t>(in.size()), &L.rec.axis))
+    return false;
+  return loss(L, params);
+}
 bool silence(Layer&, std::vector<Shape>*) { return true; }
 
 // The layer types the parser understands.  A new type needs a rule and a row here, and a row in native_producer.cpp's
@@ -680,7 +701,7 @@ const struct { const char* type; Rule rule; } kRules[] = {
     {"Softmax", same_shape}, {"Power", same_shape}, {"AbsVal", same_shape}, {"BNLL", same_shape}, {"ELU", same_shape},
     {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape},
     {"Split", split}, {"Eltwise", eltwise}, {"Scale", scale}, {"Flatten", flatten}, {"Concat", concat},
-    {"SoftmaxWithLoss", loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
+    {"SoftmaxWithLoss", softmax_loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
     {"HingeLoss", loss}, {"MultinomialLogisticLoss", loss},
     {"BatchNorm", batch_norm}, {"Slice", slice}, {"ContrastiveLoss", contrastive_loss}, {"Silence", silence},
 };

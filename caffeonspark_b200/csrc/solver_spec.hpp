@@ -34,6 +34,7 @@ struct NetLayer {
   // whether it is shared (a later use of a named param)
   std::vector<int> blobs;
   std::vector<bool> shared;
+  // axis: InnerProduct's, Slice's, Concat's, Scale's, and SoftmaxWithLoss's class axis (softmax_param, canonical)
   int64_t num_output = 0, axis = 1, group = 1;
   int64_t kernel_h = 0, kernel_w = 0, stride_h = 1, stride_w = 1, pad_h = 0, pad_w = 0, dilation_h = 1, dilation_w = 1;
   bool bias_term = true, transpose = false, global_pooling = false;
