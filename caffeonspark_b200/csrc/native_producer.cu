@@ -362,9 +362,10 @@ __global__ void slice_copy_kernel(const float* src, float* dst, int64_t total, i
 // One block.  Pair r: d = a_r - b_r, dist_sq = sum over c of d_c^2 in c order.  A similar pair (static_cast<int>(sim)
 // nonzero) adds dist_sq to the loss and gets da = alpha * d.  A dissimilar pair adds max(margin - dist_sq, 0)
 // (legacy_version) or max(margin - dist, 0)^2, and gets da = beta * d while mdist = margin - dist_sq (legacy) or
-// margin - dist is > 0, else 0, with beta = -alpha (legacy) or -alpha * mdist / (dist + 1e-4).  alpha = loss_weight / N
-// and db = -da.  Pairs are summed per thread in order, then by a fixed tree; *loss = loss_weight * (sum / N / 2).  A
-// non-finite sim sets *status and its pair contributes neither loss nor gradient.  da / db are null for a staged bottom.
+// margin - dist is > 0, else an exact 0, with beta = -alpha (legacy) or -alpha * mdist / (dist + 1e-4).  alpha =
+// loss_weight / N and db = -da.  As in Caffe, a NaN in d makes a dissimilar pair's loss NaN and its gradient 0.  Pairs
+// are summed per thread in order, then by a fixed tree; *loss = loss_weight * (sum / N / 2).  A non-finite sim sets
+// *status and its pair contributes neither loss nor gradient.  da / db are null for a staged bottom.
 // Made for the narrow embeddings of siamese nets (C of a few to a few dozen: each thread walks its pairs' C channels
 // twice).  For wide embeddings and few pairs most threads idle and the row loads are not coalesced.
 __global__ void __launch_bounds__(kThreads) contrastive_loss_kernel(const float* a, const float* b, const float* sim,
@@ -384,26 +385,28 @@ __global__ void __launch_bounds__(kThreads) contrastive_loss_kernel(const float*
     }
     const float s = sim[r];
     float scale = 0.f;  // gradient of a = scale * d
+    bool zero = true;   // gradient an exact 0 (caffe_set), not 0 * d: a NaN or infinite d stays out of it
     if (!isfinite(s)) {
       *reinterpret_cast<volatile int*>(status) = kStatusBadLabel;
     } else if (static_cast<int>(s)) {
       part = __fadd_rn(part, dist_sq);
-      scale = alpha;
+      scale = alpha, zero = false;
     } else if (legacy) {
+      // std::max(mdist, 0) returns its first argument unless mdist < 0: a NaN mdist reaches the loss
       const float mdist = __fsub_rn(margin, dist_sq);
-      part = __fadd_rn(part, fmaxf(mdist, 0.f));
-      if (mdist > 0.f) scale = -alpha;
+      part = __fadd_rn(part, mdist < 0.f ? 0.f : mdist);
+      if (mdist > 0.f) scale = -alpha, zero = false;
     } else {
       const float dist = __fsqrt_rn(dist_sq);
       const float mdist = __fsub_rn(margin, dist);
-      const float m = fmaxf(mdist, 0.f);
+      const float m = mdist < 0.f ? 0.f : mdist;
       part = __fadd_rn(part, __fmul_rn(m, m));
-      if (mdist > 0.f) scale = __fdiv_rn(__fmul_rn(-alpha, mdist), __fadd_rn(dist, 1e-4f));
+      if (mdist > 0.f) scale = __fdiv_rn(__fmul_rn(-alpha, mdist), __fadd_rn(dist, 1e-4f)), zero = false;
     }
     for (int c = 0; c < C; ++c) {
-      const float g = __fmul_rn(scale, __fsub_rn(ar[c], br[c]));
+      const float g = zero ? 0.f : __fmul_rn(scale, __fsub_rn(ar[c], br[c]));
       if (da) da[(size_t)r * C + c] = g;
-      if (db) db[(size_t)r * C + c] = -g;
+      if (db) db[(size_t)r * C + c] = zero ? 0.f : -g;
     }
   }
   part = block_sum(part, sh);

@@ -342,7 +342,9 @@ def contrastive_loss(a, b, sim, margin=1.0, legacy=False, loss_weight=1.0):
             per = torch.where(similar, dist_sq, dissimilar)
             n = a.shape[0]
             scale = torch.where(similar, torch.ones_like(beta), torch.where(mdist > 0, beta, torch.zeros_like(beta)))
-            ctx.save_for_backward(scale[:, None] * d)
+            # caffe_set: an exact 0 where a dissimilar pair has !(mdist > 0), not 0 * d (a NaN d stays out of it)
+            on = (similar | (mdist > 0))[:, None]
+            ctx.save_for_backward(torch.where(on, scale[:, None] * d, torch.zeros_like(d)))
             ctx.shapes = (a.shape, b.shape)
             return loss_weight * (per.sum() / n / 2)
 

@@ -1,5 +1,6 @@
-"""Float64 references, with Caffe's rules, of the built-in producer's Convolution, Pooling, InnerProduct, ReLU, Sigmoid
-and SoftmaxWithLoss ops (DESIGN.md section 14), and per-element error bounds derived from each op's rounding count.
+"""Float64 references, with Caffe's rules, of the built-in producer's Convolution, Pooling, InnerProduct, ReLU, Sigmoid,
+SoftmaxWithLoss, Slice, Concat, Split, Eltwise, Scale, EuclideanLoss and ContrastiveLoss ops (DESIGN.md section 14),
+and per-element error bounds derived from each op's rounding count.
 
 Every reference takes the fp32 inputs exactly (as float64) and returns float64.  A dot-product bound is
 (n + extra) * 2^-24 * sum |a_i * b_i|: n is the number of FMAs of one accumulation, extra the further roundings of
@@ -307,12 +308,230 @@ def softmax_loss_bounds(x, label, axis=1, loss_weight=1.0):
     return loss_bound, dx_bound.reshape(np.shape(x))
 
 
+# ------------------------------------------------------------------ Slice, Concat, Split (slice_layer, concat_layer, split_layer)
+def slice_bounds(size, points=None, tops=None):
+    """slice_layer.cpp Reshape: the [begin, end) of every top along the axis, from slice_points or an equal split"""
+    cuts = list(points) if points else [t * (size // tops) for t in range(1, tops)]
+    return list(zip([0] + cuts, cuts + [size]))
+
+
+def slice_forward(x, axis, ranges):
+    """pure copies: every value, NaN, infinity and subnormal, comes through unchanged"""
+    idx = [slice(None)] * x.ndim
+    out = []
+    for b, e in ranges:
+        idx[axis] = slice(b, e)
+        out.append(np.asarray(x)[tuple(idx)])
+    return out
+
+
+def split_backward32(ds, reverse=False):
+    """split_layer.cpp: the gradients of the read tops added in fp32 in top order (`reverse`: a mutation)"""
+    ds = [np.asarray(d, np.float32) for d in (ds[::-1] if reverse else ds)]
+    acc = ds[0].copy()
+    for d in ds[1:]:
+        acc = acc + d
+    return acc
+
+
+def split_backward_bound(ds):
+    """k tops: k - 1 roundings, each at most u times the running sum's magnitude"""
+    return (len(ds) - 1) * U * sum(np.abs(np.asarray(d, np.float64)) for d in ds)
+
+
+def rel(n):
+    """relative error of n roundings, (1 + u)^n - 1, from above"""
+    return n * U * (1 + n * U)
+
+
+# ------------------------------------------------------------------ Eltwise (eltwise_layer.cpp, the CPU order)
+def eltwise_sum(xs, coeffs):
+    """-> y (float64), its bound and the gradients' scale: y = c0 x0 rounded, then one fma per further bottom, so k
+    roundings each at most u times the sum of |c_i x_i|"""
+    c = [float(np.float32(v)) for v in coeffs]
+    terms = [ci * np.asarray(x, np.float64) for ci, x in zip(c, xs)]
+    return sum(terms), len(xs) * U * sum(np.abs(t) for t in terms) + len(xs) * TINY
+
+
+def eltwise_sum_backward32(dy, coeff):
+    """a copy when the coefficient is 1, else fl(c * dy)"""
+    dy = np.asarray(dy, np.float32)
+    return dy.copy() if np.float32(coeff) == 1 else np.float32(coeff) * dy
+
+
+def eltwise_prod(xs):
+    """-> y (float64) and its bound: x0 x1, then times each further bottom, k - 1 roundings"""
+    y = np.prod([np.asarray(x, np.float64) for x in xs], axis=0)
+    return y, rel(len(xs) - 1) * np.abs(y) + TINY
+
+
+def eltwise_prod_backward(xs, dy, stable):
+    """-> per-bottom (dx (float64), bound).  stable_prod_grad: the product of the other bottoms, then times dy (k - 1
+    roundings).  Otherwise caffe_div(y, x_i) then times dy: y carries k - 1 roundings and the two operations add two
+    more, and the division makes NaN exactly where x_i is 0 or infinite (0 / 0, inf / inf)."""
+    xs = [np.asarray(x, np.float64) for x in xs]
+    dy = np.asarray(dy, np.float64)
+    out = []
+    with np.errstate(invalid="ignore", over="ignore"):
+        for i in range(len(xs)):
+            g = np.prod([x for j, x in enumerate(xs) if j != i], axis=0) * dy
+            if stable:
+                out.append((g, rel(len(xs) - 1) * np.abs(g) + TINY))
+            else:
+                g = np.where((xs[i] == 0) | np.isinf(xs[i]), np.nan, g)
+                out.append((g, rel(len(xs) + 1) * np.abs(g) + 2 * TINY))
+    return out
+
+
+def eltwise_max(xs, later_wins_ties=False):
+    """-> y, winner index.  eltwise_layer.cpp Forward_cpu: bottom 0 wins over bottom 1 only when strictly greater;
+    every later bottom takes over only when strictly greater than y, so a NaN wins when it is bottom 1 and is passed
+    over elsewhere.  `later_wins_ties` (a later bottom taking over on >=, as in Caffe's GPU kernel) is a mutation for
+    the bound tests."""
+    xs = [np.asarray(x, np.float32) for x in xs]
+    gt = np.greater_equal if later_wins_ties else np.greater
+    first = ~np.greater(xs[0], xs[1])
+    y = np.where(first, xs[1], xs[0])
+    idx = first.astype(np.int64)
+    for b in range(2, len(xs)):
+        take = gt(xs[b], y)
+        y = np.where(take, xs[b], y)
+        idx = np.where(take, b, idx)
+    return y, idx
+
+
+def eltwise_max_backward(dy, idx, k):
+    dy = np.asarray(dy, np.float32)
+    return [np.where(idx == b, dy, np.float32(0)) for b in range(k)]
+
+
+# ------------------------------------------------------------------ Scale (scale_layer.cu)
+def scale_view(shape, axis, num_axes):
+    """-> (outer, dim, inner) of scale_layer.cpp for a canonical axis and num_axes (-1: to the end)"""
+    end = len(shape) if num_axes == -1 else axis + num_axes
+    if end == axis:  # a scalar scale applies from axis 0 (ScaleLayer::Reshape)
+        axis = end = 0
+    return (int(np.prod(shape[:axis], dtype=np.int64)), int(np.prod(shape[axis:end], dtype=np.int64)),
+            int(np.prod(shape[end:], dtype=np.int64)))
+
+
+def scale_forward(x, s, b, view, two_roundings=False):
+    """-> y (float64) and its bound: x * s + b rounded once (one fma): half an ulp, plus the float64 rounding of the
+    reference itself and the subnormal floor.  `two_roundings` (the product rounded to fp32 first) is a mutation."""
+    outer, dim, inner = view
+    x3 = np.asarray(x, np.float64).reshape(outer, dim, inner)
+    s3 = np.asarray(s, np.float64).reshape(1, dim, 1)
+    p = x3 * s3
+    if two_roundings:
+        p = p.astype(np.float32).astype(np.float64)
+    y = p if b is None else p + np.asarray(b, np.float64).reshape(1, dim, 1)
+    return y.reshape(np.shape(x)), (ulp(y) / 2 + 2.0 ** -53 * np.abs(y) + TINY).reshape(np.shape(x))
+
+
+def scale_backward(x, s, dy, view):
+    """-> ds, db (float64) and their bounds (one fma per product in scale_grad_kernel, bias_grad_kernel's order), and
+    dx = fl(dy * s) in fp32"""
+    outer, dim, inner = view
+    x3, dy3 = np.asarray(x, np.float64).reshape(outer, dim, inner), np.asarray(dy, np.float64).reshape(outer, dim, inner)
+    n = bias_grad_count(outer * inner)
+    ds, db = (x3 * dy3).sum(axis=(0, 2)), dy3.sum(axis=(0, 2))
+    bs, bb = n * U * np.abs(x3 * dy3).sum(axis=(0, 2)), n * U * np.abs(dy3).sum(axis=(0, 2))
+    dx = (np.asarray(dy, np.float32).reshape(outer, dim, inner) * np.asarray(s, np.float32).reshape(1, dim, 1))
+    return ds, bs + TINY, db, bb + TINY, dx.reshape(np.shape(x))
+
+
+# ------------------------------------------------------------------ EuclideanLoss (euclidean_loss_layer.cpp)
+def euclidean_loss(a, b, loss_weight=1.0):
+    """-> loss (float64) and its bound: d = a - b and d^2 round (rel(3) each), the per-thread in-order sums and the
+    8-level tree add ceil(count / 256) + 8 roundings, then / num and * loss_weight one each (/ 2 is exact)."""
+    num = np.shape(a)[0]
+    d = np.asarray(a, np.float64).ravel() - np.asarray(b, np.float64).ravel()
+    dot = float(np.sum(d * d))
+    loss = loss_weight * (dot / num / 2)
+    adds = -(-d.size // BLOCK) + 8
+    with np.errstate(invalid="ignore"):
+        bound = abs(loss_weight) / num / 2 * (rel(3) + adds * U) * dot * (1 + rel(2)) + rel(2) * abs(loss) + TINY
+    return loss, bound
+
+
+def euclidean_grads32(a, b, loss_weight=1.0):
+    """da = fl(fl(loss_weight / num) * fl(a - b)), db = fl(-fl(loss_weight / num) * fl(a - b)), as numpy float32"""
+    alpha = np.float32(loss_weight) / np.float32(np.shape(a)[0])
+    d = (np.asarray(a, np.float32).reshape(np.shape(a)[0], -1) - np.asarray(b, np.float32).reshape(np.shape(a)[0], -1))
+    return (alpha * d).reshape(np.shape(a)), (-alpha * d).reshape(np.shape(b))
+
+
+# ------------------------------------------------------------------ ContrastiveLoss (contrastive_loss_layer.cpp)
+EPS_DIST = float(np.float32(1e-4))  # Dtype(1e-4)
+
+
+def contrastive_loss(a, b, sim, margin=1.0, legacy=False, loss_weight=1.0, eps=EPS_DIST, legacy_grad_without_d=False):
+    """-> loss, da, db, mdist (float64) with Caffe's CPU rules: static_cast<int>(sim) truncates; a dissimilar pair adds
+    std::max(mdist, 0), which keeps a NaN mdist; its gradient is beta * d while mdist > 0 and an exact 0 otherwise
+    (caffe_set), beta = -alpha (legacy) or -alpha * mdist / (dist + 1e-4).  `eps` and `legacy_grad_without_d` (the
+    legacy gradient written as beta alone, as Caffe's GPU kernel does) are mutations for the bound tests."""
+    n = np.shape(a)[0]
+    d = np.asarray(a, np.float64).reshape(n, -1) - np.asarray(b, np.float64).reshape(n, -1)
+    similar = np.trunc(np.asarray(sim, np.float64).ravel()) != 0
+    alpha = loss_weight / n
+    with np.errstate(invalid="ignore", over="ignore"):
+        dsq = np.sum(d * d, axis=1)
+        dist = np.sqrt(dsq)
+        mdist = margin - (dsq if legacy else dist)
+        m = np.where(mdist < 0, 0.0, mdist)
+        per = np.where(similar, dsq, m if legacy else m * m)
+        beta = np.full(n, -alpha) if legacy else -alpha * mdist / (dist + eps)
+        scale = np.where(similar, alpha, np.where(mdist > 0, beta, 0.0))
+        grad = scale[:, None] * d
+        if legacy and legacy_grad_without_d:
+            grad = np.where((~similar & (mdist > 0))[:, None], beta[:, None] * np.ones_like(d), grad)
+        grad = np.where((similar | (mdist > 0))[:, None], grad, 0.0)  # caffe_set: not 0 * NaN
+    loss = loss_weight * float(np.sum(per)) / n / 2
+    return loss, grad.reshape(np.shape(a)), (-grad).reshape(np.shape(b)), mdist
+
+
+def contrastive_bounds(a, b, sim, margin=1.0, legacy=False, loss_weight=1.0):
+    """-> (loss bound, gradient bound, mdist bound), all first order in u.  dist_sq: d and d^2 round (rel(3)) and C - 1
+    in-order adds; sqrt one more (half the relative error of dist_sq, plus u); mdist one subtraction.  A dissimilar
+    pair's max(mdist, 0)^2 doubles mdist's relative error and rounds once.  The loss adds ceil(N / 256) + 8 roundings,
+    then / N and * loss_weight.  The gradient: alpha, d and the product one rounding each; the non-legacy beta adds
+    the product and quotient roundings, dist + 1e-4 (one) and mdist's error relative to its size."""
+    with np.errstate(invalid="ignore", over="ignore"):
+        return _contrastive_bounds(a, b, sim, margin, legacy, loss_weight)
+
+
+def _contrastive_bounds(a, b, sim, margin, legacy, loss_weight):
+    n = np.shape(a)[0]
+    d = np.asarray(a, np.float64).reshape(n, -1) - np.asarray(b, np.float64).reshape(n, -1)
+    c = d.shape[1]
+    similar = np.trunc(np.asarray(sim, np.float64).ravel()) != 0
+    dsq = np.sum(d * d, axis=1)
+    e_dsq = (rel(3) + (c - 1) * U) * dsq + c * TINY
+    dist = np.sqrt(dsq)
+    e_dist = np.where(dsq > 0, e_dsq / (2 * np.maximum(dist, FLT_MIN)), np.sqrt(e_dsq)) + U * dist
+    mdist = margin - (dsq if legacy else dist)
+    e_md = (e_dsq if legacy else e_dist) + U * np.abs(mdist)
+    m = np.maximum(mdist, 0)
+    e_per = np.where(similar, e_dsq, np.where(mdist > 0, e_md if legacy else 2 * m * e_md + e_md ** 2 + U * m * m, 0))
+    per = np.where(similar, dsq, m if legacy else m * m)
+    adds = -(-n // BLOCK) + 8
+    alpha = abs(loss_weight) / n
+    loss_bound = alpha / 2 * (e_per.sum() + adds * U * per.sum()) * (1 + rel(2)) + rel(2) * alpha / 2 * per.sum() + TINY
+    den = dist + EPS_DIST
+    g_rel = np.where(similar | legacy, rel(3), rel(6) + (e_dist + U * den) / den)
+    g_abs = np.where(similar | legacy, 0.0, alpha * e_md / den)
+    ref_scale = np.where(similar | legacy, alpha, alpha * np.abs(mdist) / den)
+    on = similar | (mdist > 0)
+    bound = np.where(on[:, None], (ref_scale * g_rel + g_abs)[:, None] * np.abs(d), 0.0) + 2 * TINY
+    return loss_bound, bound.reshape(np.shape(a)), e_md
+
+
 # ------------------------------------------------------------------ inputs
 def dyadic(rng, shape, bits=3, top=4):
     """Integers in [-top, top] times 2^-bits: ties are real ties, and every sum of a few thousand products of such
     values is exact in fp32."""
-    return (rng.randint(-top, top + 1, size=shape) * 2.0 ** -bits).astype(np.float32)
+    return np.asarray(rng.randint(-top, top + 1, size=shape) * 2.0 ** -bits).astype(np.float32)
 
 
 def gaussian(rng, shape, scale=1.0):
-    return (rng.randn(*shape) * scale).astype(np.float32)
+    return np.asarray(rng.randn(*shape) * scale).astype(np.float32)
