@@ -1,9 +1,12 @@
 """Forward/backward time of the built-in producer against the PyTorch fp32 producer (DESIGN.md section 14).
 
-Workloads: the six nets the engine runs, at their reference batch sizes (LeNet b64, CIFAR-10-quick b100,
+Workloads: the eight nets the engine runs, at their reference batch sizes (LeNet b64, CIFAR-10-quick b100,
 cifar10_full_bn b100, cifar10_full b100, the siamese MNIST example b64 of 2x28x28 pairs: its two LeNet trunks share
 their weights and end in a ContrastiveLoss, timed against the PyTorch module that runs one trunk twice; and the
-ResNet-20 fixture b100, timed against nets.resnet20_module, whose BatchNorms run the same native kernels).  For each, one process times the native engine, the PyTorch module with TF32 off and with
+ResNet-20 fixture b100, timed against nets.resnet20_module, whose BatchNorms run the same native kernels; the two
+autoencoder fixtures b100 of 1x28x28, Caffe's MNIST autoencoder and the convolutional one with Deconvolutions, each
+scoring its reconstruction against its input with SigmoidCrossEntropyLoss, timed against nets.autoencoder_module and
+nets.conv_autoencoder_module).  For each, one process times the native engine, the PyTorch module with TF32 off and with
 TF32 on (cuDNN's default, here applied to matmuls too), alternating the three in every round; each sample is CUDA events around `--iters`
 back-to-back forward/backward calls on one stream after `--warmup` untimed ones.  Prints one JSON line per
 workload with median / min / max ms per call and images/s, and the card's name and power limit.
@@ -24,7 +27,9 @@ import tempfile
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full", "mnist_siamese", "cifar10_resnet20")
+WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full", "mnist_siamese", "cifar10_resnet20",
+             "mnist_autoencoder", "mnist_conv_autoencoder")
+FIXTURES = ("cifar10_resnet20", "mnist_autoencoder", "mnist_conv_autoencoder")  # nets kept under tests/golden/configs
 FP32_PEAK = 67e12  # H100 SXM data sheet, dense FP32, at up to 700 W
 
 
@@ -53,14 +58,14 @@ def siamese_solver(directory):
     return path
 
 
-def resnet20_solver(directory):
-    """The ResNet-20 fixture's solver, pointed at the fixture's net wherever this runs from."""
+def fixture_solver(directory, name):
+    """A fixture's solver, pointed at the fixture's net wherever this runs from."""
     configs = os.path.join(ROOT, "tests", "golden", "configs")
-    solver = open(os.path.join(configs, "cifar10_resnet20_solver.prototxt")).read()
-    path = os.path.join(directory, "cifar10_resnet20_solver.prototxt")
+    solver = open(os.path.join(configs, f"{name}_solver.prototxt")).read()
+    path = os.path.join(directory, f"{name}_solver.prototxt")
     with open(path, "w") as f:
-        f.write(solver.replace('net: "cifar10_resnet20_train_test.prototxt"',
-                               f'net: "{os.path.join(configs, "cifar10_resnet20_train_test.prototxt")}"'))
+        f.write(solver.replace(f'net: "{name}_train_test.prototxt"',
+                               f'net: "{os.path.join(configs, f"{name}_train_test.prototxt")}"'))
     return path
 
 
@@ -76,7 +81,16 @@ def plan_gemms(text):
         w = int(re.search(r" w=\d+:(\d+)", line).group(1)) if " w=" in line else 0
         # the plan's rule: no data gradient into a staged input, nor into a blob with no learnable blob before it
         need_dx = " staged-bottom" not in line and " no-bottom-grad" not in line
-        if kind in ("Convolution", "ConvBiasReLUMaxPool"):
+        if kind == "Deconvolution":  # the transpose of the convolution from its top to its bottom
+            kh, kw = (int(v) for v in re.search(r" k(\d+)x(\d+)", line).groups())
+            n, cin, h, wd = ins
+            cout, oh, ow = (int(v) for v in f[6].split("x")[1:])
+            fwd.append((f"{name} forward", 2 * cout * n * oh * ow * cin * kh * kw))
+            back = [(f"{name} weight gradient", 2 * cin * cout * kh * kw * n * h * wd)]
+            if need_dx:
+                back.append((f"{name} data gradient", 2 * cin * n * h * wd * cout * kh * kw))
+            bwd.append(back if " no-backward" not in line else [])
+        elif kind in ("Convolution", "ConvBiasReLUMaxPool"):
             kh, kw = (int(v) for v in re.search(r" k(\d+)x(\d+)", line).groups())
             sh, sw = (int(v) for v in re.search(r" s(\d+)x(\d+)", line).groups())
             ph, pw = (int(v) for v in re.search(r" p(\d+)x(\d+)", line).groups())
@@ -88,7 +102,7 @@ def plan_gemms(text):
             back = [(f"{name} weight gradient", 2 * cout * k * cols)]
             if need_dx:
                 back.append((f"{name} data gradient", 2 * cin * n * h * wd * cout * kh * kw))
-            bwd.append(back)
+            bwd.append(back if " no-backward" not in line else [])
         elif kind == "InnerProduct":
             b = ins[0]
             k = 1
@@ -99,7 +113,7 @@ def plan_gemms(text):
             back = [(f"{name} weight gradient", 2 * nout * k * b)]
             if need_dx:
                 back.append((f"{name} data gradient", 2 * b * k * nout))
-            bwd.append(back)
+            bwd.append(back if " no-backward" not in line else [])
     return fwd + [g for back in reversed(bwd) for g in back]
 
 
@@ -124,12 +138,15 @@ def main():
     tmp = tempfile.mkdtemp(prefix="bench_native_producer_")
     for name in args.workloads.split(","):
         siamese, resnet = name == "mnist_siamese", name == "cifar10_resnet20"
-        solver = siamese_solver(tmp) if siamese else resnet20_solver(tmp) if resnet else nets.write_prototxts(name, tmp)
+        autoencoder = name in ("mnist_autoencoder", "mnist_conv_autoencoder")
+        solver = (siamese_solver(tmp) if siamese else fixture_solver(tmp, name) if name in FIXTURES
+                  else nets.write_prototxts(name, tmp))
         net = C.CaffeNet(solver, "", "", 1, 1, 0, True, C.CaffeNet.NONE, -1, 0)
         net.use_native_producer(fill_weights=False)
         net.fill("data", 1, 0, 0.05)
         torch.cuda.synchronize()
-        spec = nets.RESNET20 if resnet else None if siamese else nets.NETS[name]
+        spec = (nets.RESNET20 if resnet else None if siamese else nets.AUTOENCODER if name == "mnist_autoencoder"
+                else nets.CONV_AUTOENCODER if autoencoder else nets.NETS[name])
         batch = 64 if siamese else spec["batch"]
         rng = np.random.RandomState(0)
         shape = (2, 28, 28) if siamese else spec["input"]
@@ -142,10 +159,14 @@ def main():
         torch.cuda.synchronize()
         torch.cuda.set_stream(stream)
 
-        def native():
-            assert net.forward_backward([x, y], loss.data_ptr(), stream=stream.cuda_stream), net.last_error()
+        inputs = [x] if autoencoder else [x, y]  # an autoencoder's one staged input is its target too
 
-        module = (nets.siamese_module() if siamese else nets.resnet20_module() if resnet else nets.torch_module(name)).cuda()
+        def native():
+            assert net.forward_backward(inputs, loss.data_ptr(), stream=stream.cuda_stream), net.last_error()
+
+        module = (nets.siamese_module() if siamese else nets.resnet20_module() if resnet
+                  else nets.autoencoder_module() if name == "mnist_autoencoder"
+                  else nets.conv_autoencoder_module() if autoencoder else nets.torch_module(name)).cuda()
         with torch.no_grad():
             w, off = net.data().clone(), 0
             for p in module.parameters():
@@ -157,6 +178,9 @@ def main():
             if siamese:
                 a, b = module(x)
                 nets.contrastive_loss(a, b, y).backward()
+                return
+            if autoencoder:
+                nets.sigmoid_cross_entropy_loss(module(x), x).backward()
                 return
             out = module(x)
             F.cross_entropy(out, ylong).backward()

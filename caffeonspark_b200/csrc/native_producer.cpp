@@ -29,6 +29,10 @@ bool filler_ok(const FillerSpec& f, std::string* reason) {
     *reason = "filler variance_norm '" + f.variance_norm + "' is not FAN_IN, FAN_OUT or AVERAGE";
     return false;
   }
+  if (f.sparse != -1 && (f.type != "gaussian" || f.sparse < -1)) {  // filler.hpp's CHECKs
+    *reason = f.type != "gaussian" ? "Sparsity not supported by this Filler." : "Check failed: sparse >= -1";
+    return false;
+  }
   return true;
 }
 
@@ -49,8 +53,8 @@ bool fusable_pool(const NetLayer& L) {
          L.top_shapes[0][3] == pooled_size(static_cast<int>(L.bottom_shapes[0][3]), k, s);
 }
 
-// The weight (and bias) of a Convolution, InnerProduct or Scale: a shared param uses its owner's offsets, and only the
-// owner's filler fills the blob.  False when a filler is one the engine cannot draw.
+// The weight (and bias) of a Convolution, Deconvolution, InnerProduct or Scale: a shared param uses its owner's
+// offsets, and only the owner's filler fills the blob.  False when a filler is one the engine cannot draw.
 bool set_params(const NetLayer& L, Op* op, Plan* P, std::string* err) {
   std::string reason;
   if (!filler_ok(L.weight_filler, &reason) || (L.bias_term && !filler_ok(L.bias_filler, &reason))) {
@@ -66,8 +70,9 @@ bool set_params(const NetLayer& L, Op* op, Plan* P, std::string* err) {
   return true;
 }
 
-// euclidean_loss_layer.cpp, after LossLayer::Reshape's check
-bool euclidean_shapes_ok(const NetLayer& L, std::string* err) {
+// LossLayer::Reshape's check, then euclidean_loss_layer.cpp's or sigmoid_cross_entropy_loss_layer.cpp's: the two
+// bottoms hold as many values (per item, or in all: the same once the numbers agree), with the layer's own wording
+bool loss_shapes_ok(const NetLayer& L, const char* count_message, std::string* err) {
   const std::vector<int64_t>& a = L.bottom_shapes[0];
   const std::vector<int64_t>& b = L.bottom_shapes[1];
   if (a.empty() || b.empty() || a[0] != b[0]) {
@@ -75,7 +80,7 @@ bool euclidean_shapes_ok(const NetLayer& L, std::string* err) {
     return false;
   }
   if (shape_count(a, 1) != shape_count(b, 1)) {
-    *err = why(L, "Inputs must have the same dimension.");
+    *err = why(L, count_message);
     return false;
   }
   return true;
@@ -106,15 +111,19 @@ const LayerType kLayerTypes[] = {
     {"Concat", OpKind::kConcat, -1},
     {"Eltwise", OpKind::kEltwise, -1},
     {"Scale", OpKind::kScale},  // the one-bottom form
+    {"Deconvolution", OpKind::kDeconv},
+    {"Flatten", OpKind::kFlatten},  // axis 1 to the end only
     {"SoftmaxWithLoss", OpKind::kSoftmaxLoss, 2, false, 1, "label", true},
     {"ContrastiveLoss", OpKind::kContrastiveLoss, 3, false, 2, "sim", true},  // a, b, sim
     {"EuclideanLoss", OpKind::kEuclideanLoss, 2, false, -1, nullptr, true},
+    {"SigmoidCrossEntropyLoss", OpKind::kSigmoidCrossEntropyLoss, 2, false, 1, "target", true},
 };
 
 // Plan::text's name of each OpKind
 const char* const kKindNames[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling", "InnerProduct", "ReLU", "Sigmoid",
                                   "BatchNorm", "SoftmaxWithLoss", "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss",
-                                  "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale"};
+                                  "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale", "Deconvolution", "Flatten",
+                                  "SigmoidCrossEntropyLoss"};
 static_assert(std::size(kKindNames) == static_cast<size_t>(OpKind::kCount), "one name per OpKind");
 
 }  // namespace
@@ -157,13 +166,16 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
   for (size_t i = 0; i < layers.size(); ++i) {
     const NetLayer& L = layers[i];
     if (is_data_layer(L.type) || L.type == "Accuracy" || L.type == "Silence") continue;  // no TRAIN work
+    const LayerType* row = nullptr;
+    for (const LayerType& r : kLayerTypes)
+      if (L.type == r.type) row = &r;
+    // Net::Init gives a loss layer of weight 0 no backward, and its value never reaches the objective: no TRAIN work
+    // either (a monitor such as the MNIST autoencoder's l2_error), so its bottoms do not count as read
+    if (row && row->loss && L.loss_weight == 0.f) continue;
     if (L.has_loss_param) {
       *err = why(L, "loss_param is not supported (only the default VALID normalisation without ignore_label is)");
       return false;
     }
-    const LayerType* row = nullptr;
-    for (const LayerType& r : kLayerTypes)
-      if (L.type == r.type) row = &r;
     if (!row || (row->kind == OpKind::kLRNWithin && L.norm_region != "WITHIN_CHANNEL")) {
       *err = why(L, "layer type not supported");
       return false;
@@ -223,7 +235,11 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         *err = why(L, "a second loss layer is not supported");
         return false;
       }
-      if (row->kind == OpKind::kEuclideanLoss && !euclidean_shapes_ok(L, err)) return false;
+      if (row->kind == OpKind::kEuclideanLoss && !loss_shapes_ok(L, "Inputs must have the same dimension.", err))
+        return false;
+      if (row->kind == OpKind::kSigmoidCrossEntropyLoss &&
+          !loss_shapes_ok(L, "SIGMOID_CROSS_ENTROPY_LOSS layer inputs must have the same count.", err))
+        return false;
     }
     if (op.kind == OpKind::kSlice) {  // one op per top, each copying its range of the bottom (and back, in the backward)
       op.slice_axis = static_cast<int>(L.axis);
@@ -267,7 +283,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     }
     int storage = -1;
     const std::string* top = auto_top ? nullptr : &L.tops[0];
-    if (op.kind == OpKind::kConv) {
+    if (op.kind == OpKind::kConv || op.kind == OpKind::kDeconv) {
       if (L.group != 1) {
         *err = why(L, "group " + std::to_string(L.group) + " > 1 is not supported");
         return false;
@@ -281,7 +297,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.sh = static_cast<int>(L.stride_h), op.sw = static_cast<int>(L.stride_w);
       op.ph = static_cast<int>(L.pad_h), op.pw = static_cast<int>(L.pad_w);
       // conv + bias followed by ReLU and MAX pool in either order: the existing fused block (caffe_layers.cu)
-      if (L.bias_term && i + 2 < layers.size()) {
+      if (op.kind == OpKind::kConv && L.bias_term && i + 2 < layers.size()) {
         const NetLayer& a = layers[i + 1];
         const NetLayer& b = layers[i + 2];
         const bool order = (fusable_relu(a) && fusable_pool(b)) || (fusable_pool(a) && fusable_relu(b));
@@ -329,6 +345,22 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       const int in = op.bottoms[0];
       op.in_place = L.tops[0] == L.bottoms[0] && in >= P.ninputs && !P.data_alias[in];
       if (op.in_place) storage = P.storage[in];
+    } else if (op.kind == OpKind::kFlatten) {  // flatten_layer.cpp: no copy either way (ShareData, ShareDiff)
+      if (L.tops[0] == L.bottoms[0]) {
+        *err = why(L, "Flatten Layer does not allow in-place computation.");
+        return false;
+      }
+      const int64_t naxes = static_cast<int64_t>(op.in_shape.size());
+      const int64_t first = L.flatten_axis < 0 ? L.flatten_axis + naxes : L.flatten_axis;
+      const int64_t last = L.flatten_end_axis < 0 ? L.flatten_end_axis + naxes : L.flatten_end_axis;
+      if (first != 1 || last != naxes - 1) {
+        *err = why(L, "flatten_param axis " + std::to_string(L.flatten_axis) + ", end_axis " +
+                          std::to_string(L.flatten_end_axis) + " is not supported (axis 1 to the last axis is)");
+        return false;
+      }
+      // the top's gradient is the bottom's, except on a staged input, whose gradient buffer nothing may share
+      const int in = op.bottoms[0];
+      if (in >= P.ninputs) storage = P.storage[in];
     } else if (op.kind == OpKind::kBatchNorm) {
       if (!op.shares.empty()) {
         *err = why(L, "shared BatchNorm statistics are not supported");
@@ -385,25 +417,42 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       }
     }
     op.out = new_tensor(shape_count(op.out_shape), storage);
+    if (op.kind == OpKind::kFlatten) P.data_alias[op.out] = true;
     // BatchNorm's blobs are statistics, with no gradient
     wants_grad[op.out] = top_grad || (op.kind != OpKind::kBatchNorm && (op.w_off >= 0 || op.b_off >= 0));
     if (top) cur[*top] = op.out;
     if (row->loss) loss_top = op.out, loss_layer = L.name;
     P.ops.push_back(op);
   }
-  // the op of each Split's top 0 sums the gradients of the tops some layer reads (consumer[] is complete now)
+  if (losses == 0) {
+    *err = "the net has no SoftmaxWithLoss, ContrastiveLoss, EuclideanLoss or SigmoidCrossEntropyLoss layer with a "
+           "non-zero loss_weight in its TRAIN phase (native producer)";
+    return false;
+  }
+  // Caffe's blobs_under_loss: the loss's top, and every non-label bottom of an op whose top is under the loss.  Every
+  // blob has one reader (Splits aside), so one pass in reverse order finds them.  An op whose top is not under the loss
+  // runs no backward; a Split top that is not adds nothing to its bottom's gradient, and a Slice top's op still writes
+  // its range of the bottom's gradient (zeros), which the other ranges' readers need.
+  std::vector<bool> under_loss(P.tensor_count.size(), false);
+  under_loss[loss_top] = true;
+  for (size_t i = P.ops.size(); i-- > 0;) {
+    Op& op = P.ops[i];
+    if (!under_loss[op.out]) {
+      if (op.kind == OpKind::kSplit) op.split_unread = true;
+      else if (op.kind != OpKind::kSlice) op.no_backward = true;
+      continue;
+    }
+    for (size_t b = 0; b < op.bottoms.size(); ++b)
+      if (static_cast<int>(b) != op.label_bottom) under_loss[op.bottoms[b]] = true;
+  }
+  // the op of each Split's top 0 sums the gradients of the tops under the loss, in top order
   for (size_t i = 0; i < P.ops.size(); ++i) {
     if (P.ops[i].kind != OpKind::kSplit || P.ops[i].split_top != 0) continue;
     for (size_t j = i; j < P.ops.size() && P.ops[j].kind == OpKind::kSplit && P.ops[j].bottoms[0] == P.ops[i].bottoms[0];
          ++j) {
       if (j > i && P.ops[j].split_top == 0) break;  // the next Split of the same bottom
-      if (consumer[P.ops[j].out].empty()) P.ops[j].split_unread = true;
-      else P.ops[i].split_sum.push_back(P.ops[j].out);
+      if (!P.ops[j].split_unread) P.ops[i].split_sum.push_back(P.ops[j].out);
     }
-  }
-  if (losses == 0) {
-    *err = "the net has no SoftmaxWithLoss, ContrastiveLoss or EuclideanLoss layer in its TRAIN phase (native producer)";
-    return false;
   }
   for (size_t t = 0; t < P.tensor_count.size(); ++t) {
     if (P.tensor_count[t] <= 0 || P.tensor_count[t] >= (int64_t(1) << 31)) {
@@ -430,7 +479,8 @@ std::string Plan::text() const {
     if (op.kind == OpKind::kPool) os << "(" << (op.max_pool ? "MAX" : "AVE") << ")";
     if (op.kind == OpKind::kEltwise) os << "(" << eltwise_ops[op.eltwise_op] << ")";
     os << " " << op.name << " " << shape_text(op.in_shape) << " -> " << shape_text(op.out_shape);
-    if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kPool)
+    if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kPool ||
+        op.kind == OpKind::kDeconv)
       os << " k" << op.kh << "x" << op.kw << " s" << op.sh << "x" << op.sw << " p" << op.ph << "x" << op.pw;
     if (op.kind == OpKind::kConvBiasReluMaxPool) os << " pool" << op.pool_kernel << "/" << op.pool_stride;
     if (op.kind == OpKind::kReLU && op.slope != 0.f) os << " slope=" << op.slope;
@@ -450,6 +500,9 @@ std::string Plan::text() const {
       os << " second=" << op.bottoms[1] << " sim=" << op.bottoms[2] << " margin=" << op.margin
          << (op.legacy ? " legacy" : "") << " loss_weight=" << op.loss_weight;
     if (op.kind == OpKind::kEuclideanLoss) os << " second=" << op.bottoms[1] << " loss_weight=" << op.loss_weight;
+    if (op.kind == OpKind::kSigmoidCrossEntropyLoss)
+      os << " target=" << op.bottoms[1] << " loss_weight=" << op.loss_weight;
+    if (op.kind == OpKind::kFlatten) os << " data=bottom" << (storage[op.out] != op.out ? " diff=bottom" : "");
     if (op.kind == OpKind::kSplit) os << " top=" << op.split_top << " data=bottom" << (op.split_unread ? " unread" : "");
     if (op.kind == OpKind::kEltwise) {
       os << " bottoms=" << op.bottoms.size();
@@ -468,6 +521,7 @@ std::string Plan::text() const {
       os << (op.bottoms[j] < ninputs ? " staged-bottom" : " no-bottom-grad");
       break;
     }
+    if (op.no_backward) os << " no-backward";
     os << "\n";
   }
   os << "params " << param_count << " blobs " << blob_count.size() << "\n";

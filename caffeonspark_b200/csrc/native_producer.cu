@@ -3,7 +3,8 @@
 // One fp32 GEMM core serves every convolution and inner product, forward and both backwards: a 64x64x16 shared-memory
 // tile with FFMA and fp32 accumulation, templated on how it gathers its A and B operands and how it stores C.
 // Convolutions are implicit GEMMs (the tile loader gathers im2col, or the transposed-convolution window for the data
-// gradient, on the fly; no column buffer exists).  No TF32, no atomics: every output element is one thread's sum over
+// gradient, on the fly; no column buffer exists).  A Deconvolution runs as the convolution from its top to its bottom,
+// on the same three instantiations.  No TF32, no atomics: every output element is one thread's sum over
 // k in increasing order, and weight gradients reduce over N*OH*OW in fixed chunks (split_chunk) whose partials a
 // second kernel adds in chunk order.  Bias gradients are fixed-shape block reductions.  So a forward/backward is bitwise
 // reproducible run to run.
@@ -296,9 +297,11 @@ __global__ void relu_backward_kernel(const float* x, const float* dy, float* dx,
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
     dx[i] = x[i] > 0.f ? dy[i] : __fmul_rn(dy[i], slope);
 }
+__device__ __forceinline__ float sigmoid(float x) {  // sigmoid_layer.cu
+  return __fadd_rn(__fmul_rn(0.5f, tanhf(__fmul_rn(0.5f, x))), 0.5f);
+}
 __global__ void sigmoid_forward_kernel(const float* x, float* y, int n) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
-    y[i] = __fadd_rn(__fmul_rn(0.5f, tanhf(__fmul_rn(0.5f, x[i]))), 0.5f);  // sigmoid_layer.cu
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) y[i] = sigmoid(x[i]);
 }
 __global__ void sigmoid_backward_kernel(const float* y, const float* dy, float* dx, int n) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -436,6 +439,36 @@ __global__ void __launch_bounds__(kThreads) euclidean_loss_kernel(const float* a
     *loss = __fmul_rn(loss_weight, __fdiv_rn(__fdiv_rn(part, static_cast<float>(num)), 2.f));
 }
 
+// ------------------------------------------------------------------ SigmoidCrossEntropyLoss
+// (sigmoid_cross_entropy_loss_layer.cpp) Element i of the `count` scores x and targets t costs -(x * (t - [x >= 0]) -
+// log(1 + exp(x - 2 * x * [x >= 0]))), Caffe's stable form, each operation rounded once in float.  Each block sums its
+// threads' elements (each thread in index order, then a fixed tree) into partial[blockIdx.x]; the grid is grid_for(count),
+// so the partials depend on the shape alone.  dx = (sigmoid(x) - t) * (loss_weight / num), one rounding each, with the
+// Sigmoid op's sigmoid; null when the scores want no gradient.  A NaN or infinite x or t reaches the loss, as in Caffe.
+__global__ void __launch_bounds__(kThreads) sigmoid_xent_loss_kernel(const float* x, const float* t, float* dx,
+                                                                     float* partial, int count, int num,
+                                                                     float loss_weight) {
+  __shared__ float sh[kThreads];
+  const float scale = __fdiv_rn(loss_weight, static_cast<float>(num));
+  float part = 0.f;
+  for (int i = blockIdx.x * kThreads + threadIdx.x; i < count; i += gridDim.x * kThreads) {
+    const float v = x[i], target = t[i];
+    const float pos = v >= 0.f ? 1.f : 0.f;
+    const float e = logf(__fadd_rn(1.f, expf(__fsub_rn(v, __fmul_rn(__fmul_rn(2.f, v), pos)))));
+    part = __fsub_rn(part, __fsub_rn(__fmul_rn(v, __fsub_rn(target, pos)), e));
+    if (dx) dx[i] = __fmul_rn(__fsub_rn(sigmoid(v), target), scale);
+  }
+  part = block_sum(part, sh);
+  if (threadIdx.x == 0) partial[blockIdx.x] = part;
+}
+// *loss = loss_weight * (sum / num), the partials added in block order
+__global__ void sigmoid_xent_loss_total_kernel(const float* partial, int blocks, int num, float loss_weight,
+                                               float* loss) {
+  float sum = 0.f;
+  for (int b = 0; b < blocks; ++b) sum = __fadd_rn(sum, partial[b]);
+  *loss = __fmul_rn(loss_weight, __fdiv_rn(sum, static_cast<float>(num)));
+}
+
 // ------------------------------------------------------------------ Split, Eltwise (split_layer.cpp, eltwise_layer.cpp)
 // dst = a + b: the Split backward's first two read tops (later ones go through accumulate_kernel, in top order)
 __global__ void add_kernel(const float* a, const float* b, float* dst, int n) {
@@ -521,6 +554,12 @@ __global__ void gaussian_fill_kernel(float* p, const float* u2, int n, float mea
   }
 }
 
+// GaussianFiller's sparse mask: p[i] stays with probability prob (u3 in [-1, 1): kept when (u3 + 1) / 2 < prob), else 0
+__global__ void sparse_mask_kernel(float* p, const float* u3, int n, float prob) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    if (!((u3[i] + 1.f) * 0.5f < prob)) p[i] = 0.f;
+}
+
 int grid_for(int64_t n) {
   const int64_t g = (n + kThreads - 1) / kThreads;
   return static_cast<int>(g < 1 ? 1 : (g > kTargetSms * 16 ? kTargetSms * 16 : g));
@@ -529,8 +568,19 @@ int grid_for(int64_t n) {
 struct ConvDims {
   int N, Cin, H, W, Cout, OH, OW;
 };
+// A Deconvolution's dims are those of the convolution from its top to its bottom (the same weight blob, [Cin, Cout,
+// KH, KW] of the deconvolution): its forward is that convolution's data gradient, its data gradient that
+// convolution's forward, and its weight gradient that convolution's with the bottom as dy.
 ConvDims conv_dims(const Op& op) {
   ConvDims d;
+  if (op.kind == OpKind::kDeconv) {
+    d.N = static_cast<int>(op.in_shape[0]);
+    d.Cin = static_cast<int>(op.out_shape[1]), d.H = static_cast<int>(op.out_shape[2]);
+    d.W = static_cast<int>(op.out_shape[3]);
+    d.Cout = static_cast<int>(op.in_shape[1]), d.OH = static_cast<int>(op.in_shape[2]);
+    d.OW = static_cast<int>(op.in_shape[3]);
+    return d;
+  }
   d.N = static_cast<int>(op.in_shape[0]), d.Cin = static_cast<int>(op.in_shape[1]);
   d.H = static_cast<int>(op.in_shape[2]), d.W = static_cast<int>(op.in_shape[3]);
   d.Cout = static_cast<int>(op.w_count / (static_cast<int64_t>(d.Cin) * op.kh * op.kw));
@@ -563,26 +613,52 @@ int64_t slice_inner(const Op& op) {
 int64_t slice_span(const Op& op, const std::vector<int64_t>& shape) { return shape[op.slice_axis] * slice_inner(op); }
 int ip_k(const Op& op) { return static_cast<int>(op.w_count / (op.w_count > 0 ? op.out_shape[1] : 1)); }
 
-// conv weight / bias gradients and the data gradient, from dy = the conv output's gradient
-cudaError_t conv_backward(const Op& op, const float* x, const float* dy, float* dx, const float* w, float* diff,
-                          float* ws, bool bias_grad, cudaStream_t s) {
-  const ConvDims d = conv_dims(op);
+// The three GEMMs of a convolution of dims d: y = W * im2col(x) (+ bias); dx = W^T * dy gathered back to the input
+// (+ bias); dst += dW = dy * im2col(x)^T, split over N * OH * OW in fixed chunks added in chunk order.
+cudaError_t conv_forward(const Op& op, const ConvDims& d, const float* x, const float* w, const float* bias, float* y,
+                         cudaStream_t s) {
+  const int K = d.Cin * op.kh * op.kw;
+  return gemm(DenseRM{w, K}, Im2col{x, geom(d, op)}, StoreNCHW{y, bias, d.Cout, d.OH * d.OW}, d.Cout,
+              d.N * d.OH * d.OW, K, K, s);
+}
+cudaError_t conv_data_grad(const Op& op, const ConvDims& d, const float* dy, const float* w, const float* bias, float* dx,
+                           cudaStream_t s) {
+  const int KD = d.Cout * op.kh * op.kw;
+  return gemm(WeightT{w, d.Cin, op.kh * op.kw},
+              Col2imGather{dy, d.Cout, d.H, d.W, op.kh, op.kw, op.sh, op.sw, op.ph, op.pw, d.OH, d.OW},
+              StoreNCHW{dx, bias, d.Cin, d.H * d.W}, d.Cin, d.N * d.H * d.W, KD, KD, s);
+}
+cudaError_t conv_weight_grad(const Op& op, const ConvDims& d, const float* x, const float* dy, float* ws, float* dst,
+                             cudaStream_t s) {
   const int K = d.N * d.OH * d.OW, KW = d.Cin * op.kh * op.kw;
   cudaError_t e = gemm(ChanMajor{dy, d.Cout, d.OH * d.OW}, Transposed<Im2col>{Im2col{x, geom(d, op)}},
                        StorePartial{ws, d.Cout, KW}, d.Cout, KW, K, split_chunk(K), s);
   if (e != cudaSuccess) return e;
-  reduce_partials_kernel<<<grid_for(op.w_count), kThreads, 0, s>>>(ws, splits_of(K), static_cast<int>(op.w_count),
-                                                                     diff + op.w_off);
-  if (bias_grad) bias_grad_kernel<<<d.Cout, kThreads, 0, s>>>(dy, d.N, d.Cout, d.OH * d.OW, diff + op.b_off);
-  if (dx) {
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    const int KD = d.Cout * op.kh * op.kw;
-    return gemm(WeightT{w, d.Cin, op.kh * op.kw},
-                Col2imGather{dy, d.Cout, d.H, d.W, op.kh, op.kw, op.sh, op.sw, op.ph, op.pw, d.OH, d.OW},
-                StoreNCHW{dx, nullptr, d.Cin, d.H * d.W}, d.Cin, d.N * d.H * d.W, KD, KD, s);
-  }
+  reduce_partials_kernel<<<grid_for(op.w_count), kThreads, 0, s>>>(ws, splits_of(K), static_cast<int>(op.w_count), dst);
   return cudaGetLastError();
+}
+
+// conv weight / bias gradients and the data gradient, from dy = the conv output's gradient
+cudaError_t conv_backward(const Op& op, const float* x, const float* dy, float* dx, const float* w, float* diff,
+                          float* ws, bool bias_grad, cudaStream_t s) {
+  const ConvDims d = conv_dims(op);
+  cudaError_t e = conv_weight_grad(op, d, x, dy, ws, diff + op.w_off, s);
+  if (e != cudaSuccess) return e;
+  if (bias_grad) bias_grad_kernel<<<d.Cout, kThreads, 0, s>>>(dy, d.N, d.Cout, d.OH * d.OW, diff + op.b_off);
+  if ((e = cudaGetLastError()) != cudaSuccess || !dx) return e;
+  return conv_data_grad(op, d, dy, w, nullptr, dx, s);
+}
+
+// Deconvolution (deconv_layer.cpp) from dy = its top's gradient: the weight gradient of the convolution from top to
+// bottom with the bottom x as that convolution's dy, the bias gradient over dy, and dx = that convolution's forward of dy
+cudaError_t deconv_backward(const Op& op, const float* x, const float* dy, float* dx, const float* w, float* diff,
+                            float* ws, cudaStream_t s) {
+  const ConvDims d = conv_dims(op);
+  cudaError_t e = conv_weight_grad(op, d, dy, x, ws, diff + op.w_off, s);
+  if (e != cudaSuccess) return e;
+  if (op.b_off >= 0) bias_grad_kernel<<<d.Cin, kThreads, 0, s>>>(dy, d.N, d.Cin, d.H * d.W, diff + op.b_off);
+  if ((e = cudaGetLastError()) != cudaSuccess || !dx) return e;
+  return conv_forward(op, d, dy, w, nullptr, dx, s);
 }
 
 }  // namespace
@@ -669,7 +745,7 @@ bool NativeProducer::allocate(std::string* err) {
   for (size_t i = 0; i < plan_.ops.size(); ++i) {
     const Op& op = plan_.ops[i];
     const int64_t out = plan_.tensor_count[op.out];
-    if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool) {
+    if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kDeconv) {
       const ConvDims d = conv_dims(op);
       const size_t K = static_cast<size_t>(d.N) * d.OH * d.OW;
       ws = std::max(ws, static_cast<size_t>(splits_of(static_cast<int>(K))) * op.w_count);
@@ -690,6 +766,8 @@ bool NativeProducer::allocate(std::string* err) {
       bn_dims(op, &n, &c, &hw);
       if (!alloc(2 * static_cast<size_t>(c) * sizeof(float), &op_aux_[i])) return false;
       ws = std::max(ws, bn_workspace_floats(n, c));
+    } else if (op.kind == OpKind::kSigmoidCrossEntropyLoss) {
+      ws = std::max(ws, static_cast<size_t>(grid_for(plan_.tensor_count[op.bottoms[0]])));  // the per-block partials
     }
   }
   if ((e = cudaEventCreateWithFlags(&done_, cudaEventDisableTiming)) != cudaSuccess) {
@@ -740,6 +818,13 @@ bool NativeProducer::fill(uint64_t seed, cudaStream_t s, std::string* err) {
       e = launch_fill(p, n, seed, k, 1.f, s);
       if (e == cudaSuccess) e = launch_fill(tmp, n, seed, k + (uint64_t(1) << 32), 1.f, s);
       if (e == cudaSuccess) gaussian_fill_kernel<<<grid_for(n), kThreads, 0, s>>>(p, tmp, n, mean, sd);
+      // filler.hpp: sparse >= 0 keeps each weight with probability sparse / num_outputs (shape(0)), drawn under stream
+      // index + 2^33
+      if (e == cudaSuccess && f.type == "gaussian" && f.sparse >= 0) {
+        const float prob = static_cast<float>(f.sparse) / static_cast<float>(sh.empty() ? 1 : sh[0]);
+        e = launch_fill(tmp, n, seed, k + (uint64_t(2) << 32), 1.f, s);
+        if (e == cudaSuccess) sparse_mask_kernel<<<grid_for(n), kThreads, 0, s>>>(p, tmp, n, prob);
+      }
     }
     if (e == cudaSuccess) e = cudaGetLastError();
   }
@@ -785,12 +870,10 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
     case OpKind::kConv:
     case OpKind::kConvBiasReluMaxPool: {
       const ConvDims d = conv_dims(op);
-      const int K = d.Cin * op.kh * op.kw;
       const bool fused = op.kind == OpKind::kConvBiasReluMaxPool;
       const float* bias = (!fused && op.b_off >= 0) ? data_ + op.b_off : nullptr;
       float* z = fused ? op_z_[i] : y;
-      cudaError_t e = gemm(DenseRM{data_ + op.w_off, K}, Im2col{x, geom(d, op)}, StoreNCHW{z, bias, d.Cout, d.OH * d.OW},
-                           d.Cout, d.N * d.OH * d.OW, K, K, s);
+      cudaError_t e = conv_forward(op, d, x, data_ + op.w_off, bias, z, s);
       if (e != cudaSuccess || !fused) return e;
       return bias_relu_maxpool_forward(z, data_ + op.b_off, y, static_cast<uint8_t*>(op_aux_[i]), d.N, d.Cout, d.OH,
                                        d.OW, op.pool_kernel, op.pool_stride, static_cast<int>(op.out_shape[2]),
@@ -831,7 +914,10 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
                                                            op.slice_begin * slice_inner(op), true);
       return cudaGetLastError();
     }
+    case OpKind::kDeconv:  // the data gradient of the convolution from top to bottom, with the bias in its store
+      return conv_data_grad(op, conv_dims(op), x, data_ + op.w_off, op.b_off >= 0 ? data_ + op.b_off : nullptr, y, s);
     case OpKind::kSplit:  // no copy: the top reads the bottom's memory
+    case OpKind::kFlatten:
       act_[op.out] = act_[op.bottoms[0]];
       return cudaSuccess;
     case OpKind::kEltwise: {
@@ -883,6 +969,15 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
                                                    static_cast<int>(plan_.tensor_count[op.bottoms[0]]),
                                                    static_cast<int>(op.in_shape[0]), op.loss_weight);
       return cudaGetLastError();
+    case OpKind::kSigmoidCrossEntropyLoss: {
+      const int count = static_cast<int>(plan_.tensor_count[op.bottoms[0]]), num = static_cast<int>(op.in_shape[0]);
+      const int blocks = grid_for(count);
+      sigmoid_xent_loss_kernel<<<blocks, kThreads, 0, s>>>(x, act_[op.bottoms[1]],
+                                                           op.bottom_grad[0] ? grad_[op.bottoms[0]] : nullptr,
+                                                           workspace_, count, num, op.loss_weight);
+      sigmoid_xent_loss_total_kernel<<<1, 1, 0, s>>>(workspace_, blocks, num, op.loss_weight, loss_dev);
+      return cudaGetLastError();
+    }
     default:
       return cudaErrorInvalidValue;
   }
@@ -893,9 +988,12 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
   const float* dy = grad_[op.out];
   float* dx = op.bottom_grad[0] ? grad_[op.bottoms[0]] : nullptr;
   const int nin = static_cast<int>(plan_.tensor_count[op.bottoms[0]]);
+  if (op.no_backward) return cudaSuccess;  // no gradient reaches the top
   switch (op.kind) {
     case OpKind::kConv:
       return conv_backward(op, x, dy, dx, data_ + op.w_off, diff_, workspace_, op.b_off >= 0, s);
+    case OpKind::kDeconv:
+      return deconv_backward(op, x, dy, dx, data_ + op.w_off, diff_, workspace_, s);
     case OpKind::kConvBiasReluMaxPool: {
       const ConvDims d = conv_dims(op);
       float* partials = workspace_;
@@ -1011,6 +1109,8 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
     case OpKind::kSoftmaxLoss:  // the loss kernels wrote their bottoms' gradients in the forward pass
     case OpKind::kContrastiveLoss:
     case OpKind::kEuclideanLoss:
+    case OpKind::kSigmoidCrossEntropyLoss:
+    case OpKind::kFlatten:  // the top's gradient is the bottom's memory
       return cudaSuccess;
     default:
       return cudaErrorInvalidValue;

@@ -1,10 +1,13 @@
 // native_producer.hpp -- the built-in gradient producer (Net::ForwardBackward for the TRAIN phase of the LeNet,
-// CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, least-squares regression nets and
-// residual nets built of Split, Eltwise and Scale; DESIGN.md section 14).
+// CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, least-squares regression nets,
+// residual nets built of Split, Eltwise and Scale, and autoencoders built of Flatten, Deconvolution and
+// SigmoidCrossEntropyLoss; DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
-// of every learnable blob, or refuses the net naming the first layer it cannot run.  NativeProducer holds the device
+// of every learnable blob, or refuses the net naming the first layer it cannot run.  Only the ops under the loss run a
+// backward (Caffe's layer_need_backward): an op whose top no gradient reaches runs its forward alone.  A loss layer
+// with loss_weight 0 does no TRAIN work at all.  NativeProducer holds the device
 // buffers of one plan on one device and enqueues forward + backward (native_producer.cu).
 #ifndef COS_NATIVE_PRODUCER_HPP_
 #define COS_NATIVE_PRODUCER_HPP_
@@ -22,7 +25,7 @@ namespace cosb {
 
 enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
-  kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale,
+  kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale, kDeconv, kFlatten, kSigmoidCrossEntropyLoss,
   kCount  // the number of kinds (Plan::text names each)
 };
 
@@ -36,21 +39,25 @@ struct Op {
   // SoftmaxWithLoss writes its bottom's gradient whatever the flag says.
   std::vector<int> bottoms;
   std::vector<bool> bottom_grad;
-  // the label-like bottom (SoftmaxWithLoss's label, ContrastiveLoss's sim), or -1: read, never differentiated, and not
-  // counted as its blob's reader
+  // the label-like bottom (SoftmaxWithLoss's label, ContrastiveLoss's sim, SigmoidCrossEntropyLoss's target), or -1:
+  // read, never differentiated, and not counted as its blob's reader
   int label_bottom = -1;
+  // no gradient reaches the top (it is read by no layer under the loss, or only as a label): the op runs its forward
+  // and no backward.  Never set on a Split op (such a top is split_unread) nor a Slice op (it still writes its range of
+  // the bottom's gradient).
+  bool no_backward = false;
   int out = -1;                        // tensor id of the top
   std::vector<int64_t> in_shape, out_shape;  // in_shape: bottoms[0]'s
   bool in_place = false;               // ReLU / Sigmoid with top == bottom: out shares bottoms[0]'s storage (never a
                                        // staged input's: those are not written)
-  // Convolution, Pooling, the fused block's convolution
+  // Convolution, Deconvolution, Pooling, the fused block's convolution
   int kh = 0, kw = 0, sh = 1, sw = 1, ph = 0, pw = 0;
   bool max_pool = true;
   int pool_kernel = 0, pool_stride = 0;  // the fused block's MAX pool (square, pad 0)
   int64_t w_off = -1, w_count = 0, b_off = -1, b_count = 0;  // flat offsets into data_ / diff_
   std::vector<int> shares;             // learnable blobs this op uses as a sharer of a named param (owned elsewhere)
   float slope = 0.f;                   // ReLU negative_slope
-  float loss_weight = 1.f;             // SoftmaxWithLoss, ContrastiveLoss, EuclideanLoss
+  float loss_weight = 1.f;             // SoftmaxWithLoss, ContrastiveLoss, EuclideanLoss, SigmoidCrossEntropyLoss
   // SoftmaxWithLoss (softmax_loss_layer.cpp Reshape): the class axis and its C classes; rows = count(0, axis) *
   // inner, one label each, with inner = count(axis + 1)
   int softmax_axis = 1;
@@ -82,8 +89,9 @@ struct Plan {
   std::vector<Op> ops;
   std::vector<int64_t> tensor_count;   // elements per tensor id
   std::vector<int> storage;            // tensor id -> tensor id that owns its memory (itself unless in place)
-  // per tensor id: its activation is another tensor's memory, set when the forward reaches it (a Split top reads its
-  // bottom's, as Caffe's ShareData); its gradient is still its own
+  // per tensor id: its activation is another tensor's memory, set when the forward reaches it (a Split or Flatten top
+  // reads its bottom's, as Caffe's ShareData).  A Split top's gradient is still its own; a Flatten top's is its bottom's
+  // (storage, as Caffe's ShareDiff) unless the bottom is a staged input.
   std::vector<bool> data_alias;
   int ninputs = 0;                     // tensors 0 .. ninputs-1 are the staged inputs, in data-layer top order
   std::vector<std::string> input_names;
@@ -134,7 +142,8 @@ class NativeProducer {
                                           // BN save
   std::vector<float*> op_z_, op_dz_;      // fused block: conv output without bias and its gradient
   cudaEvent_t done_ = nullptr;            // recorded at the end of every call: the destructor waits for it
-  float* workspace_ = nullptr;            // split-K partials, bias partials, BatchNorm scratch (ops run in order)
+  float* workspace_ = nullptr;            // split-K partials, bias partials, BatchNorm scratch, the sigmoid
+                                          // cross-entropy's per-block partials (ops run in order)
   size_t workspace_floats_ = 0;
   std::vector<void*> allocations_;
 };

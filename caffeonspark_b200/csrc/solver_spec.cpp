@@ -287,6 +287,7 @@ FillerSpec filler(const Node* f) {
   s.mean = static_cast<float>(f->num("mean", 0.0));
   s.std = static_cast<float>(f->num("std", 1.0));
   s.variance_norm = f->str("variance_norm", "FAN_IN");
+  s.sparse = f->integer("sparse", -1);
   return s;
 }
 
@@ -573,6 +574,10 @@ bool flatten(Layer& L, std::vector<Shape>*) {  // flatten_layer.cpp with its def
   Shape in;
   int64_t axis;  // CanonicalAxisIndex(1) refuses a 0-axis bottom; a 1-axis one, which Caffe refuses too, gives N x 1
   if (!L.bottom(0, &in) || (in.empty() && !canonical_axis(L, 1, 0, &axis))) return false;
+  if (const Node* p = L.node.first("flatten_param")) {  // recorded for the engine, which runs the default alone
+    L.rec.flatten_axis = p->integer("axis", 1);
+    L.rec.flatten_end_axis = p->integer("end_axis", -1);
+  }
   L.set_top(0, {in[0], shape_count(in, 1)});
   return true;
 }

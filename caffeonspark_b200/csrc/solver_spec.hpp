@@ -21,6 +21,7 @@ struct FillerSpec {
   std::string type = "constant";
   float value = 0.f, min = 0.f, max = 1.f, mean = 0.f, std = 1.f;
   std::string variance_norm = "FAN_IN";
+  int64_t sparse = -1;  // gaussian: keep each value with probability sparse / shape(0), as filler.hpp (-1: all)
 };
 
 // One TRAIN-phase layer as the layout parser saw it: its blobs' shapes (from the same shape inference that derives
@@ -61,6 +62,8 @@ struct NetLayer {
   std::string eltwise_op = "SUM";
   std::vector<float> coeffs;
   bool stable_prod_grad = true;
+  // Flatten (caffe.proto FlattenParameter) as written: flatten_axis and flatten_end_axis, negative counted from the end
+  int64_t flatten_axis = 1, flatten_end_axis = -1;
   FillerSpec weight_filler, bias_filler;
 };
 

@@ -417,3 +417,44 @@ def resnet20_module():
             return self.fc10(y.mean(dim=(2, 3)))
 
     return ResNet20()
+
+
+# caffe-public/examples/mnist/mnist_autoencoder.prototxt (tests/golden/configs/mnist_autoencoder_train_test.prototxt):
+# InnerProducts 784-1000-500-250-30-250-500-1000-784 with a Sigmoid after each but the code layer (encode4) and the
+# output, whose logits go to SigmoidCrossEntropyLoss against the flattened input.  2,837,314 parameters in 16 blobs.
+AUTOENCODER = dict(input=(1, 28, 28), batch=100, widths=(784, 1000, 500, 250, 30, 250, 500, 1000, 784))
+AUTOENCODER_PARAM_COUNT = 2837314
+# tests/golden/configs/mnist_conv_autoencoder_train_test.prototxt: 13,264 parameters in 7 blobs
+CONV_AUTOENCODER = dict(input=(1, 28, 28), batch=100)
+CONV_AUTOENCODER_PARAM_COUNT = 13264
+
+
+def autoencoder_module():
+    """The MNIST autoencoder as one PyTorch module, parameters in learnable_params() order.  forward(x [N, 1, 28, 28])
+    -> logits [N, 784]."""
+    import torch.nn as nn
+    w = AUTOENCODER["widths"]
+    code, mods = w.index(min(w)), [nn.Flatten()]
+    for i in range(1, len(w)):
+        mods.append(nn.Linear(w[i - 1], w[i]))
+        if i not in (code, len(w) - 1):  # no Sigmoid on the code layer (encode4) nor on the logits (decode1)
+            mods.append(nn.Sigmoid())
+    return nn.Sequential(*mods)
+
+
+def conv_autoencoder_module():
+    """The convolutional autoencoder fixture as one PyTorch module (nn.ConvTranspose2d's weight is [Cin, Cout, KH, KW],
+    Caffe's Deconvolution layout).  forward(x [N, 1, 28, 28]) -> logits [N, 1, 28, 28]."""
+    import torch.nn as nn
+    return nn.Sequential(nn.Conv2d(1, 16, 3, stride=2, padding=1), nn.ReLU(),
+                         nn.Conv2d(16, 32, 3, stride=2, padding=1), nn.ReLU(),
+                         nn.ConvTranspose2d(32, 16, 4, stride=2, padding=1), nn.ReLU(),
+                         nn.ConvTranspose2d(16, 1, 4, stride=2, padding=1, bias=False))
+
+
+def sigmoid_cross_entropy_loss(logits, target, loss_weight=1.0):
+    """Caffe's SigmoidCrossEntropyLoss: the summed cross-entropy of sigmoid(logits) against target, over num =
+    logits.shape[0]; its gradient is (sigmoid(logits) - target) * loss_weight / num."""
+    import torch.nn.functional as F
+    t = target.reshape(logits.shape)
+    return loss_weight * F.binary_cross_entropy_with_logits(logits, t, reduction="sum") / logits.shape[0]
