@@ -6,7 +6,8 @@ their weights and end in a ContrastiveLoss, timed against the PyTorch module tha
 ResNet-20 fixture b100, timed against nets.resnet20_module, whose BatchNorms run the same native kernels; the two
 autoencoder fixtures b100 of 1x28x28, Caffe's MNIST autoencoder and the convolutional one with Deconvolutions, each
 scoring its reconstruction against its input with SigmoidCrossEntropyLoss, timed against nets.autoencoder_module and
-nets.conv_autoencoder_module).  For each, one process times the native engine, the PyTorch module with TF32 off and with
+nets.conv_autoencoder_module; the TanH LeNet fixture b64, whose head is Softmax + MultinomialLogisticLoss, and the
+PReLU CIFAR-10-quick fixture b100, timed against nets.lenet_tanh_module and nets.cifar10_quick_prelu_module).  For each, one process times the native engine, the PyTorch module with TF32 off and with
 TF32 on (cuDNN's default, here applied to matmuls too), alternating the three in every round; each sample is CUDA events around `--iters`
 back-to-back forward/backward calls on one stream after `--warmup` untimed ones.  Prints one JSON line per
 workload with median / min / max ms per call and images/s, and the card's name and power limit.
@@ -28,8 +29,9 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full", "mnist_siamese", "cifar10_resnet20",
-             "mnist_autoencoder", "mnist_conv_autoencoder")
-FIXTURES = ("cifar10_resnet20", "mnist_autoencoder", "mnist_conv_autoencoder")  # nets kept under tests/golden/configs
+             "mnist_autoencoder", "mnist_conv_autoencoder", "lenet_tanh", "cifar10_quick_prelu")
+FIXTURES = ("cifar10_resnet20", "mnist_autoencoder", "mnist_conv_autoencoder", "lenet_tanh",
+            "cifar10_quick_prelu")  # nets kept under tests/golden/configs
 FP32_PEAK = 67e12  # H100 SXM data sheet, dense FP32, at up to 700 W
 
 
@@ -59,13 +61,15 @@ def siamese_solver(directory):
 
 
 def fixture_solver(directory, name):
-    """A fixture's solver, pointed at the fixture's net wherever this runs from."""
+    """A fixture's solver and net, the net without a mean_file (the timed batches are staged as they are)."""
     configs = os.path.join(ROOT, "tests", "golden", "configs")
+    net = open(os.path.join(configs, f"{name}_train_test.prototxt")).read()
+    with open(os.path.join(directory, f"{name}_train_test.prototxt"), "w") as f:
+        f.write(net.replace('mean_file: "mean.binaryproto"', ""))
     solver = open(os.path.join(configs, f"{name}_solver.prototxt")).read()
     path = os.path.join(directory, f"{name}_solver.prototxt")
     with open(path, "w") as f:
-        f.write(solver.replace(f'net: "{name}_train_test.prototxt"',
-                               f'net: "{os.path.join(configs, f"{name}_train_test.prototxt")}"'))
+        f.write(solver)
     return path
 
 
@@ -146,7 +150,8 @@ def main():
         net.fill("data", 1, 0, 0.05)
         torch.cuda.synchronize()
         spec = (nets.RESNET20 if resnet else None if siamese else nets.AUTOENCODER if name == "mnist_autoencoder"
-                else nets.CONV_AUTOENCODER if autoencoder else nets.NETS[name])
+                else nets.CONV_AUTOENCODER if autoencoder else nets.LENET_TANH if name == "lenet_tanh"
+                else nets.CIFAR10_QUICK_PRELU if name == "cifar10_quick_prelu" else nets.NETS[name])
         batch = 64 if siamese else spec["batch"]
         rng = np.random.RandomState(0)
         shape = (2, 28, 28) if siamese else spec["input"]
@@ -166,7 +171,9 @@ def main():
 
         module = (nets.siamese_module() if siamese else nets.resnet20_module() if resnet
                   else nets.autoencoder_module() if name == "mnist_autoencoder"
-                  else nets.conv_autoencoder_module() if autoencoder else nets.torch_module(name)).cuda()
+                  else nets.conv_autoencoder_module() if autoencoder else nets.lenet_tanh_module() if name == "lenet_tanh"
+                  else nets.cifar10_quick_prelu_module() if name == "cifar10_quick_prelu"
+                  else nets.torch_module(name)).cuda()
         with torch.no_grad():
             w, off = net.data().clone(), 0
             for p in module.parameters():
@@ -183,6 +190,9 @@ def main():
                 nets.sigmoid_cross_entropy_loss(module(x), x).backward()
                 return
             out = module(x)
+            if name == "lenet_tanh":
+                nets.multinomial_logistic_loss(out, y).backward()
+                return
             F.cross_entropy(out, ylong).backward()
 
         default_tf32 = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)

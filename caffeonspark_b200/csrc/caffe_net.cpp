@@ -449,6 +449,14 @@ bool CaffeNet::check_status(std::string* err) {
            "loss and no gradient (status 500)";
     return false;
   }
+  if (s == kStatusBadMultinomialLabel || s == kStatusBadHingeLabel) {  // native_producer.cu mll / hinge loss kernels
+    os << (s == kStatusBadHingeLabel ? "HingeLoss" : "MultinomialLogisticLoss")
+       << ": a label outside [0, count / num) reached the native producer; its row added no loss and a zero gradient "
+          "(status "
+       << s << ")";
+    *err = os.str();
+    return false;
+  }
   if (s == 300) {  // fused_sync_sgd_tma.cu: an mbarrier never completed (a bulk copy was lost or a peer died mid-tile)
     os << "device-side TMA pipeline timed out after " << opt_timeout_ms_
        << " ms waiting for a bulk copy to complete (status 300)";

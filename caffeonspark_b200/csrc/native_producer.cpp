@@ -117,14 +117,147 @@ const LayerType kLayerTypes[] = {
     {"ContrastiveLoss", OpKind::kContrastiveLoss, 3, false, 2, "sim", true},  // a, b, sim
     {"EuclideanLoss", OpKind::kEuclideanLoss, 2, false, -1, nullptr, true},
     {"SigmoidCrossEntropyLoss", OpKind::kSigmoidCrossEntropyLoss, 2, false, 1, "target", true},
+    // the other neuron layers, Softmax and the classification losses; none shares memory with its bottom
+    {"TanH", OpKind::kTanH},
+    {"ELU", OpKind::kELU},
+    {"AbsVal", OpKind::kAbsVal},
+    {"BNLL", OpKind::kBNLL},
+    {"Power", OpKind::kPower},
+    {"Exp", OpKind::kExp},
+    {"Log", OpKind::kLog},
+    {"Threshold", OpKind::kThreshold},  // forward only: refused where a gradient would have to pass it
+    {"PReLU", OpKind::kPReLU},
+    {"Softmax", OpKind::kSoftmax},
+    {"MultinomialLogisticLoss", OpKind::kMultinomialLogisticLoss, 2, false, 1, "label", true},
+    {"HingeLoss", OpKind::kHingeLoss, 2, false, 1, "label", true},
 };
 
 // Plan::text's name of each OpKind
 const char* const kKindNames[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling", "InnerProduct", "ReLU", "Sigmoid",
                                   "BatchNorm", "SoftmaxWithLoss", "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss",
                                   "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale", "Deconvolution", "Flatten",
-                                  "SigmoidCrossEntropyLoss"};
+                                  "SigmoidCrossEntropyLoss", "TanH", "ELU", "AbsVal", "BNLL", "Power", "Exp", "Log",
+                                  "Threshold", "PReLU", "Softmax", "MultinomialLogisticLoss", "HingeLoss"};
 static_assert(std::size(kKindNames) == static_cast<size_t>(OpKind::kCount), "one name per OpKind");
+
+// LossLayer::Reshape's check, then multinomial_logistic_loss_layer.cpp's: the label holds one value per item, with
+// Blob::channels(), height() and width() all 1 (mll only)
+bool label_shapes_ok(const NetLayer& L, bool mll, std::string* err) {
+  const std::vector<int64_t>& a = L.bottom_shapes[0];
+  const std::vector<int64_t>& b = L.bottom_shapes[1];
+  if (a.empty() || b.empty() || a[0] != b[0]) {
+    *err = why(L, "The data and label should have the same number.");
+    return false;
+  }
+  static const char* legacy[] = {"channels", "height", "width"};
+  for (size_t k = 1; mll && k < 4; ++k) {
+    const int64_t v = k < b.size() ? b[k] : 1;  // Blob::LegacyShape
+    if (v != 1) {
+      *err = why(L, std::string("Check failed: bottom[1]->") + legacy[k - 1] + "() == 1 (" + std::to_string(v) +
+                        " vs. 1)");
+      return false;
+    }
+  }
+  return true;
+}
+
+std::string float_text(float v) {
+  std::ostringstream os;
+  os << v;
+  return os.str();
+}
+
+// The neuron ops, Softmax and the two classification losses: their parameters as Caffe's LayerSetUp derives them (in
+// float), and its refusals.  None shares memory with its bottom, in place or not.  True for every other kind.
+bool neuron_op(const NetLayer& L, Op* op, Plan* P, std::string* err) {
+  switch (op->kind) {
+    case OpKind::kELU:
+      op->alpha = L.elu_alpha;
+      return true;
+    case OpKind::kAbsVal:
+      if (L.tops[0] == L.bottoms[0]) {
+        *err = why(L, "AbsVal Layer does not allow in-place computation.");
+        return false;
+      }
+      return true;
+    case OpKind::kPower:
+      op->power = L.power, op->scale = L.scale, op->shift = L.shift;
+      return true;
+    case OpKind::kExp:
+    case OpKind::kLog: {  // exp_layer.cpp, log_layer.cpp
+      op->base = L.base, op->scale = L.scale, op->shift = L.shift;
+      if (L.base != -1.f && !(L.base > 0.f)) {
+        *err = why(L, "base must be strictly positive.");
+        return false;
+      }
+      const float log_base = L.base == -1.f ? 1.f : std::log(L.base);
+      if (!std::isfinite(log_base)) {
+        *err = why(L, "Inf result: log(base) = log(" + float_text(L.base) + ") = " + float_text(log_base));
+        return false;
+      }
+      if (op->kind == OpKind::kExp) {
+        op->inner_scale = log_base * L.scale;
+        op->outer_scale = L.shift == 0.f ? 1.f : L.base != -1.f ? std::pow(L.base, L.shift) : std::exp(L.shift);
+        return true;
+      }
+      op->base_scale = 1.f / log_base;
+      if (!std::isfinite(op->base_scale)) {
+        *err = why(L, "Inf result: 1/log(base) = 1/log(" + float_text(L.base) + ") = " + float_text(op->base_scale));
+        return false;
+      }
+      op->backward_num_scale = L.scale / log_base;
+      return true;
+    }
+    case OpKind::kThreshold:
+      op->threshold = L.threshold;
+      return true;
+    case OpKind::kPReLU: {  // prelu_layer.cpp: one slope per channel of axis 1, or one for the whole blob
+      if (op->in_shape.size() < 2) {
+        *err = why(L, "Number of axes of bottom blob must be >=2.");
+        return false;
+      }
+      std::string reason;
+      if (!filler_ok(L.weight_filler, &reason)) {
+        *err = why(L, reason);
+        return false;
+      }
+      op->w_off = P->blob_off[L.blobs[0]], op->w_count = P->blob_count[L.blobs[0]];
+      if (!L.shared[0]) P->blob_filler[L.blobs[0]] = L.weight_filler;
+      op->channel_shared = L.channel_shared;
+      op->prelu_channels = op->in_shape[1];
+      if (!L.channel_shared && op->prelu_channels > kMaxPReLUChannels) {  // the slope gradient's gridDim.y
+        *err = why(L, std::to_string(op->prelu_channels) + " channels is more than the " +
+                          std::to_string(kMaxPReLUChannels) + " per-channel slopes the engine supports");
+        return false;
+      }
+      op->prelu_dim = shape_count(op->in_shape, 2);
+      return true;
+    }
+    case OpKind::kSoftmax: {  // softmax_layer.cpp Reshape: CanonicalAxisIndex(softmax_param.axis)
+      const int64_t naxes = static_cast<int64_t>(op->in_shape.size());
+      const int64_t axis = L.softmax_axis < 0 ? L.softmax_axis + naxes : L.softmax_axis;
+      if (axis < 0 || axis >= naxes) {
+        *err = why(L, "axis " + std::to_string(L.softmax_axis) + " out of range for " + std::to_string(naxes) +
+                          "-D Blob");
+        return false;
+      }
+      op->softmax_axis = static_cast<int>(axis);
+      op->classes = op->in_shape[axis];
+      op->inner = shape_count(op->in_shape, axis + 1);
+      op->outer = shape_count(std::vector<int64_t>(op->in_shape.begin(), op->in_shape.begin() + axis));
+      return true;
+    }
+    case OpKind::kHingeLoss:
+      if (L.hinge_norm != "L1" && L.hinge_norm != "L2") {
+        *err = why(L, "Unknown Norm");
+        return false;
+      }
+      op->hinge_l2 = L.hinge_norm == "L2";
+      return true;
+    default:
+      return true;
+  }
+}
 
 }  // namespace
 
@@ -239,6 +372,9 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         return false;
       if (row->kind == OpKind::kSigmoidCrossEntropyLoss &&
           !loss_shapes_ok(L, "SIGMOID_CROSS_ENTROPY_LOSS layer inputs must have the same count.", err))
+        return false;
+      if ((row->kind == OpKind::kMultinomialLogisticLoss || row->kind == OpKind::kHingeLoss) &&
+          !label_shapes_ok(L, row->kind == OpKind::kMultinomialLogisticLoss, err))
         return false;
     }
     if (op.kind == OpKind::kSlice) {  // one op per top, each copying its range of the bottom (and back, in the backward)
@@ -396,6 +532,8 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.lrn_size = static_cast<int>(L.local_size);
       op.lrn_alpha = L.lrn_alpha;
       op.lrn_beta = L.lrn_beta;
+    } else if (!neuron_op(L, &op, &P, err)) {
+      return false;
     } else if (op.kind == OpKind::kContrastiveLoss) {  // the parser checked the shapes: a, b N x C (x 1 x 1), sim N values
       op.margin = L.margin;
       op.legacy = L.legacy_version;
@@ -444,6 +582,15 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     }
     for (size_t b = 0; b < op.bottoms.size(); ++b)
       if (static_cast<int>(b) != op.label_bottom) under_loss[op.bottoms[b]] = true;
+  }
+  // threshold_layer.cpp has no backward: a Threshold runs only where Caffe never calls it (its top off the loss, or no
+  // gradient wanted at its bottom), such as one that binarises a staged target
+  for (const Op& op : P.ops) {
+    if (op.kind == OpKind::kThreshold && !op.no_backward && op.bottom_grad[0]) {
+      *err = "layer '" + op.name + "' (Threshold): Not Implemented Yet: Threshold has no backward, and a gradient "
+             "reaches it and is wanted at its bottom (native producer)";
+      return false;
+    }
   }
   // the op of each Split's top 0 sums the gradients of the tops under the loss, in top order
   for (size_t i = 0; i < P.ops.size(); ++i) {
@@ -514,6 +661,16 @@ std::string Plan::text() const {
     }
     if (op.kind == OpKind::kScale)
       os << " outer=" << op.scale_outer << " dim=" << op.scale_dim << " inner=" << op.scale_inner;
+    if (op.kind == OpKind::kELU) os << " alpha=" << op.alpha;
+    if (op.kind == OpKind::kPower) os << " power=" << op.power << " scale=" << op.scale << " shift=" << op.shift;
+    if (op.kind == OpKind::kExp || op.kind == OpKind::kLog)
+      os << " base=" << op.base << " scale=" << op.scale << " shift=" << op.shift;
+    if (op.kind == OpKind::kThreshold) os << " threshold=" << op.threshold;
+    if (op.kind == OpKind::kPReLU && op.channel_shared) os << " channel_shared";
+    if (op.kind == OpKind::kSoftmax) os << " axis=" << op.softmax_axis;
+    if (op.kind == OpKind::kMultinomialLogisticLoss) os << " label=" << op.bottoms[1] << " loss_weight=" << op.loss_weight;
+    if (op.kind == OpKind::kHingeLoss)
+      os << " label=" << op.bottoms[1] << " norm=" << (op.hinge_l2 ? "L2" : "L1") << " loss_weight=" << op.loss_weight;
     if (op.in_place) os << " in-place";
     // the first bottom that gets no data gradient: a staged input, or a blob with no learnable blob before it
     for (size_t j = 0; j < op.bottoms.size(); ++j) {

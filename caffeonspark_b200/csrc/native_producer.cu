@@ -461,7 +461,7 @@ __global__ void __launch_bounds__(kThreads) sigmoid_xent_loss_kernel(const float
   part = block_sum(part, sh);
   if (threadIdx.x == 0) partial[blockIdx.x] = part;
 }
-// *loss = loss_weight * (sum / num), the partials added in block order
+// *loss = loss_weight * (sum / num), the partials added in block order (also HingeLoss's)
 __global__ void sigmoid_xent_loss_total_kernel(const float* partial, int blocks, int num, float loss_weight,
                                                float* loss) {
   float sum = 0.f;
@@ -535,6 +535,266 @@ __global__ void __launch_bounds__(kThreads) scale_grad_kernel(const float* dy, c
   }
   s = block_sum(s, sh);
   if (threadIdx.x == 0) dst[d] = __fadd_rn(dst[d], s);
+}
+
+// ------------------------------------------------------------------ the other neuron layers
+// (tanh_layer.cu, elu_layer.cu, absval_layer.cu, bnll_layer.cu, power_layer.cpp, exp_layer.cpp, log_layer.cpp,
+// threshold_layer.cu): Caffe's formulas, each operation rounded once in float.  x is the bottom's activation, y the
+// top's; the top has storage of its own, so x is the bottom as it was even when the layer is written in place.
+__global__ void tanh_forward_kernel(const float* x, float* y, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) y[i] = tanhf(x[i]);
+}
+__global__ void tanh_backward_kernel(const float* y, const float* dy, float* dx, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float t = y[i];
+    dx[i] = __fmul_rn(dy[i], __fsub_rn(1.f, __fmul_rn(t, t)));
+  }
+}
+__global__ void elu_forward_kernel(const float* x, float* y, int n, float alpha) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = x[i];
+    y[i] = v > 0.f ? v : __fmul_rn(alpha, __fsub_rn(expf(v), 1.f));
+  }
+}
+__global__ void elu_backward_kernel(const float* x, const float* y, const float* dy, float* dx, int n, float alpha) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    dx[i] = x[i] > 0.f ? dy[i] : __fmul_rn(dy[i], __fadd_rn(y[i], alpha));
+}
+__global__ void absval_forward_kernel(const float* x, float* y, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) y[i] = fabsf(x[i]);
+}
+// dx = dy * sign(x), caffe_gpu_sign's sign: 0 for a zero (and a NaN)
+__global__ void absval_backward_kernel(const float* x, const float* dy, float* dx, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = x[i];
+    dx[i] = __fmul_rn(dy[i], static_cast<float>((0.f < v) - (v < 0.f)));
+  }
+}
+constexpr float kBnllThreshold = 50.f;  // bnll_layer.cu kBNLL_THRESHOLD
+__global__ void bnll_forward_kernel(const float* x, float* y, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = x[i];
+    y[i] = v > 0.f ? __fadd_rn(v, logf(__fadd_rn(1.f, expf(-v)))) : logf(__fadd_rn(1.f, expf(v)));
+  }
+}
+__global__ void bnll_backward_kernel(const float* x, const float* dy, float* dx, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float e = expf(fminf(x[i], kBnllThreshold));  // CUDA's min: a NaN x takes the threshold, as in bnll_layer.cu
+    dx[i] = __fdiv_rn(__fmul_rn(dy[i], e), __fadd_rn(e, 1.f));
+  }
+}
+// Power, Exp and Log transform their input as Caffe's scal and add_scalar calls do: a factor of 1 or a shift of 0 is
+// skipped (so a -0 stays -0)
+__device__ __forceinline__ float scale_shift(float v, float scale, float shift) {
+  if (scale != 1.f) v = __fmul_rn(scale, v);
+  if (shift != 0.f) v = __fadd_rn(v, shift);
+  return v;
+}
+// y = (shift + scale * x)^power; `constant` (power * scale == 0) writes power == 0 ? 1 : shift^power everywhere
+__global__ void power_forward_kernel(const float* x, float* y, int n, float power, float scale, float shift,
+                                     bool constant, float value) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (constant) {
+      y[i] = value;
+      continue;
+    }
+    const float v = scale_shift(x[i], scale, shift);
+    y[i] = power != 1.f ? powf(v, power) : v;
+  }
+}
+// power_layer.cpp Backward_cpu's four branches with diff_scale = power * scale: the constant diff_scale (power 1, or
+// diff_scale 0, which is not multiplied by dy); power 2: diff_scale * scale * x (+ diff_scale * shift); shift 0:
+// power * y / x (NaN at x = 0, as in Caffe); else diff_scale * y / (shift + scale * x).  Then times dy.
+__global__ void power_backward_kernel(const float* x, const float* y, const float* dy, float* dx, int n, float power,
+                                      float scale, float shift, float diff_scale, float ds_scale, float ds_shift) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float g;
+    if (diff_scale == 0.f || power == 1.f) {
+      g = diff_scale;
+    } else if (power == 2.f) {
+      g = __fmul_rn(ds_scale, x[i]);
+      if (shift != 0.f) g = __fadd_rn(g, ds_shift);
+    } else if (shift == 0.f) {
+      g = __fmul_rn(__fdiv_rn(y[i], x[i]), power);
+    } else {
+      g = __fdiv_rn(y[i], scale_shift(x[i], scale, shift));
+      if (diff_scale != 1.f) g = __fmul_rn(diff_scale, g);
+    }
+    dx[i] = diff_scale != 0.f ? __fmul_rn(dy[i], g) : g;
+  }
+}
+// y = outer * exp(inner * x), each factor of 1 skipped; dx = inner * (y * dy)
+__global__ void exp_forward_kernel(const float* x, float* y, int n, float inner, float outer) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float v = expf(inner != 1.f ? __fmul_rn(inner, x[i]) : x[i]);
+    y[i] = outer != 1.f ? __fmul_rn(outer, v) : v;
+  }
+}
+__global__ void exp_backward_kernel(const float* y, const float* dy, float* dx, int n, float inner) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float g = __fmul_rn(y[i], dy[i]);
+    dx[i] = inner != 1.f ? __fmul_rn(inner, g) : g;
+  }
+}
+// y = base_scale * log(shift + scale * x); dx = dy * (backward_num_scale * (shift + scale * x)^-1), the power -1 a
+// correctly rounded reciprocal
+__global__ void log_forward_kernel(const float* x, float* y, int n, float scale, float shift, float base_scale) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = logf(scale_shift(x[i], scale, shift));
+    y[i] = base_scale != 1.f ? __fmul_rn(base_scale, v) : v;
+  }
+}
+__global__ void log_backward_kernel(const float* x, const float* dy, float* dx, int n, float scale, float shift,
+                                    float num_scale) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float g = __frcp_rn(scale_shift(x[i], scale, shift));
+    if (num_scale != 1.f) g = __fmul_rn(num_scale, g);
+    dx[i] = __fmul_rn(dy[i], g);
+  }
+}
+__global__ void threshold_forward_kernel(const float* x, float* y, int n, float threshold) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    y[i] = x[i] > threshold ? 1.f : 0.f;
+}
+
+// ------------------------------------------------------------------ PReLU (prelu_layer.cpp)
+// Channel c of element i is (i / dim) % C, or 0 with channel_shared.  y = max(x, 0) + a_c * min(x, 0), with std::max
+// and std::min's rules for zeros and NaN; dx = dy * ((x > 0) + a_c * (x <= 0)).
+__global__ void prelu_forward_kernel(const float* x, const float* slope, float* y, int n, int C, int dim, bool shared) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = x[i], a = __ldg(slope + (shared ? 0 : (i / dim) % C));
+    const float hi = v < 0.f ? 0.f : v, lo = 0.f < v ? 0.f : v;
+    y[i] = __fadd_rn(hi, __fmul_rn(a, lo));
+  }
+}
+__global__ void prelu_backward_kernel(const float* x, const float* slope, const float* dy, float* dx, int n, int C,
+                                      int dim, bool shared) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const float v = x[i], a = __ldg(slope + (shared ? 0 : (i / dim) % C));
+    const float pos = v > 0.f ? 1.f : 0.f, neg = v <= 0.f ? 1.f : 0.f;
+    dx[i] = __fmul_rn(dy[i], __fadd_rn(pos, __fmul_rn(a, neg)));
+  }
+}
+// The slope gradient sums dy * x * (x <= 0) over the M = N * dim elements of each channel (M = count with
+// channel_shared) in fixed chunks of kPreluChunk: block (k, c) sums chunk k of channel c (each thread in index order,
+// then block_sum's tree) into partial[c * chunks + k], and prelu_slope_total_kernel adds the partials in chunk order,
+// then once into the gradient.  The order depends on the shape alone; no atomics.  The grid is (chunks, slopes):
+// build_plan refuses more than kMaxPReLUChannels slopes, gridDim.y's limit.
+constexpr int kPreluChunk = 8192;
+__global__ void __launch_bounds__(kThreads) prelu_slope_partial_kernel(const float* x, const float* dy, float* partial,
+                                                                       int M, int C, int dim, bool shared,
+                                                                       int chunks) {
+  __shared__ float sh[kThreads];
+  const int c = blockIdx.y, k = blockIdx.x;
+  const int end = min(M, (k + 1) * kPreluChunk);
+  float s = 0.f;
+  for (int j = k * kPreluChunk + threadIdx.x; j < end; j += kThreads) {
+    const size_t i = shared ? static_cast<size_t>(j) : ((size_t)(j / dim) * C + c) * dim + j % dim;
+    const float v = x[i];
+    s = __fadd_rn(s, __fmul_rn(__fmul_rn(dy[i], v), v <= 0.f ? 1.f : 0.f));
+  }
+  s = block_sum(s, sh);
+  if (threadIdx.x == 0) partial[(size_t)c * chunks + k] = s;
+}
+__global__ void prelu_slope_total_kernel(const float* partial, int chunks, int slopes, float* dst) {
+  for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < slopes; c += gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int k = 0; k < chunks; ++k) s = __fadd_rn(s, partial[(size_t)c * chunks + k]);
+    dst[c] = __fadd_rn(dst[c], s);
+  }
+}
+
+// ------------------------------------------------------------------ Softmax (softmax_layer.cu)
+// Row r = (o, s) of x[o, c, s] (outer o, class c along the axis, inner s): max over c (from -FLT_MAX, CUDA's max),
+// y = exp(x - max), their sum in c order, y / sum.  One thread per row, looping over the classes: made for
+// classification heads; a wide axis over few rows leaves most of the GPU idle.
+__global__ void softmax_forward_kernel(const float* x, float* y, int rows, int C, int inner) {
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += gridDim.x * blockDim.x) {
+    const size_t base = (size_t)(r / inner) * C * inner + r % inner;
+    float m = -FLT_MAX;
+    for (int c = 0; c < C; ++c) m = fmaxf(x[base + (size_t)c * inner], m);
+    float sum = 0.f;
+    for (int c = 0; c < C; ++c) {
+      const float e = expf(__fsub_rn(x[base + (size_t)c * inner], m));
+      y[base + (size_t)c * inner] = e;
+      sum = __fadd_rn(sum, e);
+    }
+    for (int c = 0; c < C; ++c) y[base + (size_t)c * inner] = __fdiv_rn(y[base + (size_t)c * inner], sum);
+  }
+}
+// dx = (dy - sum over c of dy * y) * y, the dot in c order
+__global__ void softmax_backward_kernel(const float* y, const float* dy, float* dx, int rows, int C, int inner) {
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += gridDim.x * blockDim.x) {
+    const size_t base = (size_t)(r / inner) * C * inner + r % inner;
+    float dot = 0.f;
+    for (int c = 0; c < C; ++c) dot = __fadd_rn(dot, __fmul_rn(dy[base + (size_t)c * inner], y[base + (size_t)c * inner]));
+    for (int c = 0; c < C; ++c) {
+      const size_t i = base + (size_t)c * inner;
+      dx[i] = __fmul_rn(__fsub_rn(dy[i], dot), y[i]);
+    }
+  }
+}
+
+// ------------------------------------------------------------------ MultinomialLogisticLoss
+// (multinomial_logistic_loss_layer.cpp) One block over the num rows of x [num, dim]: p = max(x[r, label_r], 1e-20),
+// the loss sums -log(p) (each thread over its rows in order, then a fixed tree) and *loss = loss_weight * (sum / num).
+// dx (null when not wanted) is (-loss_weight / num) / p at the label and an exact 0 elsewhere, written whole.  A label
+// outside [0, dim) (or NaN) sets *status; its row adds no loss and gets a zero gradient.  Made for classification
+// heads of a few to a few thousand classes.
+constexpr float kLogThreshold = 1e-20f;  // loss_layer.hpp kLOG_THRESHOLD
+__global__ void __launch_bounds__(kThreads) mll_loss_kernel(const float* x, const float* label, float* dx, float* loss,
+                                                            int num, int dim, float loss_weight, int* status) {
+  __shared__ float sh[kThreads];
+  const float scale = __fdiv_rn(-loss_weight, static_cast<float>(num));
+  float part = 0.f;
+  for (int r = threadIdx.x; r < num; r += kThreads) {
+    const float lf = label[r];
+    const bool bad = !(lf >= 0.f && lf < static_cast<float>(dim));
+    if (bad) *reinterpret_cast<volatile int*>(status) = kStatusBadMultinomialLabel;
+    const int l = bad ? -1 : static_cast<int>(lf);
+    float p = 0.f;
+    if (!bad) {
+      p = x[(size_t)r * dim + l];
+      p = p < kLogThreshold ? kLogThreshold : p;  // std::max(p, threshold): a NaN p stays
+      part = __fsub_rn(part, logf(p));
+    }
+    if (dx)
+      for (int j = 0; j < dim; ++j) dx[(size_t)r * dim + j] = j == l ? __fdiv_rn(scale, p) : 0.f;
+  }
+  part = block_sum(part, sh);
+  if (threadIdx.x == 0) *loss = __fmul_rn(loss_weight, __fdiv_rn(part, static_cast<float>(num)));
+}
+
+// ------------------------------------------------------------------ HingeLoss (hinge_loss_layer.cpp)
+// Element (r, j) of x [num, dim]: v = x, negated at j = label_r; h = std::max(0, 1 + v) (a NaN gives 0).  The loss sums
+// h (L1) or h * h (L2): each block over its threads' elements in index order, then a fixed tree, into
+// partial[blockIdx.x] (the grid is grid_for(count)); sigmoid_xent_loss_total_kernel adds the partials in block order.
+// dx (null when not wanted) is g = +-h (negated at the label) times: sign(g) * (loss_weight / num) for L1, with
+// sign(0) = 0; g * (loss_weight * 2 / num) for L2.  A bad label sets *status; its row adds no loss and a zero gradient.
+__global__ void __launch_bounds__(kThreads) hinge_loss_kernel(const float* x, const float* label, float* dx,
+                                                              float* partial, int count, int dim, int num, bool l2,
+                                                              float loss_weight, int* status) {
+  __shared__ float sh[kThreads];
+  const float s1 = __fdiv_rn(loss_weight, static_cast<float>(num));
+  const float s2 = __fdiv_rn(__fmul_rn(loss_weight, 2.f), static_cast<float>(num));
+  float part = 0.f;
+  for (int i = blockIdx.x * kThreads + threadIdx.x; i < count; i += gridDim.x * kThreads) {
+    const float lf = label[i / dim];
+    if (!(lf >= 0.f && lf < static_cast<float>(dim))) {
+      *reinterpret_cast<volatile int*>(status) = kStatusBadHingeLabel;
+      if (dx) dx[i] = 0.f;
+      continue;
+    }
+    const bool at = i % dim == static_cast<int>(lf);
+    const float t = __fadd_rn(1.f, at ? -x[i] : x[i]);
+    const float h = 0.f < t ? t : 0.f;
+    part = __fadd_rn(part, l2 ? __fmul_rn(h, h) : h);
+    if (!dx) continue;
+    const float g = at ? -h : h;
+    dx[i] = l2 ? __fmul_rn(g, s2) : __fmul_rn(static_cast<float>((0.f < g) - (g < 0.f)), s1);
+  }
+  part = block_sum(part, sh);
+  if (threadIdx.x == 0) partial[blockIdx.x] = part;
 }
 
 // ------------------------------------------------------------------ fillers (u: the cos_net_fill value in [-1, 1))
@@ -612,6 +872,12 @@ int64_t slice_inner(const Op& op) {
 }
 int64_t slice_span(const Op& op, const std::vector<int64_t>& shape) { return shape[op.slice_axis] * slice_inner(op); }
 int ip_k(const Op& op) { return static_cast<int>(op.w_count / (op.w_count > 0 ? op.out_shape[1] : 1)); }
+// PReLU: the elements each slope reduces over, the number of slopes, and the chunks of the slope gradient
+int prelu_span(const Op& op) {
+  return static_cast<int>(op.channel_shared ? shape_count(op.in_shape) : op.in_shape[0] * op.prelu_dim);
+}
+int prelu_slopes(const Op& op) { return op.channel_shared ? 1 : static_cast<int>(op.prelu_channels); }
+int prelu_chunks(const Op& op) { return (prelu_span(op) + kPreluChunk - 1) / kPreluChunk; }
 
 // The three GEMMs of a convolution of dims d: y = W * im2col(x) (+ bias); dx = W^T * dy gathered back to the input
 // (+ bias); dst += dW = dy * im2col(x)^T, split over N * OH * OW in fixed chunks added in chunk order.
@@ -766,8 +1032,10 @@ bool NativeProducer::allocate(std::string* err) {
       bn_dims(op, &n, &c, &hw);
       if (!alloc(2 * static_cast<size_t>(c) * sizeof(float), &op_aux_[i])) return false;
       ws = std::max(ws, bn_workspace_floats(n, c));
-    } else if (op.kind == OpKind::kSigmoidCrossEntropyLoss) {
+    } else if (op.kind == OpKind::kSigmoidCrossEntropyLoss || op.kind == OpKind::kHingeLoss) {
       ws = std::max(ws, static_cast<size_t>(grid_for(plan_.tensor_count[op.bottoms[0]])));  // the per-block partials
+    } else if (op.kind == OpKind::kPReLU) {
+      ws = std::max(ws, static_cast<size_t>(prelu_slopes(op)) * prelu_chunks(op));  // the slope gradient's partials
     }
   }
   if ((e = cudaEventCreateWithFlags(&done_, cudaEventDisableTiming)) != cudaSuccess) {
@@ -978,6 +1246,60 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
       sigmoid_xent_loss_total_kernel<<<1, 1, 0, s>>>(workspace_, blocks, num, op.loss_weight, loss_dev);
       return cudaGetLastError();
     }
+    case OpKind::kTanH:
+      tanh_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n);
+      return cudaGetLastError();
+    case OpKind::kELU:
+      elu_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n, op.alpha);
+      return cudaGetLastError();
+    case OpKind::kAbsVal:
+      absval_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n);
+      return cudaGetLastError();
+    case OpKind::kBNLL:
+      bnll_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n);
+      return cudaGetLastError();
+    case OpKind::kPower: {  // power_layer.cpp: the constant is pow(shift, power) in float, on the host
+      const bool constant = op.power * op.scale == 0.f;
+      const float value = op.power == 0.f ? 1.f : std::pow(op.shift, op.power);
+      power_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n, op.power, op.scale, op.shift, constant, value);
+      return cudaGetLastError();
+    }
+    case OpKind::kExp:
+      exp_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n, op.inner_scale, op.outer_scale);
+      return cudaGetLastError();
+    case OpKind::kLog:
+      log_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n, op.scale, op.shift, op.base_scale);
+      return cudaGetLastError();
+    case OpKind::kThreshold:
+      threshold_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n, op.threshold);
+      return cudaGetLastError();
+    case OpKind::kPReLU:
+      prelu_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, data_ + op.w_off, y, n,
+                                                            static_cast<int>(op.prelu_channels),
+                                                            static_cast<int>(op.prelu_dim), op.channel_shared);
+      return cudaGetLastError();
+    case OpKind::kSoftmax: {
+      const int rows = static_cast<int>(op.outer * op.inner);
+      softmax_forward_kernel<<<grid_for(rows), kThreads, 0, s>>>(x, y, rows, static_cast<int>(op.classes),
+                                                                 static_cast<int>(op.inner));
+      return cudaGetLastError();
+    }
+    case OpKind::kMultinomialLogisticLoss: {
+      const int num = static_cast<int>(op.in_shape[0]);
+      mll_loss_kernel<<<1, kThreads, 0, s>>>(x, act_[op.bottoms[1]], op.bottom_grad[0] ? grad_[op.bottoms[0]] : nullptr,
+                                             loss_dev, num, static_cast<int>(plan_.tensor_count[op.bottoms[0]] / num),
+                                             op.loss_weight, status_);
+      return cudaGetLastError();
+    }
+    case OpKind::kHingeLoss: {
+      const int count = static_cast<int>(plan_.tensor_count[op.bottoms[0]]), num = static_cast<int>(op.in_shape[0]);
+      const int blocks = grid_for(count);
+      hinge_loss_kernel<<<blocks, kThreads, 0, s>>>(x, act_[op.bottoms[1]],
+                                                    op.bottom_grad[0] ? grad_[op.bottoms[0]] : nullptr, workspace_,
+                                                    count, count / num, num, op.hinge_l2, op.loss_weight, status_);
+      sigmoid_xent_loss_total_kernel<<<1, 1, 0, s>>>(workspace_, blocks, num, op.loss_weight, loss_dev);
+      return cudaGetLastError();
+    }
     default:
       return cudaErrorInvalidValue;
   }
@@ -1106,10 +1428,58 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
       if (dx) scale_forward_kernel<<<grid_for(nin), kThreads, 0, s>>>(dy, data_ + op.w_off, nullptr, dx, nin, dim, inner);
       return cudaGetLastError();
     }
+    case OpKind::kTanH:
+      if (dx) tanh_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(act_[op.out], dy, dx, nin);
+      return cudaGetLastError();
+    case OpKind::kELU:
+      if (dx) elu_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(x, act_[op.out], dy, dx, nin, op.alpha);
+      return cudaGetLastError();
+    case OpKind::kAbsVal:
+      if (dx) absval_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(x, dy, dx, nin);
+      return cudaGetLastError();
+    case OpKind::kBNLL:
+      if (dx) bnll_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(x, dy, dx, nin);
+      return cudaGetLastError();
+    case OpKind::kPower: {  // the products of diff_scale are float, as Caffe forms them
+      const float ds = op.power * op.scale;
+      if (dx)
+        power_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(x, act_[op.out], dy, dx, nin, op.power, op.scale,
+                                                                 op.shift, ds, ds * op.scale, ds * op.shift);
+      return cudaGetLastError();
+    }
+    case OpKind::kExp:
+      if (dx) exp_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(act_[op.out], dy, dx, nin, op.inner_scale);
+      return cudaGetLastError();
+    case OpKind::kLog:
+      if (dx)
+        log_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(x, dy, dx, nin, op.scale, op.shift,
+                                                               op.backward_num_scale);
+      return cudaGetLastError();
+    case OpKind::kThreshold:  // build_plan refuses a Threshold whose bottom would need a gradient
+      return dx ? cudaErrorInvalidValue : cudaSuccess;
+    case OpKind::kPReLU: {  // the slope gradient first, then the data gradient (prelu_layer.cpp's order)
+      const int C = static_cast<int>(op.prelu_channels), dim = static_cast<int>(op.prelu_dim);
+      const int chunks = prelu_chunks(op), slopes = prelu_slopes(op);
+      prelu_slope_partial_kernel<<<dim3(chunks, slopes), kThreads, 0, s>>>(x, dy, workspace_, prelu_span(op), C, dim,
+                                                                           op.channel_shared, chunks);
+      prelu_slope_total_kernel<<<grid_for(slopes), kThreads, 0, s>>>(workspace_, chunks, slopes, diff_ + op.w_off);
+      if (dx)
+        prelu_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(x, data_ + op.w_off, dy, dx, nin, C, dim,
+                                                                 op.channel_shared);
+      return cudaGetLastError();
+    }
+    case OpKind::kSoftmax:
+      if (dx)
+        softmax_backward_kernel<<<grid_for(op.outer * op.inner), kThreads, 0, s>>>(
+            act_[op.out], dy, dx, static_cast<int>(op.outer * op.inner), static_cast<int>(op.classes),
+            static_cast<int>(op.inner));
+      return cudaGetLastError();
     case OpKind::kSoftmaxLoss:  // the loss kernels wrote their bottoms' gradients in the forward pass
     case OpKind::kContrastiveLoss:
     case OpKind::kEuclideanLoss:
     case OpKind::kSigmoidCrossEntropyLoss:
+    case OpKind::kMultinomialLogisticLoss:
+    case OpKind::kHingeLoss:
     case OpKind::kFlatten:  // the top's gradient is the bottom's memory
       return cudaSuccess;
     default:

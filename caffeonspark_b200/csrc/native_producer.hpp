@@ -26,6 +26,7 @@ namespace cosb {
 enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
   kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale, kDeconv, kFlatten, kSigmoidCrossEntropyLoss,
+  kTanH, kELU, kAbsVal, kBNLL, kPower, kExp, kLog, kThreshold, kPReLU, kSoftmax, kMultinomialLogisticLoss, kHingeLoss,
   kCount  // the number of kinds (Plan::text names each)
 };
 
@@ -83,6 +84,19 @@ struct Op {
   bool stable_prod_grad = true;
   // Scale: y[o, d, i] = x[o, d, i] * s[d] (+ b[d]) over outer o, scale_dim d and inner i; w_off / b_off are s and b
   int64_t scale_outer = 1, scale_dim = 1, scale_inner = 1;
+  // The neuron ops (Caffe's *_layer.cpp LayerSetUp, computed in float as Caffe does): ELU's alpha; Power's power, scale
+  // and shift; Exp's inner_scale = log(base) * scale and outer_scale = base^shift; Log's scale, shift, base_scale =
+  // 1 / log(base) and backward_num_scale = scale / log(base); Threshold's threshold.  base is kept for the plan line.
+  float alpha = 1.f, power = 1.f, scale = 1.f, shift = 0.f, base = -1.f;
+  float inner_scale = 1.f, outer_scale = 1.f, base_scale = 1.f, backward_num_scale = 1.f;
+  float threshold = 0.f;
+  // PReLU: the slope blob is w_off; y[n, c, p] uses slope[channel_shared ? 0 : c] over prelu_channels C and
+  // prelu_dim = count(2) elements per (n, c)
+  bool channel_shared = false;
+  int64_t prelu_channels = 1, prelu_dim = 1;
+  // Softmax: softmax_axis, classes and inner as SoftmaxWithLoss's, outer = count(0, axis)
+  int64_t outer = 1;
+  bool hinge_l2 = false;               // HingeLoss: L2 norm (else L1)
 };
 
 struct Plan {
@@ -110,6 +124,11 @@ bool plan_from_prototxt(const std::string& path, SolverSpec* spec, Plan* plan, s
 
 // Status word value of a label outside [0, classes) (CaffeNet::check_status turns it into an error).
 constexpr int kStatusBadLabel = 500;
+// ... of a MultinomialLogisticLoss or HingeLoss label outside [0, dim) (or NaN): its row adds no loss and gets a zero
+// gradient
+constexpr int kStatusBadMultinomialLabel = 501, kStatusBadHingeLabel = 502;
+// PReLU's slope gradient runs one grid row per slope (gridDim.y), so a per-channel PReLU has at most this many channels
+constexpr int64_t kMaxPReLUChannels = 65535;
 
 class NativeProducer {
  public:

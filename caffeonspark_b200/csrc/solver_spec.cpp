@@ -493,6 +493,35 @@ bool same_shape(Layer& L, std::vector<Shape>*) {  // ReLU, LRN, Dropout, Sigmoid
     if (r.norm_region == "0") r.norm_region = "ACROSS_CHANNELS";  // the enum's numeric form
     if (r.norm_region == "1") r.norm_region = "WITHIN_CHANNEL";
   }
+  // the neuron layers' parameters with caffe.proto's defaults; the engine's plan checks them
+  if (const Node* p = L.node.first("power_param")) {
+    r.power = static_cast<float>(p->num("power", 1.0));
+    r.scale = static_cast<float>(p->num("scale", 1.0));
+    r.shift = static_cast<float>(p->num("shift", 0.0));
+  }
+  const Node* exp_log = r.type == "Exp" ? L.node.first("exp_param") : r.type == "Log" ? L.node.first("log_param") : nullptr;
+  if (exp_log) {
+    r.base = static_cast<float>(exp_log->num("base", -1.0));
+    r.scale = static_cast<float>(exp_log->num("scale", 1.0));
+    r.shift = static_cast<float>(exp_log->num("shift", 0.0));
+  }
+  if (const Node* p = L.node.first("elu_param")) r.elu_alpha = static_cast<float>(p->num("alpha", 1.0));
+  if (const Node* p = L.node.first("threshold_param")) r.threshold = static_cast<float>(p->num("threshold", 0.0));
+  if (const Node* p = L.node.first("softmax_param")) r.softmax_axis = p->integer("axis", 1);
+  return true;
+}
+
+bool prelu(Layer& L, std::vector<Shape>* params) {  // prelu_layer.cpp LayerSetUp: one slope per channel, or a scalar
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  const Node* p = L.node.first("prelu_param");
+  NetLayer& r = L.rec;
+  r.channel_shared = p && p->boolean("channel_shared", false);
+  if (p && p->first("filler")) r.weight_filler = filler(p->first("filler"));
+  else r.weight_filler.value = 0.25f;  // Caffe's default: constant 0.25
+  // Blob::channels() of a bottom with fewer than 2 axes is 1; the engine refuses such a bottom with Caffe's wording
+  params->push_back(r.channel_shared ? Shape{} : Shape{in.size() >= 2 ? in[1] : 1});
+  L.set_tops(in);
   return true;
 }
 
@@ -685,7 +714,15 @@ bool contrastive_loss(Layer& L, std::vector<Shape>*) {  // contrastive_loss_laye
   return true;
 }
 
-bool loss(Layer& L, std::vector<Shape>*) { L.set_tops(Shape{}); return true; }  // and Accuracy: scalar tops
+bool loss(Layer& L, std::vector<Shape>*) {  // and Accuracy: scalar tops
+  if (const Node* p = L.node.first("hinge_loss_param")) {  // caffe.proto HingeLossParameter.Norm: L1 = 1, L2 = 2
+    L.rec.hinge_norm = p->str("norm", "L1");
+    if (L.rec.hinge_norm == "1") L.rec.hinge_norm = "L1";
+    if (L.rec.hinge_norm == "2") L.rec.hinge_norm = "L2";
+  }
+  L.set_tops(Shape{});
+  return true;
+}
 
 bool softmax_loss(Layer& L, std::vector<Shape>* params) {  // softmax_loss_layer.cpp Reshape: the class axis
   Shape in;
@@ -704,7 +741,7 @@ const struct { const char* type; Rule rule; } kRules[] = {
     {"Convolution", convolution}, {"Deconvolution", convolution}, {"Pooling", pooling}, {"InnerProduct", inner_product},
     {"ReLU", same_shape}, {"LRN", same_shape}, {"Dropout", same_shape}, {"Sigmoid", same_shape}, {"TanH", same_shape},
     {"Softmax", same_shape}, {"Power", same_shape}, {"AbsVal", same_shape}, {"BNLL", same_shape}, {"ELU", same_shape},
-    {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape},
+    {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape}, {"PReLU", prelu},
     {"Split", split}, {"Eltwise", eltwise}, {"Scale", scale}, {"Flatten", flatten}, {"Concat", concat},
     {"SoftmaxWithLoss", softmax_loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
     {"HingeLoss", loss}, {"MultinomialLogisticLoss", loss},

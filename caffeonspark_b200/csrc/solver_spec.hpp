@@ -64,6 +64,15 @@ struct NetLayer {
   bool stable_prod_grad = true;
   // Flatten (caffe.proto FlattenParameter) as written: flatten_axis and flatten_end_axis, negative counted from the end
   int64_t flatten_axis = 1, flatten_end_axis = -1;
+  // Power, Exp and Log (caffe.proto PowerParameter, ExpParameter, LogParameter): power is Power's alone, base Exp's and
+  // Log's (-1: e); scale and shift each layer's own
+  float power = 1.f, scale = 1.f, shift = 0.f, base = -1.f;
+  float elu_alpha = 1.f;   // ELUParameter
+  float threshold = 0.f;   // ThresholdParameter
+  // Softmax's softmax_param axis as written (negative counted from the end; the engine's plan checks it)
+  int64_t softmax_axis = 1;
+  bool channel_shared = false;  // PReLUParameter; its filler is weight_filler (constant 0.25 when none is given)
+  std::string hinge_norm = "L1";  // HingeLossParameter: "L1" or "L2"
   FillerSpec weight_filler, bias_filler;
 };
 

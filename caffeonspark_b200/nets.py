@@ -458,3 +458,83 @@ def sigmoid_cross_entropy_loss(logits, target, loss_weight=1.0):
     import torch.nn.functional as F
     t = target.reshape(logits.shape)
     return loss_weight * F.binary_cross_entropy_with_logits(logits, t, reduction="sum") / logits.shape[0]
+
+
+# tests/golden/configs/lenet_tanh_train_test.prototxt: the reference's LeNet with a TanH after pool1 and after pool2,
+# TanH in place of relu1, and ip2 -> Softmax -> MultinomialLogisticLoss as its head.  LeNet's 431,080 parameters.
+LENET_TANH = dict(input=(1, 28, 28), batch=64, classes=10)
+LENET_TANH_PARAM_COUNT = 431080
+# tests/golden/configs/cifar10_quick_prelu_train_test.prototxt: CIFAR-10-quick with a per-channel PReLU for each ReLU
+# and a channel_shared PReLU after ip1: 145,578 + 32 + 32 + 64 + 1 = 145,707 parameters in 14 blobs.
+CIFAR10_QUICK_PRELU = dict(input=(3, 32, 32), batch=100, classes=10)
+CIFAR10_QUICK_PRELU_PARAM_COUNT = 145707
+
+
+def lenet_tanh_module():
+    """The TanH LeNet fixture as one PyTorch module, parameters in learnable_params() order.  forward(x [N, 1, 28, 28])
+    -> class probabilities [N, 10] (the Softmax's top)."""
+    import torch.nn as nn
+    return nn.Sequential(nn.Conv2d(1, 20, 5), nn.MaxPool2d(2, 2, ceil_mode=True), nn.Tanh(),
+                         nn.Conv2d(20, 50, 5), nn.MaxPool2d(2, 2, ceil_mode=True), nn.Tanh(),
+                         nn.Flatten(), nn.Linear(800, 500), nn.Tanh(), nn.Linear(500, 10), nn.Softmax(dim=1))
+
+
+def cifar10_quick_prelu_module():
+    """The PReLU CIFAR-10-quick fixture as one PyTorch module, parameters in learnable_params() order (each PReLU's
+    slopes after the layer before it; the shared slope is one value, Caffe's 0-axis blob).  forward(x [N, 3, 32, 32])
+    -> scores [N, 10]."""
+    import torch.nn as nn
+    return nn.Sequential(nn.Conv2d(3, 32, 5, padding=2), nn.MaxPool2d(3, 2, ceil_mode=True), nn.PReLU(32),
+                         nn.Conv2d(32, 32, 5, padding=2), nn.PReLU(32), nn.AvgPool2d(3, 2, ceil_mode=True),
+                         nn.Conv2d(32, 64, 5, padding=2), nn.PReLU(64), nn.AvgPool2d(3, 2, ceil_mode=True),
+                         nn.Flatten(), nn.Linear(1024, 64), nn.PReLU(1), nn.Linear(64, 10))
+
+
+def multinomial_logistic_loss(prob, label, loss_weight=1.0):
+    """Caffe's MultinomialLogisticLoss (multinomial_logistic_loss_layer.cpp): -loss_weight * sum over the num rows of
+    log(max(prob[label], 1e-20)) / num.  Its gradient is -loss_weight / num / max(prob[label], 1e-20) at the label (the
+    clamp does not stop it, unlike autograd's) and 0 elsewhere."""
+    import torch
+
+    class _Loss(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, p):
+            p2 = p.reshape(p.shape[0], -1)
+            idx = label.reshape(-1).long()[:, None]
+            picked = torch.gather(p2, 1, idx).clamp(min=1e-20)
+            g = torch.zeros_like(p2).scatter_(1, idx, -loss_weight / p2.shape[0] / picked)
+            ctx.save_for_backward(g.reshape(p.shape))
+            return -loss_weight * torch.log(picked).sum() / p2.shape[0]
+
+        @staticmethod
+        def backward(ctx, grad):
+            (g,) = ctx.saved_tensors
+            return g * grad
+
+    return _Loss.apply(prob)
+
+
+def hinge_loss(scores, label, norm="L1", loss_weight=1.0):
+    """Caffe's HingeLoss (hinge_loss_layer.cpp): h = max(0, 1 + x) off the label and max(0, 1 - x) at it, summed (L1)
+    or summed squared (L2) over num = scores.shape[0].  Its gradient is sign(g) * loss_weight / num (L1, sign(0) = 0) or
+    g * 2 * loss_weight / num (L2), with g = h off the label and -h at it."""
+    import torch
+
+    class _Loss(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, x):
+            x2 = x.reshape(x.shape[0], -1)
+            num = x2.shape[0]
+            at = torch.zeros_like(x2, dtype=torch.bool).scatter_(1, label.reshape(-1).long()[:, None], True)
+            h = torch.clamp(1 + torch.where(at, -x2, x2), min=0)
+            g = torch.where(at, -h, h)
+            g = torch.sign(g) * (loss_weight / num) if norm == "L1" else g * (loss_weight * 2 / num)
+            ctx.save_for_backward(g.reshape(x.shape))
+            return loss_weight * (h.sum() if norm == "L1" else (h * h).sum()) / num
+
+        @staticmethod
+        def backward(ctx, grad):
+            (g,) = ctx.saved_tensors
+            return g * grad
+
+    return _Loss.apply(scores)
