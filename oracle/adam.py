@@ -4,6 +4,7 @@ Only tests/ and __graft_entry__ may import this module; the product package neve
 with sync_oracle.c (on_start, scale, reduce-scatter) into _build/libadam_oracle.so with the flags of
 oracle/Makefile, so every fp32 operation is rounded once.
 """
+import concurrent.futures as cf
 import ctypes
 import os
 import subprocess
@@ -46,6 +47,7 @@ def lib():
         L.cos_oracle_step_adam.argtypes = [i32, u64, ppf, ppf, ppf, i32, pi64, pf, pf, f32, f32, f32, f32, f32, i32,
                                            i32]
         L.cos_oracle_powf_half_check.argtypes = [ctypes.c_uint32, ctypes.c_uint32, ctypes.POINTER(u64)]
+        L.cos_oracle_powf_half_fill.argtypes = [ctypes.c_uint32, ctypes.c_uint32, pf]
         _lib = L
     return _lib
 
@@ -73,6 +75,21 @@ def powf_half_check(lo, hi):
     out = (ctypes.c_uint64 * 2)()
     lib().cos_oracle_powf_half_check(lo, hi, out)
     return out[0], out[1]
+
+
+def powf_half_fill(lo, hi, out=None, threads=None):
+    """libm's powf(x, 0.5f) for the float bit patterns [lo, hi), as a float32 array (into `out` when given), filled
+    by `threads` threads (default: one per CPU); ctypes releases the GIL during each chunk."""
+    n = hi - lo
+    out = np.empty(n, np.float32) if out is None else out
+    assert out.dtype == np.float32 and out.size == n and out.flags.c_contiguous
+    k = max(1, min(threads or os.cpu_count() or 1, n))
+    cuts = [lo + n * i // k for i in range(k + 1)]
+    L = lib()
+    with cf.ThreadPoolExecutor(k) as ex:
+        list(ex.map(lambda i: L.cos_oracle_powf_half_fill(cuts[i], cuts[i + 1], O._pf(out[cuts[i] - lo:])),
+                    range(k)))
+    return out
 
 
 class AdamSimulation(O.Simulation):

@@ -120,3 +120,14 @@ void cos_oracle_powf_half_check(uint32_t lo, uint32_t hi, uint64_t* counts) {
   counts[0] = vs_sqrt;
   counts[1] = vs_device;
 }
+
+/* out[u - lo] = powf(x, 0.5f) for the bit patterns u in [lo, hi): the libm values the BatchNorm kernels' device
+ * copy of powf_half.h is checked against.  Independent ranges may be filled from separate threads. */
+void cos_oracle_powf_half_fill(uint32_t lo, uint32_t hi, float* out) {
+  for (uint64_t u = lo; u < hi; ++u) {
+    float x;
+    uint32_t b = (uint32_t)u;
+    memcpy(&x, &b, 4);
+    out[u - lo] = powf(x, 0.5f);
+  }
+}
