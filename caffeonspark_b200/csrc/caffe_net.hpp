@@ -14,7 +14,6 @@
 
 #include <cuda_runtime_api.h>
 
-#include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -22,8 +21,8 @@
 
 #include "../../include/caffedistri_b200.h"
 #include "caffe_proto_io.hpp"
-#include "data_transform.hpp"
 #include "fused_sync_sgd.hpp"
+#include "input_stager.hpp"
 #include "peer_adapter.hpp"
 #include "peer_memory.hpp"
 #include "solver_spec.hpp"
@@ -57,11 +56,11 @@ class CaffeNet {
 
   int deviceID(int solver_index) const;
   bool init(int solver_index, bool enable_nn, std::string* err);
-  bool train(int solver_index, const cos_blob* data, int ndata, std::string* err);
+  bool train(const cos_blob* data, int ndata, std::string* err);
   // one step over `passes` (== iter_size) groups of ndata blobs, one distinct micro-batch per pass
-  bool train_accumulate(int solver_index, const cos_blob* data, int ndata, int passes, std::string* err);
+  bool train_accumulate(const cos_blob* data, int ndata, int passes, std::string* err);
   // train() on untransformed blobs: each staged input's transform_param runs on the device (data_transform.hpp)
-  bool train_raw(int solver_index, const cos_raw_blob* data, int ndata, std::string* err);
+  bool train_raw(const cos_raw_blob* data, int ndata, std::string* err);
   virtual int snapshot(std::string* err);
   std::string snapshot_filename(int iter, bool is_state) const;  // Solver::SnapshotFilename
   std::vector<BlobView> blob_views(const float* flat) const;  // the learnable blobs (owners), in order
@@ -118,12 +117,7 @@ class CaffeNet {
   // Solver::Step: stage `groups` x ndata host blobs, run the producer iter_size times (pass i reads group i, or
   // group 0 when groups == 1), the loss mean, then sync_step.  With `raw` (train_raw, groups 1) the blobs come from
   // there instead of `data`, and every pass first transforms the inputs that have a transform_param.
-  bool run_step(int solver_index, const cos_blob* data, int ndata, int groups, const cos_raw_blob* raw,
-                std::string* err);
-  bool check_raw(const cos_raw_blob* data, int ndata, std::string* err);  // train_raw's argument checks
-  bool check_raw_images(const cos_raw_blob& b, const InputTransform& t,
-                        const std::function<bool(const std::string&)>& refuse);
-  bool transform_inputs(int stage, const cos_raw_blob* raw, int pass, std::string* err);
+  bool run_step(const cos_blob* data, int ndata, int groups, const cos_raw_blob* raw, std::string* err);
   int resolved_algo() const;
   int resolved_kernel() const;
 
@@ -203,35 +197,11 @@ class CaffeNet {
   std::unique_ptr<NativeProducer> native_;  // the built-in producer, when attached
   bool restored_model_ = false;             // restore() loaded weights from a model file
   int solver_index_ = 0;  // index the gradient producer sees (local device number inside the executor)
-  // Input path (row f3): the reference keeps a 2-deep Free/Full queue of host blobs between the transformer
-  // threads and the solver thread (CaffeProcessor.scala:32-35,442-452) and MemoryInputAdapter::feed points the
-  // data layer at the host blob (MemoryInputAdapter.cpp:24-32).  Here: two device-side staging sets; the H2D
-  // copy of batch t runs on its own copy stream while the compute stream still works on batch t-1; train()
-  // returns as soon as ITS batch has left host memory (the caller recycles the blobs after train() returns).
-  struct InputStage {
-    std::vector<void*> dev;            // the fp32 inputs the producer reads
-    std::vector<size_t> bytes;
-    std::vector<void*> raw;            // train_raw: the untransformed inputs that have a transform_param
-    std::vector<size_t> raw_bytes;     // (COS_RAW_U8_IMAGES: a ragged arena, grown to the largest batch seen)
-    std::vector<void*> geom;           // COS_RAW_U8_IMAGES: the call's ImageGeometry table on the device
-    std::vector<size_t> geom_bytes;
-    std::vector<void*> geom_host;      // ... and in pinned host memory, the source of its copy
-    std::vector<size_t> geom_host_bytes;
-    cudaEvent_t copied = nullptr;    // H2D of this stage finished
-    cudaEvent_t consumed = nullptr;  // the step that read this stage finished
-    bool consumed_valid = false;
-  };
-  InputStage stage_[2];
-  int stage_idx_ = 0;
-  cudaStream_t copy_stream_ = nullptr;
+  InputStager stager_;  // the input path (row f3)
   cudaEvent_t loss_ev_[2] = {nullptr, nullptr};
   bool loss_pending_[2] = {false, false};
   int loss_idx_ = 0;
   int opt_train_pipeline_ = 1;      // 0: train() returns only after the whole Step finished (reference behaviour)
-  // train_raw: the staged inputs' transforms with their means on this device, and the first call's raw shapes
-  std::vector<InputTransform> transforms_;
-  std::vector<float*> mean_dev_;
-  std::vector<cos_raw_blob> raw_shapes_;
   void harvest_losses(bool wait);
   std::vector<std::string> addr_store_;
   std::vector<const char*> addr_cstrs_;

@@ -221,7 +221,7 @@ int cos_net_train(cos_net* net, int solver_index, const cos_blob* data, int ndat
     std::string err;
     CaffeNet* r = R(net, solver_index);
     if (!r) return fail("invalid solver_index");
-    if (!r->train(0, data, ndata, &err)) return fail(err);
+    if (!r->train(data, ndata, &err)) return fail(err);
     return 1;
   })
 }
@@ -234,7 +234,7 @@ int cos_net_train_accumulate(cos_net* net, int solver_index, const cos_blob* dat
     std::string err;
     CaffeNet* r = R(net, solver_index);
     if (!r) return fail("invalid solver_index");
-    if (!r->train_accumulate(0, data, ndata, passes, &err)) return fail(err);
+    if (!r->train_accumulate(data, ndata, passes, &err)) return fail(err);
     return 1;
   })
 }
@@ -247,7 +247,7 @@ int cos_net_train_raw(cos_net* net, int solver_index, const cos_raw_blob* data, 
     std::string err;
     CaffeNet* r = R(net, solver_index);
     if (!r) return fail("invalid solver_index");
-    if (!r->train_raw(0, data, ndata, &err)) return fail(err);
+    if (!r->train_raw(data, ndata, &err)) return fail(err);
     return 1;
   })
 }
