@@ -7,7 +7,9 @@ ResNet-20 fixture b100, timed against nets.resnet20_module, whose BatchNorms run
 autoencoder fixtures b100 of 1x28x28, Caffe's MNIST autoencoder and the convolutional one with Deconvolutions, each
 scoring its reconstruction against its input with SigmoidCrossEntropyLoss, timed against nets.autoencoder_module and
 nets.conv_autoencoder_module; the TanH LeNet fixture b64, whose head is Softmax + MultinomialLogisticLoss, and the
-PReLU CIFAR-10-quick fixture b100, timed against nets.lenet_tanh_module and nets.cifar10_quick_prelu_module).  For each, one process times the native engine, the PyTorch module with TF32 off and with
+PReLU CIFAR-10-quick fixture b100, timed against nets.lenet_tanh_module and nets.cifar10_quick_prelu_module; the two
+embedding fixtures, whose staged inputs are token ids: the sentence classifier text_cnn b50 of 32 ids and the n-gram
+language model ngram_lm b128 of 4 ids, timed against nets.text_cnn_module and nets.ngram_lm_module).  For each, one process times the native engine, the PyTorch module with TF32 off and with
 TF32 on (cuDNN's default, here applied to matmuls too), alternating the three in every round; each sample is CUDA events around `--iters`
 back-to-back forward/backward calls on one stream after `--warmup` untimed ones.  Prints one JSON line per
 workload with median / min / max ms per call and images/s, and the card's name and power limit.
@@ -29,9 +31,9 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full", "mnist_siamese", "cifar10_resnet20",
-             "mnist_autoencoder", "mnist_conv_autoencoder", "lenet_tanh", "cifar10_quick_prelu")
+             "mnist_autoencoder", "mnist_conv_autoencoder", "lenet_tanh", "cifar10_quick_prelu", "text_cnn", "ngram_lm")
 FIXTURES = ("cifar10_resnet20", "mnist_autoencoder", "mnist_conv_autoencoder", "lenet_tanh",
-            "cifar10_quick_prelu")  # nets kept under tests/golden/configs
+            "cifar10_quick_prelu", "text_cnn", "ngram_lm")  # nets kept under tests/golden/configs
 FP32_PEAK = 67e12  # H100 SXM data sheet, dense FP32, at up to 700 W
 
 
@@ -149,14 +151,21 @@ def main():
         net.use_native_producer(fill_weights=False)
         net.fill("data", 1, 0, 0.05)
         torch.cuda.synchronize()
+        text = name in ("text_cnn", "ngram_lm")
         spec = (nets.RESNET20 if resnet else None if siamese else nets.AUTOENCODER if name == "mnist_autoencoder"
                 else nets.CONV_AUTOENCODER if autoencoder else nets.LENET_TANH if name == "lenet_tanh"
-                else nets.CIFAR10_QUICK_PRELU if name == "cifar10_quick_prelu" else nets.NETS[name])
+                else nets.CIFAR10_QUICK_PRELU if name == "cifar10_quick_prelu" else nets.TEXT_CNN if name == "text_cnn"
+                else nets.NGRAM_LM if name == "ngram_lm" else nets.NETS[name])
         batch = 64 if siamese else spec["batch"]
         rng = np.random.RandomState(0)
-        shape = (2, 28, 28) if siamese else spec["input"]
-        x = torch.from_numpy(rng.rand(batch, *shape).astype(np.float32)).cuda()
-        y = torch.from_numpy(rng.randint(0, 2 if siamese else 10, batch).astype(np.float32)).cuda()
+        if text:  # token ids (Zipf-skewed, as words are) and a class or next-token label
+            ids = (rng.zipf(1.2, (batch, spec["tokens"])) - 1) % spec["vocab"]
+            x = torch.from_numpy(ids.astype(np.float32)).cuda()
+            y = torch.from_numpy(rng.randint(0, spec.get("classes", spec["vocab"]), batch).astype(np.float32)).cuda()
+        else:
+            shape = (2, 28, 28) if siamese else spec["input"]
+            x = torch.from_numpy(rng.rand(batch, *shape).astype(np.float32)).cuda()
+            y = torch.from_numpy(rng.randint(0, 2 if siamese else 10, batch).astype(np.float32)).cuda()
         loss = torch.zeros(1, device="cuda")
         # a stream of its own: the legacy default stream's handle is 0, which would send the engine to the net's
         # stream, outside the events
@@ -173,6 +182,7 @@ def main():
                   else nets.autoencoder_module() if name == "mnist_autoencoder"
                   else nets.conv_autoencoder_module() if autoencoder else nets.lenet_tanh_module() if name == "lenet_tanh"
                   else nets.cifar10_quick_prelu_module() if name == "cifar10_quick_prelu"
+                  else nets.text_cnn_module() if name == "text_cnn" else nets.ngram_lm_module() if name == "ngram_lm"
                   else nets.torch_module(name)).cuda()
         with torch.no_grad():
             w, off = net.data().clone(), 0

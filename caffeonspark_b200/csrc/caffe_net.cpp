@@ -439,6 +439,11 @@ bool CaffeNet::check_status(std::string* err) {
     *err = os.str();
     return false;
   }
+  if (s == kStatusBadEmbedIndex) {  // native_producer.cu embed_forward_kernel
+    *err = "Embed: an id that is not an integer in [0, input_dim) reached the native producer; its row embedded as "
+           "zeros (plus the bias) and added no weight gradient (status 503)";
+    return false;
+  }
   if (s == 300) {  // fused_sync_sgd_tma.cu: an mbarrier never completed (a bulk copy was lost or a peer died mid-tile)
     os << "device-side TMA pipeline timed out after " << opt_timeout_ms_
        << " ms waiting for a bulk copy to complete (status 300)";

@@ -53,7 +53,7 @@ bool fusable_pool(const NetLayer& L) {
          L.top_shapes[0][3] == pooled_size(static_cast<int>(L.bottom_shapes[0][3]), k, s);
 }
 
-// The weight (and bias) of a Convolution, Deconvolution, InnerProduct or Scale: a shared param uses its owner's
+// The weight (and bias) of a Convolution, Deconvolution, InnerProduct, Scale or Embed: a shared param uses its owner's
 // offsets, and only the owner's filler fills the blob.  False when a filler is one the engine cannot draw.
 bool set_params(const NetLayer& L, Op* op, Plan* P, std::string* err) {
   std::string reason;
@@ -130,6 +130,8 @@ const LayerType kLayerTypes[] = {
     {"Softmax", OpKind::kSoftmax},
     {"MultinomialLogisticLoss", OpKind::kMultinomialLogisticLoss, 2, false, 1, "label", true},
     {"HingeLoss", OpKind::kHingeLoss, 2, false, 1, "label", true},
+    {"Embed", OpKind::kEmbed},      // its bottom's ids get no gradient
+    {"Reshape", OpKind::kReshape},  // Flatten's alias: no copy either way
 };
 
 // Plan::text's name of each OpKind
@@ -137,7 +139,8 @@ const char* const kKindNames[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling
                                   "BatchNorm", "SoftmaxWithLoss", "LRN(WITHIN_CHANNEL)", "Slice", "ContrastiveLoss",
                                   "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale", "Deconvolution", "Flatten",
                                   "SigmoidCrossEntropyLoss", "TanH", "ELU", "AbsVal", "BNLL", "Power", "Exp", "Log",
-                                  "Threshold", "PReLU", "Softmax", "MultinomialLogisticLoss", "HingeLoss"};
+                                  "Threshold", "PReLU", "Softmax", "MultinomialLogisticLoss", "HingeLoss",
+                                  "Embed", "Reshape"};
 static_assert(std::size(kKindNames) == static_cast<size_t>(OpKind::kCount), "one name per OpKind");
 
 // LossLayer::Reshape's check, then multinomial_logistic_loss_layer.cpp's: the label holds one value per item, with
@@ -481,15 +484,16 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       const int in = op.bottoms[0];
       op.in_place = L.tops[0] == L.bottoms[0] && in >= P.ninputs && !P.data_alias[in];
       if (op.in_place) storage = P.storage[in];
-    } else if (op.kind == OpKind::kFlatten) {  // flatten_layer.cpp: no copy either way (ShareData, ShareDiff)
+    } else if (op.kind == OpKind::kFlatten || op.kind == OpKind::kReshape) {
+      // flatten_layer.cpp, reshape_layer.cpp: no copy either way (ShareData, ShareDiff); the parser inferred the shape
       if (L.tops[0] == L.bottoms[0]) {
-        *err = why(L, "Flatten Layer does not allow in-place computation.");
+        *err = why(L, L.type + " Layer does not allow in-place computation.");
         return false;
       }
       const int64_t naxes = static_cast<int64_t>(op.in_shape.size());
       const int64_t first = L.flatten_axis < 0 ? L.flatten_axis + naxes : L.flatten_axis;
       const int64_t last = L.flatten_end_axis < 0 ? L.flatten_end_axis + naxes : L.flatten_end_axis;
-      if (first != 1 || last != naxes - 1) {
+      if (op.kind == OpKind::kFlatten && (first != 1 || last != naxes - 1)) {
         *err = why(L, "flatten_param axis " + std::to_string(L.flatten_axis) + ", end_axis " +
                           std::to_string(L.flatten_end_axis) + " is not supported (axis 1 to the last axis is)");
         return false;
@@ -497,6 +501,13 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       // the top's gradient is the bottom's, except on a staged input, whose gradient buffer nothing may share
       const int in = op.bottoms[0];
       if (in >= P.ninputs) storage = P.storage[in];
+    } else if (op.kind == OpKind::kEmbed) {  // embed_layer.cpp: a gather of table rows; ids have no derivative
+      if (op.bottom_grad[0]) {
+        *err = why(L, "Can't backpropagate to EmbedLayer input.");
+        return false;
+      }
+      if (!set_params(L, &op, &P, err)) return false;
+      op.input_dim = L.input_dim;
     } else if (op.kind == OpKind::kBatchNorm) {
       if (!op.shares.empty()) {
         *err = why(L, "shared BatchNorm statistics are not supported");
@@ -555,7 +566,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       }
     }
     op.out = new_tensor(shape_count(op.out_shape), storage);
-    if (op.kind == OpKind::kFlatten) P.data_alias[op.out] = true;
+    if (op.kind == OpKind::kFlatten || op.kind == OpKind::kReshape) P.data_alias[op.out] = true;
     // BatchNorm's blobs are statistics, with no gradient
     wants_grad[op.out] = top_grad || (op.kind != OpKind::kBatchNorm && (op.w_off >= 0 || op.b_off >= 0));
     if (top) cur[*top] = op.out;
@@ -632,6 +643,7 @@ std::string Plan::text() const {
     if (op.kind == OpKind::kConvBiasReluMaxPool) os << " pool" << op.pool_kernel << "/" << op.pool_stride;
     if (op.kind == OpKind::kReLU && op.slope != 0.f) os << " slope=" << op.slope;
     if (op.kind == OpKind::kLRNWithin) os << " n=" << op.lrn_size << " alpha=" << op.lrn_alpha << " beta=" << op.lrn_beta;
+    if (op.kind == OpKind::kEmbed) os << " input_dim=" << op.input_dim << " num_output=" << op.out_shape.back();
     if (op.w_off >= 0 && op.kind != OpKind::kBatchNorm) os << " w=" << op.w_off << ":" << op.w_count;
     if (op.b_off >= 0) os << " b=" << op.b_off << ":" << op.b_count;
     if (op.kind == OpKind::kBatchNorm) os << " stats=" << op.w_off;
@@ -649,7 +661,8 @@ std::string Plan::text() const {
     if (op.kind == OpKind::kEuclideanLoss) os << " second=" << op.bottoms[1] << " loss_weight=" << op.loss_weight;
     if (op.kind == OpKind::kSigmoidCrossEntropyLoss)
       os << " target=" << op.bottoms[1] << " loss_weight=" << op.loss_weight;
-    if (op.kind == OpKind::kFlatten) os << " data=bottom" << (storage[op.out] != op.out ? " diff=bottom" : "");
+    if (op.kind == OpKind::kFlatten || op.kind == OpKind::kReshape)
+      os << " data=bottom" << (storage[op.out] != op.out ? " diff=bottom" : "");
     if (op.kind == OpKind::kSplit) os << " top=" << op.split_top << " data=bottom" << (op.split_unread ? " unread" : "");
     if (op.kind == OpKind::kEltwise) {
       os << " bottoms=" << op.bottoms.size();

@@ -11,6 +11,8 @@
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <cstdint>
+#include <type_traits>
 
 #include "batch_norm.hpp"
 #include "caffe_layers.hpp"
@@ -797,6 +799,128 @@ __global__ void __launch_bounds__(kThreads) hinge_loss_kernel(const float* x, co
   if (threadIdx.x == 0) partial[blockIdx.x] = part;
 }
 
+// ------------------------------------------------------------------ Embed (embed_layer.cpp semantics)
+constexpr int kEmbedBlock = 1024;  // the one block of the offsets' scan and of the stable placement
+
+// The table row of an id, or -1 when the id is not an integer in [0, K) (negative, too large, fractional, NaN, inf).
+// K <= 2^24, so every integer below it is exact in fp32.
+__device__ __forceinline__ int embed_row(float id, int K) {
+  return id >= 0.f && id < static_cast<float>(K) && id == truncf(id) ? static_cast<int>(id) : -1;
+}
+
+// y[m, :] = w[id_m, :] (+ b, one rounding), or b (0 without a bias) for an invalid id, which sets *status.  Each thread
+// copies V consecutive floats of one row (V = 4: float4, when the row length and the pointers allow), so a warp reads
+// and writes contiguous memory.
+template <int V>
+__global__ void embed_forward_kernel(const float* ids, const float* w, const float* b, float* y, int M, int N, int K,
+                                     int* status) {
+  typedef typename std::conditional<V == 4, float4, float>::type Vec;
+  const int nv = N / V;
+  const int64_t total = static_cast<int64_t>(M) * nv;
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int m = static_cast<int>(i / nv), c = static_cast<int>(i % nv) * V;
+    const int k = embed_row(__ldg(ids + m), K);
+    if (k < 0 && c == 0) *reinterpret_cast<volatile int*>(status) = kStatusBadEmbedIndex;
+    Vec v;
+    if (k >= 0) {
+      v = __ldg(reinterpret_cast<const Vec*>(w + static_cast<size_t>(k) * N + c));
+    } else {
+      float* f = reinterpret_cast<float*>(&v);
+      for (int j = 0; j < V; ++j) f[j] = 0.f;
+    }
+    if (b) {
+      const Vec bv = __ldg(reinterpret_cast<const Vec*>(b + c));
+      float* f = reinterpret_cast<float*>(&v);
+      const float* g = reinterpret_cast<const float*>(&bv);
+      for (int j = 0; j < V; ++j) f[j] = __fadd_rn(f[j], g[j]);
+    }
+    *reinterpret_cast<Vec*>(y + static_cast<size_t>(m) * N + c) = v;
+  }
+}
+
+// count[k] = occurrences of row k among the M ids (integer atomics: the counts do not depend on their order)
+__global__ void embed_count_kernel(const float* ids, int M, int K, int* count) {
+  for (int m = blockIdx.x * blockDim.x + threadIdx.x; m < M; m += gridDim.x * blockDim.x) {
+    const int k = embed_row(__ldg(ids + m), K);
+    if (k >= 0) atomicAdd(count + k, 1);
+  }
+}
+
+// a[0 .. n) becomes its exclusive prefix sum: each thread scans a contiguous range, offset by the block's scan of the
+// range totals
+__global__ void __launch_bounds__(kEmbedBlock) exclusive_scan_kernel(int* a, int n) {
+  __shared__ int sh[kEmbedBlock];
+  const int per = (n + kEmbedBlock - 1) / kEmbedBlock;
+  const int lo = min(n, static_cast<int>(threadIdx.x) * per), hi = min(n, lo + per);
+  int sum = 0;
+  for (int i = lo; i < hi; ++i) sum += a[i];
+  sh[threadIdx.x] = sum;
+  __syncthreads();
+  for (int off = 1; off < kEmbedBlock; off <<= 1) {
+    const int v = threadIdx.x >= off ? sh[threadIdx.x - off] : 0;
+    __syncthreads();
+    sh[threadIdx.x] += v;
+    __syncthreads();
+  }
+  int run = sh[threadIdx.x] - sum;
+  for (int i = lo; i < hi; ++i) {
+    const int v = a[i];
+    a[i] = run;
+    run += v;
+  }
+}
+
+// Stable placement: order[cursor[k] ..] receives the positions m of row k in increasing m.  One block walks the ids in
+// chunks of kEmbedBlock; a position's slot is its row's cursor plus the number of earlier positions of that row in the
+// chunk, and the row's last position in the chunk advances the cursor.  On return cursor[k] is the end of k's group.
+__global__ void __launch_bounds__(kEmbedBlock) embed_place_kernel(const float* ids, int M, int K, int* cursor,
+                                                                  int* order) {
+  __shared__ int key[kEmbedBlock];
+  for (int base = 0; base < M; base += kEmbedBlock) {
+    const int m = base + static_cast<int>(threadIdx.x);
+    const int k = m < M ? embed_row(__ldg(ids + m), K) : -1;
+    key[threadIdx.x] = k;
+    __syncthreads();
+    int rank = 0;
+    bool last = true;
+    if (k >= 0) {
+      for (int j = 0; j < kEmbedBlock; ++j) {
+        if (key[j] != k) continue;
+        if (j < static_cast<int>(threadIdx.x)) ++rank;
+        else if (j > static_cast<int>(threadIdx.x)) last = false;
+      }
+    }
+    const int slot = k >= 0 ? cursor[k] + rank : 0;
+    __syncthreads();  // every cursor read of this chunk before its updates
+    if (k >= 0) {
+      order[slot] = m;
+      if (last) cursor[k] = slot + 1;
+    }
+    __syncthreads();  // the updates, and key[], before the next chunk
+  }
+}
+
+// dw[k, :] += the dy rows of k's positions, added one at a time in increasing m onto the value already in dw
+// (embed_layer.cpp Backward_cpu's order).  end[k] is the end of k's group in order[], end[K] the number of valid ids;
+// the block at a group's first slot walks the group.
+__global__ void embed_weight_grad_kernel(const float* ids, const int* order, const int* end, const float* dy,
+                                         float* dw, int N, int K) {
+  const int valid = end[K];
+  for (int j = blockIdx.x; j < valid; j += gridDim.x) {
+    const int k = static_cast<int>(__ldg(ids + order[j]));
+    if (j != (k ? end[k - 1] : 0)) continue;
+    const int stop = end[k];
+    for (int d = threadIdx.x; d < N; d += blockDim.x) {
+      float* p = dw + static_cast<size_t>(k) * N + d;
+      float s = *p;
+#pragma unroll 4
+      for (int q = j; q < stop; ++q) s = __fadd_rn(s, __ldg(dy + static_cast<size_t>(order[q]) * N + d));
+      *p = s;
+    }
+  }
+}
+
 // ------------------------------------------------------------------ fillers (u: the cos_net_fill value in [-1, 1))
 __global__ void constant_fill_kernel(float* p, int n, float v) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = v;
@@ -1036,6 +1160,8 @@ bool NativeProducer::allocate(std::string* err) {
       ws = std::max(ws, static_cast<size_t>(grid_for(plan_.tensor_count[op.bottoms[0]])));  // the per-block partials
     } else if (op.kind == OpKind::kPReLU) {
       ws = std::max(ws, static_cast<size_t>(prelu_slopes(op)) * prelu_chunks(op));  // the slope gradient's partials
+    } else if (op.kind == OpKind::kEmbed) {  // the id grouping: K + 1 counts / group ends, then the M placed positions
+      ws = std::max(ws, static_cast<size_t>(op.input_dim + 1 + plan_.tensor_count[op.bottoms[0]]));
     }
   }
   if ((e = cudaEventCreateWithFlags(&done_, cudaEventDisableTiming)) != cudaSuccess) {
@@ -1186,6 +1312,7 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
       return conv_data_grad(op, conv_dims(op), x, data_ + op.w_off, op.b_off >= 0 ? data_ + op.b_off : nullptr, y, s);
     case OpKind::kSplit:  // no copy: the top reads the bottom's memory
     case OpKind::kFlatten:
+    case OpKind::kReshape:
       act_[op.out] = act_[op.bottoms[0]];
       return cudaSuccess;
     case OpKind::kEltwise: {
@@ -1298,6 +1425,19 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
                                                     op.bottom_grad[0] ? grad_[op.bottoms[0]] : nullptr, workspace_,
                                                     count, count / num, num, op.hinge_l2, op.loss_weight, status_);
       sigmoid_xent_loss_total_kernel<<<1, 1, 0, s>>>(workspace_, blocks, num, op.loss_weight, loss_dev);
+      return cudaGetLastError();
+    }
+    case OpKind::kEmbed: {
+      const int M = static_cast<int>(plan_.tensor_count[op.bottoms[0]]), N = static_cast<int>(op.out_shape.back());
+      const int K = static_cast<int>(op.input_dim);
+      const float* w = data_ + op.w_off;
+      const float* b = op.b_off >= 0 ? data_ + op.b_off : nullptr;
+      auto aligned = [](const float* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; };
+      if (N % 4 == 0 && aligned(w) && (!b || aligned(b)) && aligned(y))
+        embed_forward_kernel<4><<<grid_for(static_cast<int64_t>(M) * N / 4), kThreads, 0, s>>>(x, w, b, y, M, N, K,
+                                                                                               status_);
+      else
+        embed_forward_kernel<1><<<grid_for(static_cast<int64_t>(M) * N), kThreads, 0, s>>>(x, w, b, y, M, N, K, status_);
       return cudaGetLastError();
     }
     default:
@@ -1481,7 +1621,23 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
     case OpKind::kMultinomialLogisticLoss:
     case OpKind::kHingeLoss:
     case OpKind::kFlatten:  // the top's gradient is the bottom's memory
+    case OpKind::kReshape:
       return cudaSuccess;
+    case OpKind::kEmbed: {  // build_plan refuses an Embed whose ids would need a gradient
+      const int N = static_cast<int>(op.out_shape.back()), K = static_cast<int>(op.input_dim);
+      int* group = reinterpret_cast<int*>(workspace_);  // counts, then offsets, then group ends: K + 1 ints
+      int* order = group + K + 1;
+      cudaError_t e = cudaMemsetAsync(group, 0, (static_cast<size_t>(K) + 1) * sizeof(int), s);
+      if (e != cudaSuccess) return e;
+      embed_count_kernel<<<grid_for(nin), kThreads, 0, s>>>(x, nin, K, group);
+      exclusive_scan_kernel<<<1, kEmbedBlock, 0, s>>>(group, K + 1);
+      embed_place_kernel<<<1, kEmbedBlock, 0, s>>>(x, nin, K, group, order);
+      const int threads = N >= kThreads ? kThreads : (N + 31) / 32 * 32;
+      embed_weight_grad_kernel<<<std::min(nin, kTargetSms * 16), threads, 0, s>>>(x, order, group, dy,
+                                                                                  diff_ + op.w_off, N, K);
+      if (op.b_off >= 0) bias_grad_kernel<<<N, kThreads, 0, s>>>(dy, nin, N, 1, diff_ + op.b_off);
+      return cudaGetLastError();
+    }
     default:
       return cudaErrorInvalidValue;
   }

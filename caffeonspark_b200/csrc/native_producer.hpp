@@ -1,7 +1,7 @@
 // native_producer.hpp -- the built-in gradient producer (Net::ForwardBackward for the TRAIN phase of the LeNet,
 // CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, least-squares regression nets,
-// residual nets built of Split, Eltwise and Scale, and autoencoders built of Flatten, Deconvolution and
-// SigmoidCrossEntropyLoss; DESIGN.md section 14).
+// residual nets built of Split, Eltwise and Scale, autoencoders built of Flatten, Deconvolution and
+// SigmoidCrossEntropyLoss, and embedding nets that read token ids through Embed and Reshape; DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -27,6 +27,7 @@ enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
   kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale, kDeconv, kFlatten, kSigmoidCrossEntropyLoss,
   kTanH, kELU, kAbsVal, kBNLL, kPower, kExp, kLog, kThreshold, kPReLU, kSoftmax, kMultinomialLogisticLoss, kHingeLoss,
+  kEmbed, kReshape,
   kCount  // the number of kinds (Plan::text names each)
 };
 
@@ -97,15 +98,18 @@ struct Op {
   // Softmax: softmax_axis, classes and inner as SoftmaxWithLoss's, outer = count(0, axis)
   int64_t outer = 1;
   bool hinge_l2 = false;               // HingeLoss: L2 norm (else L1)
+  // Embed: the vocabulary size K (w_off is the [K, num_output] table, num_output = out_shape.back()); the bottom holds
+  // M = count(bottom) ids
+  int64_t input_dim = 0;
 };
 
 struct Plan {
   std::vector<Op> ops;
   std::vector<int64_t> tensor_count;   // elements per tensor id
   std::vector<int> storage;            // tensor id -> tensor id that owns its memory (itself unless in place)
-  // per tensor id: its activation is another tensor's memory, set when the forward reaches it (a Split or Flatten top
-  // reads its bottom's, as Caffe's ShareData).  A Split top's gradient is still its own; a Flatten top's is its bottom's
-  // (storage, as Caffe's ShareDiff) unless the bottom is a staged input.
+  // per tensor id: its activation is another tensor's memory, set when the forward reaches it (a Split, Flatten or
+  // Reshape top reads its bottom's, as Caffe's ShareData).  A Split top's gradient is still its own; a Flatten or
+  // Reshape top's is its bottom's (storage, as Caffe's ShareDiff) unless the bottom is a staged input.
   std::vector<bool> data_alias;
   int ninputs = 0;                     // tensors 0 .. ninputs-1 are the staged inputs, in data-layer top order
   std::vector<std::string> input_names;
@@ -127,6 +131,9 @@ constexpr int kStatusBadLabel = 500;
 // ... of a MultinomialLogisticLoss or HingeLoss label outside [0, dim) (or NaN): its row adds no loss and gets a zero
 // gradient
 constexpr int kStatusBadMultinomialLabel = 501, kStatusBadHingeLabel = 502;
+// ... of an Embed id that is not an integer in [0, input_dim) (negative, too large, fractional, NaN or infinite): its
+// row embeds as the zero vector (plus the bias) and adds nothing to the weight gradient
+constexpr int kStatusBadEmbedIndex = 503;
 // PReLU's slope gradient runs one grid row per slope (gridDim.y), so a per-channel PReLU has at most this many channels
 constexpr int64_t kMaxPReLUChannels = 65535;
 
@@ -162,7 +169,8 @@ class NativeProducer {
   std::vector<float*> op_z_, op_dz_;      // fused block: conv output without bias and its gradient
   cudaEvent_t done_ = nullptr;            // recorded at the end of every call: the destructor waits for it
   float* workspace_ = nullptr;            // split-K partials, bias partials, BatchNorm scratch, the sigmoid
-                                          // cross-entropy's per-block partials (ops run in order)
+                                          // cross-entropy's per-block partials, Embed's id grouping (int32; ops run
+                                          // in order)
   size_t workspace_floats_ = 0;
   std::vector<void*> allocations_;
 };

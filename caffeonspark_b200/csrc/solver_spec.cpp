@@ -611,6 +611,85 @@ bool flatten(Layer& L, std::vector<Shape>*) {  // flatten_layer.cpp with its def
   return true;
 }
 
+// Ids reach the engine as fp32, which holds every integer exactly only up to 2^24
+constexpr int64_t kMaxEmbedInputDim = int64_t(1) << 24;
+
+bool embed(Layer& L, std::vector<Shape>* params) {  // embed_layer.cpp LayerSetUp and Reshape, with its CHECK messages
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  const Node* p = L.node.first("embed_param");
+  NetLayer& r = L.rec;
+  r.num_output = p ? p->integer("num_output", 0) : 0;
+  r.input_dim = p ? p->integer("input_dim", 0) : 0;
+  if (r.num_output <= 0) return L.refuse("EmbedLayer num_output must be positive.");
+  if (r.input_dim <= 0) return L.refuse("EmbedLayer input_dim must be positive.");
+  if (r.input_dim > kMaxEmbedInputDim)
+    return L.refuse("input_dim " + std::to_string(r.input_dim) + " is more than 2^24 = " +
+                    std::to_string(kMaxEmbedInputDim) + ": ids arrive as fp32, which is not exact above it");
+  r.bias_term = !p || p->boolean("bias_term", true);
+  r.weight_filler = filler(p ? p->first("weight_filler") : nullptr);
+  r.bias_filler = filler(p ? p->first("bias_filler") : nullptr);
+  params->push_back({r.input_dim, r.num_output});  // transposed from InnerProduct's: one row per id
+  if (r.bias_term) params->push_back({r.num_output});
+  Shape out = in;
+  out.push_back(r.num_output);
+  L.set_top(0, out);
+  return true;
+}
+
+bool reshape(Layer& L, std::vector<Shape>*) {  // reshape_layer.cpp LayerSetUp and Reshape, with its CHECK messages
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  const Node* p = L.node.first("reshape_param");
+  const Node* shape = p ? p->first("shape") : nullptr;
+  Shape dims;
+  if (shape) for (const Node* d : shape->all("dim")) dims.push_back(atol(d->value.c_str()));
+  int64_t inferred = -1, constant = 1;
+  std::vector<int64_t> copies;
+  for (size_t i = 0; i < dims.size(); ++i) {
+    if (dims[i] == 0) {
+      copies.push_back(static_cast<int64_t>(i));
+    } else if (dims[i] == -1) {
+      if (inferred != -1)
+        return L.refuse("new shape contains multiple -1 dims; at most a single (1) value of -1 may be specified");
+      inferred = static_cast<int64_t>(i);
+    } else if (dims[i] < 0) {  // Blob::Reshape
+      return L.refuse("Check failed: shape[" + std::to_string(i) + "] >= 0 (" + std::to_string(dims[i]) + " vs. 0)");
+    } else {
+      constant *= dims[i];
+    }
+  }
+  const int64_t naxes = static_cast<int64_t>(in.size());
+  const int64_t given = p ? p->integer("axis", 0) : 0;
+  const int64_t start = given >= 0 ? given : naxes + given + 1;
+  if (start < 0) return L.refuse("axis " + std::to_string(given) + " out of range");
+  if (start > naxes)
+    return L.refuse("axis " + std::to_string(given) + " out of range for " + std::to_string(naxes) + "-D input blob");
+  const int64_t num_axes = p ? p->integer("num_axes", -1) : -1;
+  if (num_axes < -1) return L.refuse("num_axes must be >= 0, or -1 for all");
+  const int64_t end = num_axes == -1 ? naxes : start + num_axes;
+  if (end > naxes) return L.refuse("end_axis = axis + num_axes is out of range");
+  Shape out(in.begin(), in.begin() + start);
+  out.insert(out.end(), dims.begin(), dims.end());
+  out.insert(out.end(), in.begin() + end, in.end());
+  for (int64_t c : copies) {
+    if (naxes <= start + c)
+      return L.refuse("new shape contains a 0, but there was no corresponding bottom axis to copy");
+    out[start + c] = in[start + c];
+  }
+  if (inferred >= 0) {
+    int64_t explicit_count = constant * shape_count(Shape(in.begin(), in.begin() + start)) * shape_count(in, end);
+    for (int64_t c : copies) explicit_count *= out[start + c];
+    if (explicit_count == 0 || shape_count(in) % explicit_count != 0)
+      return L.refuse("bottom count (" + std::to_string(shape_count(in)) + ") must be divisible by the product of the "
+                      "specified dimensions (" + std::to_string(explicit_count) + ")");
+    out[start + inferred] = shape_count(in) / explicit_count;
+  }
+  if (shape_count(out) != shape_count(in)) return L.refuse("output count must match input count");
+  L.set_top(0, out);
+  return true;
+}
+
 bool concat(Layer& L, std::vector<Shape>*) {  // concat_layer.cpp LayerSetUp and Reshape, with its CHECK messages
   Shape out;
   if (!L.bottom(0, &out)) return false;
@@ -743,6 +822,7 @@ const struct { const char* type; Rule rule; } kRules[] = {
     {"Softmax", same_shape}, {"Power", same_shape}, {"AbsVal", same_shape}, {"BNLL", same_shape}, {"ELU", same_shape},
     {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape}, {"PReLU", prelu},
     {"Split", split}, {"Eltwise", eltwise}, {"Scale", scale}, {"Flatten", flatten}, {"Concat", concat},
+    {"Embed", embed}, {"Reshape", reshape},
     {"SoftmaxWithLoss", softmax_loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
     {"HingeLoss", loss}, {"MultinomialLogisticLoss", loss},
     {"BatchNorm", batch_norm}, {"Slice", slice}, {"ContrastiveLoss", contrastive_loss}, {"Silence", silence},

@@ -73,6 +73,9 @@ struct NetLayer {
   int64_t softmax_axis = 1;
   bool channel_shared = false;  // PReLUParameter; its filler is weight_filler (constant 0.25 when none is given)
   std::string hinge_norm = "L1";  // HingeLossParameter: "L1" or "L2"
+  // Embed (caffe.proto EmbedParameter): the vocabulary size; num_output, bias_term (default true) and the fillers are
+  // the fields above
+  int64_t input_dim = 0;
   FillerSpec weight_filler, bias_filler;
 };
 

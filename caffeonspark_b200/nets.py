@@ -538,3 +538,65 @@ def hinge_loss(scores, label, norm="L1", loss_weight=1.0):
             return g * grad
 
     return _Loss.apply(scores)
+
+
+# tests/golden/configs/text_cnn_train_test.prototxt: Embed 5000 x 64 (no bias) of 32 tokens, Reshape to N x 1 x 32 x 64,
+# three Convolutions of 32 filters spanning 3, 4 and 5 tokens and the whole embedding, ReLU, MAX pool over time, Concat,
+# InnerProduct 96 -> 2.  320,000 + 6,176 + 8,224 + 10,272 + 194 = 344,866 parameters in 9 blobs.
+TEXT_CNN = dict(tokens=32, batch=50, vocab=5000, dim=64, widths=(3, 4, 5), filters=32, classes=2)
+TEXT_CNN_PARAM_COUNT = 344866
+# tests/golden/configs/ngram_lm_train_test.prototxt: Embed 2000 x 32 (with its bias) of 4 context tokens, InnerProduct
+# 128 -> 128, TanH, InnerProduct 128 -> 2000.  64,032 + 16,512 + 258,000 = 338,544 parameters in 6 blobs.
+NGRAM_LM = dict(tokens=4, batch=128, vocab=2000, dim=32, hidden=128)
+NGRAM_LM_PARAM_COUNT = 338544
+
+
+def embed_module(input_dim, num_output, bias=True):
+    """Caffe's Embed as a PyTorch module: weight [input_dim, num_output] (then bias [num_output]), forward(ids of any
+    shape, float or integer) -> ids.shape + (num_output,), the table's rows (plus the bias)."""
+    import torch
+    import torch.nn as nn
+
+    class Embed(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.weight = nn.Parameter(torch.zeros(input_dim, num_output))
+            self.bias = nn.Parameter(torch.zeros(num_output)) if bias else None
+
+        def forward(self, ids):
+            y = self.weight[ids.long()]
+            return y + self.bias if self.bias is not None else y
+
+    return Embed()
+
+
+def text_cnn_module():
+    """The sentence classifier fixture as one PyTorch module, parameters in learnable_params() order.
+    forward(tokens [N, 32]) -> scores [N, 2]; its `convs` are the three Convolutions, each followed by ReLU and a MAX
+    pool over all its positions."""
+    import torch
+    import torch.nn as nn
+    s = TEXT_CNN
+
+    class TextCNN(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.embed = embed_module(s["vocab"], s["dim"], bias=False)
+            self.convs = nn.ModuleList(nn.Conv2d(1, s["filters"], (k, s["dim"])) for k in s["widths"])
+            self.ip = nn.Linear(s["filters"] * len(s["widths"]), s["classes"])
+
+        def forward(self, tokens):
+            x = self.embed(tokens).unsqueeze(1)  # Reshape: N x 1 x tokens x dim
+            pooled = [torch.relu(c(x)).amax(dim=(2, 3)) for c in self.convs]
+            return self.ip(torch.cat(pooled, 1))
+
+    return TextCNN()
+
+
+def ngram_lm_module():
+    """The n-gram language model fixture as one PyTorch module, parameters in learnable_params() order.
+    forward(context [N, 4]) -> next-token scores [N, 2000]."""
+    import torch.nn as nn
+    s = NGRAM_LM
+    return nn.Sequential(embed_module(s["vocab"], s["dim"]), nn.Flatten(), nn.Linear(s["tokens"] * s["dim"], s["hidden"]),
+                         nn.Tanh(), nn.Linear(s["hidden"], s["vocab"]))

@@ -254,12 +254,14 @@ COS_API int cos_net_set_forward_backward(cos_net* net, cos_forward_backward_fn f
 
 /* The built-in gradient producer (DESIGN.md section 14): a forward/backward engine built from the TRAIN phase of a
  * Caffe net prototxt, on this library's own sm_90a kernels.  It runs MemoryData / CoSData / Input, Convolution (group
- * 1, dilation 1), Pooling (MAX, AVE), InnerProduct (axis 1), ReLU, Sigmoid, BatchNorm, LRN (WITHIN_CHANNEL), Slice
- * and one loss layer, SoftmaxWithLoss or ContrastiveLoss (default normalisation); Accuracy and Silence are skipped.
+ * 1, dilation 1), Pooling (MAX, AVE), InnerProduct (axis 1), ReLU, Sigmoid, BatchNorm, LRN (WITHIN_CHANNEL), Slice,
+ * Embed over fp32 token ids (a CoSData INT_ARRAY top) and Reshape, the other layers DESIGN.md section 14 lists, and one
+ * loss layer, SoftmaxWithLoss or ContrastiveLoss among them (default normalisation); Accuracy and Silence are skipped.
  * Named params are shared as in Caffe.  Every other layer, and loss_param or an unknown filler type, is refused with an
  * error naming the layer.  Every use of a learnable blob adds its gradient into diff_ once per call; results are
  * bitwise reproducible.
- * A label outside [0, classes) sets the net's device status word: the next synchronising call fails with a message. */
+ * A label outside [0, classes), or an Embed id that is not an integer in [0, input_dim), sets the net's device status
+ * word: the next synchronising call fails with a message. */
 /* Attach the built-in engine to every local solver of `net` and register it as the producer.
  * net_prototxt NULL = the net the solver file named at allocate; otherwise a solver or net prototxt whose layout must
  * equal the net's.  fill_weights 1 = initialise data_ from the prototxt fillers (only when no model_file was
