@@ -132,6 +132,9 @@ const LayerType kLayerTypes[] = {
     {"HingeLoss", OpKind::kHingeLoss, 2, false, 1, "label", true},
     {"Embed", OpKind::kEmbed},      // its bottom's ids get no gradient
     {"Reshape", OpKind::kReshape},  // Flatten's alias: no copy either way
+    // x, cont and the optional x_static (the parser checked the count); cont is read, never differentiated, so two
+    // RNNs may read one cont blob
+    {"RNN", OpKind::kRNN, -1, false, 1, "cont"},
 };
 
 // Plan::text's name of each OpKind
@@ -140,7 +143,7 @@ const char* const kKindNames[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling
                                   "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale", "Deconvolution", "Flatten",
                                   "SigmoidCrossEntropyLoss", "TanH", "ELU", "AbsVal", "BNLL", "Power", "Exp", "Log",
                                   "Threshold", "PReLU", "Softmax", "MultinomialLogisticLoss", "HingeLoss",
-                                  "Embed", "Reshape"};
+                                  "Embed", "Reshape", "RNN"};
 static_assert(std::size(kKindNames) == static_cast<size_t>(OpKind::kCount), "one name per OpKind");
 
 // LossLayer::Reshape's check, then multinomial_logistic_loss_layer.cpp's: the label holds one value per item, with
@@ -316,6 +319,10 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       *err = why(L, "layer type not supported");
       return false;
     }
+    if (row->kind == OpKind::kRNN && L.expose_hidden) {
+      *err = why(L, "expose_hidden: true is not supported");
+      return false;
+    }
     if (row->kind == OpKind::kScale && L.bottoms.size() == 2) {
       *err = why(L, "the two-bottom form (the scale read from bottom[1]) is not supported");
       return false;
@@ -471,8 +478,10 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         *err = why(L, "transpose: true is not supported");
         return false;
       }
-      if (L.axis != 1) {
-        *err = why(L, "axis other than 1 is not supported");
+      // inner_product_layer.cpp: count(0, axis) rows of K = count(axis) inputs each; the parser made the axis canonical
+      const int64_t naxes = static_cast<int64_t>(op.in_shape.size());
+      if (L.axis >= naxes) {
+        *err = why(L, "axis " + std::to_string(L.axis) + " out of range for " + std::to_string(naxes) + "-D Blob");
         return false;
       }
       if (!set_params(L, &op, &P, err)) return false;
@@ -508,6 +517,19 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       }
       if (!set_params(L, &op, &P, err)) return false;
       op.input_dim = L.input_dim;
+    } else if (op.kind == OpKind::kRNN) {  // recurrent_layer.cpp, rnn_layer.cpp; the parser checked the shapes
+      std::string reason;
+      if (!filler_ok(L.weight_filler, &reason) || !filler_ok(L.bias_filler, &reason)) {
+        *err = why(L, reason);
+        return false;
+      }
+      // the layer's params in the parser's order; W_xh_static only with x_static
+      std::vector<int> roles = {Op::kWxh, Op::kBh, Op::kWhh, Op::kWho, Op::kBo};
+      if (L.static_input) roles.insert(roles.begin() + 2, Op::kWxhStatic);
+      for (size_t j = 0; j < roles.size(); ++j) {
+        op.rnn_off[roles[j]] = P.blob_off[L.blobs[j]];
+        if (!L.shared[j]) P.blob_filler[L.blobs[j]] = L.bias_param[j] ? L.bias_filler : L.weight_filler;
+      }
     } else if (op.kind == OpKind::kBatchNorm) {
       if (!op.shares.empty()) {
         *err = why(L, "shared BatchNorm statistics are not supported");
@@ -568,7 +590,8 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     op.out = new_tensor(shape_count(op.out_shape), storage);
     if (op.kind == OpKind::kFlatten || op.kind == OpKind::kReshape) P.data_alias[op.out] = true;
     // BatchNorm's blobs are statistics, with no gradient
-    wants_grad[op.out] = top_grad || (op.kind != OpKind::kBatchNorm && (op.w_off >= 0 || op.b_off >= 0));
+    wants_grad[op.out] = top_grad || op.kind == OpKind::kRNN ||
+                         (op.kind != OpKind::kBatchNorm && (op.w_off >= 0 || op.b_off >= 0));
     if (top) cur[*top] = op.out;
     if (row->loss) loss_top = op.out, loss_layer = L.name;
     P.ops.push_back(op);
@@ -600,6 +623,13 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
     if (op.kind == OpKind::kThreshold && !op.no_backward && op.bottom_grad[0]) {
       *err = "layer '" + op.name + "' (Threshold): Not Implemented Yet: Threshold has no backward, and a gradient "
              "reaches it and is wanted at its bottom (native producer)";
+      return false;
+    }
+  }
+  // recurrent_layer.cpp Backward_cpu: an RNN under the loss whose cont would get a gradient (Caffe's propagate_down[1])
+  for (const Op& op : P.ops) {
+    if (op.kind == OpKind::kRNN && !op.no_backward && wants_grad[op.bottoms[1]]) {
+      *err = "layer '" + op.name + "' (RNN): Cannot backpropagate to sequence indicators. (native producer)";
       return false;
     }
   }
@@ -644,6 +674,13 @@ std::string Plan::text() const {
     if (op.kind == OpKind::kReLU && op.slope != 0.f) os << " slope=" << op.slope;
     if (op.kind == OpKind::kLRNWithin) os << " n=" << op.lrn_size << " alpha=" << op.lrn_alpha << " beta=" << op.lrn_beta;
     if (op.kind == OpKind::kEmbed) os << " input_dim=" << op.input_dim << " num_output=" << op.out_shape.back();
+    if (op.kind == OpKind::kRNN) {
+      static const char* roles[] = {"w_xh", "b_h", "w_xh_static", "w_hh", "w_ho", "b_o"};
+      os << " T=" << op.in_shape[0] << " N=" << op.in_shape[1] << " H=" << op.out_shape[2] << " cont=" << op.bottoms[1];
+      if (op.bottoms.size() > 2) os << " static=" << op.bottoms[2];
+      for (int r = 0; r < Op::kRnnBlobs; ++r)
+        if (op.rnn_off[r] >= 0) os << " " << roles[r] << "=" << op.rnn_off[r];
+    }
     if (op.w_off >= 0 && op.kind != OpKind::kBatchNorm) os << " w=" << op.w_off << ":" << op.w_count;
     if (op.b_off >= 0) os << " b=" << op.b_off << ":" << op.b_count;
     if (op.kind == OpKind::kBatchNorm) os << " stats=" << op.w_off;

@@ -108,6 +108,68 @@ struct StorePartial {  // split-K partial z of C[M, N]
   __device__ void operator()(int m, int n, int z, float v) const { ws[((size_t)z * M + m) * N + n] = v; }
 };
 
+// ------------------------------------------------------------------ the RNN's gathers and epilogues (rnn_layer.cpp's
+// unrolled net: each Caffe layer's operation rounded once, in its order)
+// hc[r, c] = cont[r] * h[r, c]: the Scale layer h_conted_{t-1} = cont_t * h_{t-1}, over one step's rows or all T N
+struct ContGather {
+  const float* h;
+  const float* cont;
+  int ld;
+  __device__ float operator()(int r, int c) const { return __fmul_rn(__ldg(cont + r), __ldg(h + (size_t)r * ld + c)); }
+};
+// h_t = tanh(fl(fl(W_hh hc_{t-1} + g_t) + z)): the Eltwise SUM in bottom order (z only with x_static), then TanH
+struct RnnStep {
+  const float* g;
+  const float* z;
+  float* h;
+  int ld;
+  __device__ void operator()(int m, int n, int, float v) const {
+    const size_t i = (size_t)m * ld + n;
+    float a = __fadd_rn(v, __ldg(g + i));
+    if (z) a = __fadd_rn(a, __ldg(z + i));
+    h[i] = tanhf(a);
+  }
+};
+struct StoreTanhRM {  // out[m * ld + n] = tanh(fl(v + bias[n])): W_ho_h_t then o_neuron_t
+  float* out;
+  const float* bias;
+  int ld;
+  __device__ void operator()(int m, int n, int, float v) const {
+    out[(size_t)m * ld + n] = tanhf(__fadd_rn(v, __ldg(bias + n)));
+  }
+};
+// dho = dzo W_ho, the gradient W_ho_h_t sends to h_t.  h_{T-1} has that one reader, so on the last step's rows
+// (m >= last) it is already the hidden TanH's: dpre = dho * (1 - h^2).
+struct RnnOutGrad {
+  float* dho;
+  float* dpre;
+  const float* h;
+  int ld, last;
+  __device__ void operator()(int m, int n, int, float v) const {
+    const size_t i = (size_t)m * ld + n;
+    dho[i] = v;
+    if (m >= last) {
+      const float t = __ldg(h + i);
+      dpre[i] = __fmul_rn(v, __fsub_rn(1.f, __fmul_rn(t, t)));
+    }
+  }
+};
+// One step of backpropagation through time, v = (dpre_t W_hh)[m, n]: the Scale's backward cont_t * v, the implicit
+// Split of h_{t-1} (its W_ho reader first), then h_neuron_{t-1}'s TanH: dpre_{t-1} = fl(dho_{t-1} + cont_t v) (1 - h^2)
+struct RnnBackStep {
+  const float* cont;  // cont_t
+  const float* dho;   // these three at step t - 1
+  const float* h;
+  float* dpre;
+  int ld;
+  __device__ void operator()(int m, int n, int, float v) const {
+    const size_t i = (size_t)m * ld + n;
+    const float d = __fadd_rn(__ldg(dho + i), __fmul_rn(__ldg(cont + m), v));
+    const float t = __ldg(h + i);
+    dpre[i] = __fmul_rn(d, __fsub_rn(1.f, __fmul_rn(t, t)));
+  }
+};
+
 // C = A[M, K] * B[K, N]; blockIdx.z covers k in [z * kchunk, min(K, (z + 1) * kchunk)).
 template <class GA, class GB, class EPI>
 __global__ void __launch_bounds__(kGemmThreads) gemm_kernel(GA ga, GB gb, EPI epi, int M, int N, int K, int kchunk) {
@@ -198,6 +260,15 @@ __global__ void __launch_bounds__(kThreads) bias_grad_kernel(const float* dy, in
   for (int i = threadIdx.x; i < N * HW; i += kThreads) s = __fadd_rn(s, dy[((size_t)(i / HW) * C + c) * HW + i % HW]);
   s = block_sum(s, sh);
   if (threadIdx.x == 0) dst[c] = __fadd_rn(dst[c], s);
+}
+
+// out[i] = d[0][i] + d[1][i] + ... in step order: the implicit Split of x_static's transform, read by every step
+__global__ void sum_steps_kernel(const float* d, int steps, int n, float* out) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float a = d[i];
+    for (int t = 1; t < steps; ++t) a = __fadd_rn(a, d[(size_t)t * n + i]);
+    out[i] = a;
+  }
 }
 
 __global__ void accumulate_kernel(float* dst, const float* src, int n) {
@@ -995,7 +1066,20 @@ int64_t slice_inner(const Op& op) {
   return n;
 }
 int64_t slice_span(const Op& op, const std::vector<int64_t>& shape) { return shape[op.slice_axis] * slice_inner(op); }
-int ip_k(const Op& op) { return static_cast<int>(op.w_count / (op.w_count > 0 ? op.out_shape[1] : 1)); }
+// InnerProduct: K = count(axis) inputs per row (the weight is [num_output, K]), and count(0, axis) rows
+int ip_k(const Op& op) { return static_cast<int>(op.w_count / (op.w_count > 0 ? op.out_shape.back() : 1)); }
+int ip_rows(const Op& op) { return static_cast<int>(shape_count(op.in_shape) / std::max(ip_k(op), 1)); }
+// RNN: T steps of N streams, H hidden units, I = count(x, 2) inputs per step and S = count(x_static, 1)
+struct RnnDims {
+  int T, N, H, I, S;
+};
+RnnDims rnn_dims(const Op& op, const std::vector<int64_t>& tensor_count) {
+  RnnDims d;
+  d.T = static_cast<int>(op.in_shape[0]), d.N = static_cast<int>(op.in_shape[1]);
+  d.H = static_cast<int>(op.out_shape[2]), d.I = static_cast<int>(shape_count(op.in_shape, 2));
+  d.S = op.bottoms.size() > 2 ? static_cast<int>(tensor_count[op.bottoms[2]] / d.N) : 0;
+  return d;
+}
 // PReLU: the elements each slope reduces over, the number of slopes, and the chunks of the slope gradient
 int prelu_span(const Op& op) {
   return static_cast<int>(op.channel_shared ? shape_count(op.in_shape) : op.in_shape[0] * op.prelu_dim);
@@ -1131,6 +1215,7 @@ bool NativeProducer::allocate(std::string* err) {
   op_aux_.assign(plan_.ops.size(), nullptr);
   op_z_.assign(plan_.ops.size(), nullptr);
   op_dz_.assign(plan_.ops.size(), nullptr);
+  rnn_.assign(plan_.ops.size(), RnnBuffers());
   size_t ws = 1;
   for (size_t i = 0; i < plan_.ops.size(); ++i) {
     const Op& op = plan_.ops[i];
@@ -1150,7 +1235,30 @@ bool NativeProducer::allocate(std::string* err) {
                (op.kind == OpKind::kEltwise && op.eltwise_op == kEltwiseMax)) {
       if (!alloc(out * sizeof(int), &op_aux_[i])) return false;
     } else if (op.kind == OpKind::kInnerProduct) {
-      ws = std::max(ws, static_cast<size_t>(splits_of(static_cast<int>(op.in_shape[0]))) * op.w_count);
+      ws = std::max(ws, static_cast<size_t>(splits_of(ip_rows(op))) * op.w_count);
+    } else if (op.kind == OpKind::kRNN) {
+      const RnnDims d = rnn_dims(op, plan_.tensor_count);
+      const size_t step = static_cast<size_t>(d.N) * d.H, seq = step * d.T;
+      RnnBuffers& b = rnn_[i];
+      void *g, *h, *state, *dzo, *dho, *dpre;
+      if (!alloc(seq * sizeof(float), &g) || !alloc(seq * sizeof(float) + step * sizeof(float), &h) ||
+          !alloc(step * sizeof(float), &state) || !alloc(seq * sizeof(float), &dzo) ||
+          !alloc(seq * sizeof(float), &dho) || !alloc(seq * sizeof(float), &dpre))
+        return false;
+      b.g = static_cast<float*>(g), b.h = static_cast<float*>(h), b.state = static_cast<float*>(state);
+      b.dzo = static_cast<float*>(dzo), b.dho = static_cast<float*>(dho), b.dpre = static_cast<float*>(dpre);
+      if (cudaMemset(b.state, 0, step * sizeof(float)) != cudaSuccess) {  // the first call starts from h = 0
+        *err = "native producer: cudaMemset failed";
+        return false;
+      }
+      const size_t seq_splits = static_cast<size_t>(splits_of(d.T * d.N));
+      ws = std::max(ws, seq_splits * d.H * std::max(d.H, d.I));  // dW_hh, dW_ho and dW_xh
+      if (d.S > 0) {
+        void *z, *dz;
+        if (!alloc(step * sizeof(float), &z) || !alloc(step * sizeof(float), &dz)) return false;
+        b.z = static_cast<float*>(z), b.dz = static_cast<float*>(dz);
+        ws = std::max(ws, static_cast<size_t>(splits_of(d.N)) * d.H * d.S);
+      }
     } else if (op.kind == OpKind::kBatchNorm) {
       int n, c, hw;
       bn_dims(op, &n, &c, &hw);
@@ -1280,7 +1388,7 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
         ave_pool_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, pool_geom(op));
       return cudaGetLastError();
     case OpKind::kInnerProduct: {
-      const int B = static_cast<int>(op.in_shape[0]), N = static_cast<int>(op.out_shape[1]), K = ip_k(op);
+      const int B = ip_rows(op), N = static_cast<int>(op.out_shape.back()), K = ip_k(op);
       return gemm(DenseRM{x, K}, DenseCM{data_ + op.w_off, K},
                   StoreRM{y, op.b_off >= 0 ? data_ + op.b_off : nullptr, N}, B, N, K, K, s);
     }
@@ -1440,6 +1548,32 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
         embed_forward_kernel<1><<<grid_for(static_cast<int64_t>(M) * N), kThreads, 0, s>>>(x, w, b, y, M, N, K, status_);
       return cudaGetLastError();
     }
+    case OpKind::kRNN: {  // recurrent_layer.cpp Forward_cpu without expose_hidden, over rnn_layer.cpp's unrolled net
+      const RnnDims d = rnn_dims(op, plan_.tensor_count);
+      const RnnBuffers& b = rnn_[i];
+      const float* cont = act_[op.bottoms[1]];
+      const float* whh = data_ + op.rnn_off[Op::kWhh];
+      const size_t step = static_cast<size_t>(d.N) * d.H;
+      const int TN = d.T * d.N;
+      // g = x W_xh^T + b_h over every step, z = x_static W_xh_static^T, and h_{-1} = the carried state
+      cudaError_t e = gemm(DenseRM{x, d.I}, DenseCM{data_ + op.rnn_off[Op::kWxh], d.I},
+                           StoreRM{b.g, data_ + op.rnn_off[Op::kBh], d.H}, TN, d.H, d.I, d.I, s);
+      if (e == cudaSuccess && b.z)
+        e = gemm(DenseRM{act_[op.bottoms[2]], d.S}, DenseCM{data_ + op.rnn_off[Op::kWxhStatic], d.S},
+                 StoreRM{b.z, nullptr, d.H}, d.N, d.H, d.S, d.S, s);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(b.h, b.state, step * sizeof(float), cudaMemcpyDeviceToDevice, s);
+      // one launch per step: h_t from cont_t * h_{t-1}
+      for (int t = 0; t < d.T && e == cudaSuccess; ++t)
+        e = gemm(ContGather{b.h + t * step, cont + static_cast<size_t>(t) * d.N, d.H}, DenseCM{whh, d.H},
+                 RnnStep{b.g + t * step, b.z, b.h + (t + 1) * step, d.H}, d.N, d.H, d.H, d.H, s);
+      // the top o = tanh(h W_ho^T + b_o) over every step, and h_{T-1} carried to the next call
+      if (e == cudaSuccess)
+        e = gemm(DenseRM{b.h + step, d.H}, DenseCM{data_ + op.rnn_off[Op::kWho], d.H},
+                 StoreTanhRM{y, data_ + op.rnn_off[Op::kBo], d.H}, TN, d.H, d.H, d.H, s);
+      if (e == cudaSuccess)
+        e = cudaMemcpyAsync(b.state, b.h + d.T * step, step * sizeof(float), cudaMemcpyDeviceToDevice, s);
+      return e;
+    }
     default:
       return cudaErrorInvalidValue;
   }
@@ -1477,7 +1611,7 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
         ave_pool_backward_kernel<<<grid_for(nin), kThreads, 0, s>>>(dy, dx, pool_geom(op));
       return cudaGetLastError();
     case OpKind::kInnerProduct: {
-      const int B = static_cast<int>(op.in_shape[0]), N = static_cast<int>(op.out_shape[1]), K = ip_k(op);
+      const int B = ip_rows(op), N = static_cast<int>(op.out_shape.back()), K = ip_k(op);
       cudaError_t e = gemm(DenseCM{dy, N}, DenseRM{x, K}, StorePartial{workspace_, N, K}, N, K, B, split_chunk(B), s);
       if (e != cudaSuccess) return e;
       reduce_partials_kernel<<<grid_for(op.w_count), kThreads, 0, s>>>(workspace_, splits_of(B),
@@ -1637,6 +1771,59 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
                                                                                   diff_ + op.w_off, N, K);
       if (op.b_off >= 0) bias_grad_kernel<<<N, kThreads, 0, s>>>(dy, nin, N, 1, diff_ + op.b_off);
       return cudaGetLastError();
+    }
+    case OpKind::kRNN: {  // backpropagation through time inside this call; nothing crosses into the previous one
+      const RnnDims d = rnn_dims(op, plan_.tensor_count);
+      const RnnBuffers& b = rnn_[i];
+      const float* cont = act_[op.bottoms[1]];
+      const float* whh = data_ + op.rnn_off[Op::kWhh];
+      const size_t step = static_cast<size_t>(d.N) * d.H;
+      const int TN = d.T * d.N;
+      // the weight gradient C[M, N] = A B over K products, split in fixed chunks and added once into dst
+      auto weight_grad = [&](auto ga, auto gb, int M, int N, int K, float* dst) {
+        cudaError_t e = gemm(ga, gb, StorePartial{workspace_, M, N}, M, N, K, split_chunk(K), s);
+        if (e != cudaSuccess) return e;
+        reduce_partials_kernel<<<grid_for(static_cast<int64_t>(M) * N), kThreads, 0, s>>>(workspace_, splits_of(K),
+                                                                                          M * N, dst);
+        return cudaGetLastError();
+      };
+      // the output: dzo = dtop (1 - top^2), then W_ho, b_o and dho over every step
+      tanh_backward_kernel<<<grid_for(static_cast<int64_t>(TN) * d.H), kThreads, 0, s>>>(act_[op.out], dy, b.dzo,
+                                                                                        TN * d.H);
+      cudaError_t e = cudaGetLastError();
+      if (e == cudaSuccess)
+        e = weight_grad(DenseCM{b.dzo, d.H}, DenseRM{b.h + step, d.H}, d.H, d.H, TN, diff_ + op.rnn_off[Op::kWho]);
+      if (e != cudaSuccess) return e;
+      bias_grad_kernel<<<d.H, kThreads, 0, s>>>(b.dzo, TN, d.H, 1, diff_ + op.rnn_off[Op::kBo]);
+      if ((e = cudaGetLastError()) != cudaSuccess) return e;
+      e = gemm(DenseRM{b.dzo, d.H}, DenseRM{data_ + op.rnn_off[Op::kWho], d.H},
+               RnnOutGrad{b.dho, b.dpre, b.h + step, d.H, (d.T - 1) * d.N}, TN, d.H, d.H, d.H, s);
+      // one launch per step, t = T-1 .. 1: dpre_{t-1} from dpre_t (step 0's gradient at h_{-1} is not needed)
+      for (int t = d.T - 1; t >= 1 && e == cudaSuccess; --t)
+        e = gemm(DenseRM{b.dpre + t * step, d.H}, DenseRM{whh, d.H},
+                 RnnBackStep{cont + static_cast<size_t>(t) * d.N, b.dho + (t - 1) * step, b.h + t * step,
+                             b.dpre + (t - 1) * step, d.H},
+                 d.N, d.H, d.H, d.H, s);
+      // W_hh against hc_{t-1} = cont_t h_{t-1}, regathered; W_xh, b_h and dx over every step
+      if (e == cudaSuccess)
+        e = weight_grad(DenseCM{b.dpre, d.H}, ContGather{b.h, cont, d.H}, d.H, d.H, TN, diff_ + op.rnn_off[Op::kWhh]);
+      if (e == cudaSuccess)
+        e = weight_grad(DenseCM{b.dpre, d.H}, DenseRM{x, d.I}, d.H, d.I, TN, diff_ + op.rnn_off[Op::kWxh]);
+      if (e != cudaSuccess) return e;
+      bias_grad_kernel<<<d.H, kThreads, 0, s>>>(b.dpre, TN, d.H, 1, diff_ + op.rnn_off[Op::kBh]);
+      if ((e = cudaGetLastError()) == cudaSuccess && dx)
+        e = gemm(DenseRM{b.dpre, d.H}, DenseRM{data_ + op.rnn_off[Op::kWxh], d.I}, StoreRM{dx, nullptr, d.I}, TN, d.I,
+                 d.H, d.H, s);
+      if (e != cudaSuccess || !b.z) return e;
+      // x_static: its transform is read by every step, so its gradient is dpre summed over t in step order
+      sum_steps_kernel<<<grid_for(step), kThreads, 0, s>>>(b.dpre, d.T, static_cast<int>(step), b.dz);
+      const float* xs = act_[op.bottoms[2]];
+      if ((e = cudaGetLastError()) == cudaSuccess)
+        e = weight_grad(DenseCM{b.dz, d.H}, DenseRM{xs, d.S}, d.H, d.S, d.N, diff_ + op.rnn_off[Op::kWxhStatic]);
+      if (e == cudaSuccess && op.bottom_grad[2])
+        e = gemm(DenseRM{b.dz, d.H}, DenseRM{data_ + op.rnn_off[Op::kWxhStatic], d.S},
+                 StoreRM{grad_[op.bottoms[2]], nullptr, d.S}, d.N, d.S, d.H, d.H, s);
+      return e;
     }
     default:
       return cudaErrorInvalidValue;

@@ -1,7 +1,8 @@
 // native_producer.hpp -- the built-in gradient producer (Net::ForwardBackward for the TRAIN phase of the LeNet,
 // CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, least-squares regression nets,
 // residual nets built of Split, Eltwise and Scale, autoencoders built of Flatten, Deconvolution and
-// SigmoidCrossEntropyLoss, and embedding nets that read token ids through Embed and Reshape; DESIGN.md section 14).
+// SigmoidCrossEntropyLoss, embedding nets that read token ids through Embed and Reshape, and recurrent nets built of
+// RNN layers over time-major inputs; DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -27,7 +28,7 @@ enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
   kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale, kDeconv, kFlatten, kSigmoidCrossEntropyLoss,
   kTanH, kELU, kAbsVal, kBNLL, kPower, kExp, kLog, kThreshold, kPReLU, kSoftmax, kMultinomialLogisticLoss, kHingeLoss,
-  kEmbed, kReshape,
+  kEmbed, kReshape, kRNN,
   kCount  // the number of kinds (Plan::text names each)
 };
 
@@ -101,6 +102,11 @@ struct Op {
   // Embed: the vocabulary size K (w_off is the [K, num_output] table, num_output = out_shape.back()); the bottom holds
   // M = count(bottom) ids
   int64_t input_dim = 0;
+  // RNN: x is [T, N, ...] (in_shape), the top [T, N, H]; bottoms[1] is cont [T, N] (the label-like bottom) and
+  // bottoms[2], when there, x_static [N, ...].  The flat offsets of its blobs, by role: W_xh, b_h, W_xh_static (-1
+  // without x_static), W_hh, W_ho, b_o.
+  enum { kWxh, kBh, kWxhStatic, kWhh, kWho, kBo, kRnnBlobs };
+  int64_t rnn_off[kRnnBlobs] = {-1, -1, -1, -1, -1, -1};
 };
 
 struct Plan {
@@ -167,6 +173,15 @@ class NativeProducer {
   std::vector<void*> op_aux_;             // per op: MAX pool / Eltwise MAX argmax (int32), fused block index (uint8),
                                           // BN save
   std::vector<float*> op_z_, op_dz_;      // fused block: conv output without bias and its gradient
+  // per op, an RNN's buffers (null for other ops), all [rows, H] with rows as named: g = x W_xh^T + b_h (T N), z =
+  // x_static W_xh_static^T (N), h = h_{-1} .. h_{T-1} ((T + 1) N), state = the hidden state carried from call to call
+  // (N; zero at creation, h_{T-1} after every forward), dzo = the output tanh's input gradient (T N), dho = its
+  // gradient at h (T N), dpre = the hidden tanh's input gradient (T N), dz = dpre summed over t (N)
+  struct RnnBuffers {
+    float *g = nullptr, *z = nullptr, *h = nullptr, *state = nullptr, *dzo = nullptr, *dho = nullptr,
+          *dpre = nullptr, *dz = nullptr;
+  };
+  std::vector<RnnBuffers> rnn_;
   cudaEvent_t done_ = nullptr;            // recorded at the end of every call: the destructor waits for it
   float* workspace_ = nullptr;            // split-K partials, bias partials, BatchNorm scratch, the sigmoid
                                           // cross-entropy's per-block partials, Embed's id grouping (int32; ops run

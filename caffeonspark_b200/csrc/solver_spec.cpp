@@ -346,9 +346,11 @@ void data_top(Layer& L, size_t i, Shape s, const Node* transform_param) {
   L.spec->inputs.push_back(in);
 }
 
-void data_input(Layer& L, const Shape& s) {  // the first data layer to call it gives the net's batch and input shape
+// The first data layer to call it gives the net's batch and input shape; the batch is s[0] unless given (a transposed
+// CoSData top is [channels, batch_size]).
+void data_input(Layer& L, const Shape& s, int64_t batch = -1) {
   if (!L.first_data) return;
-  L.spec->batch_size = static_cast<int>(s[0]);
+  L.spec->batch_size = static_cast<int>(batch >= 0 ? batch : s[0]);
   L.spec->input_shape.assign(s.begin(), s.end());
   L.first_data = false;
 }
@@ -368,18 +370,25 @@ bool cos_data(Layer& L, std::vector<Shape>*) {
   const Node* p = L.node.first("cos_data_param");
   if (!p) { *L.err = "CoSData layer without cos_data_param"; return false; }
   auto tb = p->all("top");
+  const int64_t batch = p->integer("batch_size", 0);
   for (size_t i = 0; i < L.rec.tops.size(); ++i) {
-    Shape s{p->integer("batch_size", 0)};
+    Shape s{batch};
     if (i < tb.size()) {
       int64_t c = tb[i]->integer("out_channels", 0), h = tb[i]->integer("out_height", 0), w = tb[i]->integer("out_width", 0);
       if (!c) c = tb[i]->integer("channels", 0);
       if (!h) h = tb[i]->integer("height", 0);
       if (!w) w = tb[i]->integer("width", 0);
-      Shape full{c, h, w};
-      for (int64_t a = 0; a < tb[i]->integer("sample_num_axes", 3) && a < 3; ++a) s.push_back(full[a] ? full[a] : 1);
+      const int64_t axes = tb[i]->integer("sample_num_axes", 3);
+      if (tb[i]->boolean("transpose", false)) {  // cos_data_layer.cpp: time-major [channels, batch_size]
+        if (axes != 1) return L.refuse("each sample must be a 1d-vector if transpose is used");
+        s = {c, batch};
+      } else {
+        Shape full{c, h, w};
+        for (int64_t a = 0; a < axes && a < 3; ++a) s.push_back(full[a] ? full[a] : 1);
+      }
     }
     data_top(L, i, s, i < tb.size() ? tb[i]->first("transform_param") : nullptr);
-    if (i == 0) data_input(L, s);
+    if (i == 0) data_input(L, s, batch);
   }
   return true;
 }
@@ -690,6 +699,49 @@ bool reshape(Layer& L, std::vector<Shape>*) {  // reshape_layer.cpp LayerSetUp a
   return true;
 }
 
+// recurrent_layer.cpp LayerSetUp (after Layer::CheckBlobCounts) and rnn_layer.cpp FillUnrolledNet, with their CHECK
+// messages.  The learnable blobs are the unrolled net's, in the order of their first use there: W_xh [H, I], b_h [H],
+// W_xh_static [H, S] (with x_static), W_hh [H, H], W_ho [H, H], b_o [H], with I = count(x, 2) and S = count(x_static, 1).
+bool rnn(Layer& L, std::vector<Shape>* params) {
+  const Node* p = L.node.first("recurrent_param");
+  NetLayer& r = L.rec;
+  r.num_output = p ? p->integer("num_output", 0) : 0;
+  r.expose_hidden = p && p->boolean("expose_hidden", false);
+  const size_t least = 2 + (r.expose_hidden ? 1 : 0), tops = 1 + (r.expose_hidden ? 1 : 0);
+  const std::string type = r.type + " Layer ";
+  if (r.bottoms.size() < least)
+    return L.refuse(type + "takes at least " + std::to_string(least) + " bottom blob(s) as input.");
+  if (r.bottoms.size() > least + 1)
+    return L.refuse(type + "takes at most " + std::to_string(least + 1) + " bottom blob(s) as input.");
+  if (r.tops.size() != tops) return L.refuse(type + "produces " + std::to_string(tops) + " top blob(s) as output.");
+  Shape x, cont, xs;
+  if (!L.bottom(0, &x) || !L.bottom(1, &cont)) return false;
+  if (x.size() < 2) return L.refuse("bottom[0] must have at least 2 axes -- (#timesteps, #streams, ...)");
+  if (cont.size() != 2) return L.refuse("bottom[1] must have exactly 2 axes -- (#timesteps, #streams)");
+  auto eq = [&](const char* what, int64_t a, int64_t b) {
+    return a == b || L.refuse(std::string("Check failed: ") + what + " (" + std::to_string(a) + " vs. " +
+                              std::to_string(b) + ")");
+  };
+  if (!eq("T_ == bottom[1]->shape(0)", x[0], cont[0]) || !eq("N_ == bottom[1]->shape(1)", x[1], cont[1])) return false;
+  r.static_input = r.bottoms.size() > least;
+  if (r.static_input) {
+    if (!L.bottom(2, &xs)) return false;
+    if (xs.empty()) return L.refuse("Check failed: bottom[2]->num_axes() >= 1 (0 vs. 1)");
+    if (!eq("N_ == bottom[2]->shape(0)", x[1], xs[0])) return false;
+  }
+  if (r.num_output <= 0) return L.refuse("num_output must be positive");
+  const int64_t H = r.num_output;
+  r.weight_filler = filler(p->first("weight_filler")), r.bias_filler = filler(p->first("bias_filler"));  // p: H > 0
+  *params = {{H, shape_count(x, 2)}, {H}};
+  r.bias_param = {false, true};
+  if (r.static_input) params->push_back({H, shape_count(xs, 1)}), r.bias_param.push_back(false);
+  params->insert(params->end(), {{H, H}, {H, H}, {H}});
+  r.bias_param.insert(r.bias_param.end(), {false, false, true});
+  L.set_top(0, {x[0], x[1], H});
+  if (r.expose_hidden) L.set_top(1, {1, x[1], H});
+  return true;
+}
+
 bool concat(Layer& L, std::vector<Shape>*) {  // concat_layer.cpp LayerSetUp and Reshape, with its CHECK messages
   Shape out;
   if (!L.bottom(0, &out)) return false;
@@ -822,7 +874,7 @@ const struct { const char* type; Rule rule; } kRules[] = {
     {"Softmax", same_shape}, {"Power", same_shape}, {"AbsVal", same_shape}, {"BNLL", same_shape}, {"ELU", same_shape},
     {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape}, {"PReLU", prelu},
     {"Split", split}, {"Eltwise", eltwise}, {"Scale", scale}, {"Flatten", flatten}, {"Concat", concat},
-    {"Embed", embed}, {"Reshape", reshape},
+    {"Embed", embed}, {"Reshape", reshape}, {"RNN", rnn},
     {"SoftmaxWithLoss", softmax_loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
     {"HingeLoss", loss}, {"MultinomialLogisticLoss", loss},
     {"BatchNorm", batch_norm}, {"Slice", slice}, {"ContrastiveLoss", contrastive_loss}, {"Silence", silence},

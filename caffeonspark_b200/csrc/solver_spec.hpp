@@ -76,7 +76,14 @@ struct NetLayer {
   // Embed (caffe.proto EmbedParameter): the vocabulary size; num_output, bias_term (default true) and the fillers are
   // the fields above
   int64_t input_dim = 0;
+  // RNN (caffe.proto RecurrentParameter): num_output is H; bottoms x, cont and the optional x_static (a fourth bottom
+  // and a second top with expose_hidden, which the parser lays out and the engine refuses)
+  bool expose_hidden = false;
+  bool static_input = false;
   FillerSpec weight_filler, bias_filler;
+  // per param: whether bias_filler fills it rather than weight_filler.  Empty for the layers whose params are a
+  // weight and then (with bias_term) a bias.
+  std::vector<bool> bias_param;
 };
 
 // A later use of a named param (net.cpp AppendParam): it reads the owner's data and adds its gradient into the owner's

@@ -600,3 +600,99 @@ def ngram_lm_module():
     s = NGRAM_LM
     return nn.Sequential(embed_module(s["vocab"], s["dim"]), nn.Flatten(), nn.Linear(s["tokens"] * s["dim"], s["hidden"]),
                          nn.Tanh(), nn.Linear(s["hidden"], s["vocab"]))
+
+
+# tests/golden/configs/rnn_lm_train_test.prototxt: time-major sentences of 20 tokens in 32 streams, Embed 2000 x 128 (no
+# bias), RNN of 256 units, InnerProduct 256 -> 2000 on axis 2.  256,000 + (32,768 + 256 + 65,536 + 65,536 + 256) +
+# (512,000 + 2,000) = 934,352 parameters in 8 blobs.
+RNN_LM = dict(steps=20, batch=32, vocab=2000, dim=128, hidden=256)
+RNN_LM_PARAM_COUNT = 934352
+# tests/golden/configs/rnn_caption_train_test.prototxt: a 1x28x28 image through LeNet's conv/pool stack and ip1 (256) +
+# ReLU into x_static of rnn1 (128 units, over Embed 1000 x 64 of the caption), rnn2 (128) over rnn1, both reading one
+# cont, InnerProduct 128 -> 1000 on axis 2; 12 timesteps of 16 streams.  547,018 parameters in 20 blobs.
+RNN_CAPTION = dict(steps=12, batch=16, vocab=1000, dim=64, hidden=128, image=256)
+RNN_CAPTION_PARAM_COUNT = 547018
+
+
+def rnn_module(input_dim, num_output, static_dim=0):
+    """Caffe's RNN layer (rnn_layer.cpp's unrolled net, without expose_hidden) as a PyTorch module, parameters in its
+    blobs' order: W_xh [H, I], b_h [H], W_xh_static [H, S] (with static_dim), W_hh [H, H], W_ho [H, H], b_o [H].
+    forward(x [T, N, ...], cont [T, N], h0 [N, H], x_static [N, ...] or None) -> (o [T, N, H], h_{T-1} [N, H]), with
+    h_t = tanh(W_hh (cont_t h_{t-1}) + W_xh x_t + b_h (+ W_xh_static x_static)) and o_t = tanh(W_ho h_t + b_o).  The
+    caller carries h_{T-1} into the next call's h0, detached: no gradient crosses calls."""
+    import torch
+    import torch.nn as nn
+
+    class RNN(nn.Module):
+        def __init__(self):
+            super().__init__()
+            H = num_output
+            self.w_xh = nn.Parameter(torch.zeros(H, input_dim))
+            self.b_h = nn.Parameter(torch.zeros(H))
+            self.w_xh_static = nn.Parameter(torch.zeros(H, static_dim)) if static_dim else None
+            self.w_hh = nn.Parameter(torch.zeros(H, H))
+            self.w_ho = nn.Parameter(torch.zeros(H, H))
+            self.b_o = nn.Parameter(torch.zeros(H))
+
+        def forward(self, x, cont, h0, x_static=None):
+            g = x.flatten(2) @ self.w_xh.t() + self.b_h
+            z = x_static.flatten(1) @ self.w_xh_static.t() if self.w_xh_static is not None else None
+            h, hs = h0, []
+            for t in range(x.shape[0]):
+                a = (cont[t].unsqueeze(1) * h) @ self.w_hh.t() + g[t]
+                h = torch.tanh(a + z if z is not None else a)
+                hs.append(h)
+            hs = torch.stack(hs)
+            return torch.tanh(hs @ self.w_ho.t() + self.b_o), h
+
+    return RNN()
+
+
+def rnn_lm_module():
+    """The RNN language model fixture as one PyTorch module, parameters in learnable_params() order.
+    forward(tokens [T, N], cont [T, N], h0 [N, 256]) -> (scores [T, N, 2000], h_{T-1})."""
+    import torch.nn as nn
+    s = RNN_LM
+
+    class RNNLM(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.embed = embed_module(s["vocab"], s["dim"], bias=False)
+            self.rnn = rnn_module(s["dim"], s["hidden"])
+            self.predict = nn.Linear(s["hidden"], s["vocab"])
+
+        def forward(self, tokens, cont, h0):
+            o, h = self.rnn(self.embed(tokens), cont, h0)
+            return self.predict(o), h
+
+    return RNNLM()
+
+
+def rnn_caption_module():
+    """The miniature LRCN fixture as one PyTorch module, parameters in learnable_params() order.
+    forward(image [N, 1, 28, 28], cont [T, N], tokens [T, N], (h1, h2) [N, 128] each) -> (scores [T, N, 1000],
+    (h1_{T-1}, h2_{T-1}))."""
+    import torch
+    import torch.nn as nn
+    s = RNN_CAPTION
+
+    class RNNCaption(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.conv1 = nn.Conv2d(1, 20, 5)
+            self.conv2 = nn.Conv2d(20, 50, 5)
+            self.ip1 = nn.Linear(800, s["image"])
+            self.embed = embed_module(s["vocab"], s["dim"], bias=False)
+            self.rnn1 = rnn_module(s["dim"], s["hidden"], s["image"])
+            self.rnn2 = rnn_module(s["hidden"], s["hidden"])
+            self.predict = nn.Linear(s["hidden"], s["vocab"])
+
+        def forward(self, image, cont, tokens, h0):
+            f = nn.functional.max_pool2d(self.conv1(image), 2, 2)
+            f = nn.functional.max_pool2d(self.conv2(f), 2, 2)
+            f = torch.relu(self.ip1(f.flatten(1)))
+            o1, h1 = self.rnn1(self.embed(tokens), cont, h0[0], f)
+            o2, h2 = self.rnn2(o1, cont, h0[1])
+            return self.predict(o2), (h1, h2)
+
+    return RNNCaption()

@@ -254,8 +254,10 @@ COS_API int cos_net_set_forward_backward(cos_net* net, cos_forward_backward_fn f
 
 /* The built-in gradient producer (DESIGN.md section 14): a forward/backward engine built from the TRAIN phase of a
  * Caffe net prototxt, on this library's own sm_90a kernels.  It runs MemoryData / CoSData / Input, Convolution (group
- * 1, dilation 1), Pooling (MAX, AVE), InnerProduct (axis 1), ReLU, Sigmoid, BatchNorm, LRN (WITHIN_CHANNEL), Slice,
- * Embed over fp32 token ids (a CoSData INT_ARRAY top) and Reshape, the other layers DESIGN.md section 14 lists, and one
+ * 1, dilation 1), Pooling (MAX, AVE), InnerProduct (any axis), ReLU, Sigmoid, BatchNorm, LRN (WITHIN_CHANNEL), Slice,
+ * Embed over fp32 token ids (a CoSData INT_ARRAY top), Reshape, RNN (without expose_hidden; its hidden state is kept
+ * per engine from call to call, zero at first, and not snapshotted) over time-major CoSData tops (transpose: true),
+ * the other layers DESIGN.md section 14 lists, and one
  * loss layer, SoftmaxWithLoss or ContrastiveLoss among them (default normalisation); Accuracy and Silence are skipped.
  * Named params are shared as in Caffe.  Every other layer, and loss_param or an unknown filler type, is refused with an
  * error naming the layer.  Every use of a learnable blob adds its gradient into diff_ once per call; results are
