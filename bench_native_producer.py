@@ -9,7 +9,9 @@ scoring its reconstruction against its input with SigmoidCrossEntropyLoss, timed
 nets.conv_autoencoder_module; the TanH LeNet fixture b64, whose head is Softmax + MultinomialLogisticLoss, and the
 PReLU CIFAR-10-quick fixture b100, timed against nets.lenet_tanh_module and nets.cifar10_quick_prelu_module; the two
 embedding fixtures, whose staged inputs are token ids: the sentence classifier text_cnn b50 of 32 ids and the n-gram
-language model ngram_lm b128 of 4 ids, timed against nets.text_cnn_module and nets.ngram_lm_module).  For each, one process times the native engine, the PyTorch module with TF32 off and with
+language model ngram_lm b128 of 4 ids, timed against nets.text_cnn_module and nets.ngram_lm_module; and the two MVN
+fixtures: cifar10_quick_mvn b100 and the layer-normalised RNN language model rnn_lm_ln of 20 steps x 32 streams, timed
+against nets.cifar10_quick_mvn_module and nets.rnn_lm_ln_module, whose MVNs run the same native kernels).  For each, one process times the native engine, the PyTorch module with TF32 off and with
 TF32 on (cuDNN's default, here applied to matmuls too), alternating the three in every round; each sample is CUDA events around `--iters`
 back-to-back forward/backward calls on one stream after `--warmup` untimed ones.  Prints one JSON line per
 workload with median / min / max ms per call and images/s, and the card's name and power limit.
@@ -31,9 +33,10 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 WORKLOADS = ("lenet", "cifar10_quick", "cifar10_full_bn", "cifar10_full", "mnist_siamese", "cifar10_resnet20",
-             "mnist_autoencoder", "mnist_conv_autoencoder", "lenet_tanh", "cifar10_quick_prelu", "text_cnn", "ngram_lm")
+             "mnist_autoencoder", "mnist_conv_autoencoder", "lenet_tanh", "cifar10_quick_prelu", "text_cnn", "ngram_lm",
+             "cifar10_quick_mvn", "rnn_lm_ln")
 FIXTURES = ("cifar10_resnet20", "mnist_autoencoder", "mnist_conv_autoencoder", "lenet_tanh",
-            "cifar10_quick_prelu", "text_cnn", "ngram_lm")  # nets kept under tests/golden/configs
+            "cifar10_quick_prelu", "text_cnn", "ngram_lm", "cifar10_quick_mvn", "rnn_lm_ln")  # nets kept under tests/golden/configs
 FP32_PEAK = 67e12  # H100 SXM data sheet, dense FP32, at up to 700 W
 
 
@@ -151,14 +154,20 @@ def main():
         net.use_native_producer(fill_weights=False)
         net.fill("data", 1, 0, 0.05)
         torch.cuda.synchronize()
-        text = name in ("text_cnn", "ngram_lm")
+        text, lm = name in ("text_cnn", "ngram_lm"), name == "rnn_lm_ln"
         spec = (nets.RESNET20 if resnet else None if siamese else nets.AUTOENCODER if name == "mnist_autoencoder"
                 else nets.CONV_AUTOENCODER if autoencoder else nets.LENET_TANH if name == "lenet_tanh"
                 else nets.CIFAR10_QUICK_PRELU if name == "cifar10_quick_prelu" else nets.TEXT_CNN if name == "text_cnn"
-                else nets.NGRAM_LM if name == "ngram_lm" else nets.NETS[name])
+                else nets.NGRAM_LM if name == "ngram_lm" else nets.CIFAR10_QUICK_MVN if name == "cifar10_quick_mvn"
+                else nets.RNN_LM if lm else nets.NETS[name])
         batch = 64 if siamese else spec["batch"]
         rng = np.random.RandomState(0)
-        if text:  # token ids (Zipf-skewed, as words are) and a class or next-token label
+        if lm:  # time-major sentences [steps, batch]: cont (0 where a sentence starts), tokens and next tokens
+            ids = (rng.zipf(1.2, (spec["steps"] + 1, batch)) - 1) % spec["vocab"]
+            cont = torch.from_numpy((rng.rand(spec["steps"], batch) > 0.15).astype(np.float32)).cuda()
+            x = torch.from_numpy(ids[:-1].astype(np.float32)).cuda()
+            y = torch.from_numpy(ids[1:].astype(np.float32)).cuda()
+        elif text:  # token ids (Zipf-skewed, as words are) and a class or next-token label
             ids = (rng.zipf(1.2, (batch, spec["tokens"])) - 1) % spec["vocab"]
             x = torch.from_numpy(ids.astype(np.float32)).cuda()
             y = torch.from_numpy(rng.randint(0, spec.get("classes", spec["vocab"]), batch).astype(np.float32)).cuda()
@@ -173,7 +182,8 @@ def main():
         torch.cuda.synchronize()
         torch.cuda.set_stream(stream)
 
-        inputs = [x] if autoencoder else [x, y]  # an autoencoder's one staged input is its target too
+        # an autoencoder's one staged input is its target too
+        inputs = [x] if autoencoder else [cont, x, y] if lm else [x, y]
 
         def native():
             assert net.forward_backward(inputs, loss.data_ptr(), stream=stream.cuda_stream), net.last_error()
@@ -183,6 +193,8 @@ def main():
                   else nets.conv_autoencoder_module() if autoencoder else nets.lenet_tanh_module() if name == "lenet_tanh"
                   else nets.cifar10_quick_prelu_module() if name == "cifar10_quick_prelu"
                   else nets.text_cnn_module() if name == "text_cnn" else nets.ngram_lm_module() if name == "ngram_lm"
+                  else nets.cifar10_quick_mvn_module() if name == "cifar10_quick_mvn"
+                  else nets.rnn_lm_ln_module() if lm
                   else nets.torch_module(name)).cuda()
         with torch.no_grad():
             w, off = net.data().clone(), 0
@@ -198,6 +210,11 @@ def main():
                 return
             if autoencoder:
                 nets.sigmoid_cross_entropy_loss(module(x), x).backward()
+                return
+            if lm:  # each call from a zero hidden state, as the engine's first call
+                h0 = torch.zeros(batch, spec["hidden"], device="cuda")
+                scores, _ = module(x.long(), cont, h0)
+                F.cross_entropy(scores.reshape(-1, spec["vocab"]), ylong.reshape(-1)).backward()
                 return
             out = module(x)
             if name == "lenet_tanh":

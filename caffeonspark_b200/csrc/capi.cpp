@@ -18,6 +18,7 @@
 #include "caffe_net.hpp"
 #include "caffe_proto_io.hpp"
 #include "hdf5_io.hpp"
+#include "mvn.hpp"
 #include "native_producer.hpp"
 #include "peer_adapter.hpp"
 #include "solver_spec.hpp"
@@ -735,6 +736,37 @@ int cos_batch_norm_backward(const float* x, const float* dy, float* dx, const fl
   return launched(cosb::batch_norm_backward(x, dy, dx, save, workspace, num, channels, height, width,
                                             use_global_stats != 0, eps, static_cast<cudaStream_t>(cuda_stream)),
                   "cos_batch_norm_backward");
+}
+
+namespace {
+const char* mvn_args(const void* a, const void* b, const void* c, const float* stats, const float* workspace,
+                     long long rows, long long dim) {
+  if (!a || !b || !c || !stats) return "NULL tensor";
+  if (rows < 1 || dim < 1 || rows > ((1ll << 31) - 1) / dim) return "bad shape";  // rows * dim < 2^31
+  if (!workspace && cosb::mvn_workspace_floats(rows, dim) > 0) return "NULL workspace";
+  return nullptr;
+}
+}  // namespace
+
+long long cos_mvn_workspace_floats(long long rows, long long dim) {
+  return rows < 1 || dim < 1 ? 0 : static_cast<long long>(cosb::mvn_workspace_floats(rows, dim));
+}
+
+int cos_mvn_forward(const float* x, float* y, float* stats, float* workspace, long long rows, long long dim,
+                    int normalize_variance, float eps, void* cuda_stream) {
+  if (const char* e = mvn_args(x, y, y, stats, workspace, rows, dim)) return fail(e);
+  if (!std::isfinite(eps)) return fail("MVN needs a finite eps");
+  return launched(cosb::mvn_forward(x, y, stats, workspace, rows, dim, normalize_variance != 0, eps,
+                                    static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_mvn_forward");
+}
+
+int cos_mvn_backward(const float* y, const float* dy, float* dx, float* stats, float* workspace, long long rows,
+                     long long dim, int normalize_variance, void* cuda_stream) {
+  if (const char* e = mvn_args(y, dy, dx, stats, workspace, rows, dim)) return fail(e);
+  return launched(cosb::mvn_backward(y, dy, dx, stats, workspace, rows, dim, normalize_variance != 0,
+                                     static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_mvn_backward");
 }
 
 int cos_batch_norm_forward_bf16(const uint16_t* x, uint16_t* y, float* mean_blob, float* var_blob, float* scale_blob,

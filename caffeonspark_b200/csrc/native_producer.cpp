@@ -135,6 +135,7 @@ const LayerType kLayerTypes[] = {
     // x, cont and the optional x_static (the parser checked the count); cont is read, never differentiated, so two
     // RNNs may read one cont blob
     {"RNN", OpKind::kRNN, -1, false, 1, "cont"},
+    {"MVN", OpKind::kMVN},
 };
 
 // Plan::text's name of each OpKind
@@ -143,7 +144,7 @@ const char* const kKindNames[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling
                                   "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale", "Deconvolution", "Flatten",
                                   "SigmoidCrossEntropyLoss", "TanH", "ELU", "AbsVal", "BNLL", "Power", "Exp", "Log",
                                   "Threshold", "PReLU", "Softmax", "MultinomialLogisticLoss", "HingeLoss",
-                                  "Embed", "Reshape", "RNN"};
+                                  "Embed", "Reshape", "RNN", "MVN"};
 static_assert(std::size(kKindNames) == static_cast<size_t>(OpKind::kCount), "one name per OpKind");
 
 // LossLayer::Reshape's check, then multinomial_logistic_loss_layer.cpp's: the label holds one value per item, with
@@ -530,6 +531,14 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         op.rnn_off[roles[j]] = P.blob_off[L.blobs[j]];
         if (!L.shared[j]) P.blob_filler[L.blobs[j]] = L.bias_param[j] ? L.bias_filler : L.weight_filler;
       }
+    } else if (op.kind == OpKind::kMVN) {  // mvn_layer.cpp; the parser gave the top the bottom's legacy 4-D shape
+      // The top gets storage of its own even when top == bottom, unlike Caffe: its in-place Backward_gpu overwrites
+      // top_diff with y * dy and then sums that again as if it were dy (DESIGN.md section 14)
+      op.normalize_variance = L.normalize_variance;
+      op.across_channels = L.across_channels;
+      op.eps = L.eps;
+      op.mvn_rows = op.out_shape[0] * (L.across_channels ? 1 : op.out_shape[1]);
+      op.mvn_dim = shape_count(op.out_shape) / op.mvn_rows;
     } else if (op.kind == OpKind::kBatchNorm) {
       if (!op.shares.empty()) {
         *err = why(L, "shared BatchNorm statistics are not supported");
@@ -680,6 +689,11 @@ std::string Plan::text() const {
       if (op.bottoms.size() > 2) os << " static=" << op.bottoms[2];
       for (int r = 0; r < Op::kRnnBlobs; ++r)
         if (op.rnn_off[r] >= 0) os << " " << roles[r] << "=" << op.rnn_off[r];
+    }
+    if (op.kind == OpKind::kMVN) {
+      os << " rows=" << op.mvn_rows << " dim=" << op.mvn_dim << " eps=" << op.eps;
+      if (op.across_channels) os << " across";
+      if (!op.normalize_variance) os << " mean-only";
     }
     if (op.w_off >= 0 && op.kind != OpKind::kBatchNorm) os << " w=" << op.w_off << ":" << op.w_count;
     if (op.b_off >= 0) os << " b=" << op.b_off << ":" << op.b_count;

@@ -17,6 +17,7 @@
 #include "batch_norm.hpp"
 #include "caffe_layers.hpp"
 #include "fused_sync_sgd.hpp"
+#include "mvn.hpp"
 #include "native_producer.hpp"
 
 namespace cosb {
@@ -1264,6 +1265,9 @@ bool NativeProducer::allocate(std::string* err) {
       bn_dims(op, &n, &c, &hw);
       if (!alloc(2 * static_cast<size_t>(c) * sizeof(float), &op_aux_[i])) return false;
       ws = std::max(ws, bn_workspace_floats(n, c));
+    } else if (op.kind == OpKind::kMVN) {  // the per-row statistics, and the long rows' chunk partials
+      if (!alloc(5 * static_cast<size_t>(op.mvn_rows) * sizeof(float), &op_aux_[i])) return false;
+      ws = std::max(ws, mvn_workspace_floats(op.mvn_rows, op.mvn_dim));
     } else if (op.kind == OpKind::kSigmoidCrossEntropyLoss || op.kind == OpKind::kHingeLoss) {
       ws = std::max(ws, static_cast<size_t>(grid_for(plan_.tensor_count[op.bottoms[0]])));  // the per-block partials
     } else if (op.kind == OpKind::kPReLU) {
@@ -1405,6 +1409,9 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
       return batch_norm_forward(x, y, m, m + c, m + 2 * c, static_cast<float*>(op_aux_[i]), workspace_, bn, c, hw, 1,
                                 op.global_stats, op.fraction, op.eps, s);
     }
+    case OpKind::kMVN:
+      return mvn_forward(x, y, static_cast<float*>(op_aux_[i]), workspace_, op.mvn_rows, op.mvn_dim,
+                         op.normalize_variance, op.eps, s);
     case OpKind::kSlice:
       slice_copy_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, n, slice_span(op, op.out_shape), slice_span(op, op.in_shape),
                                                          op.slice_begin * slice_inner(op), false);
@@ -1635,6 +1642,10 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
       return batch_norm_backward(x, dy, dx, static_cast<const float*>(op_aux_[i]), workspace_, bn, c, hw, 1,
                                  op.global_stats, op.eps, s);
     }
+    case OpKind::kMVN:  // reads its own top y, not x
+      if (!dx) return cudaSuccess;
+      return mvn_backward(act_[op.out], dy, dx, static_cast<float*>(op_aux_[i]), workspace_, op.mvn_rows, op.mvn_dim,
+                          op.normalize_variance, s);
     case OpKind::kLRNWithin:
       if (!dx) return cudaSuccess;
       return lrn_within_backward(x, dy, dx, static_cast<int>(op.in_shape[0]), static_cast<int>(op.in_shape[1]),

@@ -1,8 +1,8 @@
 // native_producer.hpp -- the built-in gradient producer (Net::ForwardBackward for the TRAIN phase of the LeNet,
 // CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, least-squares regression nets,
 // residual nets built of Split, Eltwise and Scale, autoencoders built of Flatten, Deconvolution and
-// SigmoidCrossEntropyLoss, embedding nets that read token ids through Embed and Reshape, and recurrent nets built of
-// RNN layers over time-major inputs; DESIGN.md section 14).
+// SigmoidCrossEntropyLoss, embedding nets that read token ids through Embed and Reshape, recurrent nets built of
+// RNN layers over time-major inputs, and nets normalised by MVN; DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -28,7 +28,7 @@ enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
   kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale, kDeconv, kFlatten, kSigmoidCrossEntropyLoss,
   kTanH, kELU, kAbsVal, kBNLL, kPower, kExp, kLog, kThreshold, kPReLU, kSoftmax, kMultinomialLogisticLoss, kHingeLoss,
-  kEmbed, kReshape, kRNN,
+  kEmbed, kReshape, kRNN, kMVN,
   kCount  // the number of kinds (Plan::text names each)
 };
 
@@ -107,6 +107,10 @@ struct Op {
   // without x_static), W_hh, W_ho, b_o.
   enum { kWxh, kBh, kWxhStatic, kWhh, kWho, kBo, kRnnBlobs };
   int64_t rnn_off[kRnnBlobs] = {-1, -1, -1, -1, -1, -1};
+  // MVN: mvn_rows contiguous rows of mvn_dim elements each (num * channels rows, or num with across_channels), each
+  // normalised on its own; eps is added to the standard deviation.  Mean-only without normalize_variance.
+  int64_t mvn_rows = 0, mvn_dim = 0;
+  bool normalize_variance = true, across_channels = false;
 };
 
 struct Plan {
@@ -171,7 +175,7 @@ class NativeProducer {
   int* status_;
   std::vector<float*> act_, grad_;        // per tensor id (staged inputs: act_ is the caller's buffer, set per call)
   std::vector<void*> op_aux_;             // per op: MAX pool / Eltwise MAX argmax (int32), fused block index (uint8),
-                                          // BN save
+                                          // BN save, MVN's per-row statistics (mvn.hpp)
   std::vector<float*> op_z_, op_dz_;      // fused block: conv output without bias and its gradient
   // per op, an RNN's buffers (null for other ops), all [rows, H] with rows as named: g = x W_xh^T + b_h (T N), z =
   // x_static W_xh_static^T (N), h = h_{-1} .. h_{T-1} ((T + 1) N), state = the hidden state carried from call to call
@@ -184,8 +188,8 @@ class NativeProducer {
   std::vector<RnnBuffers> rnn_;
   cudaEvent_t done_ = nullptr;            // recorded at the end of every call: the destructor waits for it
   float* workspace_ = nullptr;            // split-K partials, bias partials, BatchNorm scratch, the sigmoid
-                                          // cross-entropy's per-block partials, Embed's id grouping (int32; ops run
-                                          // in order)
+                                          // cross-entropy's per-block partials, Embed's id grouping (int32), MVN's
+                                          // chunk partials (ops run in order)
   size_t workspace_floats_ = 0;
   std::vector<void*> allocations_;
 };

@@ -785,6 +785,28 @@ bool batch_norm(Layer& L, std::vector<Shape>* params) {
   return true;
 }
 
+// mvn_layer.cpp Reshape: the top is the bottom's legacy 4-D shape (num, channels, height, width), with Blob::LegacyShape's
+// CHECK; a zero dimension would make Forward divide by a zero count, so it is refused too
+bool mvn(Layer& L, std::vector<Shape>*) {
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  if (in.size() > 4) return L.refuse("Cannot use legacy accessors on Blobs with > 4 axes.");
+  Shape top(4, 1);
+  for (size_t a = 0; a < in.size(); ++a) {
+    if (in[a] == 0) return L.refuse("a bottom of shape " + shape_text(in) + " has no elements to normalise");
+    top[a] = in[a];
+  }
+  L.set_tops(top);
+  NetLayer& r = L.rec;
+  r.eps = 1e-9f;
+  if (const Node* p = L.node.first("mvn_param")) {
+    r.normalize_variance = p->boolean("normalize_variance", true);
+    r.across_channels = p->boolean("across_channels", false);
+    r.eps = static_cast<float>(p->num("eps", 1e-9));
+  }
+  return true;
+}
+
 bool slice(Layer& L, std::vector<Shape>*) {  // slice_layer.cpp Reshape
   Shape in;
   if (!L.bottom(0, &in)) return false;
@@ -874,7 +896,7 @@ const struct { const char* type; Rule rule; } kRules[] = {
     {"Softmax", same_shape}, {"Power", same_shape}, {"AbsVal", same_shape}, {"BNLL", same_shape}, {"ELU", same_shape},
     {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape}, {"PReLU", prelu},
     {"Split", split}, {"Eltwise", eltwise}, {"Scale", scale}, {"Flatten", flatten}, {"Concat", concat},
-    {"Embed", embed}, {"Reshape", reshape}, {"RNN", rnn},
+    {"Embed", embed}, {"Reshape", reshape}, {"RNN", rnn}, {"MVN", mvn},
     {"SoftmaxWithLoss", softmax_loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
     {"HingeLoss", loss}, {"MultinomialLogisticLoss", loss},
     {"BatchNorm", batch_norm}, {"Slice", slice}, {"ContrastiveLoss", contrastive_loss}, {"Silence", silence},

@@ -42,7 +42,9 @@ struct NetLayer {
   std::string pool = "MAX";
   float negative_slope = 0.f;
   bool use_global_stats = false;  // BatchNorm in TRAIN: default false
-  float moving_average_fraction = 0.999f, eps = 1e-5f;
+  float moving_average_fraction = 0.999f, eps = 1e-5f;  // eps: BatchNorm's, or MVN's (the parser sets its 1e-9)
+  // MVN (caffe.proto MVNParameter defaults)
+  bool normalize_variance = true, across_channels = false;
   float loss_weight = 1.f;
   bool has_loss_param = false;
   // LRN (caffe.proto LRNParameter defaults); norm_region is "ACROSS_CHANNELS" or "WITHIN_CHANNEL"

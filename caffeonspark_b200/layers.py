@@ -1,6 +1,7 @@
 """Native producer layers: autograd Functions and modules over the library's LRN (across and within channels) and fused
-conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10) and its
-BatchNorm entry points (csrc/batch_norm.cu, DESIGN.md section 13).
+conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10), its
+BatchNorm entry points (csrc/batch_norm.cu, DESIGN.md section 13) and its MVN entry points (csrc/mvn.cu, DESIGN.md
+section 14).
 
 Activations may be fp32 or bf16 (the mixed-precision producer runs these layers under
 torch.autocast, where the convolutions hand them bf16).  bf16 tensors take the bf16 entry points,
@@ -215,6 +216,81 @@ def batch_norm_composite(x, mean, variance, scale, use_global_stats=False, movin
     sd = torch.pow(var + eps, 0.5)
     y = (xf - mu.view(1, c, 1)) / sd.view(1, c, 1)
     return y.reshape(x.shape).to(x.dtype)
+
+
+def legacy_shape(shape):
+    """Blob::LegacyShape's (num, channels, height, width) of a shape of at most 4 axes: the missing axes are 1."""
+    if len(shape) > 4:
+        raise CosError("Cannot use legacy accessors on Blobs with > 4 axes.")
+    return tuple(shape) + (1,) * (4 - len(shape))
+
+
+def _mvn_formula_forward(x, rows, dim, normalize_variance, eps):
+    """mvn_layer.cu Forward_gpu in x's dtype: -> (y, s) with y [rows, dim] and s [rows, 1] (None mean-only)."""
+    alpha = torch.tensor(1.0 / dim, dtype=x.dtype)
+    xr = x.reshape(rows, dim)
+    y = xr - xr.sum(1, keepdim=True) * alpha
+    if not normalize_variance:
+        return y, None
+    s = torch.pow((y * y).sum(1, keepdim=True) * alpha, 0.5) + torch.tensor(eps, dtype=x.dtype)
+    return y / s, s
+
+
+def _mvn_formula_backward(y, dy, s, dim):
+    """mvn_layer.cu Backward_gpu's formula (the exact derivative only where s >> eps) in y's dtype."""
+    if s is None:
+        return dy - dy.sum(1, keepdim=True) * torch.tensor(1.0 / dim, dtype=y.dtype)
+    a, b = (y * dy).sum(1, keepdim=True), dy.sum(1, keepdim=True)
+    return (dy + torch.tensor(-1.0 / dim, dtype=y.dtype) * (y * a + b)) / s
+
+
+class MVN(torch.autograd.Function):
+    """Caffe's MVN layer: MVN.apply(x, normalize_variance=True, across_channels=False, eps=1e-9) -> the normalised x
+    in the bottom's legacy 4-D shape (num, channels, height, width), as mvn_layer.cpp reshapes its top.  Each of the
+    num * channels rows (num with across_channels) of count / rows elements is centred on its mean and, with
+    normalize_variance, divided by s = sqrt(mean of squared deviations) + eps.  The backward is Caffe's formula
+    dx = (dy - (y * sum(y dy) + sum(dy)) / dim) / s (dy - mean(dy) mean-only), which is the exact derivative only
+    where s >> eps.  fp32 CUDA tensors take the native kernels; CPU tensors, of any float dtype, the same formulas
+    in PyTorch."""
+
+    @staticmethod
+    def forward(ctx, x, normalize_variance=True, across_channels=False, eps=1e-9):
+        shape = legacy_shape(x.shape)
+        if x.numel() == 0:
+            raise CosError(f"MVN needs a bottom with no zero dimension, got {tuple(x.shape)}")
+        rows = shape[0] * (1 if across_channels else shape[1])
+        dim = x.numel() // rows
+        ctx.geom, ctx.in_shape = (rows, dim, bool(normalize_variance)), x.shape
+        if not x.is_cuda:
+            y, s = _mvn_formula_forward(x, rows, dim, normalize_variance, eps)
+            ctx.save_for_backward(y, s)
+            return y.reshape(shape)
+        if x.dtype != torch.float32:
+            raise CosError(f"MVN takes fp32 CUDA tensors (or CPU tensors), got {x.dtype} on {x.device}")
+        x = x.contiguous()
+        y = torch.empty(shape, dtype=torch.float32, device=x.device)
+        stats = torch.empty(5 * rows, dtype=torch.float32, device=x.device)
+        work = torch.empty(max(1, _lib.lib().cos_mvn_workspace_floats(rows, dim)), dtype=torch.float32,
+                           device=x.device)
+        _call(_lib.lib().cos_mvn_forward, x.data_ptr(), y.data_ptr(), stats.data_ptr(), work.data_ptr(), rows, dim,
+              int(bool(normalize_variance)), float(eps), _stream())
+        ctx.save_for_backward(y, stats)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        rows, dim, normalize_variance = ctx.geom
+        y, saved = ctx.saved_tensors
+        if not y.is_cuda:
+            return _mvn_formula_backward(y, dy.reshape(rows, dim), saved, dim).reshape(ctx.in_shape), None, None, None
+        dy = dy.contiguous().float()
+        dx = torch.empty(ctx.in_shape, dtype=torch.float32, device=y.device)
+        work = torch.empty(max(1, _lib.lib().cos_mvn_workspace_floats(rows, dim)), dtype=torch.float32,
+                           device=y.device)
+        stats = saved.clone()  # the backward writes its row sums A and B into stats; the saved tensor stays as it was
+        _call(_lib.lib().cos_mvn_backward, y.data_ptr(), dy.data_ptr(), dx.data_ptr(), stats.data_ptr(),
+              work.data_ptr(), rows, dim, int(normalize_variance), _stream())
+        return dx, None, None, None
 
 
 class LRN(nn.Module):

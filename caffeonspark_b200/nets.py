@@ -468,6 +468,54 @@ LENET_TANH_PARAM_COUNT = 431080
 # and a channel_shared PReLU after ip1: 145,578 + 32 + 32 + 64 + 1 = 145,707 parameters in 14 blobs.
 CIFAR10_QUICK_PRELU = dict(input=(3, 32, 32), batch=100, classes=10)
 CIFAR10_QUICK_PRELU_PARAM_COUNT = 145707
+# tests/golden/configs/cifar10_quick_mvn_train_test.prototxt: CIFAR-10-quick with MVN on the staged input, after conv2
+# (then a Scale with a bias), after pool2 (mean-only), after pool3 (eps 0.001, then a Scale with a bias) and across
+# ip1's channels: 145,578 + 64 + 128 = 145,770 parameters in 14 blobs.
+CIFAR10_QUICK_MVN = dict(input=(3, 32, 32), batch=100, classes=10)
+CIFAR10_QUICK_MVN_PARAM_COUNT = 145770
+
+
+def scale_module(dim, axis=1):
+    """Caffe's one-bottom Scale with bias_term over `dim` elements of axis `axis`: y = x * s + b (scale_layer.cpp),
+    s filled with 1 and b with 0."""
+    import torch
+    import torch.nn as nn
+
+    class Scale(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.weight = nn.Parameter(torch.ones(dim))
+            self.bias = nn.Parameter(torch.zeros(dim))
+
+        def forward(self, x):
+            shape = (dim,) + (1,) * (x.dim() - axis - 1)
+            return x * self.weight.view(shape) + self.bias.view(shape)
+
+    return Scale()
+
+
+def mvn_module(normalize_variance=True, across_channels=False, eps=1e-9):
+    """Caffe's MVN (layers.MVN) as a module: its top has the bottom's legacy 4-D shape."""
+    import torch.nn as nn
+    from .layers import MVN
+
+    class _MVN(nn.Module):
+        def forward(self, x):
+            return MVN.apply(x, normalize_variance, across_channels, eps)
+
+    return _MVN()
+
+
+def cifar10_quick_mvn_module():
+    """The MVN CIFAR-10-quick fixture as one PyTorch module, parameters in learnable_params() order.
+    forward(x [N, 3, 32, 32]) -> scores [N, 10]."""
+    import torch.nn as nn
+    return nn.Sequential(mvn_module(), nn.Conv2d(3, 32, 5, padding=2), nn.MaxPool2d(3, 2, ceil_mode=True), nn.ReLU(),
+                         nn.Conv2d(32, 32, 5, padding=2), mvn_module(), scale_module(32), nn.ReLU(),
+                         nn.AvgPool2d(3, 2, ceil_mode=True), mvn_module(normalize_variance=False),
+                         nn.Conv2d(32, 64, 5, padding=2), nn.ReLU(), nn.AvgPool2d(3, 2, ceil_mode=True),
+                         mvn_module(eps=1e-3), scale_module(64), nn.Flatten(), nn.Linear(1024, 64),
+                         mvn_module(across_channels=True), nn.Flatten(), nn.Linear(64, 10))
 
 
 def lenet_tanh_module():
@@ -612,6 +660,9 @@ RNN_LM_PARAM_COUNT = 934352
 # cont, InnerProduct 128 -> 1000 on axis 2; 12 timesteps of 16 streams.  547,018 parameters in 20 blobs.
 RNN_CAPTION = dict(steps=12, batch=16, vocab=1000, dim=64, hidden=128, image=256)
 RNN_CAPTION_PARAM_COUNT = 547018
+# tests/golden/configs/rnn_lm_ln_train_test.prototxt: rnn_lm with an MVN over each timestep's 256 hidden outputs and a
+# Scale with a bias on axis 2 before the scores: 934,352 + 512 = 934,864 parameters in 10 blobs.
+RNN_LM_LN_PARAM_COUNT = 934864
 
 
 def rnn_module(input_dim, num_output, static_dim=0):
@@ -696,3 +747,25 @@ def rnn_caption_module():
             return self.predict(o2), (h1, h2)
 
     return RNNCaption()
+
+
+def rnn_lm_ln_module():
+    """The layer-normalised RNN language model fixture as one PyTorch module, parameters in learnable_params() order.
+    forward(tokens [T, N], cont [T, N], h0 [N, 256]) -> (scores [T, N, 2000], h_{T-1})."""
+    import torch.nn as nn
+    s = RNN_LM
+
+    class RNNLMLN(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.embed = embed_module(s["vocab"], s["dim"], bias=False)
+            self.rnn = rnn_module(s["dim"], s["hidden"])
+            self.ln = mvn_module()
+            self.scale = scale_module(s["hidden"], axis=2)
+            self.predict = nn.Linear(s["hidden"], s["vocab"])
+
+        def forward(self, tokens, cont, h0):
+            o, h = self.rnn(self.embed(tokens), cont, h0)
+            return self.predict(self.scale(self.ln(o)).flatten(2)), h
+
+    return RNNLMLN()

@@ -257,6 +257,7 @@ COS_API int cos_net_set_forward_backward(cos_net* net, cos_forward_backward_fn f
  * 1, dilation 1), Pooling (MAX, AVE), InnerProduct (any axis), ReLU, Sigmoid, BatchNorm, LRN (WITHIN_CHANNEL), Slice,
  * Embed over fp32 token ids (a CoSData INT_ARRAY top), Reshape, RNN (without expose_hidden; its hidden state is kept
  * per engine from call to call, zero at first, and not snapshotted) over time-major CoSData tops (transpose: true),
+ * MVN (its top the bottom's legacy 4-D shape; in place it computes the out-of-place result),
  * the other layers DESIGN.md section 14 lists, and one
  * loss layer, SoftmaxWithLoss or ContrastiveLoss among them (default normalisation); Accuracy and Silence are skipped.
  * Named params are shared as in Caffe.  Every other layer, and loss_param or an unknown filler type, is refused with an
@@ -452,6 +453,24 @@ COS_API int cos_batch_norm_forward_bf16(const uint16_t* x, uint16_t* y, float* m
 COS_API int cos_batch_norm_backward_bf16(const uint16_t* x, const uint16_t* dy, uint16_t* dx, const float* save,
                                          float* workspace, int num, int channels, int height, int width,
                                          int use_global_stats, float eps, void* cuda_stream);
+
+/* Caffe's MVN layer (mvn_layer.cu; DESIGN.md section 14): `rows` contiguous rows of `dim` fp32 elements, each
+ * normalised on its own (a Caffe bottom has num * channels rows, or num with across_channels).  With
+ * alpha = (float)(1.0 / dim) and one fp32 rounding per operation:
+ *   forward   y = x - mu, mu = sum(x) * alpha; with normalize_variance y = (x - mu) / s, s = powf(var, 0.5) + eps
+ *             (glibc's powf), var = sum((x - mu)^2) * alpha
+ *   backward  with normalize_variance dx = (dy + c * (y * A + B)) / s, c = (float)(-1.0 / dim), A = sum(y * dy),
+ *             B = sum(dy) (Caffe's formula, the exact derivative only where s >> eps); mean-only dx = dy - B * alpha
+ * stats holds 5 * rows floats, row vectors in this order: sum(x), sum((x - mu)^2) and s (written by the forward;
+ * 0 and 1 mean-only), then A and B (written by the backward, which reads s).  workspace is
+ * cos_mvn_workspace_floats(rows, dim) floats (NULL when that is 0).  The row sums' order is fixed by (rows, dim):
+ * results are bitwise identical from run to run.  y may be x, and dx may be y or dy.  Same launch rules as the
+ * calls above; rows * dim must be below 2^31 (else "bad shape"). */
+COS_API long long cos_mvn_workspace_floats(long long rows, long long dim);
+COS_API int cos_mvn_forward(const float* x, float* y, float* stats, float* workspace, long long rows, long long dim,
+                            int normalize_variance, float eps, void* cuda_stream);
+COS_API int cos_mvn_backward(const float* y, const float* dy, float* dx, float* stats, float* workspace,
+                             long long rows, long long dim, int normalize_variance, void* cuda_stream);
 
 /* --------------------- transport object (reference: util/socket.hpp) ------ */
 /* PeerAdapter = SocketAdapter + SocketChannel of the reference
