@@ -1,6 +1,7 @@
 // native_producer.cpp -- the built-in producer's net plan (host only); see native_producer.hpp.
 #include "native_producer.hpp"
 
+#include <algorithm>
 #include <cmath>
 #include <iterator>
 #include <map>
@@ -263,6 +264,24 @@ bool neuron_op(const NetLayer& L, Op* op, Plan* P, std::string* err) {
       return true;
     default:
       return true;
+  }
+}
+
+// The largest M of the op's GEMMs (0 for an op without one): the channels of a convolution's forward and data gradient
+// (either side, as a Deconvolution swaps them), an InnerProduct's rows (forward, data gradient) and num_output (weight
+// gradient), an RNN's T * N rows and its num_output
+int64_t gemm_rows(const Op& op) {
+  switch (op.kind) {
+    case OpKind::kConv:
+    case OpKind::kConvBiasReluMaxPool:
+    case OpKind::kDeconv:
+      return std::max(op.in_shape[1], op.out_shape[1]);
+    case OpKind::kInnerProduct:
+      return std::max(shape_count(op.out_shape) / op.out_shape.back(), op.out_shape.back());
+    case OpKind::kRNN:
+      return std::max(op.in_shape[0] * op.in_shape[1], op.out_shape[2]);
+    default:
+      return 0;
   }
 }
 
@@ -595,6 +614,12 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
                           " rows of the scores along axis " + std::to_string(axis));
         return false;
       }
+    }
+    const int64_t rows = gemm_rows(op);
+    if (rows > kMaxGemmRows) {
+      *err = why(L, "a GEMM of " + std::to_string(rows) + " rows is more than the " + std::to_string(kMaxGemmRows) +
+                        " the engine supports");
+      return false;
     }
     op.out = new_tensor(shape_count(op.out_shape), storage);
     if (op.kind == OpKind::kFlatten || op.kind == OpKind::kReshape) P.data_alias[op.out] = true;

@@ -146,6 +146,9 @@ constexpr int kStatusBadMultinomialLabel = 501, kStatusBadHingeLabel = 502;
 constexpr int kStatusBadEmbedIndex = 503;
 // PReLU's slope gradient runs one grid row per slope (gridDim.y), so a per-channel PReLU has at most this many channels
 constexpr int64_t kMaxPReLUChannels = 65535;
+// The GEMM core puts its M rows on gridDim.y in tiles of 64, so one GEMM has at most this many rows: an InnerProduct's
+// rows or num_output, a convolution's input or output channels, an RNN's T * N or num_output
+constexpr int64_t kMaxGemmRows = 65535 * 64;
 
 class NativeProducer {
  public:

@@ -16,7 +16,7 @@ from conftest import ROOT
 from gpu_util import assert_bits_equal, to_host
 from test_gpu_least_squares import _near
 from test_gpu_native_producer import _UpdateCheck, _grads, _load
-from test_gpu_producer_ops import FAMILIES, _check, _close, _engine, _forward, _probe
+from test_gpu_producer_ops import FAMILIES, _check, _close, _engine, _exact_depth, _forward, _probe
 
 pytestmark = pytest.mark.gpu
 
@@ -94,6 +94,8 @@ DECONV_CASES = [  # (N, Cin, H, W, Cout, (kh, kw, sh, sw, ph, pw), bias)
     (1, 5, 3, 3, 65, (2, 2, 2, 2, 0, 0), True),  # Cout across the 64-row tile edge of the forward
     (1, 65, 3, 3, 2, (1, 1, 1, 1, 0, 0), True),  # Cin across it for the data gradient
     (2, 2, 20, 20, 2, (3, 3, 1, 1, 1, 1), True),  # N H W = 800: two chunks of the weight gradient
+    (1, 2, 3, 43691, 2, (1, 1, 1, 1, 0, 0), True),  # N H W = 131,073: 249 widened chunks of 528
+    (256, 2, 55, 55, 2, (1, 1, 1, 1, 0, 0), True),  # N H W = 774,400: 255 chunks of 3,040
 ]
 
 
@@ -113,6 +115,10 @@ def test_deconvolution(cos, tmp_path, family, n, cin, h, w, cout, geo, bias):
     B = _probe(y64, rng, family)
     r = _engine(cos, tmp_path, [x], _deconv_layer(cout, geo, bias), [wt] + ([b] if bias else []), y64.shape, B)
     d = r["d"]
+    if exact:  # x and d are dyadic in 2^-3
+        adw, adb, _ = A.deconv_backward(np.abs(x), np.abs(wt), np.abs(d), geo)
+        _exact_depth(adw, 2.0 ** -6, "dW")
+        _exact_depth(adb, 2.0 ** -3, "db")
     by, bw, bb, bx = A.deconv_bounds(x, wt, b, d, geo)
     _forward(d, y64, B, by, "y", exact)
     dw, db, dx = A.deconv_backward(x, wt, d, geo)

@@ -193,7 +193,16 @@ CONV_CASES = [  # (N, Cin, H, W, Cout, (kh, kw, sh, sw, ph, pw), bias)
     (1, 2, 8, 8, 3, (1, 1, 1, 1, 0, 0), True),
     (1, 2, 5, 13, 3, (1, 1, 1, 1, 0, 0), True),
     (2, 3, 40, 40, 4, (3, 3, 1, 1, 1, 1), True),  # N OH OW = 3200 = 6 * 512 + 128
+    # past 256 chunks of 512 the chunk widens: N OH OW = 131,073 (249 chunks of 528), 774,400 (255 of 3,040)
+    (1, 2, 3, 43691, 3, (1, 1, 1, 1, 0, 0), True),
+    (256, 2, 55, 55, 3, (1, 1, 1, 1, 0, 0), True),
 ]
+
+
+def _exact_depth(abs_sum, unit, what):
+    """On dyadic inputs a sum is exact in fp32 in any order while sum |terms| stays below 2^24 of the terms' unit: every
+    partial sum is then a multiple of the unit below 2^24 units.  The deep reductions assert it before comparing."""
+    assert np.max(abs_sum) < 2 ** 24 * unit, f"{what}: sum |terms| = {np.max(abs_sum) / unit:.0f} units, not exact"
 
 
 def _conv_params(rng, family, cin, cout, kh, kw, bias):
@@ -217,6 +226,10 @@ def test_convolution(cos, tmp_path, family, n, cin, h, w, cout, geo, bias):
     r = _engine(cos, tmp_path, [x], _conv_layer("c", "x0", "y", cout, geo, bias),
                 [wt] + ([b] if bias else []), y64.shape, B)
     d = r["d"]
+    if exact:  # x and d are dyadic in 2^-3, so dW's terms are in 2^-6 and db's in 2^-3
+        adw, adb, _ = R.conv_backward(np.abs(x), np.abs(wt), np.abs(d), geo)
+        _exact_depth(adw, 2.0 ** -6, "dW")
+        _exact_depth(adb, 2.0 ** -3, "db")
     by, bw, bb, bx = R.conv_bounds(x, wt, b, d, geo)
     _forward(d, y64, B, by, "y", exact)
     dw, db, dx = R.conv_backward(x, wt, d, geo)
@@ -325,6 +338,7 @@ IP_CASES = [  # (bottom shape, N, bias)
     ((600, 1000), 10, True), ((1100, 17), 65, True), ((65, 1000), 129, True),
     ((5, 3, 4, 5), 10, True),  # a 4-D bottom: K = 60
     ((64, 15), 10, False),
+    ((131073, 5), 3, True), ((774400, 3), 2, True),  # rows past 256 chunks of 512: the widened chunks
 ]
 
 
@@ -346,6 +360,10 @@ def test_inner_product(cos, tmp_path, family, shape, nout, bias):
             f'num_output: {nout} bias_term: {"true" if bias else "false"} }} }}\n')
     r = _engine(cos, tmp_path, [x], body, [wt] + ([b] if bias else []), y64.shape, B)
     d = r["d"]
+    if exact:
+        adw, adb, _ = R.ip_backward(np.abs(x), np.abs(wt), np.abs(d))
+        _exact_depth(adw, 2.0 ** -6, "dW")
+        _exact_depth(adb, 2.0 ** -3, "db")
     by, bw, bb, bx = R.ip_bounds(x, wt, b, d)
     _forward(d, y64, B, by, "y", exact)
     dw, db, dx = R.ip_backward(x, wt, d)

@@ -158,6 +158,7 @@ OP_CASES = [
     (20, 32, 3, 64, 6, "random", True, False),
     (2, 1, 9, 257, 0, "scaled", False, False),
     (7, 32, 64, 1, 0, "start", True, False),
+    (4, 32769, 2, 3, 0, "random", True, False),  # T N = 131,076: the weight gradients take 249 widened chunks of 528
 ]
 
 

@@ -202,3 +202,19 @@ def test_a_loss_layers_top_is_not_read(cos, tmp_path):
                  'layer { name: "r" type: "ReLU" bottom: "loss" top: "loss" }\n')
     with pytest.raises(cos.CosError, match=r"^layer 'r' \(ReLU\): bottom 'loss' is the top of loss layer 'euc'"):
         cos.native_producer_plan(str(p))
+
+
+@pytest.mark.parametrize("rows,refused", [(4194240, False), (4194241, True)])
+def test_a_gemm_past_the_grids_rows_is_refused(cos, tmp_path, rows, refused):
+    # the GEMM core tiles M = 64 rows per gridDim.y block, 65,535 at most: an InnerProduct over more rows is refused by
+    # the plan (which allocates nothing) rather than failing at its first forward
+    p = tmp_path / "net.prototxt"
+    p.write_text(f'name: "t" layer {{ name: "in" type: "Input" top: "x" top: "t" input_param {{ shape {{ dim: {rows} '
+                 f'dim: 1 }} shape {{ dim: {rows} dim: 1 }} }} }}\n' + _ip("ip", "x", "y").replace("num_output: 4", "num_output: 1") +
+                 '\nlayer { name: "euc" type: "EuclideanLoss" bottom: "y" bottom: "t" top: "loss" }\n')
+    if refused:
+        with pytest.raises(cos.CosError, match=r"^layer 'ip' \(InnerProduct\): a GEMM of 4194241 rows is more than the "
+                                               r"4194240 the engine supports"):
+            cos.native_producer_plan(str(p))
+    else:
+        assert "InnerProduct ip 4194240x1 -> 4194240x1" in cos.native_producer_plan(str(p))
