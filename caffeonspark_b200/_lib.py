@@ -135,6 +135,8 @@ SYMBOLS = [
     ("cos_mvn_workspace_floats", _c.c_longlong, [_c.c_longlong, _c.c_longlong]),
     ("cos_mvn_forward", _i, [_vp, _vp, _vp, _vp, _c.c_longlong, _c.c_longlong, _i, _f, _vp]),
     ("cos_mvn_backward", _i, [_vp, _vp, _vp, _vp, _vp, _c.c_longlong, _c.c_longlong, _i, _vp]),
+    ("cos_crop_forward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    ("cos_crop_backward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
     ("cos_adapter_create", _vp, [_i, _i]),
     ("cos_adapter_destroy", None, [_vp]),
     ("cos_adapter_address", _cp, [_vp]),

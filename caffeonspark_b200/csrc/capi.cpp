@@ -769,6 +769,36 @@ int cos_mvn_backward(const float* y, const float* dy, float* dx, float* stats, f
                   "cos_mvn_backward");
 }
 
+namespace {
+// -> (bottom shape, top shape, offsets) of a crop over `naxes` axes, or an error message
+const char* crop_args(const void* a, const void* b, int naxes, const long long* bottom_shape,
+                      const long long* top_shape, const long long* offsets, std::vector<int64_t>* bs,
+                      std::vector<int64_t>* ts, std::vector<int64_t>* os) {
+  if (!a || !b || !bottom_shape || !top_shape || !offsets) return "NULL tensor or shape";
+  if (naxes < 1 || naxes > cosb::kCropMaxAxes) return "bad number of axes";
+  bs->assign(bottom_shape, bottom_shape + naxes), ts->assign(top_shape, top_shape + naxes);
+  os->assign(offsets, offsets + naxes);
+  for (int k = 0; k < naxes; ++k)
+    if ((*ts)[k] < 1 || (*os)[k] < 0 || (*os)[k] + (*ts)[k] > (*bs)[k]) return "the window leaves the bottom";
+  return nullptr;
+}
+}  // namespace
+
+int cos_crop_forward(const float* x, float* y, int naxes, const long long* bottom_shape, const long long* top_shape,
+                     const long long* offsets, void* cuda_stream) {
+  std::vector<int64_t> bs, ts, os;
+  if (const char* e = crop_args(x, y, naxes, bottom_shape, top_shape, offsets, &bs, &ts, &os)) return fail(e);
+  return launched(cosb::crop_forward(x, y, bs, ts, os, static_cast<cudaStream_t>(cuda_stream)), "cos_crop_forward");
+}
+
+int cos_crop_backward(const float* dy, float* dx, int naxes, const long long* bottom_shape,
+                      const long long* top_shape, const long long* offsets, void* cuda_stream) {
+  std::vector<int64_t> bs, ts, os;
+  if (const char* e = crop_args(dy, dx, naxes, bottom_shape, top_shape, offsets, &bs, &ts, &os)) return fail(e);
+  return launched(cosb::crop_backward(dy, dx, bs, ts, os, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_crop_backward");
+}
+
 int cos_batch_norm_forward_bf16(const uint16_t* x, uint16_t* y, float* mean_blob, float* var_blob, float* scale_blob,
                                 float* save, float* workspace, int num, int channels, int height, int width,
                                 int use_global_stats, float moving_average_fraction, float eps, void* cuda_stream) {

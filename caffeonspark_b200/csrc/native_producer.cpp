@@ -137,6 +137,8 @@ const LayerType kLayerTypes[] = {
     // RNNs may read one cont blob
     {"RNN", OpKind::kRNN, -1, false, 1, "cont"},
     {"MVN", OpKind::kMVN},
+    // the reference gives only its shape: it is never read, so it may also feed a Concat or a loss without a Split
+    {"Crop", OpKind::kCrop, 2, false, 1, "ref"},
 };
 
 // Plan::text's name of each OpKind
@@ -145,7 +147,7 @@ const char* const kKindNames[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling
                                   "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale", "Deconvolution", "Flatten",
                                   "SigmoidCrossEntropyLoss", "TanH", "ELU", "AbsVal", "BNLL", "Power", "Exp", "Log",
                                   "Threshold", "PReLU", "Softmax", "MultinomialLogisticLoss", "HingeLoss",
-                                  "Embed", "Reshape", "RNN", "MVN"};
+                                  "Embed", "Reshape", "RNN", "MVN", "Crop"};
 static_assert(std::size(kKindNames) == static_cast<size_t>(OpKind::kCount), "one name per OpKind");
 
 // LossLayer::Reshape's check, then multinomial_logistic_loss_layer.cpp's: the label holds one value per item, with
@@ -558,6 +560,14 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.eps = L.eps;
       op.mvn_rows = op.out_shape[0] * (L.across_channels ? 1 : op.out_shape[1]);
       op.mvn_dim = shape_count(op.out_shape) / op.mvn_rows;
+    } else if (op.kind == OpKind::kCrop) {  // crop_layer.cpp; the parser checked the window.  The top owns its storage
+      if (op.in_shape.size() > static_cast<size_t>(kCropMaxAxes)) {
+        *err = why(L, "a bottom of " + std::to_string(op.in_shape.size()) + " axes is more than the " +
+                          std::to_string(kCropMaxAxes) + " a blob may have");
+        return false;
+      }
+      op.crop_axis = static_cast<int>(L.axis);
+      op.crop_offsets = L.crop_offsets;
     } else if (op.kind == OpKind::kBatchNorm) {
       if (!op.shares.empty()) {
         *err = why(L, "shared BatchNorm statistics are not supported");
@@ -719,6 +729,12 @@ std::string Plan::text() const {
       os << " rows=" << op.mvn_rows << " dim=" << op.mvn_dim << " eps=" << op.eps;
       if (op.across_channels) os << " across";
       if (!op.normalize_variance) os << " mean-only";
+    }
+    if (op.kind == OpKind::kCrop) {
+      os << " axis=" << op.crop_axis << " offsets=";
+      for (size_t a = op.crop_axis; a < op.crop_offsets.size(); ++a)
+        os << (a > static_cast<size_t>(op.crop_axis) ? "," : "") << op.crop_offsets[a];
+      os << " ref=" << op.bottoms[1];
     }
     if (op.w_off >= 0 && op.kind != OpKind::kBatchNorm) os << " w=" << op.w_off << ":" << op.w_count;
     if (op.b_off >= 0) os << " b=" << op.b_off << ":" << op.b_count;

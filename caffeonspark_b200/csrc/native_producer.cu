@@ -435,6 +435,65 @@ __global__ void slice_copy_kernel(const float* src, float* dst, int64_t total, i
   }
 }
 
+// ------------------------------------------------------------------ Crop (crop_layer.cpp)
+// The window's geometry over `rank` axes, innermost first (axis 0 is the contiguous one): the top's dims, the bottom's
+// dims and the window's offset on each, in units of V (float or float4: the innermost dims and offset are divided by
+// 4 for float4).  crop_geom merges an axis into the next inner one when that one is not cropped, so a crop on H and W
+// of NCHW maps over three axes.
+struct CropGeom {
+  int rank;
+  int64_t top[kCropMaxAxes], bottom[kCropMaxAxes], off[kCropMaxAxes];
+};
+
+// q = n / d and n - q d, with 32-bit arithmetic when both fit (every index of a blob under 2^32 elements)
+__device__ __forceinline__ int64_t crop_divmod(int64_t n, int64_t d, int64_t* r) {
+  if (((n | d) >> 32) == 0) {
+    const uint32_t q = static_cast<uint32_t>(n) / static_cast<uint32_t>(d);
+    *r = static_cast<uint32_t>(n) - q * static_cast<uint32_t>(d);
+    return q;
+  }
+  const int64_t q = n / d;
+  *r = n - q * d;
+  return q;
+}
+
+// Forward: one thread per element (or float4) of the top, consecutive threads on consecutive innermost elements:
+// y[i] = x[the bottom index of i's coordinates plus the offsets].  A copy: every bit of x arrives in y.
+template <class V>
+__global__ void crop_forward_kernel(const V* __restrict__ x, V* __restrict__ y, int64_t total, CropGeom g) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    int64_t rest = i, src = 0, stride = 1;
+    for (int a = 0; a < g.rank; ++a) {
+      int64_t c = rest;
+      if (a + 1 < g.rank) rest = crop_divmod(rest, g.top[a], &c);
+      src += (c + g.off[a]) * stride;
+      stride *= g.bottom[a];
+    }
+    y[i] = x[src];
+  }
+}
+
+// Backward: one thread per element (or float4) of the bottom, each written once: dy at the mapped top index inside
+// the window, +0 outside it.  No memset, no scatter, no atomics.
+template <class V>
+__global__ void crop_backward_kernel(const V* __restrict__ dy, V* __restrict__ dx, int64_t total, CropGeom g) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    int64_t rest = i, src = 0, stride = 1;
+    bool inside = true;
+    for (int a = 0; a < g.rank; ++a) {
+      int64_t c = rest;
+      if (a + 1 < g.rank) rest = crop_divmod(rest, g.bottom[a], &c);
+      const int64_t t = c - g.off[a];
+      inside = inside && t >= 0 && t < g.top[a];
+      src += t * stride;
+      stride *= g.top[a];
+    }
+    dx[i] = inside ? dy[src] : V{};  // V{}: +0 in every lane
+  }
+}
+
 // ------------------------------------------------------------------ ContrastiveLoss (contrastive_loss_layer.cpp)
 // One block.  Pair r: d = a_r - b_r, dist_sq = sum over c of d_c^2 in c order.  A similar pair (static_cast<int>(sim)
 // nonzero) adds dist_sq to the loss and gets da = alpha * d.  A dissimilar pair adds max(margin - dist_sq, 0)
@@ -1138,6 +1197,64 @@ cudaError_t deconv_backward(const Op& op, const float* x, const float* dy, float
 
 }  // namespace
 
+// ------------------------------------------------------------------ Crop's launches
+namespace {
+// The merged geometry of a crop, innermost axis first; false for a shape the kernels do not take.  *vec4 when the
+// float4 kernels apply: the innermost run, the bottom's innermost dim and offset are multiples of 4 and every pointer
+// is 16-byte aligned (the bottom's rows then start aligned too).
+bool crop_geom(const std::vector<int64_t>& bottom, const std::vector<int64_t>& top, const std::vector<int64_t>& offsets,
+               std::initializer_list<const void*> ptrs, CropGeom* g, bool* vec4) {
+  const size_t n = bottom.size();
+  if (n == 0 || n > static_cast<size_t>(kCropMaxAxes) || top.size() != n || offsets.size() != n) return false;
+  g->rank = 0;
+  for (size_t k = n; k-- > 0;) {
+    if (top[k] < 1 || offsets[k] < 0 || offsets[k] + top[k] > bottom[k]) return false;
+    const int r = g->rank - 1;
+    if (r >= 0 && g->top[r] == g->bottom[r] && g->off[r] == 0) {  // the inner axis is whole: merge this one into it
+      g->off[r] = offsets[k] * g->bottom[r];
+      g->top[r] *= top[k];
+      g->bottom[r] *= bottom[k];
+    } else {
+      g->top[g->rank] = top[k], g->bottom[g->rank] = bottom[k], g->off[g->rank] = offsets[k];
+      ++g->rank;
+    }
+  }
+  bool aligned = true;
+  for (const void* p : ptrs) aligned = aligned && reinterpret_cast<uintptr_t>(p) % 16 == 0;
+  *vec4 = aligned && g->top[0] % 4 == 0 && g->bottom[0] % 4 == 0 && g->off[0] % 4 == 0;
+  if (*vec4) g->top[0] /= 4, g->bottom[0] /= 4, g->off[0] /= 4;
+  return true;
+}
+}  // namespace
+
+cudaError_t crop_forward(const float* x, float* y, const std::vector<int64_t>& bottom_shape,
+                         const std::vector<int64_t>& top_shape, const std::vector<int64_t>& offsets, cudaStream_t s) {
+  CropGeom g;
+  bool vec4;
+  if (!crop_geom(bottom_shape, top_shape, offsets, {x, y}, &g, &vec4)) return cudaErrorInvalidValue;
+  const int64_t n = shape_count(top_shape) / (vec4 ? 4 : 1);
+  if (vec4)
+    crop_forward_kernel<float4><<<grid_for(n), kThreads, 0, s>>>(reinterpret_cast<const float4*>(x),
+                                                                  reinterpret_cast<float4*>(y), n, g);
+  else
+    crop_forward_kernel<float><<<grid_for(n), kThreads, 0, s>>>(x, y, n, g);
+  return cudaGetLastError();
+}
+
+cudaError_t crop_backward(const float* dy, float* dx, const std::vector<int64_t>& bottom_shape,
+                          const std::vector<int64_t>& top_shape, const std::vector<int64_t>& offsets, cudaStream_t s) {
+  CropGeom g;
+  bool vec4;
+  if (!crop_geom(bottom_shape, top_shape, offsets, {dy, dx}, &g, &vec4)) return cudaErrorInvalidValue;
+  const int64_t n = shape_count(bottom_shape) / (vec4 ? 4 : 1);
+  if (vec4)
+    crop_backward_kernel<float4><<<grid_for(n), kThreads, 0, s>>>(reinterpret_cast<const float4*>(dy),
+                                                                   reinterpret_cast<float4*>(dx), n, g);
+  else
+    crop_backward_kernel<float><<<grid_for(n), kThreads, 0, s>>>(dy, dx, n, g);
+  return cudaGetLastError();
+}
+
 // ------------------------------------------------------------------ engine
 
 NativeProducer* NativeProducer::create(const Plan& plan, int device, float* data, float* diff, int* status,
@@ -1423,6 +1540,8 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
                                                            op.slice_begin * slice_inner(op), true);
       return cudaGetLastError();
     }
+    case OpKind::kCrop:
+      return crop_forward(x, y, op.in_shape, op.out_shape, op.crop_offsets, s);
     case OpKind::kDeconv:  // the data gradient of the convolution from top to bottom, with the bias in its store
       return conv_data_grad(op, conv_dims(op), x, data_ + op.w_off, op.b_off >= 0 ? data_ + op.b_off : nullptr, y, s);
     case OpKind::kSplit:  // no copy: the top reads the bottom's memory
@@ -1665,6 +1784,8 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
                                                            slice_span(op, op.out_shape),
                                                            op.slice_begin * slice_inner(op), false);
       return cudaGetLastError();
+    case OpKind::kCrop:  // writes every element of dx: the engine's data gradients are written, not accumulated
+      return dx ? crop_backward(dy, dx, op.in_shape, op.out_shape, op.crop_offsets, s) : cudaSuccess;
     case OpKind::kSplit: {  // top 0's op: dx = the read tops' gradients summed in top order; the other tops' do nothing
       if (!dx || op.split_top != 0) return cudaSuccess;
       const std::vector<int>& g = op.split_sum;

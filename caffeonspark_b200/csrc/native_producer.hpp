@@ -2,7 +2,8 @@
 // CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, least-squares regression nets,
 // residual nets built of Split, Eltwise and Scale, autoencoders built of Flatten, Deconvolution and
 // SigmoidCrossEntropyLoss, embedding nets that read token ids through Embed and Reshape, recurrent nets built of
-// RNN layers over time-major inputs, and nets normalised by MVN; DESIGN.md section 14).
+// RNN layers over time-major inputs, nets normalised by MVN, and U-Net segmentation nets that Crop their skips and
+// per-pixel labels; DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -28,7 +29,7 @@ enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
   kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale, kDeconv, kFlatten, kSigmoidCrossEntropyLoss,
   kTanH, kELU, kAbsVal, kBNLL, kPower, kExp, kLog, kThreshold, kPReLU, kSoftmax, kMultinomialLogisticLoss, kHingeLoss,
-  kEmbed, kReshape, kRNN, kMVN,
+  kEmbed, kReshape, kRNN, kMVN, kCrop,
   kCount  // the number of kinds (Plan::text names each)
 };
 
@@ -42,8 +43,8 @@ struct Op {
   // SoftmaxWithLoss writes its bottom's gradient whatever the flag says.
   std::vector<int> bottoms;
   std::vector<bool> bottom_grad;
-  // the label-like bottom (SoftmaxWithLoss's label, ContrastiveLoss's sim, SigmoidCrossEntropyLoss's target), or -1:
-  // read, never differentiated, and not counted as its blob's reader
+  // the label-like bottom (SoftmaxWithLoss's label, ContrastiveLoss's sim, SigmoidCrossEntropyLoss's target, RNN's
+  // cont, Crop's shape-only reference), or -1: never differentiated, and not counted as its blob's reader
   int label_bottom = -1;
   // no gradient reaches the top (it is read by no layer under the loss, or only as a label): the op runs its forward
   // and no backward.  Never set on a Split op (such a top is split_unread) nor a Slice op (it still writes its range of
@@ -111,6 +112,10 @@ struct Op {
   // normalised on its own; eps is added to the standard deviation.  Mean-only without normalize_variance.
   int64_t mvn_rows = 0, mvn_dim = 0;
   bool normalize_variance = true, across_channels = false;
+  // Crop: out[i] = bottoms[0][i + crop_offsets[i]] per axis, over the top's shape (crop_offsets[a] = 0 for a <
+  // crop_axis); bottoms[1] gives only its shape and is never read
+  int crop_axis = 0;
+  std::vector<int64_t> crop_offsets;
 };
 
 struct Plan {
@@ -146,6 +151,16 @@ constexpr int kStatusBadMultinomialLabel = 501, kStatusBadHingeLabel = 502;
 constexpr int kStatusBadEmbedIndex = 503;
 // PReLU's slope gradient runs one grid row per slope (gridDim.y), so a per-channel PReLU has at most this many channels
 constexpr int64_t kMaxPReLUChannels = 65535;
+// Blob::Reshape's kMaxBlobAxes: Crop's kernels map indices over at most this many axes
+constexpr int kCropMaxAxes = 32;
+// Crop's kernels (native_producer.cu): the copy of the window at per-axis `offsets` (one per axis) of a contiguous
+// bottom of `bottom_shape` into a contiguous top of `top_shape`, and its gradient: every element of dx written once,
+// dy's inside the window and +0 outside.  Bit-exact copies; one launch each.  cudaErrorInvalidValue for a shape the
+// kernels do not take (more than kCropMaxAxes axes, or a window that leaves the bottom).
+cudaError_t crop_forward(const float* x, float* y, const std::vector<int64_t>& bottom_shape,
+                         const std::vector<int64_t>& top_shape, const std::vector<int64_t>& offsets, cudaStream_t s);
+cudaError_t crop_backward(const float* dy, float* dx, const std::vector<int64_t>& bottom_shape,
+                          const std::vector<int64_t>& top_shape, const std::vector<int64_t>& offsets, cudaStream_t s);
 // The GEMM core puts its M rows on gridDim.y in tiles of 64, so one GEMM has at most this many rows: an InnerProduct's
 // rows or num_output, a convolution's input or output channels, an RNN's T * N or num_output
 constexpr int64_t kMaxGemmRows = 65535 * 64;

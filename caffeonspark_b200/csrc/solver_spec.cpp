@@ -807,6 +807,43 @@ bool mvn(Layer& L, std::vector<Shape>*) {
   return true;
 }
 
+// crop_layer.cpp LayerSetUp and Reshape (after Layer::CheckBlobCounts), with their CHECK messages: bottom[0] cropped to
+// bottom[1]'s size on every axis from `axis` on, at per-axis offsets.  bottom[1] gives only its shape.
+bool crop(Layer& L, std::vector<Shape>*) {
+  NetLayer& r = L.rec;
+  if (r.bottoms.size() != 2) return L.refuse("Crop Layer takes 2 bottom blob(s) as input.");
+  if (r.tops.size() != 1) return L.refuse("Crop Layer produces 1 top blob(s) as output.");
+  const Node* p = L.node.first("crop_param");
+  std::vector<int64_t> given;  // crop_param offset, a repeated uint32
+  for (const Node* o : p ? p->all("offset") : std::vector<const Node*>()) {
+    given.push_back(atol(o->value.c_str()));
+    if (given.back() < 0) return L.refuse("crop_param offset " + o->value + ": Expected integer, got: -");
+  }
+  Shape in, ref;
+  if (!L.bottom(0, &in) || !L.bottom(1, &ref)) return false;
+  if (r.tops[0] == r.bottoms[0]) return L.refuse("Crop Layer does not allow in-place computation.");
+  const int64_t naxes = static_cast<int64_t>(in.size());
+  int64_t axis;
+  if (!canonical_axis(L, p ? p->integer("axis", 2) : 2, naxes, &axis)) return false;
+  if (given.size() > 1 && axis + static_cast<int64_t>(given.size()) != naxes)
+    return L.refuse("number of offset values specified must be equal to the number of dimensions following axis.");
+  Shape top = in;
+  r.crop_offsets.assign(in.size(), 0);
+  for (int64_t i = axis; i < naxes; ++i) {
+    int64_t i_ref;  // Blob::shape(i) of the reference: CanonicalAxisIndex's CHECK
+    if (!canonical_axis(L, i, static_cast<int64_t>(ref.size()), &i_ref)) return false;
+    const int64_t offset = given.empty() ? 0 : given.size() == 1 ? given[0] : given[i - axis];
+    if (in[i] - offset < ref[i])
+      return L.refuse("the crop for dimension " + std::to_string(i) + " is out-of-bounds with size " +
+                      std::to_string(ref[i]) + " and offset " + std::to_string(offset));
+    top[i] = ref[i];
+    r.crop_offsets[i] = offset;
+  }
+  r.axis = axis;
+  L.set_top(0, top);
+  return true;
+}
+
 bool slice(Layer& L, std::vector<Shape>*) {  // slice_layer.cpp Reshape
   Shape in;
   if (!L.bottom(0, &in)) return false;
@@ -896,7 +933,7 @@ const struct { const char* type; Rule rule; } kRules[] = {
     {"Softmax", same_shape}, {"Power", same_shape}, {"AbsVal", same_shape}, {"BNLL", same_shape}, {"ELU", same_shape},
     {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape}, {"PReLU", prelu},
     {"Split", split}, {"Eltwise", eltwise}, {"Scale", scale}, {"Flatten", flatten}, {"Concat", concat},
-    {"Embed", embed}, {"Reshape", reshape}, {"RNN", rnn}, {"MVN", mvn},
+    {"Embed", embed}, {"Reshape", reshape}, {"RNN", rnn}, {"MVN", mvn}, {"Crop", crop},
     {"SoftmaxWithLoss", softmax_loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
     {"HingeLoss", loss}, {"MultinomialLogisticLoss", loss},
     {"BatchNorm", batch_norm}, {"Slice", slice}, {"ContrastiveLoss", contrastive_loss}, {"Silence", silence},

@@ -82,6 +82,9 @@ struct NetLayer {
   // and a second top with expose_hidden, which the parser lays out and the engine refuses)
   bool expose_hidden = false;
   bool static_input = false;
+  // Crop (crop_layer.cpp): `axis` is the first cropped axis (canonical), and the offset of every axis of bottom[0]
+  // (0 before `axis`)
+  std::vector<int64_t> crop_offsets;
   FillerSpec weight_filler, bias_filler;
   // per param: whether bias_filler fills it rather than weight_filler.  Empty for the layers whose params are a
   // weight and then (with bias_term) a bias.

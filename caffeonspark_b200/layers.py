@@ -1,7 +1,7 @@
 """Native producer layers: autograd Functions and modules over the library's LRN (across and within channels) and fused
 conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10), its
-BatchNorm entry points (csrc/batch_norm.cu, DESIGN.md section 13) and its MVN entry points (csrc/mvn.cu, DESIGN.md
-section 14).
+BatchNorm entry points (csrc/batch_norm.cu, DESIGN.md section 13), its MVN entry points (csrc/mvn.cu, DESIGN.md
+section 14) and its Crop kernels (csrc/native_producer.cu, DESIGN.md section 14).
 
 Activations may be fp32 or bf16 (the mixed-precision producer runs these layers under
 torch.autocast, where the convolutions hand them bf16).  bf16 tensors take the bf16 entry points,
@@ -13,6 +13,8 @@ kernels: a missing library or a failed launch raises.  The modules evaluate CPU 
 PyTorch composition that defines the layer, so a producer module can still be checked on a
 GPU-less host; the autograd Functions themselves take CUDA tensors only.
 """
+import ctypes
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -358,3 +360,27 @@ class ConvReluMaxPool(nn.Module):
         if not z.is_cuda:
             return F.max_pool2d(F.relu(z + c.bias.view(1, -1, 1, 1)), self.kernel, self.stride, ceil_mode=True)
         return BiasReluMaxPoolFunction.apply(z, c.bias, self.kernel, self.stride)
+
+
+def _crop_call(fn, src, dst, bottom_shape, top_shape, offsets):
+    n = len(bottom_shape)
+    if not (src.is_cuda and dst.is_cuda and src.dtype == dst.dtype == torch.float32 and src.is_contiguous() and
+            dst.is_contiguous()) or len(top_shape) != n or len(offsets) != n:
+        raise CosError("Crop takes contiguous fp32 CUDA tensors and one top dim and offset per bottom axis")
+    arr = ctypes.c_longlong * n
+    _call(fn, src.data_ptr(), dst.data_ptr(), n, arr(*bottom_shape), arr(*top_shape), arr(*offsets), _stream())
+    return dst
+
+
+def crop_forward(x, top_shape, offsets, out=None):
+    """Caffe's Crop forward on the native kernel: x[o_0:o_0 + t_0, .., o_n:o_n + t_n] for top_shape t and one offset o
+    per axis of x, copied bit for bit into `out` (a new tensor when None)."""
+    out = torch.empty(tuple(top_shape), dtype=torch.float32, device=x.device) if out is None else out
+    return _crop_call(_lib.lib().cos_crop_forward, x, out, tuple(x.shape), tuple(top_shape), offsets)
+
+
+def crop_backward(dy, bottom_shape, offsets, out=None):
+    """Crop's data gradient on the native kernel: dx of bottom_shape, dy's bits inside the window at `offsets` and +0
+    outside it; every element of `out` (a new tensor when None) is written."""
+    out = torch.empty(tuple(bottom_shape), dtype=torch.float32, device=dy.device) if out is None else out
+    return _crop_call(_lib.lib().cos_crop_backward, dy, out, tuple(bottom_shape), tuple(dy.shape), offsets)

@@ -769,3 +769,61 @@ def rnn_lm_ln_module():
             return self.predict(self.scale(self.ln(o)).flatten(2)), h
 
     return RNNLMLN()
+
+
+# tests/golden/configs/unet_train_test.prototxt: a three-level U-Net over 1 x 92 x 92 images and their per-pixel labels
+# (batch 8): unpadded 3x3 convolutions at 16, 32 and 64 channels, each followed by ReLU, 2/2 MAX pools, 2x2 stride-2
+# up-convolutions (Deconvolution) with ReLU, skips cropped to the up-convolutions' size and concatenated before them,
+# and a 1x1 score convolution to 2 classes at 52 x 52.  116,770 parameters in 26 blobs.
+UNET = dict(input=(1, 92, 92), batch=8, classes=2, score=52)
+UNET_PARAM_COUNT = 116770
+
+
+def crop(x, size, offsets):
+    """Caffe's Crop from axis 2 by slicing: x[:, :, o_h:o_h + h, o_w:o_w + w] for size (h, w), offsets (o_h, o_w)."""
+    return x[:, :, offsets[0]:offsets[0] + size[0], offsets[1]:offsets[1] + size[1]]
+
+
+def unet_module():
+    """The U-Net fixture as one PyTorch module, parameters in learnable_params() order.  forward(images [N, 1, 92, 92])
+    -> scores [N, 2, 52, 52]; crop_label(labels [N, 1, 92, 92]) -> the labels of the scored pixels.  Every ReLU and
+    MAX pool goes through relu() and pool(), so that a caller can fix their branches."""
+    import torch
+    import torch.nn as nn
+    import torch.nn.functional as F
+
+    class UNet(nn.Module):
+        def __init__(self):
+            super().__init__()
+            conv = lambda cin, cout: nn.Conv2d(cin, cout, 3)  # noqa: E731
+            self.conv1a, self.conv1b = conv(1, 16), conv(16, 16)
+            self.conv2a, self.conv2b = conv(16, 32), conv(32, 32)
+            self.conv3a, self.conv3b = conv(32, 64), conv(64, 64)
+            self.upconv2 = nn.ConvTranspose2d(64, 32, 2, stride=2)
+            self.conv4a, self.conv4b = conv(64, 32), conv(32, 32)
+            self.upconv1 = nn.ConvTranspose2d(32, 16, 2, stride=2)
+            self.conv5a, self.conv5b = conv(32, 16), conv(16, 16)
+            self.score = nn.Conv2d(16, 2, 1)
+
+        def relu(self, x):
+            return torch.relu(x)
+
+        def pool(self, x):
+            return F.max_pool2d(x, 2, 2, ceil_mode=True)
+
+        def forward(self, x):
+            r = self.relu
+            d1 = r(self.conv1b(r(self.conv1a(x))))
+            d2 = r(self.conv2b(r(self.conv2a(self.pool(d1)))))
+            d3 = r(self.conv3b(r(self.conv3a(self.pool(d2)))))
+            u2 = r(self.upconv2(d3))
+            h = torch.cat([crop(d2, u2.shape[2:], (4, 4)), u2], 1)
+            u1 = r(self.upconv1(r(self.conv4b(r(self.conv4a(h))))))
+            h = torch.cat([crop(d1, u1.shape[2:], (16, 16)), u1], 1)
+            return self.score(r(self.conv5b(r(self.conv5a(h)))))
+
+        @staticmethod
+        def crop_label(label):
+            return crop(label, (UNET["score"], UNET["score"]), (20, 20))
+
+    return UNet()

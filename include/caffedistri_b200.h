@@ -257,9 +257,10 @@ COS_API int cos_net_set_forward_backward(cos_net* net, cos_forward_backward_fn f
  * 1, dilation 1), Pooling (MAX, AVE), InnerProduct (any axis), ReLU, Sigmoid, BatchNorm, LRN (WITHIN_CHANNEL), Slice,
  * Embed over fp32 token ids (a CoSData INT_ARRAY top), Reshape, RNN (without expose_hidden; its hidden state is kept
  * per engine from call to call, zero at first, and not snapshotted) over time-major CoSData tops (transpose: true),
- * MVN (its top the bottom's legacy 4-D shape; in place it computes the out-of-place result),
- * the other layers DESIGN.md section 14 lists, and one
- * loss layer, SoftmaxWithLoss or ContrastiveLoss among them (default normalisation); Accuracy and Silence are skipped.
+ * MVN (its top the bottom's legacy 4-D shape; in place it computes the out-of-place result), Crop (its reference
+ * bottom only gives a shape, so a per-pixel CoSData label can be cropped to a score map), the other layers DESIGN.md
+ * section 14 lists, and one loss layer, SoftmaxWithLoss or ContrastiveLoss among them (default normalisation);
+ * Accuracy and Silence are skipped.
  * Named params are shared as in Caffe.  Every other layer, and loss_param or an unknown filler type, is refused with an
  * error naming the layer.  Every use of a learnable blob adds its gradient into diff_ once per call; results are
  * bitwise reproducible.
@@ -471,6 +472,16 @@ COS_API int cos_mvn_forward(const float* x, float* y, float* stats, float* works
                             int normalize_variance, float eps, void* cuda_stream);
 COS_API int cos_mvn_backward(const float* y, const float* dy, float* dx, float* stats, float* workspace,
                              long long rows, long long dim, int normalize_variance, void* cuda_stream);
+
+/* Caffe's Crop layer (crop_layer.cpp; DESIGN.md section 14) over contiguous fp32 blobs of `naxes` axes (1 to 32):
+ *   forward   y[i_0, .., i_{n-1}] = x[i_0 + offsets[0], .., i_{n-1} + offsets[n-1]] over top_shape
+ *   backward  dx over bottom_shape: dy at the mapped index inside the window, +0 outside it; every element written
+ * Both are bit-exact copies (NaN payloads, infinities, subnormals and -0 arrive as they are), one launch each.  The
+ * window must lie inside the bottom (else "the window leaves the bottom").  Same launch rules as the calls above. */
+COS_API int cos_crop_forward(const float* x, float* y, int naxes, const long long* bottom_shape,
+                             const long long* top_shape, const long long* offsets, void* cuda_stream);
+COS_API int cos_crop_backward(const float* dy, float* dx, int naxes, const long long* bottom_shape,
+                              const long long* top_shape, const long long* offsets, void* cuda_stream);
 
 /* --------------------- transport object (reference: util/socket.hpp) ------ */
 /* PeerAdapter = SocketAdapter + SocketChannel of the reference
