@@ -137,6 +137,10 @@ SYMBOLS = [
     ("cos_mvn_backward", _i, [_vp, _vp, _vp, _vp, _vp, _c.c_longlong, _c.c_longlong, _i, _vp]),
     ("cos_crop_forward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
     ("cos_crop_backward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    ("cos_conv_workspace_floats", _c.c_longlong, [_i] * 12),
+    ("cos_conv_forward", _i, [_vp, _vp, _vp, _vp] + [_i] * 12 + [_vp]),
+    ("cos_conv_backward_data", _i, [_vp, _vp, _vp] + [_i] * 12 + [_vp]),
+    ("cos_conv_backward_filter", _i, [_vp, _vp, _vp, _vp] + [_i] * 12 + [_vp]),
     ("cos_adapter_create", _vp, [_i, _i]),
     ("cos_adapter_destroy", None, [_vp]),
     ("cos_adapter_address", _cp, [_vp]),

@@ -18,6 +18,7 @@
 #include "caffe_net.hpp"
 #include "caffe_proto_io.hpp"
 #include "hdf5_io.hpp"
+#include "conv_tf32.hpp"
 #include "mvn.hpp"
 #include "native_producer.hpp"
 #include "peer_adapter.hpp"
@@ -767,6 +768,53 @@ int cos_mvn_backward(const float* y, const float* dy, float* dx, float* stats, f
   return launched(cosb::mvn_backward(y, dy, dx, stats, workspace, rows, dim, normalize_variance != 0,
                                      static_cast<cudaStream_t>(cuda_stream)),
                   "cos_mvn_backward");
+}
+
+namespace {
+// -> the convolution's geometry (output plane filled in) or an error message
+const char* conv_args(const void* a, const void* b, const void* c, int n, int ch, int h, int w, int k, int r, int s,
+                      int stride_h, int stride_w, int pad_h, int pad_w, int groups, cosb::ConvGeom* g) {
+  *g = cosb::ConvGeom{n, ch, h, w, k, r, s, stride_h, stride_w, pad_h, pad_w, groups, 0, 0};
+  if (const char* e = cosb::conv_geometry(g)) return e;
+  if (!a || !b || !c) return "NULL tensor";
+  return nullptr;
+}
+}  // namespace
+
+long long cos_conv_workspace_floats(int n, int c, int h, int w, int k, int r, int s, int stride_h, int stride_w,
+                                    int pad_h, int pad_w, int groups) {
+  cosb::ConvGeom g{n, c, h, w, k, r, s, stride_h, stride_w, pad_h, pad_w, groups, 0, 0};
+  return cosb::conv_geometry(&g) ? 0 : static_cast<long long>(cosb::conv_workspace_floats(g));
+}
+
+int cos_conv_forward(const float* x, const float* weight, const float* bias, float* y, int n, int c, int h, int w,
+                     int k, int r, int s, int stride_h, int stride_w, int pad_h, int pad_w, int groups,
+                     void* cuda_stream) {
+  cosb::ConvGeom g;
+  if (const char* e = conv_args(x, weight, y, n, c, h, w, k, r, s, stride_h, stride_w, pad_h, pad_w, groups, &g))
+    return fail(std::string("cos_conv_forward: ") + e);
+  return launched(cosb::conv_forward(x, weight, bias, y, g, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_conv_forward");
+}
+
+int cos_conv_backward_data(const float* dy, const float* weight, float* dx, int n, int c, int h, int w, int k, int r,
+                           int s, int stride_h, int stride_w, int pad_h, int pad_w, int groups, void* cuda_stream) {
+  cosb::ConvGeom g;
+  if (const char* e = conv_args(dy, weight, dx, n, c, h, w, k, r, s, stride_h, stride_w, pad_h, pad_w, groups, &g))
+    return fail(std::string("cos_conv_backward_data: ") + e);
+  return launched(cosb::conv_backward_data(dy, weight, dx, g, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_conv_backward_data");
+}
+
+int cos_conv_backward_filter(const float* x, const float* dy, float* dweight, float* workspace, int n, int c, int h,
+                             int w, int k, int r, int s, int stride_h, int stride_w, int pad_h, int pad_w, int groups,
+                             void* cuda_stream) {
+  cosb::ConvGeom g;
+  if (const char* e = conv_args(x, dy, dweight, n, c, h, w, k, r, s, stride_h, stride_w, pad_h, pad_w, groups, &g))
+    return fail(std::string("cos_conv_backward_filter: ") + e);
+  if (!workspace && cosb::conv_workspace_floats(g) > 0) return fail("cos_conv_backward_filter: NULL workspace");
+  return launched(cosb::conv_backward_filter(x, dy, dweight, workspace, g, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_conv_backward_filter");
 }
 
 namespace {

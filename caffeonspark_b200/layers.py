@@ -1,7 +1,8 @@
 """Native producer layers: autograd Functions and modules over the library's LRN (across and within channels) and fused
 conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10), its
 BatchNorm entry points (csrc/batch_norm.cu, DESIGN.md section 13), its MVN entry points (csrc/mvn.cu, DESIGN.md
-section 14) and its Crop kernels (csrc/native_producer.cu, DESIGN.md section 14).
+section 14), its Crop kernels (csrc/native_producer.cu, DESIGN.md section 14) and its TF32 convolutions
+(csrc/conv_tf32.cu, DESIGN.md section 10.2).
 
 Activations may be fp32 or bf16 (the mixed-precision producer runs these layers under
 torch.autocast, where the convolutions hand them bf16).  bf16 tensors take the bf16 entry points,
@@ -345,6 +346,84 @@ class BatchNorm(nn.Module):
         return BatchNormFunction.apply(x, self.mean, self.variance, self.scale_factor, *hyper)
 
 
+def _conv_geometry(x, weight, stride, padding, groups):
+    n, c, h, w = x.shape
+    k, _, r, s = weight.shape
+    return (n, c, h, w, k, r, s, stride[0], stride[1], padding[0], padding[1], groups)
+
+
+class ConvFunction(torch.autograd.Function):
+    """A convolution on the native TF32 implicit-GEMM kernels (csrc/conv_tf32.cu): fp32 CUDA tensors, NCHW in and
+    out.  The data gradient is skipped when x needs none (a net's first layer)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, stride, padding, groups):
+        x, weight = x.contiguous(), weight.contiguous()
+        geom = _conv_geometry(x, weight, stride, padding, groups)
+        n, _, h, w, k, r, s, sh, sw, ph, pw, _ = geom
+        y = torch.empty((n, k, (h + 2 * ph - r) // sh + 1, (w + 2 * pw - s) // sw + 1), dtype=x.dtype, device=x.device)
+        _call(_lib.lib().cos_conv_forward, x.data_ptr(), weight.data_ptr(),
+              None if bias is None else bias.contiguous().data_ptr(), y.data_ptr(), *geom, _stream())
+        ctx.save_for_backward(x, weight)
+        ctx.geom, ctx.has_bias = geom, bias is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight = ctx.saved_tensors
+        dy, geom = dy.contiguous(), ctx.geom
+        dx = dw = db = None
+        L = _lib.lib()
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty_like(x)
+            _call(L.cos_conv_backward_data, dy.data_ptr(), weight.data_ptr(), dx.data_ptr(), *geom, _stream())
+        if ctx.needs_input_grad[1]:
+            dw = torch.empty_like(weight)
+            work = torch.empty(max(1, L.cos_conv_workspace_floats(*geom)), dtype=torch.float32, device=x.device)
+            _call(L.cos_conv_backward_filter, x.data_ptr(), dy.data_ptr(), dw.data_ptr(), work.data_ptr(), *geom,
+                  _stream())
+        if ctx.has_bias and ctx.needs_input_grad[2]:
+            db = dy.sum((0, 2, 3))
+        return dx, dw, db, None, None, None
+
+
+# The geometry where the native kernels beat cuDNN (DESIGN.md section 10.2): few input channels per group, where
+# cuDNN's channels-last kernels are poorly filled, and a reduction long enough to fill the k-tiles.  At CaffeNet
+# conv1 (3 channels, 363 taps) the native calls take half of cuDNN's forward time and three quarters of its
+# weight-gradient time.  From 48 channels up (CaffeNet conv2 to conv5) cuDNN is 1.4 to 5 times faster than this
+# mma.sync mainloop, and CIFAR-10-quick (conv1: 3 channels, 75 taps) trained 9 % slower with its conv1 native.
+NATIVE_CONV_MAX_GROUP_CHANNELS = 4
+NATIVE_CONV_MIN_TAPS = 128
+
+
+def native_conv(x, weight):
+    """Whether conv2d runs on the native TF32 kernels: where cuDNN would run TF32 anyway (fp32 CUDA tensors, autocast
+    off, torch.backends.cudnn.allow_tf32 set) and the geometry is one where they are faster (few input channels per
+    group, many taps)."""
+    return (x.is_cuda and x.dtype == torch.float32 and weight.dtype == torch.float32 and x.dim() == 4 and
+            not torch.is_autocast_enabled("cuda") and torch.backends.cudnn.allow_tf32 and
+            weight.dim() == 4 and weight.shape[1] <= NATIVE_CONV_MAX_GROUP_CHANNELS and
+            weight.shape[1] * weight.shape[2] * weight.shape[3] >= NATIVE_CONV_MIN_TAPS)
+
+
+def conv2d(x, weight, bias=None, stride=(1, 1), padding=(0, 0), dilation=(1, 1), groups=1):
+    """F.conv2d with int pairs for stride, padding and dilation, on the native kernels where native_conv() holds
+    (and the dilation is 1)."""
+    if native_conv(x, weight) and tuple(dilation) == (1, 1):
+        return ConvFunction.apply(x, weight, bias, tuple(stride), tuple(padding), groups)
+    return F.conv2d(x, weight, bias, stride, padding, dilation, groups)
+
+
+class Conv2d(nn.Conv2d):
+    """nn.Conv2d (same parameters, initialisation and type name) whose zero-padded convolution runs through
+    conv2d() above."""
+
+    def forward(self, x):
+        if self.padding_mode != "zeros" or isinstance(self.padding, str):
+            return super().forward(x)
+        return conv2d(x, self.weight, self.bias, self.stride, self.padding, self.dilation, self.groups)
+
+
 class ConvReluMaxPool(nn.Module):
     """conv -> ReLU -> MAX pool (or conv -> MAX pool -> ReLU, the same function).  `conv` holds the weight and the
     bias; the convolution runs without bias and the native block adds it."""
@@ -356,7 +435,7 @@ class ConvReluMaxPool(nn.Module):
 
     def forward(self, x):
         c = self.conv
-        z = F.conv2d(x, c.weight, None, c.stride, c.padding, c.dilation, c.groups)
+        z = conv2d(x, c.weight, None, c.stride, c.padding, c.dilation, c.groups)
         if not z.is_cuda:
             return F.max_pool2d(F.relu(z + c.bias.view(1, -1, 1, 1)), self.kernel, self.stride, ceil_mode=True)
         return BiasReluMaxPoolFunction.apply(z, c.bias, self.kernel, self.stride)

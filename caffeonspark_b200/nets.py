@@ -251,7 +251,7 @@ def torch_module(name):
 
 def _sequential(net):
     import torch.nn as nn
-    from .layers import LRN, BatchNorm, ConvReluMaxPool
+    from .layers import LRN, BatchNorm, Conv2d, ConvReluMaxPool
     c, h, w = net["input"]
     layers = net["layers"]
     mods, flat, skip = [], None, 0
@@ -262,7 +262,7 @@ def _sequential(net):
         kind = L[0]
         if kind == "conv":
             _, _, cout, k, s, p, g, _, pb = L
-            conv = nn.Conv2d(c, cout, k, stride=s, padding=p, groups=g, bias=pb is not None)
+            conv = Conv2d(c, cout, k, stride=s, padding=p, groups=g, bias=pb is not None)
             h, w, c = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1, cout
             pool = _relu_maxpool_after(layers, i) if pb is not None else None
             if pool is None:

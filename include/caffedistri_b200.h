@@ -483,6 +483,26 @@ COS_API int cos_crop_forward(const float* x, float* y, int naxes, const long lon
 COS_API int cos_crop_backward(const float* dy, float* dx, int naxes, const long long* bottom_shape,
                               const long long* top_shape, const long long* offsets, void* cuda_stream);
 
+/* Convolution on TF32 tensor cores (DESIGN.md section 10.2): x [n, c, h, w], w [k, c / groups, r, s] and
+ * y [n, k, p, q] contiguous fp32 NCHW, p = (h + 2 pad_h - r) / stride_h + 1, q likewise; any geometry whose tensors
+ * have fewer than 2^31 elements.  Every operand is rounded to TF32 (cvt.rna) and the products are summed in fp32, in
+ * an order fixed by the shape: repeated calls give the same bits.
+ *   forward          y = conv(x, w) (+ bias[k] when bias is not NULL)
+ *   backward_data    dx from dy and w (any stride)
+ *   backward_filter  dw from x and dy; workspace is cos_conv_workspace_floats(...) floats (NULL when that is 0)
+ * Same launch rules as the calls above. */
+COS_API long long cos_conv_workspace_floats(int n, int c, int h, int w, int k, int r, int s, int stride_h,
+                                            int stride_w, int pad_h, int pad_w, int groups);
+COS_API int cos_conv_forward(const float* x, const float* weight, const float* bias, float* y, int n, int c, int h,
+                             int w, int k, int r, int s, int stride_h, int stride_w, int pad_h, int pad_w, int groups,
+                             void* cuda_stream);
+COS_API int cos_conv_backward_data(const float* dy, const float* weight, float* dx, int n, int c, int h, int w, int k,
+                                   int r, int s, int stride_h, int stride_w, int pad_h, int pad_w, int groups,
+                                   void* cuda_stream);
+COS_API int cos_conv_backward_filter(const float* x, const float* dy, float* dweight, float* workspace, int n, int c,
+                                     int h, int w, int k, int r, int s, int stride_h, int stride_w, int pad_h,
+                                     int pad_w, int groups, void* cuda_stream);
+
 /* --------------------- transport object (reference: util/socket.hpp) ------ */
 /* PeerAdapter = SocketAdapter + SocketChannel of the reference
  * (socket.hpp:22-89): a listener thread on a per-process endpoint whose
