@@ -847,6 +847,22 @@ int cos_crop_backward(const float* dy, float* dx, int naxes, const long long* bo
                   "cos_crop_backward");
 }
 
+int cos_spp_forward(const float* x, float* y, int* argmax, int num, int channels, int height, int width,
+                    int pyramid_height, int max_pool, void* cuda_stream) {
+  if (!x || !y || (max_pool && !argmax)) return fail("NULL tensor");
+  return launched(cosb::spp_forward(x, y, argmax, num, channels, height, width, pyramid_height, max_pool != 0,
+                                    static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_spp_forward");
+}
+
+int cos_spp_backward(const float* dy, const int* argmax, float* dx, int num, int channels, int height, int width,
+                     int pyramid_height, int max_pool, void* cuda_stream) {
+  if (!dy || !dx || (max_pool && !argmax)) return fail("NULL tensor");
+  return launched(cosb::spp_backward(dy, argmax, dx, num, channels, height, width, pyramid_height, max_pool != 0,
+                                     static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_spp_backward");
+}
+
 int cos_batch_norm_forward_bf16(const uint16_t* x, uint16_t* y, float* mean_blob, float* var_blob, float* scale_blob,
                                 float* save, float* workspace, int num, int channels, int height, int width,
                                 int use_global_stats, float moving_average_fraction, float eps, void* cuda_stream) {

@@ -139,6 +139,7 @@ const LayerType kLayerTypes[] = {
     {"MVN", OpKind::kMVN},
     // the reference gives only its shape: it is never read, so it may also feed a Concat or a loss without a Split
     {"Crop", OpKind::kCrop, 2, false, 1, "ref"},
+    {"SPP", OpKind::kSPP},
 };
 
 // Plan::text's name of each OpKind
@@ -147,7 +148,7 @@ const char* const kKindNames[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling
                                   "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale", "Deconvolution", "Flatten",
                                   "SigmoidCrossEntropyLoss", "TanH", "ELU", "AbsVal", "BNLL", "Power", "Exp", "Log",
                                   "Threshold", "PReLU", "Softmax", "MultinomialLogisticLoss", "HingeLoss",
-                                  "Embed", "Reshape", "RNN", "MVN", "Crop"};
+                                  "Embed", "Reshape", "RNN", "MVN", "Crop", "SPP"};
 static_assert(std::size(kKindNames) == static_cast<size_t>(OpKind::kCount), "one name per OpKind");
 
 // LossLayer::Reshape's check, then multinomial_logistic_loss_layer.cpp's: the label holds one value per item, with
@@ -568,6 +569,22 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       }
       op.crop_axis = static_cast<int>(L.axis);
       op.crop_offsets = L.crop_offsets;
+    } else if (op.kind == OpKind::kSPP) {  // spp_layer.cpp; the parser checked every level.  The top owns its storage
+      if (L.pool != "MAX" && L.pool != "AVE") {
+        *err = why(L, "pool method " + L.pool + " is not supported (MAX and AVE are)");
+        return false;
+      }
+      if (L.tops[0] == L.bottoms[0]) {
+        *err = why(L, L.type + " Layer does not allow in-place computation.");
+        return false;
+      }
+      if (L.pyramid_height > kSppMaxLevels) {
+        *err = why(L, "pyramid_height " + std::to_string(L.pyramid_height) + " is more than the " +
+                          std::to_string(kSppMaxLevels) + " levels the engine supports");
+        return false;
+      }
+      op.max_pool = L.pool == "MAX";
+      op.spp_levels = static_cast<int>(L.pyramid_height);
     } else if (op.kind == OpKind::kBatchNorm) {
       if (!op.shares.empty()) {
         *err = why(L, "shared BatchNorm statistics are not supported");
@@ -708,7 +725,7 @@ std::string Plan::text() const {
   for (size_t i = 0; i < ops.size(); ++i) {
     const Op& op = ops[i];
     os << "op " << i << " " << kKindNames[static_cast<int>(op.kind)];
-    if (op.kind == OpKind::kPool) os << "(" << (op.max_pool ? "MAX" : "AVE") << ")";
+    if (op.kind == OpKind::kPool || op.kind == OpKind::kSPP) os << "(" << (op.max_pool ? "MAX" : "AVE") << ")";
     if (op.kind == OpKind::kEltwise) os << "(" << eltwise_ops[op.eltwise_op] << ")";
     os << " " << op.name << " " << shape_text(op.in_shape) << " -> " << shape_text(op.out_shape);
     if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kPool ||
@@ -729,6 +746,11 @@ std::string Plan::text() const {
       os << " rows=" << op.mvn_rows << " dim=" << op.mvn_dim << " eps=" << op.eps;
       if (op.across_channels) os << " across";
       if (!op.normalize_variance) os << " mean-only";
+    }
+    for (int l = 0; op.kind == OpKind::kSPP && l < op.spp_levels; ++l) {
+      const SppLevel v = spp_level(op.in_shape[2], op.in_shape[3], l);
+      os << " level" << l << " " << v.bins << "x" << v.bins << " k" << v.kernel_h << "x" << v.kernel_w << " p"
+         << v.pad_h << "x" << v.pad_w;
     }
     if (op.kind == OpKind::kCrop) {
       os << " axis=" << op.crop_axis << " offsets=";

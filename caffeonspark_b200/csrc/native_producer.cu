@@ -282,23 +282,43 @@ struct PoolGeom {
   int N, C, H, W, PH, PW, KH, KW, SH, SW, PADH, PADW;
 };
 
+// Output (ph, pw)'s window: rows [*hs, *he) and columns [*ws, *we) of the plane, the padding clipped off
+__device__ __forceinline__ void pool_window(int ph, int pw, const PoolGeom& g, int* hs, int* he, int* ws, int* we) {
+  *hs = ph * g.SH - g.PADH, *ws = pw * g.SW - g.PADW;
+  *he = min(*hs + g.KH, g.H), *we = min(*ws + g.KW, g.W);
+  *hs = max(*hs, 0), *ws = max(*ws, 0);
+}
+
+// MAX over a window in (h, w) order from -FLT_MAX: the first value > the running maximum wins, so NaN never does, and
+// *mi is -1 when no value is > -FLT_MAX
+__device__ __forceinline__ float window_max(const float* plane, int W, int hs, int he, int ws, int we, int* mi) {
+  float m = -FLT_MAX;
+  *mi = -1;
+  for (int h = hs; h < he; ++h)
+    for (int w = ws; w < we; ++w)
+      if (plane[h * W + w] > m) {  // the first maximum wins
+        *mi = h * W + w;
+        m = plane[*mi];
+      }
+  return m;
+}
+
+// AVE's sum over a window: row-major, one rounding per add, from +0
+__device__ __forceinline__ float window_sum(const float* plane, int W, int hs, int he, int ws, int we) {
+  float s = 0.f;
+  for (int h = hs; h < he; ++h)
+    for (int w = ws; w < we; ++w) s = __fadd_rn(s, plane[h * W + w]);
+  return s;
+}
+
 __global__ void max_pool_forward_kernel(const float* x, float* y, int* idx, PoolGeom g) {
   const int total = g.N * g.C * g.PH * g.PW;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int pw = i % g.PW, ph = (i / g.PW) % g.PH, nc = i / (g.PW * g.PH);
-    int hs = ph * g.SH - g.PADH, ws = pw * g.SW - g.PADW;
-    const int he = min(hs + g.KH, g.H), we = min(ws + g.KW, g.W);
-    hs = max(hs, 0), ws = max(ws, 0);
-    const float* plane = x + (size_t)nc * g.H * g.W;
-    float m = -FLT_MAX;
-    int mi = -1;
-    for (int h = hs; h < he; ++h)
-      for (int w = ws; w < we; ++w)
-        if (plane[h * g.W + w] > m) {  // the first maximum wins
-          mi = h * g.W + w;
-          m = plane[mi];
-        }
-    y[i] = m;
+    int hs, he, ws, we;
+    pool_window(ph, pw, g, &hs, &he, &ws, &we);
+    int mi;
+    y[i] = window_max(x + (size_t)nc * g.H * g.W, g.W, hs, he, ws, we, &mi);
     idx[i] = mi;
   }
 }
@@ -332,15 +352,10 @@ __global__ void ave_pool_forward_kernel(const float* x, float* y, PoolGeom g) {
   const int total = g.N * g.C * g.PH * g.PW;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int pw = i % g.PW, ph = (i / g.PW) % g.PH, nc = i / (g.PW * g.PH);
-    const int size = ave_pool_size(ph, pw, g);
-    int hs = ph * g.SH - g.PADH, ws = pw * g.SW - g.PADW;
-    const int he = min(hs + g.KH, g.H), we = min(ws + g.KW, g.W);
-    hs = max(hs, 0), ws = max(ws, 0);
-    const float* plane = x + (size_t)nc * g.H * g.W;
-    float s = 0.f;
-    for (int h = hs; h < he; ++h)
-      for (int w = ws; w < we; ++w) s = __fadd_rn(s, plane[h * g.W + w]);
-    y[i] = __fdiv_rn(s, static_cast<float>(size));
+    int hs, he, ws, we;
+    pool_window(ph, pw, g, &hs, &he, &ws, &we);
+    y[i] = __fdiv_rn(window_sum(x + (size_t)nc * g.H * g.W, g.W, hs, he, ws, we),
+                     static_cast<float>(ave_pool_size(ph, pw, g)));
   }
 }
 
@@ -355,6 +370,69 @@ __global__ void ave_pool_backward_kernel(const float* dy, float* dx, PoolGeom g)
     for (int ph = phs; ph < phe; ++ph)
       for (int pw = pws; pw < pwe; ++pw)
         s = __fadd_rn(s, __fdiv_rn(dy[o + ph * g.PW + pw], static_cast<float>(ave_pool_size(ph, pw, g))));
+    dx[i] = s;
+  }
+}
+
+// ------------------------------------------------------------------ SPP (spp_layer.cpp)
+// The pyramid over one [N, C, H, W] bottom: level l pools bins = 2^l windows per side with kernel kh[l] x kw[l], stride
+// equal to the kernel and pad padh[l] x padw[l] (spp_level); the top holds per_sample = C * sum of 4^l values per
+// sample, level l's from C * (4^l - 1) / 3 on, ordered (c, ph, pw): the Concat of each level's Flatten.
+struct SppGeom {
+  int N, C, H, W, levels, per_sample;
+  int kh[kSppMaxLevels], kw[kSppMaxLevels], padh[kSppMaxLevels], padw[kSppMaxLevels];
+};
+
+// Level l as the Pooling layer Caffe's SPP builds for it
+__device__ __forceinline__ PoolGeom spp_pool_geom(const SppGeom& g, int l) {
+  return PoolGeom{g.N, g.C, g.H, g.W, 1 << l, 1 << l, g.kh[l], g.kw[l], g.kh[l], g.kw[l], g.padh[l], g.padw[l]};
+}
+
+// Forward: one thread per top element over every level, written straight to its place in the top (no Split, per-level
+// buffer or Concat copy), with the pooling kernels' window arithmetic: MAX's first maximum and argmax, or AVE's
+// row-major sum over the clipped window divided by ave_pool_size.
+__global__ void spp_forward_kernel(const float* __restrict__ x, float* __restrict__ y, int* __restrict__ idx,
+                                   SppGeom g, bool max_pool) {
+  const int total = g.N * g.per_sample;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int n = i / g.per_sample;
+    int r = i - n * g.per_sample, l = 0;
+    while (r >= (g.C << (2 * l))) r -= g.C << (2 * l), ++l;  // level l holds C * 4^l values
+    const int bins = 1 << l, pw = r % bins, ph = (r / bins) % bins, c = r / (bins * bins);
+    const PoolGeom pg = spp_pool_geom(g, l);
+    int hs, he, ws, we;
+    pool_window(ph, pw, pg, &hs, &he, &ws, &we);
+    const float* plane = x + ((size_t)n * g.C + c) * g.H * g.W;
+    if (max_pool) {
+      int mi;
+      y[i] = window_max(plane, g.W, hs, he, ws, we, &mi);
+      idx[i] = mi;
+    } else {
+      y[i] = __fdiv_rn(window_sum(plane, g.W, hs, he, ws, we), static_cast<float>(ave_pool_size(ph, pw, pg)));
+    }
+  }
+}
+
+// Backward: one thread per bottom element, each written once.  Stride equals kernel, so the element lies in one window
+// per level; that level's term is what its Pooling backward writes there (0 + dy for MAX's argmax, else +0; 0 + dy /
+// size for AVE), and the terms are added in level order, ((g0 + g1) + g2) + .., as Split's backward sums its tops.
+__global__ void spp_backward_kernel(const float* __restrict__ dy, const int* __restrict__ idx, float* __restrict__ dx,
+                                    SppGeom g, bool max_pool) {
+  const int total = g.N * g.C * g.H * g.W;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int w = i % g.W, h = (i / g.W) % g.H, nc = i / (g.W * g.H), n = nc / g.C, c = nc - n * g.C;
+    size_t level = (size_t)n * g.per_sample;  // where level l starts in the top
+    float s = 0.f;
+    for (int l = 0; l < g.levels; ++l) {
+      const PoolGeom pg = spp_pool_geom(g, l);
+      const int ph = (h + pg.PADH) / pg.KH, pw = (w + pg.PADW) / pg.KW;
+      const size_t o = level + ((size_t)c * pg.PH + ph) * pg.PW + pw;
+      float t = 0.f;
+      if (!max_pool) t = __fadd_rn(0.f, __fdiv_rn(dy[o], static_cast<float>(ave_pool_size(ph, pw, pg))));
+      else if (idx[o] == h * g.W + w) t = __fadd_rn(0.f, dy[o]);
+      s = l == 0 ? t : __fadd_rn(s, t);
+      level += (size_t)g.C << (2 * l);
+    }
     dx[i] = s;
   }
 }
@@ -1255,6 +1333,46 @@ cudaError_t crop_backward(const float* dy, float* dx, const std::vector<int64_t>
   return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------ SPP's launches
+namespace {
+// The pyramid of spp_level() over a num x channels x height x width bottom; false for one the kernels do not take
+bool spp_geom(int num, int channels, int height, int width, int levels, SppGeom* g) {
+  if (num < 1 || channels < 1 || height < 1 || width < 1 || levels < 1 || levels > kSppMaxLevels) return false;
+  *g = SppGeom{num, channels, height, width, levels, 0, {}, {}, {}, {}};
+  int64_t per_sample = 0;
+  for (int l = 0; l < levels; ++l) {
+    const SppLevel v = spp_level(height, width, l);
+    // pad < kernel (the parser's check) puts every window's start inside the map, so each level pools bins x bins
+    if (v.pad_h >= v.kernel_h || v.pad_w >= v.kernel_w) return false;
+    g->kh[l] = static_cast<int>(v.kernel_h), g->kw[l] = static_cast<int>(v.kernel_w);
+    g->padh[l] = static_cast<int>(v.pad_h), g->padw[l] = static_cast<int>(v.pad_w);
+    per_sample += static_cast<int64_t>(channels) * v.bins * v.bins;
+  }
+  const int64_t limit = int64_t(1) << 31;
+  if (per_sample * num >= limit || static_cast<int64_t>(num) * channels * height * width >= limit) return false;
+  g->per_sample = static_cast<int>(per_sample);
+  return true;
+}
+}  // namespace
+
+cudaError_t spp_forward(const float* x, float* y, int* argmax, int num, int channels, int height, int width, int levels,
+                        bool max_pool, cudaStream_t s) {
+  SppGeom g;
+  if (!spp_geom(num, channels, height, width, levels, &g) || (max_pool && !argmax)) return cudaErrorInvalidValue;
+  const int n = g.N * g.per_sample;
+  spp_forward_kernel<<<grid_for(n), kThreads, 0, s>>>(x, y, argmax, g, max_pool);
+  return cudaGetLastError();
+}
+
+cudaError_t spp_backward(const float* dy, const int* argmax, float* dx, int num, int channels, int height, int width,
+                         int levels, bool max_pool, cudaStream_t s) {
+  SppGeom g;
+  if (!spp_geom(num, channels, height, width, levels, &g) || (max_pool && !argmax)) return cudaErrorInvalidValue;
+  const int n = num * channels * height * width;
+  spp_backward_kernel<<<grid_for(n), kThreads, 0, s>>>(dy, argmax, dx, g, max_pool);
+  return cudaGetLastError();
+}
+
 // ------------------------------------------------------------------ engine
 
 NativeProducer* NativeProducer::create(const Plan& plan, int device, float* data, float* diff, int* status,
@@ -1349,7 +1467,7 @@ bool NativeProducer::allocate(std::string* err) {
         op_z_[i] = static_cast<float*>(z), op_dz_[i] = static_cast<float*>(dz), op_aux_[i] = idx;
         ws = std::max(ws, static_cast<size_t>(d.N + 1) * d.Cout);  // bias partials + dbias
       }
-    } else if ((op.kind == OpKind::kPool && op.max_pool) ||
+    } else if (((op.kind == OpKind::kPool || op.kind == OpKind::kSPP) && op.max_pool) ||
                (op.kind == OpKind::kEltwise && op.eltwise_op == kEltwiseMax)) {
       if (!alloc(out * sizeof(int), &op_aux_[i])) return false;
     } else if (op.kind == OpKind::kInnerProduct) {
@@ -1542,6 +1660,10 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
     }
     case OpKind::kCrop:
       return crop_forward(x, y, op.in_shape, op.out_shape, op.crop_offsets, s);
+    case OpKind::kSPP:
+      return spp_forward(x, y, static_cast<int*>(op_aux_[i]), static_cast<int>(op.in_shape[0]),
+                         static_cast<int>(op.in_shape[1]), static_cast<int>(op.in_shape[2]),
+                         static_cast<int>(op.in_shape[3]), op.spp_levels, op.max_pool, s);
     case OpKind::kDeconv:  // the data gradient of the convolution from top to bottom, with the bias in its store
       return conv_data_grad(op, conv_dims(op), x, data_ + op.w_off, op.b_off >= 0 ? data_ + op.b_off : nullptr, y, s);
     case OpKind::kSplit:  // no copy: the top reads the bottom's memory
@@ -1786,6 +1908,11 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
       return cudaGetLastError();
     case OpKind::kCrop:  // writes every element of dx: the engine's data gradients are written, not accumulated
       return dx ? crop_backward(dy, dx, op.in_shape, op.out_shape, op.crop_offsets, s) : cudaSuccess;
+    case OpKind::kSPP:  // writes every element of dx
+      if (!dx) return cudaSuccess;
+      return spp_backward(dy, static_cast<const int*>(op_aux_[i]), dx, static_cast<int>(op.in_shape[0]),
+                          static_cast<int>(op.in_shape[1]), static_cast<int>(op.in_shape[2]),
+                          static_cast<int>(op.in_shape[3]), op.spp_levels, op.max_pool, s);
     case OpKind::kSplit: {  // top 0's op: dx = the read tops' gradients summed in top order; the other tops' do nothing
       if (!dx || op.split_top != 0) return cudaSuccess;
       const std::vector<int>& g = op.split_sum;

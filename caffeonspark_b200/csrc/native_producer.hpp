@@ -2,8 +2,8 @@
 // CIFAR-10-quick, CIFAR-10-full, CIFAR-10-full-BN and siamese MNIST family of nets, least-squares regression nets,
 // residual nets built of Split, Eltwise and Scale, autoencoders built of Flatten, Deconvolution and
 // SigmoidCrossEntropyLoss, embedding nets that read token ids through Embed and Reshape, recurrent nets built of
-// RNN layers over time-major inputs, nets normalised by MVN, and U-Net segmentation nets that Crop their skips and
-// per-pixel labels; DESIGN.md section 14).
+// RNN layers over time-major inputs, nets normalised by MVN, U-Net segmentation nets that Crop their skips and
+// per-pixel labels, and nets with a spatial-pyramid-pooling (SPP) head; DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -29,7 +29,7 @@ enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
   kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale, kDeconv, kFlatten, kSigmoidCrossEntropyLoss,
   kTanH, kELU, kAbsVal, kBNLL, kPower, kExp, kLog, kThreshold, kPReLU, kSoftmax, kMultinomialLogisticLoss, kHingeLoss,
-  kEmbed, kReshape, kRNN, kMVN, kCrop,
+  kEmbed, kReshape, kRNN, kMVN, kCrop, kSPP,
   kCount  // the number of kinds (Plan::text names each)
 };
 
@@ -116,6 +116,9 @@ struct Op {
   // crop_axis); bottoms[1] gives only its shape and is never read
   int crop_axis = 0;
   std::vector<int64_t> crop_offsets;
+  // SPP: spp_levels pyramid levels over in_shape's H x W (spp_level() gives each one's geometry), MAX or AVE by
+  // max_pool; the top holds every level's bins, level after level within each sample
+  int spp_levels = 0;
 };
 
 struct Plan {
@@ -161,6 +164,18 @@ cudaError_t crop_forward(const float* x, float* y, const std::vector<int64_t>& b
                          const std::vector<int64_t>& top_shape, const std::vector<int64_t>& offsets, cudaStream_t s);
 cudaError_t crop_backward(const float* dy, float* dx, const std::vector<int64_t>& bottom_shape,
                           const std::vector<int64_t>& top_shape, const std::vector<int64_t>& offsets, cudaStream_t s);
+// SPP's kernels (native_producer.cu) take at most this many pyramid levels: a 17th would give even one channel more
+// than the 2^31 elements a blob of the engine may hold
+constexpr int kSppMaxLevels = 16;
+// SPP's kernels: spp_layer.cpp's Split, `levels` Poolings (MAX or AVE, spp_level()'s geometry), Flattens and Concat as
+// one launch per direction over a contiguous [num, channels, height, width] bottom.  The forward writes y, [num,
+// channels * sum of 4^l], and with MAX one int32 argmax per output (-1 for a window with no value > -FLT_MAX); the
+// backward writes every element of dx once, each level's term added in level order.  cudaErrorInvalidValue for a
+// geometry the kernels do not take (no level, more than kSppMaxLevels, a level whose pad is not below its kernel).
+cudaError_t spp_forward(const float* x, float* y, int* argmax, int num, int channels, int height, int width, int levels,
+                        bool max_pool, cudaStream_t s);
+cudaError_t spp_backward(const float* dy, const int* argmax, float* dx, int num, int channels, int height, int width,
+                         int levels, bool max_pool, cudaStream_t s);
 // The GEMM core puts its M rows on gridDim.y in tiles of 64, so one GEMM has at most this many rows: an InnerProduct's
 // rows or num_output, a convolution's input or output channels, an RNN's T * N or num_output
 constexpr int64_t kMaxGemmRows = 65535 * 64;
@@ -192,7 +207,8 @@ class NativeProducer {
   float* diff_;
   int* status_;
   std::vector<float*> act_, grad_;        // per tensor id (staged inputs: act_ is the caller's buffer, set per call)
-  std::vector<void*> op_aux_;             // per op: MAX pool / Eltwise MAX argmax (int32), fused block index (uint8),
+  std::vector<void*> op_aux_;             // per op: MAX pool, SPP and Eltwise MAX argmax (int32), fused block index
+                                          // (uint8),
                                           // BN save, MVN's per-row statistics (mvn.hpp)
   std::vector<float*> op_z_, op_dz_;      // fused block: conv output without bias and its gradient
   // per op, an RNN's buffers (null for other ops), all [rows, H] with rows as named: g = x W_xh^T + b_h (T N), z =

@@ -82,6 +82,16 @@ std::string shape_text(const std::vector<int64_t>& s) {
   return s.empty() ? "scalar" : t;
 }
 
+SppLevel spp_level(int64_t height, int64_t width, int level) {
+  SppLevel v;
+  v.bins = int64_t(1) << level;
+  v.kernel_h = (height + v.bins - 1) / v.bins;  // ceil(bottom_h / double(num_bins)) for positive sizes
+  v.kernel_w = (width + v.bins - 1) / v.bins;
+  v.pad_h = (v.kernel_h * v.bins - height + 1) / 2;
+  v.pad_w = (v.kernel_w * v.bins - width + 1) / 2;
+  return v;
+}
+
 namespace {
 
 typedef std::vector<int64_t> Shape;
@@ -433,6 +443,25 @@ bool convolution(Layer& L, std::vector<Shape>* params) {  // and Deconvolution; 
   return true;
 }
 
+// pooling_layer.cpp's pad < kernel CHECKs (LayerSetUp), with `at` after their wording, and its pooled size (Reshape)
+bool pooled(const Layer& L, HW in, HW k, HW st, HW pad, const std::string& at, HW* out) {
+  // a window that lay entirely in the padding would pool nothing
+  if (pad.h >= k.h)
+    return L.refuse("Check failed: pad_h_ < kernel_h_ (" + std::to_string(pad.h) + " vs. " + std::to_string(k.h) + ")" +
+                    at);
+  if (pad.w >= k.w)
+    return L.refuse("Check failed: pad_w_ < kernel_w_ (" + std::to_string(pad.w) + " vs. " + std::to_string(k.w) + ")" +
+                    at);
+  // ceil((H + 2p - k) / s) + 1, clipped so the last window starts inside
+  out->h = static_cast<int64_t>(ceil(static_cast<float>(in.h + 2 * pad.h - k.h) / st.h)) + 1;
+  out->w = static_cast<int64_t>(ceil(static_cast<float>(in.w + 2 * pad.w - k.w) / st.w)) + 1;
+  if (pad.h || pad.w) {
+    if ((out->h - 1) * st.h >= in.h + pad.h) --out->h;
+    if ((out->w - 1) * st.w >= in.w + pad.w) --out->w;
+  }
+  return true;
+}
+
 bool pooling(Layer& L, std::vector<Shape>*) {
   const Node* p = L.node.first("pooling_param");
   Shape in;
@@ -448,22 +477,39 @@ bool pooling(Layer& L, std::vector<Shape>*) {
   if (k.h <= 0 || k.w <= 0 || st.h <= 0 || st.w <= 0 || pad.h < 0 || pad.w < 0) return L.bad("pooling_param");
   if (global && (pad.h || pad.w || st.h != 1 || st.w != 1))
     return L.refuse("With Global_pooling: true; only pad = 0 and stride = 1");
-  // a window that lay entirely in the padding would pool nothing
-  if (pad.h >= k.h)
-    return L.refuse("Check failed: pad_h_ < kernel_h_ (" + std::to_string(pad.h) + " vs. " + std::to_string(k.h) + ")");
-  if (pad.w >= k.w)
-    return L.refuse("Check failed: pad_w_ < kernel_w_ (" + std::to_string(pad.w) + " vs. " + std::to_string(k.w) + ")");
-  // pooling_layer.cpp: ceil((H + 2p - k) / s) + 1, clipped so the last window starts inside
-  int64_t oh = static_cast<int64_t>(ceil(static_cast<float>(in[2] + 2 * pad.h - k.h) / st.h)) + 1;
-  int64_t ow = static_cast<int64_t>(ceil(static_cast<float>(in[3] + 2 * pad.w - k.w) / st.w)) + 1;
-  if (pad.h || pad.w) {
-    if ((oh - 1) * st.h >= in[2] + pad.h) --oh;
-    if ((ow - 1) * st.w >= in[3] + pad.w) --ow;
-  }
+  HW out;
+  if (!pooled(L, {in[2], in[3]}, k, st, pad, "", &out)) return false;
   NetLayer& r = L.rec;
   r.kernel_h = k.h, r.kernel_w = k.w, r.stride_h = st.h, r.stride_w = st.w, r.pad_h = pad.h, r.pad_w = pad.w;
   r.pool = p->str("pool", "MAX"), r.global_pooling = global;
-  L.set_tops({in[0], in[1], oh, ow});
+  L.set_tops({in[0], in[1], out.h, out.w});
+  return true;
+}
+
+// spp_layer.cpp: Reshape's CHECK, LayerSetUp's, then each level's Pooling (GetPoolingParam, spp_level) through
+// pooled().  One level is Caffe's lone Pooling with its [N, C, 1, 1] top; more are the Concat of each level's
+// Flatten, [N, C * sum of bins^2].
+bool spp(Layer& L, std::vector<Shape>*) {
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  if (in.size() != 4) return L.refuse("Input must have 4 axes, corresponding to (num, channels, height, width)");
+  if (in[2] <= 0 || in[3] <= 0) return L.refuse("Input dimensions cannot be zero.");
+  const Node* p = L.node.first("spp_param");
+  NetLayer& r = L.rec;
+  r.pyramid_height = p ? p->integer("pyramid_height", 0) : 0;
+  if (r.pyramid_height < 1)
+    return L.refuse("spp_param pyramid_height must be at least 1 (a pyramid of no levels pools nothing)");
+  r.pool = p->str("pool", "MAX");
+  int64_t per_channel = 0;
+  for (int l = 0; l < r.pyramid_height; ++l) {
+    const SppLevel v = spp_level(in[2], in[3], l);
+    HW out;
+    const std::string at = " at pyramid level " + std::to_string(l) + " (" + std::to_string(v.bins) + " bins)";
+    if (!pooled(L, {in[2], in[3]}, {v.kernel_h, v.kernel_w}, {v.kernel_h, v.kernel_w}, {v.pad_h, v.pad_w}, at, &out))
+      return false;
+    per_channel += out.h * out.w;
+  }
+  L.set_top(0, r.pyramid_height == 1 ? Shape{in[0], in[1], 1, 1} : Shape{in[0], in[1] * per_channel});
   return true;
 }
 
@@ -933,7 +979,7 @@ const struct { const char* type; Rule rule; } kRules[] = {
     {"Softmax", same_shape}, {"Power", same_shape}, {"AbsVal", same_shape}, {"BNLL", same_shape}, {"ELU", same_shape},
     {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape}, {"PReLU", prelu},
     {"Split", split}, {"Eltwise", eltwise}, {"Scale", scale}, {"Flatten", flatten}, {"Concat", concat},
-    {"Embed", embed}, {"Reshape", reshape}, {"RNN", rnn}, {"MVN", mvn}, {"Crop", crop},
+    {"Embed", embed}, {"Reshape", reshape}, {"RNN", rnn}, {"MVN", mvn}, {"Crop", crop}, {"SPP", spp},
     {"SoftmaxWithLoss", softmax_loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
     {"HingeLoss", loss}, {"MultinomialLogisticLoss", loss},
     {"BatchNorm", batch_norm}, {"Slice", slice}, {"ContrastiveLoss", contrastive_loss}, {"Silence", silence},

@@ -85,6 +85,9 @@ struct NetLayer {
   // Crop (crop_layer.cpp): `axis` is the first cropped axis (canonical), and the offset of every axis of bottom[0]
   // (0 before `axis`)
   std::vector<int64_t> crop_offsets;
+  // SPP (caffe.proto SPPParameter): the number of pyramid levels; `pool` is its pool method.  Level l's geometry is
+  // spp_level()'s.
+  int64_t pyramid_height = 0;
   FillerSpec weight_filler, bias_filler;
   // per param: whether bias_filler fills it rather than weight_filler.  Empty for the layers whose params are a
   // weight and then (with bias_term) a bias.
@@ -166,6 +169,13 @@ struct SolverSpec {
 int64_t shape_count(const std::vector<int64_t>& s, size_t from = 0);
 // "2x3x4", or "scalar" for a shape without axes.
 std::string shape_text(const std::vector<int64_t>& s);
+
+// SPPLayer::GetPoolingParam: level l of a pyramid over a height x width map pools bins = 2^l windows per side, with
+// kernel k = ceil(height / bins), stride k and pad (k bins - height + 1) / 2 (the same for the width).
+struct SppLevel {
+  int64_t bins, kernel_h, kernel_w, pad_h, pad_w;
+};
+SppLevel spp_level(int64_t height, int64_t width, int level);
 
 // SocketSync::chunk (socket_sync_cpu.cpp:46-54).
 void chunk(uint64_t param_count, int cluster_size, int peer, uint64_t* offs, uint64_t* size);

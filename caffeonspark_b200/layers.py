@@ -1,7 +1,7 @@
 """Native producer layers: autograd Functions and modules over the library's LRN (across and within channels) and fused
 conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10), its
 BatchNorm entry points (csrc/batch_norm.cu, DESIGN.md section 13), its MVN entry points (csrc/mvn.cu, DESIGN.md
-section 14), its Crop kernels (csrc/native_producer.cu, DESIGN.md section 14) and its TF32 convolutions
+section 14), its Crop and SPP kernels (csrc/native_producer.cu, DESIGN.md section 14) and its TF32 convolutions
 (csrc/conv_tf32.cu, DESIGN.md section 10.2).
 
 Activations may be fp32 or bf16 (the mixed-precision producer runs these layers under
@@ -15,6 +15,7 @@ PyTorch composition that defines the layer, so a producer module can still be ch
 GPU-less host; the autograd Functions themselves take CUDA tensors only.
 """
 import ctypes
+import math
 
 import torch
 import torch.nn as nn
@@ -463,3 +464,49 @@ def crop_backward(dy, bottom_shape, offsets, out=None):
     outside it; every element of `out` (a new tensor when None) is written."""
     out = torch.empty(tuple(bottom_shape), dtype=torch.float32, device=dy.device) if out is None else out
     return _crop_call(_lib.lib().cos_crop_backward, dy, out, tuple(bottom_shape), tuple(dy.shape), offsets)
+
+
+def spp_top_shape(bottom_shape, pyramid_height):
+    """Caffe's SPP top for a [N, C, H, W] bottom: Pooling's [N, C, 1, 1] for one level, else the Concat of every level's
+    Flatten, [N, C * (4^h - 1) / 3]."""
+    n, c = bottom_shape[0], bottom_shape[1]
+    return (n, c, 1, 1) if pyramid_height == 1 else (n, c * (4 ** pyramid_height - 1) // 3)
+
+
+def _spp_check(tensors, pool):
+    if pool not in ("MAX", "AVE"):
+        raise CosError(f"SPP pool method {pool} is not supported (MAX and AVE are)")
+    for t, dtype in tensors:
+        if t is not None and not (t.is_cuda and t.dtype == dtype and t.is_contiguous()):
+            raise CosError("SPP takes contiguous CUDA tensors: fp32 data and gradients, int32 argmax")
+
+
+def spp_forward(x, pyramid_height, pool="MAX", out=None, argmax=None):
+    """Caffe's SPP forward on the native kernel (one launch): x [N, C, H, W] -> (y of spp_top_shape, argmax), with
+    argmax the int32 index in its plane of each MAX window's first maximum (-1 when no value is > -FLT_MAX), None for
+    AVE.  `out` and `argmax` are written when given, else new tensors."""
+    shape = spp_top_shape(tuple(x.shape), pyramid_height)
+    out = torch.empty(shape, dtype=torch.float32, device=x.device) if out is None else out
+    if argmax is None and pool == "MAX":
+        argmax = torch.empty(shape, dtype=torch.int32, device=x.device)
+    _spp_check([(x, torch.float32), (out, torch.float32), (argmax, torch.int32)], pool)
+    if x.dim() != 4 or out.numel() != math.prod(shape) or (argmax is not None and argmax.numel() != out.numel()):
+        raise CosError(f"SPP takes a 4-d bottom and a top of {shape}")
+    _call(_lib.lib().cos_spp_forward, x.data_ptr(), out.data_ptr(), argmax.data_ptr() if argmax is not None else None,
+          *x.shape, pyramid_height, int(pool == "MAX"), _stream())
+    return out, argmax
+
+
+def spp_backward(dy, argmax, bottom_shape, pyramid_height, pool="MAX", out=None):
+    """SPP's data gradient on the native kernel (one launch): dx of bottom_shape, each level's Pooling gradient added
+    in level order; every element of `out` (a new tensor when None) is written.  argmax is the forward's (MAX only)."""
+    out = torch.empty(tuple(bottom_shape), dtype=torch.float32, device=dy.device) if out is None else out
+    _spp_check([(dy, torch.float32), (out, torch.float32), (argmax if pool == "MAX" else None, torch.int32)], pool)
+    shape = spp_top_shape(tuple(bottom_shape), pyramid_height)
+    if (len(bottom_shape) != 4 or tuple(out.shape) != tuple(bottom_shape) or dy.numel() != math.prod(shape) or
+            (pool == "MAX" and (argmax is None or argmax.numel() != dy.numel()))):
+        raise CosError(f"SPP's backward takes a top gradient (and MAX argmax) of {shape} and a dx of {bottom_shape}")
+    _call(_lib.lib().cos_spp_backward, dy.data_ptr(), argmax.data_ptr() if pool == "MAX" else None, out.data_ptr(),
+          *bottom_shape, pyramid_height, int(pool == "MAX"), _stream())
+    return out
+

@@ -518,6 +518,59 @@ def cifar10_quick_mvn_module():
                          mvn_module(across_channels=True), nn.Flatten(), nn.Linear(64, 10))
 
 
+# tests/golden/configs/cifar10_quick_spp_train_test.prototxt: CIFAR-10-quick with conv3 padded by 1 (64 x 6 x 6) and
+# pool3 replaced by a 3-level MAX SPP (1, 2 and 4 bins per side), 1344 values into ip1: 145,578 - 65,600 + 86,080 =
+# 166,058 parameters in 10 blobs.
+CIFAR10_QUICK_SPP = dict(input=(3, 32, 32), batch=100, classes=10, pyramid_height=3)
+CIFAR10_QUICK_SPP_PARAM_COUNT = 166058
+
+
+def spp_level(height, width, level):
+    """SPPLayer::GetPoolingParam for pyramid level `level` of a height x width map: (bins, kernel_h, kernel_w, pad_h,
+    pad_w); the stride is the kernel."""
+    bins = 2 ** level
+    kh, kw = -(-height // bins), -(-width // bins)
+    return bins, kh, kw, (kh * bins - height + 1) // 2, (kw * bins - width + 1) // 2
+
+
+def spp(x, pyramid_height, pool="MAX"):
+    """Caffe's SPP as its expansion in PyTorch: each level pooled with spp_level's geometry (the padding made explicit:
+    -inf for MAX, zeros for AVE, whose divisor is the whole kernel), flattened and concatenated; one level is Pooling's
+    [N, C, 1, 1] top."""
+    import torch
+    import torch.nn.functional as F
+    parts = []
+    for level in range(pyramid_height):
+        bins, kh, kw, ph, pw = spp_level(x.shape[2], x.shape[3], level)
+        padded = F.pad(x, (pw, pw, ph, ph), value=float("-inf") if pool == "MAX" else 0.0)
+        pool_fn = F.max_pool2d if pool == "MAX" else F.avg_pool2d
+        out = pool_fn(padded, (kh, kw), (kh, kw))
+        assert out.shape[2:] == (bins, bins), (out.shape, bins)
+        parts.append(out.flatten(1))
+    return parts[0].view(x.shape[0], x.shape[1], 1, 1) if pyramid_height == 1 else torch.cat(parts, 1)
+
+
+def spp_module(pyramid_height, pool="MAX"):
+    """spp() as a module"""
+    import torch.nn as nn
+
+    class SPP(nn.Module):
+        def forward(self, x):
+            return spp(x, pyramid_height, pool)
+
+    return SPP()
+
+
+def cifar10_quick_spp_module():
+    """The SPP CIFAR-10-quick fixture as one PyTorch module, parameters in learnable_params() order.
+    forward(x [N, 3, 32, 32]) -> scores [N, 10]."""
+    import torch.nn as nn
+    return nn.Sequential(nn.Conv2d(3, 32, 5, padding=2), nn.MaxPool2d(3, 2, ceil_mode=True), nn.ReLU(),
+                         nn.Conv2d(32, 32, 5, padding=2), nn.ReLU(), nn.AvgPool2d(3, 2, ceil_mode=True),
+                         nn.Conv2d(32, 64, 5, padding=1), nn.ReLU(), spp_module(CIFAR10_QUICK_SPP["pyramid_height"]),
+                         nn.Linear(1344, 64), nn.Linear(64, 10))
+
+
 def lenet_tanh_module():
     """The TanH LeNet fixture as one PyTorch module, parameters in learnable_params() order.  forward(x [N, 1, 28, 28])
     -> class probabilities [N, 10] (the Softmax's top)."""

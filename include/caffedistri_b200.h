@@ -258,9 +258,9 @@ COS_API int cos_net_set_forward_backward(cos_net* net, cos_forward_backward_fn f
  * Embed over fp32 token ids (a CoSData INT_ARRAY top), Reshape, RNN (without expose_hidden; its hidden state is kept
  * per engine from call to call, zero at first, and not snapshotted) over time-major CoSData tops (transpose: true),
  * MVN (its top the bottom's legacy 4-D shape; in place it computes the out-of-place result), Crop (its reference
- * bottom only gives a shape, so a per-pixel CoSData label can be cropped to a score map), the other layers DESIGN.md
- * section 14 lists, and one loss layer, SoftmaxWithLoss or ContrastiveLoss among them (default normalisation);
- * Accuracy and Silence are skipped.
+ * bottom only gives a shape, so a per-pixel CoSData label can be cropped to a score map), SPP (MAX or AVE), the other
+ * layers DESIGN.md section 14 lists, and one loss layer, SoftmaxWithLoss or ContrastiveLoss among them (default
+ * normalisation); Accuracy and Silence are skipped.
  * Named params are shared as in Caffe.  Every other layer, and loss_param or an unknown filler type, is refused with an
  * error naming the layer.  Every use of a learnable blob adds its gradient into diff_ once per call; results are
  * bitwise reproducible.
@@ -502,6 +502,22 @@ COS_API int cos_conv_backward_data(const float* dy, const float* weight, float* 
 COS_API int cos_conv_backward_filter(const float* x, const float* dy, float* dweight, float* workspace, int n, int c,
                                      int h, int w, int k, int r, int s, int stride_h, int stride_w, int pad_h,
                                      int pad_w, int groups, void* cuda_stream);
+
+/* Caffe's SPP layer (spp_layer.cpp; DESIGN.md section 14) over a contiguous fp32 [num, channels, height, width] bottom
+ * with pyramid_height levels (1 to 16), MAX (max_pool != 0) or AVE.  Level l pools 2^l x 2^l windows of kernel
+ * ceil(H / 2^l), stride the kernel and pad (kernel * 2^l - H + 1) / 2 (likewise for the width), as
+ * SPPLayer::GetPoolingParam sets them.
+ *   forward   y [num, channels * (4^pyramid_height - 1) / 3]: each sample's level l from channels * (4^l - 1) / 3 on,
+ *             ordered (channel, row, column), bit for bit Caffe's Split + Pooling + Flatten + Concat; with MAX,
+ *             argmax (int32, y's size) gets each window's first maximum (-1 when no value is > -FLT_MAX)
+ *   backward  dx (the bottom's size, every element written) = the levels' Pooling gradients added in level order, as
+ *             Caffe's Split adds them; argmax is the forward's (unused for AVE, may be NULL)
+ * A geometry with a level whose pad is not below its kernel is refused.  One launch each; same launch rules as the
+ * calls above. */
+COS_API int cos_spp_forward(const float* x, float* y, int* argmax, int num, int channels, int height, int width,
+                            int pyramid_height, int max_pool, void* cuda_stream);
+COS_API int cos_spp_backward(const float* dy, const int* argmax, float* dx, int num, int channels, int height,
+                             int width, int pyramid_height, int max_pool, void* cuda_stream);
 
 /* --------------------- transport object (reference: util/socket.hpp) ------ */
 /* PeerAdapter = SocketAdapter + SocketChannel of the reference
