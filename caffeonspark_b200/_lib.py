@@ -139,6 +139,8 @@ SYMBOLS = [
     ("cos_crop_backward", _i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
     ("cos_spp_forward", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     ("cos_spp_backward", _i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    ("cos_tile_forward", _i, [_vp, _vp, _i, _vp, _i, _i, _vp]),
+    ("cos_tile_backward", _i, [_vp, _vp, _i, _vp, _i, _i, _vp]),
     ("cos_conv_workspace_floats", _c.c_longlong, [_i] * 12),
     ("cos_conv_forward", _i, [_vp, _vp, _vp, _vp] + [_i] * 12 + [_vp]),
     ("cos_conv_backward_data", _i, [_vp, _vp, _vp] + [_i] * 12 + [_vp]),

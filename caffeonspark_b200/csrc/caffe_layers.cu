@@ -24,20 +24,10 @@
 #include <atomic>
 
 #include "caffe_layers.hpp"
+#include "fast_div.cuh"
 
 namespace cosb {
 namespace {
-
-// n / d for 0 <= n < 2^31 with a multiply-high and a shift instead of an integer division (a division per
-// element costs more issue slots than the element's memory traffic takes time)
-struct FastDiv {
-  unsigned d, m, s;
-  explicit FastDiv(unsigned div) : d(div), m(0), s(0) {
-    while (s < 31 && (1u << s) < d) ++s;
-    m = (unsigned)((((1ull << 32) * ((1ull << s) - d)) / d) + 1);
-  }
-  __device__ __forceinline__ unsigned div(unsigned n) const { return (__umulhi(n, m) + n) >> s; }
-};
 
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }

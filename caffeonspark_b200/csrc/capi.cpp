@@ -863,6 +863,42 @@ int cos_spp_backward(const float* dy, const int* argmax, float* dx, int num, int
                   "cos_spp_backward");
 }
 
+namespace {
+// -> (outer, inner) of a Tile along `axis` of a `naxes`-axis bottom, or an error message
+const char* tile_args(const void* a, const void* b, int naxes, const long long* bottom_shape, int axis, int tiles,
+                      int64_t* outer, int64_t* inner) {
+  if (!a || !b || !bottom_shape) return "NULL tensor or shape";
+  if (naxes < 1 || axis < 0 || axis >= naxes) return "axis out of range";
+  if (tiles < 1) return "Number of tiles must be positive.";
+  *outer = 1, *inner = 1;
+  for (int k = 0; k < naxes; ++k) {
+    if (bottom_shape[k] < 1 || bottom_shape[k] > cosb::kTileMaxTop) return "bad shape";
+    int64_t& part = k < axis ? *outer : *inner;
+    if (part > cosb::kTileMaxTop / bottom_shape[k]) return "a top of more than 2^31 - 1 elements";
+    part *= bottom_shape[k];
+  }
+  if (*outer > cosb::kTileMaxTop / *inner || *outer * *inner > cosb::kTileMaxTop / tiles)
+    return "a top of more than 2^31 - 1 elements";
+  return nullptr;
+}
+}  // namespace
+
+int cos_tile_forward(const float* x, float* y, int naxes, const long long* bottom_shape, int axis, int tiles,
+                     void* cuda_stream) {
+  int64_t outer, inner;
+  if (const char* e = tile_args(x, y, naxes, bottom_shape, axis, tiles, &outer, &inner)) return fail(e);
+  return launched(cosb::tile_forward(x, y, outer, inner, tiles, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_tile_forward");
+}
+
+int cos_tile_backward(const float* dy, float* dx, int naxes, const long long* bottom_shape, int axis, int tiles,
+                      void* cuda_stream) {
+  int64_t outer, inner;
+  if (const char* e = tile_args(dy, dx, naxes, bottom_shape, axis, tiles, &outer, &inner)) return fail(e);
+  return launched(cosb::tile_backward(dy, dx, outer, inner, tiles, static_cast<cudaStream_t>(cuda_stream)),
+                  "cos_tile_backward");
+}
+
 int cos_batch_norm_forward_bf16(const uint16_t* x, uint16_t* y, float* mean_blob, float* var_blob, float* scale_blob,
                                 float* save, float* workspace, int num, int channels, int height, int width,
                                 int use_global_stats, float moving_average_fraction, float eps, void* cuda_stream) {

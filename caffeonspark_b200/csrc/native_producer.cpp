@@ -140,6 +140,7 @@ const LayerType kLayerTypes[] = {
     // the reference gives only its shape: it is never read, so it may also feed a Concat or a loss without a Split
     {"Crop", OpKind::kCrop, 2, false, 1, "ref"},
     {"SPP", OpKind::kSPP},
+    {"Tile", OpKind::kTile},
 };
 
 // Plan::text's name of each OpKind
@@ -148,7 +149,7 @@ const char* const kKindNames[] = {"Convolution", "ConvBiasReLUMaxPool", "Pooling
                                   "Concat", "EuclideanLoss", "Split", "Eltwise", "Scale", "Deconvolution", "Flatten",
                                   "SigmoidCrossEntropyLoss", "TanH", "ELU", "AbsVal", "BNLL", "Power", "Exp", "Log",
                                   "Threshold", "PReLU", "Softmax", "MultinomialLogisticLoss", "HingeLoss",
-                                  "Embed", "Reshape", "RNN", "MVN", "Crop", "SPP"};
+                                  "Embed", "Reshape", "RNN", "MVN", "Crop", "SPP", "Tile"};
 static_assert(std::size(kKindNames) == static_cast<size_t>(OpKind::kCount), "one name per OpKind");
 
 // LossLayer::Reshape's check, then multinomial_logistic_loss_layer.cpp's: the label holds one value per item, with
@@ -585,6 +586,18 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       }
       op.max_pool = L.pool == "MAX";
       op.spp_levels = static_cast<int>(L.pyramid_height);
+    } else if (op.kind == OpKind::kTile) {  // tile_layer.cpp; the parser inferred the top.  The top owns its storage
+      if (L.tops[0] == L.bottoms[0]) {
+        *err = why(L, L.type + " Layer does not allow in-place computation.");
+        return false;
+      }
+      if (shape_count(op.out_shape) > kTileMaxTop) {
+        *err = why(L, "a top of " + std::to_string(shape_count(op.out_shape)) + " elements is more than the " +
+                          std::to_string(kTileMaxTop) + " the Tile kernels index in 32 bits");
+        return false;
+      }
+      op.tile_axis = static_cast<int>(L.axis);
+      op.tiles = L.tiles;
     } else if (op.kind == OpKind::kBatchNorm) {
       if (!op.shares.empty()) {
         *err = why(L, "shared BatchNorm statistics are not supported");
@@ -752,6 +765,8 @@ std::string Plan::text() const {
       os << " level" << l << " " << v.bins << "x" << v.bins << " k" << v.kernel_h << "x" << v.kernel_w << " p"
          << v.pad_h << "x" << v.pad_w;
     }
+    if (op.kind == OpKind::kTile)
+      os << " axis=" << op.tile_axis << " tiles=" << op.tiles << " inner=" << shape_count(op.in_shape, op.tile_axis);
     if (op.kind == OpKind::kCrop) {
       os << " axis=" << op.crop_axis << " offsets=";
       for (size_t a = op.crop_axis; a < op.crop_offsets.size(); ++a)

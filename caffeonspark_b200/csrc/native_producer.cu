@@ -16,6 +16,7 @@
 
 #include "batch_norm.hpp"
 #include "caffe_layers.hpp"
+#include "fast_div.cuh"
 #include "fused_sync_sgd.hpp"
 #include "mvn.hpp"
 #include "native_producer.hpp"
@@ -570,6 +571,95 @@ __global__ void crop_backward_kernel(const V* __restrict__ dy, V* __restrict__ d
     }
     dx[i] = inside ? dy[src] : V{};  // V{}: +0 in every lane
   }
+}
+
+// ------------------------------------------------------------------ Tile (tile_layer.cpp)
+// The top is [outer, tiles, inner] over the bottom's [outer, inner]; every index is below 2^31 (tile_forward checks the
+// top's count), so the kernels index in 32 bits.
+
+// Forward: thread k writes top elements [V k, V k + V), as one 128-bit store for V = 4.  With kVecLoad (inner a multiple
+// of 4, x 16-byte aligned) the V elements lie in one row of x and are read as one float4; otherwise each is read on its
+// own, walking (o, t, d) from the first.  A copy: every bit of x arrives in y.
+template <int V, bool kVecLoad>
+__global__ void tile_forward_kernel(const float* __restrict__ x, float* __restrict__ y, int n, int inner, int tiles,
+                                    FastDiv fd_inner, FastDiv fd_tiles) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const unsigned j = static_cast<unsigned>(k) * V;
+  const unsigned q = fd_inner.div(j);  // the top's row (o, t)
+  const unsigned o = fd_tiles.div(q);
+  unsigned d = j - q * inner, t = q - o * tiles, src = o * inner + d;
+  if constexpr (V == 1) {
+    y[j] = x[src];
+  } else if constexpr (kVecLoad) {
+    *reinterpret_cast<float4*>(y + j) = *reinterpret_cast<const float4*>(x + src);
+  } else {
+    float v[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      v[e] = x[src];
+      ++src;
+      if (++d == static_cast<unsigned>(inner)) {  // the next row: the same bottom row again, or the next one after
+        d = 0;                                   // the last tile
+        if (++t == static_cast<unsigned>(tiles)) t = 0;
+        else src -= inner;
+      }
+    }
+    *reinterpret_cast<float4*>(y + j) = make_float4(v[0], v[1], v[2], v[3]);
+  }
+}
+
+// Backward for inner >= kTileStagedMaxInner: one thread per dx element (o, d), consecutive threads on consecutive d, so
+// every load of a tile row is coalesced.  dx = dy[o, 0, d], then dy[o, t, d] added in t order.
+__global__ void tile_backward_direct_kernel(const float* __restrict__ dy, float* __restrict__ dx, int n, int inner,
+                                            int tiles) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int o = i / inner;
+  const float* p = dy + static_cast<int64_t>(o) * tiles * inner + (i - o * inner);
+  float acc = p[0];
+#pragma unroll 8
+  for (int t = 1; t < tiles; ++t) acc = __fadd_rn(acc, p[static_cast<int64_t>(t) * inner]);
+  dx[i] = acc;
+}
+
+// Backward for inner < kTileStagedMaxInner: a block owns `rows` consecutive outer rows, rows * inner <= blockDim.x
+// outputs, and walks the tiles in chunks of kTileChunk.  The block copies its rows' part of the chunk (each row's part
+// contiguous in dy) into shared memory, consecutive threads on consecutive floats, as stage[t][k] for output k = r *
+// inner + d, at a row stride `stride` congruent to inner mod 32: neither the stores (consecutive t * inner + d) nor the
+// column reads (consecutive k) meet a bank conflict.  Thread k then adds its column in t order: the first tile copied,
+// each later one added.  fd_span and fd_last divide by a full chunk's row length (kTileChunk * inner) and the last's.
+constexpr int kTileChunk = 32;
+constexpr int kTileStageStride = kThreads + 32;  // the largest `stride` tile_backward picks
+__global__ void __launch_bounds__(kThreads) tile_backward_staged_kernel(const float* __restrict__ dy,
+                                                                        float* __restrict__ dx, int outer, int inner,
+                                                                        int tiles, int rows, int stride,
+                                                                        FastDiv fd_inner, FastDiv fd_span,
+                                                                        FastDiv fd_last) {
+  __shared__ float stage[kTileChunk * kTileStageStride];
+  const int o0 = blockIdx.x * rows;
+  const int nrows = min(rows, outer - o0), outputs = nrows * inner;
+  const float* base = dy + static_cast<int64_t>(o0) * tiles * inner;
+  float acc = 0.f;
+  for (int t0 = 0; t0 < tiles; t0 += kTileChunk) {
+    const int tc = min(kTileChunk, tiles - t0), span = tc * inner;
+    const FastDiv& fd = tc == kTileChunk ? fd_span : fd_last;
+    __syncthreads();  // the previous chunk's columns are read
+#pragma unroll 4
+    for (int e = threadIdx.x; e < nrows * span; e += blockDim.x) {
+      const int r = fd.div(e), c = e - r * span;
+      const int t = fd_inner.div(c), d = c - t * inner;
+      stage[t * stride + r * inner + d] = base[(static_cast<int64_t>(r) * tiles + t0) * inner + c];
+    }
+    __syncthreads();
+    if (static_cast<int>(threadIdx.x) < outputs) {
+      const float* col = stage + threadIdx.x;
+      int t = 0;
+      if (t0 == 0) acc = col[0], t = 1;
+      for (; t < tc; ++t) acc = __fadd_rn(acc, col[t * stride]);
+    }
+  }
+  if (static_cast<int>(threadIdx.x) < outputs) dx[static_cast<int64_t>(o0) * inner + threadIdx.x] = acc;
 }
 
 // ------------------------------------------------------------------ ContrastiveLoss (contrastive_loss_layer.cpp)
@@ -1161,6 +1251,11 @@ int grid_for(int64_t n) {
 struct ConvDims {
   int N, Cin, H, W, Cout, OH, OW;
 };
+
+// Tile's outer = count(0, axis) of its bottom
+int64_t tile_outer(const Op& op) {
+  return shape_count(std::vector<int64_t>(op.in_shape.begin(), op.in_shape.begin() + op.tile_axis));
+}
 // A Deconvolution's dims are those of the convolution from its top to its bottom (the same weight blob, [Cin, Cout,
 // KH, KW] of the deconvolution): its forward is that convolution's data gradient, its data gradient that
 // convolution's forward, and its weight gradient that convolution's with the bottom as dy.
@@ -1370,6 +1465,56 @@ cudaError_t spp_backward(const float* dy, const int* argmax, float* dx, int num,
   if (!spp_geom(num, channels, height, width, levels, &g) || (max_pool && !argmax)) return cudaErrorInvalidValue;
   const int n = num * channels * height * width;
   spp_backward_kernel<<<grid_for(n), kThreads, 0, s>>>(dy, argmax, dx, g, max_pool);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------ Tile's launches
+bool tile_backward_staged(int64_t inner) { return inner < kTileStagedMaxInner; }
+
+namespace {
+bool tile_shape_ok(int64_t outer, int64_t inner, int64_t tiles) {
+  return outer >= 1 && inner >= 1 && tiles >= 1 && outer <= kTileMaxTop / inner && outer * inner <= kTileMaxTop / tiles;
+}
+bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
+}  // namespace
+
+cudaError_t tile_forward(const float* x, float* y, int64_t outer, int64_t inner, int64_t tiles, cudaStream_t s) {
+  if (!tile_shape_ok(outer, inner, tiles)) return cudaErrorInvalidValue;
+  const int64_t total = outer * tiles * inner;
+  const int in = static_cast<int>(inner), ti = static_cast<int>(tiles);
+  const FastDiv fi(static_cast<unsigned>(inner)), ft(static_cast<unsigned>(tiles));
+  if (total % 4 == 0 && aligned16(y)) {
+    const int n = static_cast<int>(total / 4);
+    const int blocks = (n + kThreads - 1) / kThreads;
+    if (inner % 4 == 0 && aligned16(x))
+      tile_forward_kernel<4, true><<<blocks, kThreads, 0, s>>>(x, y, n, in, ti, fi, ft);
+    else
+      tile_forward_kernel<4, false><<<blocks, kThreads, 0, s>>>(x, y, n, in, ti, fi, ft);
+  } else {
+    const int n = static_cast<int>(total);
+    tile_forward_kernel<1, false><<<(n + kThreads - 1) / kThreads, kThreads, 0, s>>>(x, y, n, in, ti, fi, ft);
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t tile_backward(const float* dy, float* dx, int64_t outer, int64_t inner, int64_t tiles, cudaStream_t s) {
+  if (!tile_shape_ok(outer, inner, tiles)) return cudaErrorInvalidValue;
+  const int in = static_cast<int>(inner), ti = static_cast<int>(tiles);
+  if (!tile_backward_staged(inner)) {
+    const int n = static_cast<int>(outer * inner);
+    tile_backward_direct_kernel<<<(n + kThreads - 1) / kThreads, kThreads, 0, s>>>(dy, dx, n, in, ti);
+    return cudaGetLastError();
+  }
+  // rows per block: a block's worth of outputs, fewer when that would leave the grid under two blocks per SM
+  const int64_t spread = (outer + 2 * kTargetSms - 1) / (2 * kTargetSms);
+  const int rows = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(kThreads / inner, spread)));
+  const int outputs = rows * in;
+  const int stride = outputs + ((in - outputs) % 32 + 32) % 32;  // >= outputs, congruent to inner mod 32
+  const int64_t blocks = (outer + rows - 1) / rows;
+  const int last = static_cast<int>((tiles - 1) % kTileChunk + 1);  // the last chunk's tiles
+  tile_backward_staged_kernel<<<static_cast<unsigned>(blocks), kThreads, 0, s>>>(
+      dy, dx, static_cast<int>(outer), in, ti, rows, stride, FastDiv(static_cast<unsigned>(in)),
+      FastDiv(static_cast<unsigned>(kTileChunk * in)), FastDiv(static_cast<unsigned>(last * in)));
   return cudaGetLastError();
 }
 
@@ -1664,6 +1809,8 @@ cudaError_t NativeProducer::run_op_forward(const Op& op, size_t i, float* loss_d
       return spp_forward(x, y, static_cast<int*>(op_aux_[i]), static_cast<int>(op.in_shape[0]),
                          static_cast<int>(op.in_shape[1]), static_cast<int>(op.in_shape[2]),
                          static_cast<int>(op.in_shape[3]), op.spp_levels, op.max_pool, s);
+    case OpKind::kTile:
+      return tile_forward(x, y, tile_outer(op), shape_count(op.in_shape, op.tile_axis), op.tiles, s);
     case OpKind::kDeconv:  // the data gradient of the convolution from top to bottom, with the bias in its store
       return conv_data_grad(op, conv_dims(op), x, data_ + op.w_off, op.b_off >= 0 ? data_ + op.b_off : nullptr, y, s);
     case OpKind::kSplit:  // no copy: the top reads the bottom's memory
@@ -1913,6 +2060,9 @@ cudaError_t NativeProducer::run_op_backward(const Op& op, size_t i, cudaStream_t
       return spp_backward(dy, static_cast<const int*>(op_aux_[i]), dx, static_cast<int>(op.in_shape[0]),
                           static_cast<int>(op.in_shape[1]), static_cast<int>(op.in_shape[2]),
                           static_cast<int>(op.in_shape[3]), op.spp_levels, op.max_pool, s);
+    case OpKind::kTile:  // writes every element of dx
+      return dx ? tile_backward(dy, dx, tile_outer(op), shape_count(op.in_shape, op.tile_axis), op.tiles, s)
+                : cudaSuccess;
     case OpKind::kSplit: {  // top 0's op: dx = the read tops' gradients summed in top order; the other tops' do nothing
       if (!dx || op.split_top != 0) return cudaSuccess;
       const std::vector<int>& g = op.split_sum;

@@ -3,7 +3,8 @@
 // residual nets built of Split, Eltwise and Scale, autoencoders built of Flatten, Deconvolution and
 // SigmoidCrossEntropyLoss, embedding nets that read token ids through Embed and Reshape, recurrent nets built of
 // RNN layers over time-major inputs, nets normalised by MVN, U-Net segmentation nets that Crop their skips and
-// per-pixel labels, and nets with a spatial-pyramid-pooling (SPP) head; DESIGN.md section 14).
+// per-pixel labels, nets with a spatial-pyramid-pooling (SPP) head, and squeeze-and-excitation nets that Tile their
+// gates over the map; DESIGN.md section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -29,7 +30,7 @@ enum class OpKind {
   kConv, kConvBiasReluMaxPool, kPool, kInnerProduct, kReLU, kSigmoid, kBatchNorm, kSoftmaxLoss, kLRNWithin, kSlice,
   kContrastiveLoss, kConcat, kEuclideanLoss, kSplit, kEltwise, kScale, kDeconv, kFlatten, kSigmoidCrossEntropyLoss,
   kTanH, kELU, kAbsVal, kBNLL, kPower, kExp, kLog, kThreshold, kPReLU, kSoftmax, kMultinomialLogisticLoss, kHingeLoss,
-  kEmbed, kReshape, kRNN, kMVN, kCrop, kSPP,
+  kEmbed, kReshape, kRNN, kMVN, kCrop, kSPP, kTile,
   kCount  // the number of kinds (Plan::text names each)
 };
 
@@ -119,6 +120,10 @@ struct Op {
   // SPP: spp_levels pyramid levels over in_shape's H x W (spp_level() gives each one's geometry), MAX or AVE by
   // max_pool; the top holds every level's bins, level after level within each sample
   int spp_levels = 0;
+  // Tile: the top is [outer, tiles, inner] over the bottom's [outer, inner], outer = count(0, tile_axis) and inner =
+  // count(tile_axis) of in_shape
+  int tile_axis = 0;
+  int64_t tiles = 1;
 };
 
 struct Plan {
@@ -176,6 +181,21 @@ cudaError_t spp_forward(const float* x, float* y, int* argmax, int num, int chan
                         bool max_pool, cudaStream_t s);
 cudaError_t spp_backward(const float* dy, const int* argmax, float* dx, int num, int channels, int height, int width,
                          int levels, bool max_pool, cudaStream_t s);
+// Tile's kernels index in 32 bits: a top has at most this many elements
+constexpr int64_t kTileMaxTop = (int64_t(1) << 31) - 1;
+// Tile's kernels (native_producer.cu): tile_layer.cpp over a contiguous bottom [outer, inner] and top [outer, tiles,
+// inner].  The forward writes each top element once, with 128-bit stores where y is 16-byte aligned and the top's count
+// a multiple of 4.  The backward writes each element of dx once: dy[o, 0, d], then dy[o, t, d] added for t = 1 ..
+// tiles - 1 in order, each add rounded once in fp32 (Backward_cpu's copy and axpys, so a column of -0 stays -0).  One
+// launch each; cudaErrorInvalidValue for an empty shape or a top of more than kTileMaxTop elements.
+cudaError_t tile_forward(const float* x, float* y, int64_t outer, int64_t inner, int64_t tiles, cudaStream_t s);
+cudaError_t tile_backward(const float* dy, float* dx, int64_t outer, int64_t inner, int64_t tiles, cudaStream_t s);
+// Which backward kernel tile_backward runs, from the shape alone: below kTileStagedMaxInner (a gate tiled along H, then
+// W, has inner 1) each dx element sums `tiles` consecutive runs too short to fill a sector across lanes, so a block
+// stages its rows of dy through shared memory with coalesced loads and sums each column there; from it on, one thread
+// per dx element reads dy directly, coalesced across lanes.  Both give the same bits.
+constexpr int64_t kTileStagedMaxInner = 32;
+bool tile_backward_staged(int64_t inner);
 // The GEMM core puts its M rows on gridDim.y in tiles of 64, so one GEMM has at most this many rows: an InnerProduct's
 // rows or num_output, a convolution's input or output channels, an RNN's T * N or num_output
 constexpr int64_t kMaxGemmRows = 65535 * 64;

@@ -890,6 +890,22 @@ bool crop(Layer& L, std::vector<Shape>*) {
   return true;
 }
 
+// tile_layer.cpp Reshape, with its CHECK messages: the top is the bottom with shape[axis] *= tiles (axis default 1)
+bool tile(Layer& L, std::vector<Shape>*) {
+  Shape in;
+  if (!L.bottom(0, &in)) return false;
+  const Node* p = L.node.first("tile_param");
+  NetLayer& r = L.rec;
+  if (!canonical_axis(L, p ? p->integer("axis", 1) : 1, static_cast<int64_t>(in.size()), &r.axis)) return false;
+  if (!p || !p->first("tiles")) return L.refuse("Number of tiles must be specified");
+  r.tiles = p->integer("tiles", 0);
+  if (r.tiles <= 0) return L.refuse("Number of tiles must be positive.");
+  Shape top = in;
+  top[r.axis] *= r.tiles;
+  L.set_top(0, top);
+  return true;
+}
+
 bool slice(Layer& L, std::vector<Shape>*) {  // slice_layer.cpp Reshape
   Shape in;
   if (!L.bottom(0, &in)) return false;
@@ -980,6 +996,7 @@ const struct { const char* type; Rule rule; } kRules[] = {
     {"Exp", same_shape}, {"Log", same_shape}, {"Threshold", same_shape}, {"PReLU", prelu},
     {"Split", split}, {"Eltwise", eltwise}, {"Scale", scale}, {"Flatten", flatten}, {"Concat", concat},
     {"Embed", embed}, {"Reshape", reshape}, {"RNN", rnn}, {"MVN", mvn}, {"Crop", crop}, {"SPP", spp},
+    {"Tile", tile},
     {"SoftmaxWithLoss", softmax_loss}, {"Accuracy", loss}, {"EuclideanLoss", loss}, {"SigmoidCrossEntropyLoss", loss},
     {"HingeLoss", loss}, {"MultinomialLogisticLoss", loss},
     {"BatchNorm", batch_norm}, {"Slice", slice}, {"ContrastiveLoss", contrastive_loss}, {"Silence", silence},

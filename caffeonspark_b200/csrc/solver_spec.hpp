@@ -88,6 +88,8 @@ struct NetLayer {
   // SPP (caffe.proto SPPParameter): the number of pyramid levels; `pool` is its pool method.  Level l's geometry is
   // spp_level()'s.
   int64_t pyramid_height = 0;
+  // Tile (caffe.proto TileParameter): `axis` is the tiled axis (canonical), repeated `tiles` times
+  int64_t tiles = 0;
   FillerSpec weight_filler, bias_filler;
   // per param: whether bias_filler fills it rather than weight_filler.  Empty for the layers whose params are a
   // weight and then (with bias_term) a bias.

@@ -1,7 +1,7 @@
 """Native producer layers: autograd Functions and modules over the library's LRN (across and within channels) and fused
 conv-bias + ReLU + MAX-pool entry points (csrc/caffe_layers.cu, DESIGN.md section 10), its
 BatchNorm entry points (csrc/batch_norm.cu, DESIGN.md section 13), its MVN entry points (csrc/mvn.cu, DESIGN.md
-section 14), its Crop and SPP kernels (csrc/native_producer.cu, DESIGN.md section 14) and its TF32 convolutions
+section 14), its Crop, SPP and Tile kernels (csrc/native_producer.cu, DESIGN.md section 14) and its TF32 convolutions
 (csrc/conv_tf32.cu, DESIGN.md section 10.2).
 
 Activations may be fp32 or bf16 (the mixed-precision producer runs these layers under
@@ -510,3 +510,44 @@ def spp_backward(dy, argmax, bottom_shape, pyramid_height, pool="MAX", out=None)
           *bottom_shape, pyramid_height, int(pool == "MAX"), _stream())
     return out
 
+
+def tile_top_shape(bottom_shape, axis, tiles):
+    """Caffe's Tile top: the bottom's shape with shape[axis] (negative counted from the end) multiplied by tiles."""
+    if not -len(bottom_shape) <= axis < len(bottom_shape):
+        raise CosError(f"axis {axis} out of range for {len(bottom_shape)}-D Blob")
+    shape = list(bottom_shape)
+    shape[axis] *= tiles
+    return tuple(shape)
+
+
+def _tile_call(forward, x, y, bottom_shape, axis, tiles):
+    """The forward (x to y) or the backward (y to x) over the bottom-sized x and the top-sized y"""
+    n = len(bottom_shape)
+    if tiles < 1:
+        raise CosError("Number of tiles must be positive.")
+    if not all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() for t in (x, y)):
+        raise CosError("Tile takes contiguous fp32 CUDA tensors")
+    top = tile_top_shape(bottom_shape, axis, tiles)
+    axis = axis + n if axis < 0 else axis
+    if x.numel() != math.prod(bottom_shape) or y.numel() != math.prod(top):
+        raise CosError(f"Tile takes a bottom of {tuple(bottom_shape)} and a top of {top} (axis {axis}, tiles {tiles})")
+    fn, src, dst = (_lib.lib().cos_tile_forward, x, y) if forward else (_lib.lib().cos_tile_backward, y, x)
+    _call(fn, src.data_ptr(), dst.data_ptr(), n, (ctypes.c_longlong * n)(*bottom_shape), axis, tiles, _stream())
+
+
+def tile_forward(x, axis, tiles, out=None):
+    """Caffe's Tile forward on the native kernel (one launch): x repeated `tiles` times along `axis`, every bit copied
+    into `out` (a new tensor of tile_top_shape when None)."""
+    shape = tile_top_shape(tuple(x.shape), axis, tiles)
+    out = torch.empty(shape, dtype=torch.float32, device=x.device) if out is None else out
+    _tile_call(True, x, out, tuple(x.shape), axis, tiles)
+    return out
+
+
+def tile_backward(dy, bottom_shape, axis, tiles, out=None):
+    """Tile's data gradient on the native kernel (one launch): dx of bottom_shape, each element the first tile's
+    gradient with the later tiles' added in tile order, each add rounded once (Caffe's Backward_cpu bit for bit); every
+    element of `out` (a new tensor when None) is written."""
+    out = torch.empty(tuple(bottom_shape), dtype=torch.float32, device=dy.device) if out is None else out
+    _tile_call(False, out, dy, tuple(bottom_shape), axis, tiles)
+    return out

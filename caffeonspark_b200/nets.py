@@ -362,12 +362,33 @@ def contrastive_loss(a, b, sim, margin=1.0, legacy=False, loss_weight=1.0):
 # Eltwise SUM shortcuts with a 1x1 stride-2 projection where the shape changes, global AVE pooling and a 10-way
 # InnerProduct.  Batch 100 of 3x32x32.
 RESNET20 = dict(input=(3, 32, 32), batch=100, classes=10, stages=(16, 32, 64), blocks=3)
+# tests/golden/configs/cifar10_se_resnet20_train_test.prototxt: ResNet-20 with a squeeze-and-excitation gate of reduction
+# 4 on every residual branch (after its second BatchNorm + Scale, before the Eltwise SUM).  282,547 parameters in 164
+# blobs.
+SE_RESNET20_PARAM_COUNT = 282547
 
 
 def resnet20_module():
     """ResNet-20 as one PyTorch module with its parameters in learnable_params() order: per convolution its weight, the
     BatchNorm's three statistics and the Scale's scale and bias; per block branch2a, branch2b, then the projection
     (branch1) where there is one; the InnerProduct last.  forward(x [N, 3, 32, 32]) -> scores [N, 10]."""
+    return _resnet20(se=False)
+
+
+def se_resnet20_module():
+    """The SE-ResNet-20 fixture as one PyTorch module, parameters in learnable_params() order: resnet20_module's, with
+    each block's SE gate (fc1 weight and bias, fc2 weight and bias) after branch2b and before branch1.  The gate is
+    sigmoid(fc2(relu(fc1(mean over H, W)))) per (sample, channel), broadcast over the map as Caffe's two Tiles do."""
+    return _resnet20(se=True)
+
+
+def se_gate(x, fc1, fc2, relu):
+    """x times the squeeze-and-excitation gate sigmoid(fc2(relu(fc1(x averaged over H and W)))), broadcast over H, W"""
+    import torch
+    return x * torch.sigmoid(fc2(relu(fc1(x.mean(dim=(2, 3))))))[:, :, None, None]
+
+
+def _resnet20(se):
     import torch
     import torch.nn as nn
     from .layers import BatchNorm
@@ -394,10 +415,14 @@ def resnet20_module():
             stride = 1 if cin == cout else 2
             self.branch2a = unit(cin, cout, 3, stride)
             self.branch2b = unit(cout, cout, 3, 1)
+            if se:
+                self.se_fc1, self.se_fc2 = nn.Linear(cout, cout // 4), nn.Linear(cout // 4, cout)
             self.branch1 = unit(cin, cout, 1, 2) if cin != cout else None
 
         def forward(self, x):
             y = self.branch2b(self.branch2a(x).relu())
+            if se:
+                y = se_gate(y, self.se_fc1, self.se_fc2, torch.relu)
             return (y + (self.branch1(x) if self.branch1 is not None else x)).relu()
 
     class ResNet20(nn.Module):
@@ -830,6 +855,9 @@ def rnn_lm_ln_module():
 # and a 1x1 score convolution to 2 classes at 52 x 52.  116,770 parameters in 26 blobs.
 UNET = dict(input=(1, 92, 92), batch=8, classes=2, score=52)
 UNET_PARAM_COUNT = 116770
+# tests/golden/configs/unet_scse_train_test.prototxt: the U-Net with a concurrent spatial and channel squeeze-and-
+# excitation (scSE) block after relu4b and after relu5b.  117,520 parameters in 38 blobs.
+UNET_SCSE_PARAM_COUNT = 117520
 
 
 def crop(x, size, offsets):
@@ -841,9 +869,32 @@ def unet_module():
     """The U-Net fixture as one PyTorch module, parameters in learnable_params() order.  forward(images [N, 1, 92, 92])
     -> scores [N, 2, 52, 52]; crop_label(labels [N, 1, 92, 92]) -> the labels of the scored pixels.  Every ReLU and
     MAX pool goes through relu() and pool(), so that a caller can fix their branches."""
+    return _unet(scse=False)
+
+
+def unet_scse_module():
+    """The U-Net scSE fixture as one PyTorch module, parameters in learnable_params() order: unet_module's, with the
+    scSE block after conv4b (channel gate fc1 and fc2, then the spatial gate's 1x1 convolution, each weight then bias)
+    before upconv1, and the one after conv5b before score.  Every ReLU, MAX pool and Eltwise MAX goes through relu(),
+    pool() and max(), so that a caller can fix their branches."""
+    return _unet(scse=True)
+
+
+def _unet(scse):
     import torch
     import torch.nn as nn
     import torch.nn.functional as F
+
+    class SCSE(nn.Module):
+        """Concurrent spatial and channel squeeze-and-excitation: max(x * SE gate, x * sigmoid(1x1 conv C -> 1))"""
+
+        def __init__(self, c):
+            super().__init__()
+            self.fc1, self.fc2 = nn.Linear(c, c // 4), nn.Linear(c // 4, c)
+            self.conv = nn.Conv2d(c, 1, 1)
+
+        def forward(self, x, relu, vmax):
+            return vmax(se_gate(x, self.fc1, self.fc2, relu), x * torch.sigmoid(self.conv(x)))
 
     class UNet(nn.Module):
         def __init__(self):
@@ -854,8 +905,10 @@ def unet_module():
             self.conv3a, self.conv3b = conv(32, 64), conv(64, 64)
             self.upconv2 = nn.ConvTranspose2d(64, 32, 2, stride=2)
             self.conv4a, self.conv4b = conv(64, 32), conv(32, 32)
+            self.scse4 = SCSE(32) if scse else None
             self.upconv1 = nn.ConvTranspose2d(32, 16, 2, stride=2)
             self.conv5a, self.conv5b = conv(32, 16), conv(16, 16)
+            self.scse5 = SCSE(16) if scse else None
             self.score = nn.Conv2d(16, 2, 1)
 
         def relu(self, x):
@@ -864,6 +917,12 @@ def unet_module():
         def pool(self, x):
             return F.max_pool2d(x, 2, 2, ceil_mode=True)
 
+        def max(self, a, b):  # Caffe's Eltwise MAX: b wins a tie, and the whole gradient goes to the winner
+            return torch.where(a > b, a, b)
+
+        def gate(self, block, x):
+            return block(x, self.relu, self.max) if block is not None else x
+
         def forward(self, x):
             r = self.relu
             d1 = r(self.conv1b(r(self.conv1a(x))))
@@ -871,9 +930,9 @@ def unet_module():
             d3 = r(self.conv3b(r(self.conv3a(self.pool(d2)))))
             u2 = r(self.upconv2(d3))
             h = torch.cat([crop(d2, u2.shape[2:], (4, 4)), u2], 1)
-            u1 = r(self.upconv1(r(self.conv4b(r(self.conv4a(h))))))
+            u1 = r(self.upconv1(self.gate(self.scse4, r(self.conv4b(r(self.conv4a(h)))))))
             h = torch.cat([crop(d1, u1.shape[2:], (16, 16)), u1], 1)
-            return self.score(r(self.conv5b(r(self.conv5a(h)))))
+            return self.score(self.gate(self.scse5, r(self.conv5b(r(self.conv5a(h))))))
 
         @staticmethod
         def crop_label(label):

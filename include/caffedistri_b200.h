@@ -258,9 +258,9 @@ COS_API int cos_net_set_forward_backward(cos_net* net, cos_forward_backward_fn f
  * Embed over fp32 token ids (a CoSData INT_ARRAY top), Reshape, RNN (without expose_hidden; its hidden state is kept
  * per engine from call to call, zero at first, and not snapshotted) over time-major CoSData tops (transpose: true),
  * MVN (its top the bottom's legacy 4-D shape; in place it computes the out-of-place result), Crop (its reference
- * bottom only gives a shape, so a per-pixel CoSData label can be cropped to a score map), SPP (MAX or AVE), the other
- * layers DESIGN.md section 14 lists, and one loss layer, SoftmaxWithLoss or ContrastiveLoss among them (default
- * normalisation); Accuracy and Silence are skipped.
+ * bottom only gives a shape, so a per-pixel CoSData label can be cropped to a score map), SPP (MAX or AVE), Tile (not
+ * in place), the other layers DESIGN.md section 14 lists, and one loss layer, SoftmaxWithLoss or ContrastiveLoss among
+ * them (default normalisation); Accuracy and Silence are skipped.
  * Named params are shared as in Caffe.  Every other layer, and loss_param or an unknown filler type, is refused with an
  * error naming the layer.  Every use of a learnable blob adds its gradient into diff_ once per call; results are
  * bitwise reproducible.
@@ -518,6 +518,18 @@ COS_API int cos_spp_forward(const float* x, float* y, int* argmax, int num, int 
                             int pyramid_height, int max_pool, void* cuda_stream);
 COS_API int cos_spp_backward(const float* dy, const int* argmax, float* dx, int num, int channels, int height,
                              int width, int pyramid_height, int max_pool, void* cuda_stream);
+
+/* Caffe's Tile layer (tile_layer.cpp; DESIGN.md section 14) over a contiguous fp32 bottom of `naxes` axes
+ * (bottom_shape) repeated `tiles` times along `axis` (canonical, 0 .. naxes - 1): with outer = count(0, axis) and
+ * inner = count(axis), the top is [outer, tiles, inner] in memory, at most 2^31 - 1 elements.
+ *   forward   y[o, t, d] = x[o, d], every bit copied
+ *   backward  dx[o, d] = dy[o, 0, d], then dy[o, t, d] added for t = 1 .. tiles - 1 in order, each add rounded once
+ *             in fp32: Backward_cpu's copy and axpys bit for bit (a column of -0 stays -0); every element written
+ * One launch each; same launch rules as the calls above. */
+COS_API int cos_tile_forward(const float* x, float* y, int naxes, const long long* bottom_shape, int axis, int tiles,
+                             void* cuda_stream);
+COS_API int cos_tile_backward(const float* dy, float* dx, int naxes, const long long* bottom_shape, int axis,
+                              int tiles, void* cuda_stream);
 
 /* --------------------- transport object (reference: util/socket.hpp) ------ */
 /* PeerAdapter = SocketAdapter + SocketChannel of the reference
