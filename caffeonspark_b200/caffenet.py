@@ -242,7 +242,7 @@ class _DevArray:
 
 
 def _blob_array(data):
-    """list of host arrays (numpy float32 / CPU torch float32, up to 4-D) -> cos_blob[]"""
+    """list of host arrays (numpy float32 / CPU torch float32) -> cos_blob[]"""
     blobs = (cos_blob * max(1, len(data)))()
     keep = []
     for i, a in enumerate(data):
@@ -255,9 +255,18 @@ def _blob_array(data):
             a = np.ascontiguousarray(a, dtype=np.float32)
             ptr, shape = a.ctypes.data, a.shape
         keep.append(a)
-        shape = tuple(shape) + (1,) * (4 - len(shape))
-        blobs[i].data, blobs[i].num, blobs[i].channels, blobs[i].height, blobs[i].width = ptr, *[int(s) for s in shape]
+        blobs[i].data, blobs[i].num, blobs[i].channels, blobs[i].height, blobs[i].width = ptr, *_blob_dims(shape)
     return blobs, keep
+
+
+def _blob_dims(shape):
+    """cos_blob's (num, channels, height, width) of an array's shape: missing axes are 1, and the axes from the fourth
+    on fold into width (a [N, C, D, H, W] volume is [N, C, D, H * W]); the producers check the element count"""
+    shape = tuple(int(d) for d in shape) + (1,) * (4 - len(shape))
+    width = 1
+    for d in shape[3:]:
+        width *= d
+    return shape[:3] + (width,)
 
 
 class CaffeNet:
@@ -438,8 +447,7 @@ class CaffeNet:
                 ptr, shape = a.data_ptr(), tuple(a.shape)
             else:
                 ptr, shape = a
-            shape = tuple(int(d) for d in shape) + (1,) * (4 - len(shape))
-            blobs[i].data, blobs[i].num, blobs[i].channels, blobs[i].height, blobs[i].width = ptr, *shape
+            blobs[i].data, blobs[i].num, blobs[i].channels, blobs[i].height, blobs[i].width = ptr, *_blob_dims(shape)
         return bool(self._L.cos_net_forward_backward(self._h, solver_index, blobs, len(inputs), loss_dev, stream))
 
     def param_count(self):

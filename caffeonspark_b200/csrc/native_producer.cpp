@@ -458,7 +458,7 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
         *err = why(L, "group " + std::to_string(L.group) + " > 1 is not supported");
         return false;
       }
-      if (L.dilation_h != 1 || L.dilation_w != 1) {
+      if (L.dilation_h != 1 || L.dilation_w != 1 || L.dilation_d != 1) {
         *err = why(L, "dilation other than 1 is not supported");
         return false;
       }
@@ -466,8 +466,17 @@ bool build_plan(const SolverSpec& spec, const std::vector<NetLayer>& layers, Pla
       op.kh = static_cast<int>(L.kernel_h), op.kw = static_cast<int>(L.kernel_w);
       op.sh = static_cast<int>(L.stride_h), op.sw = static_cast<int>(L.stride_w);
       op.ph = static_cast<int>(L.pad_h), op.pw = static_cast<int>(L.pad_w);
+      op.kd = static_cast<int>(L.kernel_d), op.sd = static_cast<int>(L.stride_d), op.pd = static_cast<int>(L.pad_d);
+      // the 3-D gathers index the bottom, the top and the N D H W columns of their GEMMs (fewer than either blob's
+      // elements) in 32 bits
+      const int64_t widest = std::max(shape_count(op.in_shape), shape_count(op.out_shape));
+      if (op.in_shape.size() == 5 && widest >= (int64_t(1) << 31)) {
+        *err = why(L, "a geometry of " + std::to_string(widest) + " elements reaches the 2^31 the 3-D convolution "
+                          "kernels index in 32 bits");
+        return false;
+      }
       // conv + bias followed by ReLU and MAX pool in either order: the existing fused block (caffe_layers.cu)
-      if (op.kind == OpKind::kConv && L.bias_term && i + 2 < layers.size()) {
+      if (op.kind == OpKind::kConv && L.bias_term && op.in_shape.size() == 4 && i + 2 < layers.size()) {
         const NetLayer& a = layers[i + 1];
         const NetLayer& b = layers[i + 2];
         const bool order = (fusable_relu(a) && fusable_pool(b)) || (fusable_pool(a) && fusable_relu(b));
@@ -741,8 +750,13 @@ std::string Plan::text() const {
     if (op.kind == OpKind::kPool || op.kind == OpKind::kSPP) os << "(" << (op.max_pool ? "MAX" : "AVE") << ")";
     if (op.kind == OpKind::kEltwise) os << "(" << eltwise_ops[op.eltwise_op] << ")";
     os << " " << op.name << " " << shape_text(op.in_shape) << " -> " << shape_text(op.out_shape);
-    if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kPool ||
-        op.kind == OpKind::kDeconv)
+    if ((op.kind == OpKind::kConv || op.kind == OpKind::kDeconv) && op.in_shape.size() == 5)
+      os << " k" << op.kd << "x" << op.kh << "x" << op.kw << " s" << op.sd << "x" << op.sh << "x" << op.sw << " p"
+         << op.pd << "x" << op.ph << "x" << op.pw;
+    else if ((op.kind == OpKind::kConv || op.kind == OpKind::kDeconv) && op.in_shape.size() == 3)
+      os << " k" << op.kw << " s" << op.sw << " p" << op.pw;
+    else if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kPool ||
+             op.kind == OpKind::kDeconv)
       os << " k" << op.kh << "x" << op.kw << " s" << op.sh << "x" << op.sw << " p" << op.ph << "x" << op.pw;
     if (op.kind == OpKind::kConvBiasReluMaxPool) os << " pool" << op.pool_kernel << "/" << op.pool_stride;
     if (op.kind == OpKind::kReLU && op.slope != 0.f) os << " slope=" << op.slope;

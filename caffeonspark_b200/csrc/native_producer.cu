@@ -86,6 +86,39 @@ struct Col2imGather {
     return __ldg(dy + ((size_t)(n * Cout + co) * OH + oh) * OW + ow);
   }
 };
+// The same two gathers over three spatial axes (a Convolution or Deconvolution over [N, C, D, H, W]).  ChanMajor and
+// WeightT serve the 3-D weight and data gradients as they are, with HW = OD OH OW and KK = KD KH KW.
+struct ConvGeom3 {
+  int C, D, H, W, KD, KH, KW, SD, SH, SW, PD, PH, PW, OD, OH, OW;
+};
+// B[k, j] of the forward: k = ((ci * KD + kd) * KH + kh) * KW + kw, j = ((n * OD + od) * OH + oh) * OW + ow; zero
+// padding
+struct Vol2col {
+  const float* x;
+  ConvGeom3 g;
+  __device__ float operator()(int k, int j) const {
+    const int kw = k % g.KW, t = k / g.KW, kh = t % g.KH, t1 = t / g.KH, kd = t1 % g.KD, ci = t1 / g.KD;
+    const int ow = j % g.OW, t2 = j / g.OW, oh = t2 % g.OH, t3 = t2 / g.OH, od = t3 % g.OD, n = t3 / g.OD;
+    const int d = od * g.SD - g.PD + kd, h = oh * g.SH - g.PH + kh, w = ow * g.SW - g.PW + kw;
+    if (d < 0 || d >= g.D || h < 0 || h >= g.H || w < 0 || w >= g.W) return 0.f;
+    return __ldg(x + (((size_t)(n * g.C + ci) * g.D + d) * g.H + h) * g.W + w);
+  }
+};
+// B[k2, j] of the data gradient: dy at the output position whose window puts tap (kd, kh, kw) on input voxel j =
+// ((n * D + d) * H + h) * W + w, k2 = ((co * KD + kd) * KH + kh) * KW + kw; g.C is Cout, dy's channels
+struct Col2volGather {
+  const float* dy;
+  ConvGeom3 g;
+  __device__ float operator()(int k2, int j) const {
+    const int kw = k2 % g.KW, t = k2 / g.KW, kh = t % g.KH, t1 = t / g.KH, kd = t1 % g.KD, co = t1 / g.KD;
+    const int w = j % g.W, t2 = j / g.W, h = t2 % g.H, t3 = t2 / g.H, d = t3 % g.D, n = t3 / g.D;
+    const int td = d + g.PD - kd, th = h + g.PH - kh, tw = w + g.PW - kw;
+    if (td < 0 || th < 0 || tw < 0 || td % g.SD || th % g.SH || tw % g.SW) return 0.f;
+    const int od = td / g.SD, oh = th / g.SH, ow = tw / g.SW;
+    if (od >= g.OD || oh >= g.OH || ow >= g.OW) return 0.f;
+    return __ldg(dy + (((size_t)(n * g.C + co) * g.OD + od) * g.OH + oh) * g.OW + ow);
+  }
+};
 
 // ------------------------------------------------------------------ epilogues
 struct StoreNCHW {  // C[m = channel, n = (img, pixel)] -> out[img, m, pixel] (+ bias[m])
@@ -1248,8 +1281,11 @@ int grid_for(int64_t n) {
   return static_cast<int>(g < 1 ? 1 : (g > kTargetSms * 16 ? kTargetSms * 16 : g));
 }
 
+// D and OD are 1 below three spatial axes, and H and OH are 1 for one ([N, C, L] runs as [N, C, 1, L])
 struct ConvDims {
   int N, Cin, H, W, Cout, OH, OW;
+  int D = 1, OD = 1;
+  bool vol = false;  // three spatial axes: the Vol2col / Col2volGather instantiations
 };
 
 // Tile's outer = count(0, axis) of its bottom
@@ -1261,23 +1297,36 @@ int64_t tile_outer(const Op& op) {
 // convolution's forward, and its weight gradient that convolution's with the bottom as dy.
 ConvDims conv_dims(const Op& op) {
   ConvDims d;
+  const size_t axes = op.in_shape.size();
+  d.vol = axes == 5;
+  // a blob's spatial axes as D, H, W
+  auto spatial = [axes](const std::vector<int64_t>& s, int* D, int* H, int* W) {
+    *D = axes == 5 ? static_cast<int>(s[2]) : 1;
+    *H = axes == 3 ? 1 : static_cast<int>(s[axes - 2]);
+    *W = static_cast<int>(s[axes - 1]);
+  };
   if (op.kind == OpKind::kDeconv) {
     d.N = static_cast<int>(op.in_shape[0]);
-    d.Cin = static_cast<int>(op.out_shape[1]), d.H = static_cast<int>(op.out_shape[2]);
-    d.W = static_cast<int>(op.out_shape[3]);
-    d.Cout = static_cast<int>(op.in_shape[1]), d.OH = static_cast<int>(op.in_shape[2]);
-    d.OW = static_cast<int>(op.in_shape[3]);
+    d.Cin = static_cast<int>(op.out_shape[1]);
+    spatial(op.out_shape, &d.D, &d.H, &d.W);
+    d.Cout = static_cast<int>(op.in_shape[1]);
+    spatial(op.in_shape, &d.OD, &d.OH, &d.OW);
     return d;
   }
   d.N = static_cast<int>(op.in_shape[0]), d.Cin = static_cast<int>(op.in_shape[1]);
-  d.H = static_cast<int>(op.in_shape[2]), d.W = static_cast<int>(op.in_shape[3]);
-  d.Cout = static_cast<int>(op.w_count / (static_cast<int64_t>(d.Cin) * op.kh * op.kw));
+  spatial(op.in_shape, &d.D, &d.H, &d.W);
+  d.Cout = static_cast<int>(op.w_count / (static_cast<int64_t>(d.Cin) * op.kd * op.kh * op.kw));
+  d.OD = (d.D + 2 * op.pd - op.kd) / op.sd + 1;
   d.OH = (d.H + 2 * op.ph - op.kh) / op.sh + 1;
   d.OW = (d.W + 2 * op.pw - op.kw) / op.sw + 1;
   return d;
 }
 ConvGeom geom(const ConvDims& d, const Op& op) {
   return ConvGeom{d.Cin, d.H, d.W, op.kh, op.kw, op.sh, op.sw, op.ph, op.pw, d.OH, d.OW};
+}
+// c: the channels of the blob the gather reads (Cin for Vol2col, Cout for Col2volGather)
+ConvGeom3 geom3(const ConvDims& d, const Op& op, int c) {
+  return ConvGeom3{c, d.D, d.H, d.W, op.kd, op.kh, op.kw, op.sd, op.sh, op.sw, op.pd, op.ph, op.pw, d.OD, d.OH, d.OW};
 }
 PoolGeom pool_geom(const Op& op) {
   return PoolGeom{static_cast<int>(op.in_shape[0]), static_cast<int>(op.in_shape[1]), static_cast<int>(op.in_shape[2]),
@@ -1322,14 +1371,25 @@ int prelu_chunks(const Op& op) { return (prelu_span(op) + kPreluChunk - 1) / kPr
 
 // The three GEMMs of a convolution of dims d: y = W * im2col(x) (+ bias); dx = W^T * dy gathered back to the input
 // (+ bias); dst += dW = dy * im2col(x)^T, split over N * OH * OW in fixed chunks added in chunk order.
+// Over three spatial axes the same three GEMMs run on Vol2col and Col2volGather, k and j extended by the depth axis.
 cudaError_t conv_forward(const Op& op, const ConvDims& d, const float* x, const float* w, const float* bias, float* y,
                          cudaStream_t s) {
+  if (d.vol) {
+    const int K = d.Cin * op.kd * op.kh * op.kw, OV = d.OD * d.OH * d.OW;
+    return gemm(DenseRM{w, K}, Vol2col{x, geom3(d, op, d.Cin)}, StoreNCHW{y, bias, d.Cout, OV}, d.Cout, d.N * OV, K,
+                K, s);
+  }
   const int K = d.Cin * op.kh * op.kw;
   return gemm(DenseRM{w, K}, Im2col{x, geom(d, op)}, StoreNCHW{y, bias, d.Cout, d.OH * d.OW}, d.Cout,
               d.N * d.OH * d.OW, K, K, s);
 }
 cudaError_t conv_data_grad(const Op& op, const ConvDims& d, const float* dy, const float* w, const float* bias, float* dx,
                            cudaStream_t s) {
+  if (d.vol) {
+    const int KK = op.kd * op.kh * op.kw, V = d.D * d.H * d.W;
+    return gemm(WeightT{w, d.Cin, KK}, Col2volGather{dy, geom3(d, op, d.Cout)}, StoreNCHW{dx, bias, d.Cin, V}, d.Cin,
+                d.N * V, d.Cout * KK, d.Cout * KK, s);
+  }
   const int KD = d.Cout * op.kh * op.kw;
   return gemm(WeightT{w, d.Cin, op.kh * op.kw},
               Col2imGather{dy, d.Cout, d.H, d.W, op.kh, op.kw, op.sh, op.sw, op.ph, op.pw, d.OH, d.OW},
@@ -1337,9 +1397,12 @@ cudaError_t conv_data_grad(const Op& op, const ConvDims& d, const float* dy, con
 }
 cudaError_t conv_weight_grad(const Op& op, const ConvDims& d, const float* x, const float* dy, float* ws, float* dst,
                              cudaStream_t s) {
-  const int K = d.N * d.OH * d.OW, KW = d.Cin * op.kh * op.kw;
-  cudaError_t e = gemm(ChanMajor{dy, d.Cout, d.OH * d.OW}, Transposed<Im2col>{Im2col{x, geom(d, op)}},
-                       StorePartial{ws, d.Cout, KW}, d.Cout, KW, K, split_chunk(K), s);
+  const int K = d.N * d.OD * d.OH * d.OW, KW = d.Cin * op.kd * op.kh * op.kw;
+  cudaError_t e =
+      d.vol ? gemm(ChanMajor{dy, d.Cout, d.OD * d.OH * d.OW}, Transposed<Vol2col>{Vol2col{x, geom3(d, op, d.Cin)}},
+                   StorePartial{ws, d.Cout, KW}, d.Cout, KW, K, split_chunk(K), s)
+            : gemm(ChanMajor{dy, d.Cout, d.OH * d.OW}, Transposed<Im2col>{Im2col{x, geom(d, op)}},
+                   StorePartial{ws, d.Cout, KW}, d.Cout, KW, K, split_chunk(K), s);
   if (e != cudaSuccess) return e;
   reduce_partials_kernel<<<grid_for(op.w_count), kThreads, 0, s>>>(ws, splits_of(K), static_cast<int>(op.w_count), dst);
   return cudaGetLastError();
@@ -1351,7 +1414,7 @@ cudaError_t conv_backward(const Op& op, const float* x, const float* dy, float* 
   const ConvDims d = conv_dims(op);
   cudaError_t e = conv_weight_grad(op, d, x, dy, ws, diff + op.w_off, s);
   if (e != cudaSuccess) return e;
-  if (bias_grad) bias_grad_kernel<<<d.Cout, kThreads, 0, s>>>(dy, d.N, d.Cout, d.OH * d.OW, diff + op.b_off);
+  if (bias_grad) bias_grad_kernel<<<d.Cout, kThreads, 0, s>>>(dy, d.N, d.Cout, d.OD * d.OH * d.OW, diff + op.b_off);
   if ((e = cudaGetLastError()) != cudaSuccess || !dx) return e;
   return conv_data_grad(op, d, dy, w, nullptr, dx, s);
 }
@@ -1363,7 +1426,7 @@ cudaError_t deconv_backward(const Op& op, const float* x, const float* dy, float
   const ConvDims d = conv_dims(op);
   cudaError_t e = conv_weight_grad(op, d, dy, x, ws, diff + op.w_off, s);
   if (e != cudaSuccess) return e;
-  if (op.b_off >= 0) bias_grad_kernel<<<d.Cin, kThreads, 0, s>>>(dy, d.N, d.Cin, d.H * d.W, diff + op.b_off);
+  if (op.b_off >= 0) bias_grad_kernel<<<d.Cin, kThreads, 0, s>>>(dy, d.N, d.Cin, d.D * d.H * d.W, diff + op.b_off);
   if ((e = cudaGetLastError()) != cudaSuccess || !dx) return e;
   return conv_forward(op, d, dy, w, nullptr, dx, s);
 }
@@ -1603,7 +1666,7 @@ bool NativeProducer::allocate(std::string* err) {
     const int64_t out = plan_.tensor_count[op.out];
     if (op.kind == OpKind::kConv || op.kind == OpKind::kConvBiasReluMaxPool || op.kind == OpKind::kDeconv) {
       const ConvDims d = conv_dims(op);
-      const size_t K = static_cast<size_t>(d.N) * d.OH * d.OW;
+      const size_t K = static_cast<size_t>(d.N) * d.OD * d.OH * d.OW;
       ws = std::max(ws, static_cast<size_t>(splits_of(static_cast<int>(K))) * op.w_count);
       if (op.kind == OpKind::kConvBiasReluMaxPool) {
         const size_t zb = static_cast<size_t>(d.N) * d.Cout * d.OH * d.OW * sizeof(float);

@@ -3,8 +3,9 @@
 // residual nets built of Split, Eltwise and Scale, autoencoders built of Flatten, Deconvolution and
 // SigmoidCrossEntropyLoss, embedding nets that read token ids through Embed and Reshape, recurrent nets built of
 // RNN layers over time-major inputs, nets normalised by MVN, U-Net segmentation nets that Crop their skips and
-// per-pixel labels, nets with a spatial-pyramid-pooling (SPP) head, and squeeze-and-excitation nets that Tile their
-// gates over the map; DESIGN.md section 14).
+// per-pixel labels, nets with a spatial-pyramid-pooling (SPP) head, squeeze-and-excitation nets that Tile their
+// gates over the map, and volumetric nets of N-D Convolution and Deconvolution over [N, C, D, H, W]; DESIGN.md
+// section 14).
 //
 // build_plan() turns the layout parser's TRAIN-phase layer list (solver_spec.hpp: the shape inference is shared
 // with the learnable layout) into an ordered op list with shapes, in-place aliasing and the flat data_/diff_ offset
@@ -55,8 +56,11 @@ struct Op {
   std::vector<int64_t> in_shape, out_shape;  // in_shape: bottoms[0]'s
   bool in_place = false;               // ReLU / Sigmoid with top == bottom: out shares bottoms[0]'s storage (never a
                                        // staged input's: those are not written)
-  // Convolution, Deconvolution, Pooling, the fused block's convolution
+  // Convolution, Deconvolution, Pooling, the fused block's convolution.  kd, sd and pd: the depth axis of a
+  // Convolution or Deconvolution over 5 axes [N, C, D, H, W] (1, 1, 0 over fewer); one over 3 axes [N, C, L] runs as
+  // the 2-D op over [N, C, 1, L] with kh 1, sh 1 and ph 0.
   int kh = 0, kw = 0, sh = 1, sw = 1, ph = 0, pw = 0;
+  int kd = 1, sd = 1, pd = 0;
   bool max_pool = true;
   int pool_kernel = 0, pool_stride = 0;  // the fused block's MAX pool (square, pad 0)
   int64_t w_off = -1, w_count = 0, b_off = -1, b_count = 0;  // flat offsets into data_ / diff_

@@ -415,9 +415,73 @@ bool input(Layer& L, std::vector<Shape>*) {
   return true;
 }
 
+// base_conv_layer.cpp LayerSetUp's rule for a repeated field of an N-D convolution: given once, or once per spatial
+// axis, or (with a default) not at all; the _h / _w form only in 2-D.  False, with Caffe's CHECK wording, otherwise.
+// `hw` names the 2-D form's prefix ("" for dilation, which has none).
+bool spatial_field(const Layer& L, const Node& p, const std::string& name, const std::string& hw, size_t axes,
+                   int64_t dflt, std::vector<int64_t>* out) {
+  if (!hw.empty() && (p.first(hw + "_h") || p.first(hw + "_w")))
+    return L.refuse(hw + "_h & " + hw + "_w can only be used for 2D convolution.");
+  auto reps = p.all(name);
+  if (!(reps.size() == 1 || reps.size() == axes || (reps.empty() && dflt >= 0)))
+    return L.refuse(name + " must be specified once, or once per spatial dimension (" + name + " specified " +
+                    std::to_string(reps.size()) + " times; " + std::to_string(axes) + " spatial dims).");
+  out->assign(axes, dflt);
+  for (size_t a = 0; a < axes && !reps.empty(); ++a) (*out)[a] = atol(reps[reps.size() == 1 ? 0 : a]->value.c_str());
+  return true;
+}
+
+// A Convolution or Deconvolution over a bottom of 3 or 5 axes, [N, C, L] or [N, C, D, H, W]: base_conv_layer.cpp's
+// per-axis fields and conv_layer.cpp / deconv_layer.cpp's output size on every spatial axis.  A 1-D layer is recorded
+// as the 2-D one over [N, C, 1, L] (kernel_h 1, stride_h 1, pad_h 0); a 3-D layer adds the depth fields.
+bool convolution_nd(Layer& L, const Node& p, const Shape& in, std::vector<Shape>* params) {
+  int64_t axis = 0;
+  if (!canonical_axis(L, p.integer("axis", 1), static_cast<int64_t>(in.size()), &axis)) return false;
+  if (axis != 1)
+    return L.refuse("convolution_param axis " + std::to_string(p.integer("axis", 1)) + " is not supported on a " +
+                    std::to_string(in.size()) + "-axis bottom (the channel axis must be 1)");
+  const size_t axes = in.size() - 2;
+  std::vector<int64_t> k, st, pad, dil;
+  if (!spatial_field(L, p, "kernel_size", "kernel", axes, -1, &k)) return false;
+  for (int64_t v : k)
+    if (v <= 0) return L.refuse("Filter dimensions must be nonzero.");
+  if (!spatial_field(L, p, "stride", "stride", axes, 1, &st)) return false;
+  for (int64_t v : st)
+    if (v <= 0) return L.refuse("Stride dimensions must be nonzero.");
+  if (!spatial_field(L, p, "pad", "pad", axes, 0, &pad) || !spatial_field(L, p, "dilation", "", axes, 1, &dil))
+    return false;
+  const int64_t nout = p.integer("num_output", 0), group = p.integer("group", 1);
+  bool ok = nout > 0 && group > 0 && in[1] % group == 0 && nout % group == 0;
+  for (size_t a = 0; a < axes; ++a) ok = ok && pad[a] >= 0 && dil[a] > 0;
+  if (!ok) return L.bad("convolution_param");
+  NetLayer& r = L.rec;
+  r.num_output = nout, r.group = group;
+  const size_t h = axes == 3 ? 1 : 0, w = axes - 1;  // the height and width axes among the spatial ones (1-D: H = 1)
+  if (axes == 3) r.kernel_d = k[0], r.stride_d = st[0], r.pad_d = pad[0], r.dilation_d = dil[0];
+  r.kernel_h = axes == 1 ? 1 : k[h], r.stride_h = axes == 1 ? 1 : st[h], r.pad_h = axes == 1 ? 0 : pad[h];
+  r.dilation_h = axes == 1 ? 1 : dil[h];
+  r.kernel_w = k[w], r.stride_w = st[w], r.pad_w = pad[w], r.dilation_w = dil[w];
+  r.bias_term = p.boolean("bias_term", true);
+  r.weight_filler = filler(p.first("weight_filler")), r.bias_filler = filler(p.first("bias_filler"));
+  const bool conv = r.type == "Convolution";
+  Shape weight{conv ? nout : in[1], conv ? in[1] / group : nout / group}, top{in[0], nout};
+  for (size_t a = 0; a < axes; ++a) {
+    const int64_t ke = dil[a] * (k[a] - 1) + 1;  // the dilated kernel
+    weight.push_back(k[a]);
+    top.push_back(conv ? (in[2 + a] + 2 * pad[a] - ke) / st[a] + 1 : st[a] * (in[2 + a] - 1) + ke - 2 * pad[a]);
+  }
+  params->push_back(weight);
+  L.set_top(0, top);
+  if (r.bias_term) params->push_back({nout});
+  return true;
+}
+
 bool convolution(Layer& L, std::vector<Shape>* params) {  // and Deconvolution; weight shapes of base_conv_layer.cpp
   const Node* p = L.node.first("convolution_param");
   Shape in;
+  if (p && L.bottom(0, &in) && in.size() >= 6)
+    return L.refuse("a bottom of " + std::to_string(in.size()) + " axes is not supported (at most 3 spatial axes are)");
+  if (p && (in.size() == 3 || in.size() == 5)) return convolution_nd(L, *p, in, params);
   if (!p || !L.bottom(0, &in) || in.size() != 4) return L.bad("Convolution");
   const int64_t nout = p->integer("num_output", 0), group = p->integer("group", 1);
   HW k = pair_field(*p, "kernel_size", "kernel_h", "kernel_w", 0), st = pair_field(*p, "stride", "stride_h", "stride_w", 1);

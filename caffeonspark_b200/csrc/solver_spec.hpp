@@ -38,6 +38,9 @@ struct NetLayer {
   // axis: InnerProduct's, Slice's, Concat's, Scale's, and SoftmaxWithLoss's class axis (softmax_param, canonical)
   int64_t num_output = 0, axis = 1, group = 1;
   int64_t kernel_h = 0, kernel_w = 0, stride_h = 1, stride_w = 1, pad_h = 0, pad_w = 0, dilation_h = 1, dilation_w = 1;
+  // the depth axis of a Convolution or Deconvolution over a 5-axis bottom [N, C, D, H, W] (1, 1, 0, 1 otherwise).  One
+  // over a 3-axis bottom [N, C, L] has kernel_h 1, stride_h 1 and pad_h 0: the 2-D layer over [N, C, 1, L].
+  int64_t kernel_d = 1, stride_d = 1, pad_d = 0, dilation_d = 1;
   bool bias_term = true, transpose = false, global_pooling = false;
   std::string pool = "MAX";
   float negative_slope = 0.f;

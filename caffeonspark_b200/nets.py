@@ -939,3 +939,84 @@ def _unet(scse):
             return crop(label, (UNET["score"], UNET["score"]), (20, 20))
 
     return UNet()
+
+
+# tests/golden/configs/vnet3d_train_test.prototxt: a small V-Net over 1 x 32 x 32 x 32 volumes and their per-voxel
+# labels (batch 2): padded 3x3x3 convolutions with PReLU and one residual sum per stage at 8, 16 and 32 channels,
+# stride-2 2x2x2 convolutions down and Deconvolutions up, skips concatenated after each Deconvolution, and a 1x1x1
+# score convolution to 2 classes at 32^3.  64,362 parameters in 32 blobs.
+VNET3D = dict(input=(1, 32, 32, 32), batch=2, classes=2)
+VNET3D_PARAM_COUNT = 64362
+# tests/golden/configs/c3d_clip_train_test.prototxt: a small C3D-style classifier over 3 x 8 x 56 x 56 clips (batch
+# 4): three 3-D convolutions with ReLU, given per spatial axis, then an InnerProduct to 10 classes.  87,146 parameters
+# in 8 blobs.
+C3D_CLIP = dict(input=(3, 8, 56, 56), batch=4, classes=10)
+C3D_CLIP_PARAM_COUNT = 87146
+
+
+def vnet3d_module():
+    """The V-Net fixture as one PyTorch module (F.conv3d / conv_transpose3d), parameters in learnable_params() order:
+    each convolution's weight and bias, then its PReLU's slopes.  forward(volumes [N, 1, 32, 32, 32]) -> scores [N, 2,
+    32, 32, 32]."""
+    import torch
+    import torch.nn as nn
+
+    class VNet3D(nn.Module):
+        def __init__(self):
+            super().__init__()
+
+            def block(name, cin, cout, k, stride=1, pad=0, deconv=False):
+                cls = nn.ConvTranspose3d if deconv else nn.Conv3d
+                setattr(self, name, cls(cin, cout, k, stride=stride, padding=pad))
+                setattr(self, "prelu_" + name, nn.PReLU(cout, init=0.25))
+
+            block("conv1a", 1, 8, 3, pad=1)
+            block("conv1b", 8, 8, 3, pad=1)
+            block("down1", 8, 16, 2, stride=2)
+            block("conv2", 16, 16, 3, pad=1)
+            block("down2", 16, 32, 2, stride=2)
+            block("conv3", 32, 32, 3, pad=1)
+            block("up2", 32, 16, 2, stride=2, deconv=True)
+            block("conv4", 32, 16, 3, pad=1)
+            block("up1", 16, 8, 2, stride=2, deconv=True)
+            block("conv5", 16, 8, 3, pad=1)
+            self.score = nn.Conv3d(8, 2, 1)
+
+        def act(self, name, x):
+            return getattr(self, "prelu_" + name)(getattr(self, name)(x))
+
+        def forward(self, x):
+            a = self.act
+            h = a("conv1a", x)
+            res1 = a("conv1b", h) + h
+            h = a("down1", res1)
+            res2 = a("conv2", h) + h
+            h = a("down2", res2)
+            h = a("conv3", h) + h
+            u = a("up2", h)
+            h = a("conv4", torch.cat([res2, u], 1)) + u
+            u = a("up1", h)
+            return self.score(a("conv5", torch.cat([res1, u], 1)) + u)
+
+    return VNet3D()
+
+
+def c3d_clip_module():
+    """The C3D clip fixture as one PyTorch module, parameters in learnable_params() order.  forward(clips [N, 3, 8, 56,
+    56]) -> scores [N, 10]."""
+    import torch
+    import torch.nn as nn
+
+    class C3DClip(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.conv1 = nn.Conv3d(3, 16, 3, stride=(1, 2, 2), padding=1)
+            self.conv2 = nn.Conv3d(16, 32, 3, stride=2, padding=1)
+            self.conv3 = nn.Conv3d(32, 32, (1, 3, 3), stride=(1, 2, 2), padding=(0, 1, 1))
+            self.fc4 = nn.Linear(32 * 4 * 7 * 7, 10)
+
+        def forward(self, x):
+            h = torch.relu(self.conv3(torch.relu(self.conv2(torch.relu(self.conv1(x))))))
+            return self.fc4(h.flatten(1))
+
+    return C3DClip()
